@@ -1,13 +1,16 @@
 #!/usr/bin/env python
 """North-star benchmark: ResNet-50 training images/sec on synthetic 224x224 batches (BASELINE.json configs[1]).
 
-    python bench.py --gpus N --steps K --warmup W            # this repo's B200 kernel path
+    python bench.py --gpus N --steps K --warmup W            # this repo's H100 kernel path
     python bench.py --impl reference --gpus N --steps K ...  # the reference's CPU trainer path (oracle port)
 
 One "step" = one full pass of the hot path over one batch: zero_grad -> forward -> CE loss -> backward ->
 (all-reduce) -> fused SGD step, batch 256 per GPU, bf16 compute / fp32 masters.  Prints ONE JSON line
 (rank 0).  ``value`` is the whole-job device-resident throughput, ``e2e`` the same metric through the
 public API (Trainer) with pinned HOST batches: H2D of every batch and D2H of the loss inside the timed region.
+
+--dump-outputs DIR writes what the last timed step computed (logits, loss, a fixed sample of the updated parameters)
+as float32 .npy files; inputs and initial weights are seeded, so two builds can be compared output for output.
 """
 import argparse
 import json
@@ -44,17 +47,15 @@ def parse():
     p.add_argument('--no-e2e', action='store_true')
     p.add_argument('--no-cpu-baseline', action='store_true')
     p.add_argument('--cpu-batch', type=int, default=32)
+    p.add_argument('--dump-outputs', metavar='DIR', default=None,
+                   help='write the outputs of the last timed step to DIR/<name>.npy (float32, <= 64 MB in all)')
     return p.parse_args()
 
 
 def peaks():
-    try:
-        with open(os.path.join(ROOT, 'MEASURED_PEAKS.json')) as f:
-            d = json.load(f)
-        return {'hbm_gbs': d['hbm_gbs'], 'tflops_burst': d['bf16_tflops'],
-                'tflops': d.get('bf16_tflops_sustained', d['bf16_tflops']), 'source': 'measured'}
-    except Exception:
-        return {'hbm_gbs': 6650.0, 'tflops_burst': 1590.0, 'tflops': 1400.0, 'source': 'fallback'}
+    """NVIDIA's data-sheet figures for the H100 SXM (700 W): HBM3 bandwidth and dense BF16 tensor rate.  A card with a
+    lower power limit runs lower clocks under sustained load, so shares of these peaks are upper-bound denominators."""
+    return {'hbm_gbs': 3350.0, 'tflops': 989.0, 'source': 'H100 SXM data sheet'}
 
 
 class ClockSampler(threading.Thread):
@@ -90,10 +91,6 @@ class ClockSampler(threading.Thread):
         reasons = [n for i, n in enumerate(names) if any(s[3 + i].lower().startswith('active') for s in self.samples)]
         return {'sm_mhz': sm[len(sm) // 2], 'sm_max_mhz': float(self.samples[0][1]), 'reasons': reasons,
                 'power_w_max': max(float(s[2]) for s in self.samples), 'samples': len(self.samples)}
-
-
-def default_cfg_for_traffic(args):
-    return args.model == 'resnet' and args.depth == 50 and args.size == IMG and args.batch == 256
 
 
 def usable_cores():
@@ -210,12 +207,12 @@ def main():
             loss = criterion(out, y_dev)
             loss.backward()
         else:
-            loss = replayed[1]
+            out, loss = replayed[0], replayed[1]
         trainer._allreduce_gradients()
         optimizer.set_grad_unscale(1.0, world)
         optimizer.step()
         trainer.training_steps += 1
-        return loss
+        return out, loss
 
     for _ in range(max(args.warmup, 4)):   # steps 1-2 eager, 3 captures the CUDA graph, 4+ replay it
         device_step()
@@ -228,7 +225,7 @@ def main():
     e0.record()
     t_enq = time.perf_counter()
     for _ in range(args.steps):
-        loss = device_step()
+        out, loss = device_step()
     e1.record()
     enqueue_ms = (time.perf_counter() - t_enq) * 1e3 / args.steps     # host time to launch one step (no syncs)
     torch.cuda.synchronize()
@@ -240,6 +237,8 @@ def main():
     ms = float(t)
     clocks = sampler.stop() if sampler else None
     final_loss = float(loss.detach())
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, model, out, loss)
     sync_all()
 
     # ---- end to end through the public API: pinned host batches, H2D + loss D2H inside the timed region ----
@@ -248,7 +247,7 @@ def main():
         loader = [(x_host, y_host)] * 2
         trainer.forward(loader, training=True)           # warm the path
         sync_all()
-        n_e2e = max(10, args.steps)
+        n_e2e = args.steps
         # raw pinned-host -> device bandwidth of this box (explains e2e when PCIe, not the GPU, is the bound)
         h2d_ms = float('inf')
         x_probe = torch.empty_like(x_dev)
@@ -330,19 +329,8 @@ def main():
             ach = d['bytes'] / (d['ms'] * 1e-3) / 1e9
             roof = {'kernel': dom, 'bound': 'hbm', 'achieved': ach, 'peak': pk['hbm_gbs'], 'unit': 'GB/s',
                     'frac': ach / pk['hbm_gbs'], 'traffic': None}
-        # traffic: DRAM bytes (ncu dram__bytes_read.sum + dram__bytes_write.sum) per launch of the dominant class, from
-        # the committed launch list of this same command (profiles/r02_traffic.json; tools/profile_round2.sh)
-        try:
-            with open(os.path.join(ROOT, 'profiles', 'r02_traffic.json')) as f:
-                tj = json.load(f)['classes']
-            key = dom if dom in tj else ('conv_fprop+dgrad' if dom in ('conv_fprop', 'conv_dgrad') else None)
-            if key and default_cfg_for_traffic(args):
-                roof['traffic'] = (tj[key]['dram_read_bytes'] + tj[key]['dram_write_bytes']) / max(tj[key]['launches'], 1)
-                roof['traffic_unit'] = 'bytes per launch (class average; ncu, profiles/r02_traffic.json)'
-                roof['algorithmic_bytes_per_launch'] = d['bytes'] / max(d['calls'], 1) if d.get('bytes') else None
-        except Exception:
-            pass
-        roof['peak_source'] = pk['source'] + (' sustained' if dom.startswith('conv_') else '')
+        roof['algorithmic_bytes_per_launch'] = d['bytes'] / max(d['calls'], 1) if d.get('bytes') else None
+        roof['peak_source'] = pk['source']
         roof['launches_of_kernel_per_step'] = d['calls']
         roof['avg_launch_ms'] = d['ms'] / max(d['calls'], 1)
         roof['step_share'] = d['ms'] / total_ms if total_ms else None
@@ -373,7 +361,7 @@ def main():
                                        % (name, args.size, args.size, B,
                                           ' (BASELINE.json configs[1])' if default_cfg else ''),
                            'global_batch': world * B, 'parallelism': 'dp%d' % world,
-                           'l2_policy': 'per-step working set (activations ~10 GB) >> 126 MB L2; no explicit flush'},
+                           'l2_policy': 'per-step working set (activations ~10 GB) >> 50 MB L2; no explicit flush'},
                 'clocks': clocks, 'e2e': e2e, 'gpu_launches': launches, 'roofline': roof, 'cpu_baseline': cpu_base,
                 'final_loss': final_loss,
                 'conv_tensor_pipe_frac': (world * B * args.steps * TRAIN_CONV_GFLOP_PER_IMG / (ms * 1e-3) / 1e3
@@ -381,6 +369,23 @@ def main():
         print(json.dumps(line), flush=True)
     if distributed:
         shutdown(trainer)
+
+
+DUMP_PARAM_SAMPLE = 1 << 22     # 16 MB of float32: with the logits well under 64 MB in all
+
+
+def dump_outputs(path, model, logits, loss):
+    """What the timed step hands its caller: the logits and loss of the last step and the parameters after its SGD update
+    (a fixed, seeded sample of DUMP_PARAM_SAMPLE elements of their concatenation in named_parameters() order)."""
+    import numpy as np
+    os.makedirs(path, exist_ok=True)
+    flat = torch.cat([p.detach().float().flatten() for _, p in model.named_parameters()])
+    g = torch.Generator().manual_seed(0)
+    idx = torch.randperm(flat.numel(), generator=g)[:DUMP_PARAM_SAMPLE].sort().values
+    arrays = {'logits': logits.detach().float(), 'loss': loss.detach().float().reshape(-1)[:1],
+              'params_sample': flat[idx.to(flat.device)]}
+    for name, a in arrays.items():
+        np.save(os.path.join(path, name + '.npy'), a.cpu().numpy())
 
 
 def shutdown(trainer):

@@ -1,4 +1,4 @@
-"""convnet.pytorch_b200 -- a Blackwell (sm_100a) native training hot path behind the public surface of
+"""convnet.pytorch_b200 -- a Hopper (sm_90a) native training hot path behind the public surface of
 eladhoffer/convNet.pytorch: ``trainer.Trainer``, the ``models`` registry (ResNet / ResNeXt / MobileNet-v2),
 ``utils.optim.OptimRegime`` regimes and the ``main.py`` CLI.
 

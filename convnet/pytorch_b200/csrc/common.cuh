@@ -1,10 +1,12 @@
-// Shared device helpers for the sm_100a kernels: mbarrier, TMA, tcgen05/TMEM wrappers.
-// Everything here is inline PTX for compute_100a; nothing is borrowed from a library.
+// Shared device helpers for the sm_90a kernels: mbarrier, TMA, wgmma wrappers.
+// Everything here is inline PTX for compute_90a; nothing is borrowed from a library.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
 #include <stdint.h>
+#include "wgmma.cuh"
+#include "../../../include/b200conv.h"
 
 #ifndef B200_WAIT_TIMEOUT_NS
 #define B200_WAIT_TIMEOUT_NS 4000000000ull  // 4 s
@@ -135,75 +137,50 @@ __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
 
-// ---------------------------------------------------------------- tcgen05 / TMEM
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;"
-               ::"r"(smem_u32(smem_dst)), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t addr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(addr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc], bf16 inputs, fp32 accumulate; single-thread issue
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b,
-                                          uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// all previously issued MMAs of this thread arrive on the mbarrier when complete
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];"
-               ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-// 32 lanes x 16 consecutive fp32 columns: thread t gets TMEM lane (base_lane + t), columns [col, col+16)
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-        "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr) : "memory");
+// ---------------------------------------------------------------- wgmma
+// Warpgroup MMA (sm_90a): a warpgroup (4 consecutive warps, the first a multiple of 4) issues wgmma.mma_async with both
+// operands in shared memory; the fp32 accumulators live in the issuing threads' registers (wgmma.cuh).
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// Orders ordinary register accesses of the accumulators against the asynchronous MMAs that write them.
+template <int SZ>
+__device__ __forceinline__ void wgmma_fence_acc(float (&d)[SZ]) {
+#pragma unroll
+  for (int i = 0; i < SZ; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// Shared-memory matrix descriptor (tcgen05 "version 1").
+// Shared-memory matrix descriptor of wgmma.
 //  start address [0,14) (>>4), leading byte offset [16,30) (>>4), stride byte offset [32,46) (>>4),
-//  version [46,48) = 1, layout type [61,64): 0 none, 2 = 128B swizzle, 4 = 64B, 6 = 32B.
+//  layout type [62,64): 0 none, 1 = 128B swizzle, 2 = 64B, 3 = 32B.  The swizzle is a function of the absolute
+//  shared-memory address, so a descriptor may be advanced by any multiple of 16 bytes into a TMA-written buffer.
+//  K-major: SBO = distance between 8-row groups (LBO unused with a swizzle).
+//  MN-major: LBO = distance between swizzle-width column blocks along M/N, SBO = distance between 8-row groups along K.
 __device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes,
                                                    uint32_t layout_type) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((saddr >> 4) & 0x3FFF);
   d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(layout_type & 7) << 61;
+  d |= static_cast<uint64_t>(layout_type & 3) << 62;
   return d;
 }
 __device__ __host__ __forceinline__ uint32_t layout_type_for_row_bytes(uint32_t row_bytes) {
-  return row_bytes == 128 ? 2u : (row_bytes == 64 ? 4u : 6u);
+  return row_bytes == 128 ? 1u : (row_bytes == 64 ? 2u : 3u);
 }
-// Instruction descriptor for kind::f16, bf16 x bf16 -> fp32.
-__device__ __host__ __forceinline__ uint32_t make_idesc_bf16(uint32_t M, uint32_t N, uint32_t a_mn_major,
-                                                             uint32_t b_mn_major) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | (a_mn_major << 15) | (b_mn_major << 16) |
-         ((N >> 3) << 17) | ((M >> 4) << 24);
-}
+// Accumulator fragment of m64nNk16 for thread t of the warpgroup: element i sits at row 16 * (t / 32) + (t % 32) / 4
+// + 8 * ((i / 2) % 2), column 8 * (i / 4) + 2 * (t % 4) + i % 2.
 
 // ---------------------------------------------------------------- misc
+__device__ __forceinline__ float apply_act(float v, int act) {
+  return act == B200_ACT_RELU ? fmaxf(v, 0.f) : (act == B200_ACT_RELU6 ? fminf(fmaxf(v, 0.f), 6.f) : v);
+}
+// consumer warp: its MMAs are done reading a ring slot whose empty barrier counts one arrival per consumer warp
+__device__ __forceinline__ void release_stage(uint64_t* empty_bar, int lane) {
+  __syncwarp();
+  if (lane == 0) mbar_arrive(empty_bar);
+}
 __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
   __nv_bfloat162 v = __floats2bfloat162_rn(lo, hi);
   return *reinterpret_cast<uint32_t*>(&v);

@@ -1,13 +1,13 @@
-// Implicit-GEMM convolution on tcgen05 tensor cores (sm_100a): fprop, dgrad, wgrad.
+// Implicit-GEMM convolution on Hopper tensor cores (sm_90a wgmma): fprop, dgrad, wgrad.
 //
 //   fprop : y[m, k]   = sum_{tap, c} x_im2col[m, tap, c] * w[k, tap, c]        (A K-major, B K-major)
 //   dgrad : dx[m, c]  = sum_{tap, k} dy_im2col[m, tap, k] * wt[c, tap, k]       (same kernel, tap table)
 //   wgrad : dw[k, tap, c] += sum_{pix} dy[pix, k] * x_im2col[pix, tap, c]       (A MN-major, B MN-major)
 //
 // Operand tiles are staged by TMA (im2col mode for the activation side, tiled mode for weights / dy)
-// into 32/64/128B-swizzled shared memory, consumed by single-thread-issued tcgen05.mma with fp32
-// accumulators in TMEM, drained by 4 epilogue warps with tcgen05.ld.
-// Warp roles: warp 0 = TMA producer, warp 1 = MMA issuer (+TMEM alloc), warps 2..5 = epilogue.
+// into 32/64/128B-swizzled shared memory and consumed by wgmma.mma_async with fp32 accumulators in registers.
+// Warp roles: warps 0..7 = two consumer warpgroups (rows 0-63 and 64-127 of a 128-row tile: MMA, then the epilogue),
+// warp 8 (of the third warpgroup) = TMA producer, which runs ahead through the stage ring while the consumers drain a tile.
 //
 // Replaces cuDNN's convolution behind nn.Conv2d in the reference (models/resnet.py:75-78,126-132,
 // 226-227) and its autograd backward (trainer.py:162).
@@ -19,10 +19,11 @@ namespace b200 {
 
 constexpr int kMaxStages = 8;
 constexpr int kMaxTaps = 32;
-constexpr int kThreads = 192;        // wgrad: TMA warp, MMA warp, 4 epilogue warps
-constexpr int kIgemmThreads = 320;   // igemm: TMA warp, MMA warp, 8 epilogue warps (2 per TMEM lane quarter)
+constexpr int kThreads = 384;        // two consumer warpgroups + a producer warpgroup (only warp 8 works: registers are allocated
+                                     // per warpgroup in wgmma kernels, so 288 threads would cost as much as 384)
+constexpr int kConsumers = 256;
+constexpr int kProducerWarp = 8;
 constexpr int kTileM = 128;
-constexpr uint32_t kTmemCols = 512;
 constexpr int kStatReplicas = 16;    // must match kReplicas of bn.cu (layout of the BN workspace accumulators)
 
 struct TapEntry {
@@ -53,11 +54,10 @@ struct IgemmParams {
                          // once -- and walks the m-tiles blockIdx.x / n_tiles, + gridDim.x / n_tiles, ... (the grid is a
                          // multiple of n_tiles).  Cuts the L2->SM re-streaming of the weights from once per tile to once
                          // per CTA for layers whose per-n-tile weights fit in shared memory (K <= 256 at N-tile 256)
-  int epi_bufs;          // 1 or 2 output staging tiles: with 2 the residual tile of the NEXT tile is fetched while this one
-                         // is converted and stored, and a store never waits for the previous one (write-heavy epilogues)
-  uint32_t epi_bytes;
   int window;            // > 0: block-diagonal convolution -- n-tile b (block_n == window) reads source channels
                          // [window*b, window*b + window) only; the weight operand is [N_total][taps][window]
+  int epi_bufs;          // 1 or 2 output staging tiles: with 2, a tile's staging never waits for the previous tile's store
+  uint32_t epi_bytes;
   double* stats;         // fused BN statistics accumulators [kStatReplicas][2][N_total] (BN workspace) or nullptr
   void* out;
   const void* res;
@@ -65,84 +65,55 @@ struct IgemmParams {
   TapEntry taps[kMaxTaps];
 };
 
-__device__ __forceinline__ void store_chunk16(const IgemmParams& p, const uint32_t (&v)[16], long long off,
-                                              int n0, bool row_ok) {
-  // v: 16 consecutive fp32 accumulators (as bits) for columns [n0, n0+16) of this thread's row
-  if (!row_ok) return;
-  float f[16];
-#pragma unroll
-  for (int i = 0; i < 16; ++i) f[i] = __uint_as_float(v[i]);
-  const bool full = (n0 + 16 <= p.N_total);
+// Columns n, n+1 (n even) of one output row through the generic output mapping; off = element offset of the row.
+__device__ __forceinline__ void store_pair(const IgemmParams& p, float v0, float v1, long long off, int n) {
+  if (n >= p.N_total) return;
+  const bool two = n + 1 < p.N_total;
+  const bool vec = two && (p.ldo & 1) == 0;
   if (p.bias != nullptr) {
-#pragma unroll
-    for (int i = 0; i < 16; ++i)
-      if (n0 + i < p.N_total) f[i] += __ldg(p.bias + n0 + i);
+    v0 += __ldg(p.bias + n);
+    if (two) v1 += __ldg(p.bias + n + 1);
   }
   if (p.res != nullptr) {
-    const __nv_bfloat16* r = reinterpret_cast<const __nv_bfloat16*>(p.res) + off + n0;
-    if (full && ((p.ldo & 7) == 0)) {
-      const uint4 r0 = *reinterpret_cast<const uint4*>(r);
-      const uint4 r1 = *reinterpret_cast<const uint4*>(r + 8);
-      const uint32_t rr[8] = {r0.x, r0.y, r0.z, r0.w, r1.x, r1.y, r1.z, r1.w};
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        float2 t = unpack_bf16x2(rr[i]);
-        f[2 * i] += t.x;
-        f[2 * i + 1] += t.y;
-      }
+    const __nv_bfloat16* r = reinterpret_cast<const __nv_bfloat16*>(p.res) + off + n;
+    if (vec) {
+      const float2 t = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(r));
+      v0 += t.x;
+      v1 += t.y;
     } else {
-#pragma unroll
-      for (int i = 0; i < 16; ++i)
-        if (n0 + i < p.N_total) f[i] += __bfloat162float(r[i]);
+      v0 += __bfloat162float(r[0]);
+      if (two) v1 += __bfloat162float(r[1]);
     }
   }
-  if (p.act == B200_ACT_RELU) {
-#pragma unroll
-    for (int i = 0; i < 16; ++i) f[i] = fmaxf(f[i], 0.f);
-  } else if (p.act == B200_ACT_RELU6) {
-#pragma unroll
-    for (int i = 0; i < 16; ++i) f[i] = fminf(fmaxf(f[i], 0.f), 6.f);
-  }
+  v0 = apply_act(v0, p.act);
+  v1 = apply_act(v1, p.act);
   if (p.out_fp32) {
-    float* o = reinterpret_cast<float*>(p.out) + off + n0;
-    if (full && ((p.ldo & 3) == 0)) {
-#pragma unroll
-      for (int i = 0; i < 4; ++i)
-        *reinterpret_cast<float4*>(o + 4 * i) = make_float4(f[4 * i], f[4 * i + 1], f[4 * i + 2], f[4 * i + 3]);
+    float* o = reinterpret_cast<float*>(p.out) + off + n;
+    if (vec) {
+      *reinterpret_cast<float2*>(o) = make_float2(v0, v1);
     } else {
-#pragma unroll
-      for (int i = 0; i < 16; ++i)
-        if (n0 + i < p.N_total) o[i] = f[i];
+      o[0] = v0;
+      if (two) o[1] = v1;
     }
   } else {
-    __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(p.out) + off + n0;
-    if (full && ((p.ldo & 7) == 0)) {
-      uint4 a, b;
-      a.x = pack_bf16x2(f[0], f[1]);   a.y = pack_bf16x2(f[2], f[3]);
-      a.z = pack_bf16x2(f[4], f[5]);   a.w = pack_bf16x2(f[6], f[7]);
-      b.x = pack_bf16x2(f[8], f[9]);   b.y = pack_bf16x2(f[10], f[11]);
-      b.z = pack_bf16x2(f[12], f[13]); b.w = pack_bf16x2(f[14], f[15]);
-      *reinterpret_cast<uint4*>(o) = a;
-      *reinterpret_cast<uint4*>(o + 8) = b;
+    __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(p.out) + off + n;
+    if (vec) {
+      *reinterpret_cast<uint32_t*>(o) = pack_bf16x2(v0, v1);
     } else {
-#pragma unroll
-      for (int i = 0; i < 16; ++i)
-        if (n0 + i < p.N_total) o[i] = __float2bfloat16(f[i]);
+      o[0] = __float2bfloat16(v0);
+      if (two) o[1] = __float2bfloat16(v1);
     }
   }
 }
 
-__global__ void __launch_bounds__(kIgemmThreads, 1)
+__global__ void __launch_bounds__(kThreads, 1)
 conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                   const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmR,
                   const __grid_constant__ IgemmParams p) {
   extern __shared__ uint8_t smem_raw[];
   __shared__ __align__(8) uint64_t full_bar[kMaxStages];
   __shared__ __align__(8) uint64_t empty_bar[kMaxStages];
-  __shared__ __align__(8) uint64_t tmem_full[2];
-  __shared__ __align__(8) uint64_t tmem_empty[2];
-  __shared__ __align__(8) uint64_t res_bar[2], bstat_bar;
-  __shared__ uint32_t tmem_base_s;
+  __shared__ __align__(8) uint64_t res_bar[2][2], bstat_bar;   // [warpgroup][staging buffer]
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -150,20 +121,15 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   uint8_t* smem = smem_raw + (((raw_addr + 1023u) & ~1023u) - raw_addr);
   const uint32_t stage_bytes = p.b_stationary ? p.a_bytes : p.a_bytes + p.b_bytes;
   uint8_t* sBstat = smem + p.num_stages * stage_bytes;   // stationary weight slices [tap * c_chunks + k-block]
-  uint8_t* epi_base = sBstat + (p.b_stationary ? static_cast<uint32_t>(p.ntaps * p.c_chunks) * p.b_bytes : 0u);
+  uint8_t* epi = sBstat + (p.b_stationary ? static_cast<uint32_t>(p.ntaps * p.c_chunks) * p.b_bytes : 0u);
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < p.num_stages; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
+      mbar_init(&empty_bar[s], kConsumers / 32);
     }
     mbar_init(&bstat_bar, 1);
-    mbar_init(&tmem_full[0], 1);
-    mbar_init(&tmem_full[1], 1);
-    mbar_init(&tmem_empty[0], 8);
-    mbar_init(&tmem_empty[1], 8);
-    mbar_init(&res_bar[0], 1);
-    mbar_init(&res_bar[1], 1);
+    for (int i = 0; i < 4; ++i) mbar_init(&res_bar[i >> 1][i & 1], 1);
     fence_mbar_init();
     prefetch_tmap(&tmA);
     prefetch_tmap(&tmB);
@@ -172,15 +138,8 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       if (p.res != nullptr) prefetch_tmap(&tmR);
     }
   }
-  if (warp == 1) {
-    tmem_alloc(&tmem_base_s, kTmemCols);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  pdl_wait();   // prologue above (barriers, TMEM, descriptor prefetch) overlaps the predecessor grid
-  const uint32_t tmem_base = tmem_base_s;
+  pdl_wait();   // prologue above (barriers, descriptor prefetch) overlaps the predecessor grid
 
   const int total_tiles = p.m_tiles * p.n_tiles;
   const int k_iters = p.ntaps * p.c_chunks;
@@ -190,8 +149,8 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   const int walk_end = p.own_ntile ? p.m_tiles : total_tiles;
   const int own_n = static_cast<int>(blockIdx.x) % p.n_tiles;
 
-  if (warp == 0) {
-    if (lane == 0) {
+  if (warp >= kProducerWarp) {
+    if (warp == kProducerWarp && lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
       const int IJ = p.I * p.J;
@@ -230,226 +189,171 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      const uint32_t idesc = make_idesc_bf16(kTileM, p.block_n, 0, 0);
-      const uint32_t row_bytes = p.ck * 2;
-      // The issuing thread is latency-bound per instruction: build the descriptor once and advance its address field
-      // (bytes >> 4) instead of re-encoding it for every MMA.
-      const uint64_t proto = make_smem_desc(0, 16, 8 * row_bytes, layout_type_for_row_bytes(row_bytes));
-      const int ksteps = p.ck / 16;
-      if (p.b_stationary && walk_first < walk_end) {
-        mbar_wait(&bstat_bar, 0);
-        tc_fence_after();
+    return;
+  }
+
+  // ---- consumers: warpgroup wg computes rows [64 wg, 64 wg + 64) of every tile.  The two warpgroups share the operand
+  // ring but nothing else: each stages, stores and (optionally) reduces the statistics of its own 64 rows, so one
+  // warpgroup's epilogue overlaps the other's MMAs.
+  const int wg = warp >> 2;
+  const int wt = threadIdx.x & 127;                           // thread index inside the warpgroup
+  const int r_lo = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // this thread's fragment rows: r_lo and r_lo + 8
+  const int c_lo = 2 * (lane & 3);
+  const bool leader = wt == 0;
+  const uint32_t row_bytes = p.ck * 2;
+  const uint64_t proto = make_smem_desc(0, 16, 8 * row_bytes, layout_type_for_row_bytes(row_bytes));
+  const uint32_t a_wg = (64u * row_bytes * wg) >> 4;
+  const int ksteps = p.ck / 16;
+  const uint32_t bstat_addr = smem_u32(sBstat);
+  const int nbox = p.block_n >> 6;
+  // fused-statistics bookkeeping: this thread owns columns st_col (+ 128 when block_n == 256), rows
+  // [st_row0, st_row0 + st_rows) of its warpgroup's half of each tile
+  const int st_col = wt % p.block_n;
+  const int st_ncol = p.block_n > 128 ? 2 : 1;
+  const int st_rows = 64 / (p.block_n > 128 ? 1 : 128 / p.block_n);
+  const int st_row0 = wg * 64 + (p.block_n > 128 ? 0 : (wt / p.block_n) * st_rows);
+  int st_ntile = -1;
+  float st_s1[2] = {0.f, 0.f}, st_s2[2] = {0.f, 0.f};
+  auto flush_stats = [&]() {
+    for (int u = 0; u < st_ncol; ++u) {
+      double* dst = p.stats + (blockIdx.x % kStatReplicas) * 2 * p.N_total + st_ntile * p.block_n + st_col + 128 * u;
+      atomicAdd(dst, (double)st_s1[u]);
+      atomicAdd(dst + p.N_total, (double)st_s2[u]);
+      st_s1[u] = 0.f; st_s2[u] = 0.f;
+    }
+  };
+  const int IJ = p.I * p.J;
+  if (p.b_stationary && walk_first < walk_end) mbar_wait(&bstat_bar, 0);
+
+  float acc[128];
+  int stage = 0;
+  uint32_t phase = 0;
+  int local = 0;
+  for (int tile = walk_first; tile < walk_end; tile += walk_step, ++local) {
+    const int m_tile = p.own_ntile ? tile : tile / p.n_tiles;
+    const int n_tile = p.own_ntile ? own_n : tile - m_tile * p.n_tiles;
+    const int nbase = n_tile * p.block_n;
+    const int eb = p.epi_bufs == 2 ? (local & 1) : 0;
+    uint8_t* epi_t = epi + eb * p.epi_bytes;   // staging tile of this tile: 64-column boxes of [128 rows][128 B]
+    if (p.tma_store) {
+      // This warpgroup's rows of the staging tile are reused: its store of the tile that last used the buffer must
+      // have read them and its threads must be done with their statistics reads.  Then its half of the residual tile
+      // is fetched into them, landing while the MMAs run.
+      if (leader && local > 0) {
+        if (p.epi_bufs == 2) bulk_wait_group_read1();
+        else bulk_wait_group_read0();
       }
-      const uint32_t bstat_addr = smem_u32(sBstat);
-      int local = 0;
-      for (int tile = walk_first; tile < walk_end; tile += walk_step, ++local) {
-        const int acc = local & 1;
-        const uint32_t acc_phase = (local >> 1) & 1u;
-        mbar_wait(&tmem_empty[acc], acc_phase ^ 1u);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * 256;
-        for (int it = 0; it < k_iters; ++it) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint32_t a_addr = smem_u32(smem + stage * stage_bytes);
-          const uint64_t da = proto + (a_addr >> 4);
-          const uint64_t db = proto + ((p.b_stationary ? bstat_addr + it * p.b_bytes : a_addr + p.a_bytes) >> 4);
-          if (ksteps == 4) {
-            umma_bf16(d_tmem, da, db, idesc, it != 0 ? 1u : 0u);
-            umma_bf16(d_tmem, da + 2, db + 2, idesc, 1u);
-            umma_bf16(d_tmem, da + 4, db + 4, idesc, 1u);
-            umma_bf16(d_tmem, da + 6, db + 6, idesc, 1u);
-          } else {
-            for (int k = 0; k < ksteps; ++k) umma_bf16(d_tmem, da + 2 * k, db + 2 * k, idesc, (it | k) != 0 ? 1u : 0u);
-          }
-          umma_commit(&empty_bar[stage]);
-          if (it == k_iters - 1) umma_commit(&tmem_full[acc]);
-          if (++stage == p.num_stages) { stage = 0; phase ^= 1u; }
-        }
+      named_bar_sync(1 + wg, 128);
+      if (leader && p.res != nullptr) {
+        fence_proxy_async();
+        mbar_arrive_expect_tx(&res_bar[wg][eb], static_cast<uint32_t>(nbox) * 64u * 128u);
+        for (int b = 0; b < nbox; ++b)
+          tma_load_2d(&tmR, &res_bar[wg][eb], epi_t + b * (kTileM * 128) + wg * 64 * 128, nbase + b * 64,
+                      m_tile * kTileM + wg * 64);
       }
     }
-  } else {
-    const int q = warp & 3;            // TMEM lane quarter this warp may read
-    const int half = (warp - 2) >> 2;  // the two warps of a quarter take alternate 16-column chunks
-    // fused-statistics bookkeeping: this thread owns column st_col, rows [st_row0, st_row0 + st_rows) of each tile
-    const int st_tid = threadIdx.x - 64;
-    const int st_col = st_tid % p.block_n;
-    const int st_rows = kTileM / (256 / p.block_n);
-    const int st_row0 = (st_tid / p.block_n) * st_rows;
-    int st_ntile = -1;
-    float st_s1 = 0.f, st_s2 = 0.f;
-    const int IJ = p.I * p.J;
-    int local = 0;
-    for (int tile = walk_first; tile < walk_end; tile += walk_step, ++local) {
-      const int acc = local & 1;
-      const uint32_t acc_phase = (local >> 1) & 1u;
-      const int m_tile = p.own_ntile ? tile : tile / p.n_tiles;
-      const int n_tile = p.own_ntile ? own_n : tile - m_tile * p.n_tiles;
-      const int m = m_tile * kTileM + q * 32 + lane;
-      const bool row_ok = m < p.M_total;
-      long long off = 0;
-      if (row_ok) {
-        const int img = m / IJ;
-        const int rem = m - img * IJ;
-        const int bi = rem / p.J;
-        const int bj = rem - bi * p.J;
-        off = ((static_cast<long long>(img) * p.OH + (bi * p.os + p.oh0)) * p.OW + (bj * p.os + p.ow0)) *
-              static_cast<long long>(p.ldo);
+
+    wgmma_fence_acc(acc);
+    int prev = 0;
+    for (int it = 0; it < k_iters; ++it) {
+      mbar_wait(&full_bar[stage], phase);
+      const uint32_t a_addr = smem_u32(smem + stage * stage_bytes);
+      const uint64_t da = proto + (a_addr >> 4) + a_wg;
+      const uint64_t db = proto + ((p.b_stationary ? bstat_addr + it * p.b_bytes : a_addr + p.a_bytes) >> 4);
+      wgmma_fence();
+      for (int k = 0; k < ksteps; ++k)
+        wgmma_bf16<0, 0>(acc, p.block_n, da + 2 * k, db + 2 * k, (it | k) != 0 ? 1u : 0u);
+      wgmma_commit();
+      wgmma_wait<1>();                                    // the previous iteration's MMAs are done with their stage
+      if (it > 0) release_stage(&empty_bar[prev], lane);
+      prev = stage;
+      if (++stage == p.num_stages) { stage = 0; phase ^= 1u; }
+    }
+    wgmma_wait<0>();
+    wgmma_fence_acc(acc);
+    release_stage(&empty_bar[prev], lane);
+
+    if (p.tma_store) {
+      // Dense bf16 output: stage the tile in 128B-swizzled shared memory and write it with TMA (coalesced, clipped at
+      // the M tail); the residual was fetched into the same buffer.
+      if (p.res != nullptr)
+        mbar_wait(&res_bar[wg][eb], static_cast<uint32_t>((p.epi_bufs == 2 ? local >> 1 : local) & 1));
+#pragma unroll
+      for (int j = 0; j < 128; j += 4) {
+        const int c = 2 * j + c_lo;
+        if (2 * j < p.block_n) {
+          float bias0 = 0.f, bias1 = 0.f;
+          if (p.bias != nullptr) { bias0 = __ldg(p.bias + nbase + c); bias1 = __ldg(p.bias + nbase + c + 1); }
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int row = r_lo + 8 * h;
+            uint32_t* dst = reinterpret_cast<uint32_t*>(epi_t + (c >> 6) * (kTileM * 128) + row * 128 +
+                                                        ((((c & 63) >> 3) ^ (row & 7)) << 4) + (c & 7) * 2);
+            float v0 = acc[j + 2 * h] + bias0, v1 = acc[j + 2 * h + 1] + bias1;
+            if (p.res != nullptr) {
+              const float2 t = unpack_bf16x2(*dst);
+              v0 += t.x;
+              v1 += t.y;
+            }
+            *dst = pack_bf16x2(apply_act(v0, p.act), apply_act(v1, p.act));
+          }
+        }
       }
-      const uint32_t taddr = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + acc * 256;
-      const int nbase = n_tile * p.block_n;
-      if (p.tma_store) {
-        // Dense bf16 output: stage the tile in 128B-swizzled shared memory and write it with TMA (coalesced,
-        // clipped at the M tail); the residual tile is fetched by TMA into the same buffer and updated in place.
-        const bool leader = (warp == 2 && lane == 0);
-        const int row = q * 32 + lane;
-        const int nbox = p.block_n >> 6;
-        // staging buffer of this tile; with two buffers tile i uses buffer i & 1
-        const int eb = p.epi_bufs == 2 ? (local & 1) : 0;
-        uint8_t* epi = epi_base + eb * p.epi_bytes;
-        if (leader) {
-          // the buffer about to be (re)written must no longer be read by an earlier TMA store: one buffer -> the
-          // previous store; two buffers -> the store before the previous one, unless the NEXT tile's residual is
-          // prefetched below into the buffer the previous store used
-          if (local > 0) {
-            if (p.epi_bufs == 2 && p.res == nullptr) { if (local > 1) bulk_wait_group_read1(); }
-            else bulk_wait_group_read0();
-          }
-          if (p.res != nullptr) {
-            auto fetch = [&](int t_tile, int buf) {
-              const int mt = p.own_ntile ? t_tile : t_tile / p.n_tiles;
-              const int nt = p.own_ntile ? own_n : t_tile - mt * p.n_tiles;
-              uint8_t* dst = epi_base + buf * p.epi_bytes;
-              mbar_arrive_expect_tx(&res_bar[buf], static_cast<uint32_t>(nbox) * kTileM * 128u);
-              for (int b = 0; b < nbox; ++b)
-                tma_load_2d(&tmR, &res_bar[buf], dst + b * (kTileM * 128), nt * p.block_n + b * 64, mt * kTileM);
-            };
-            if (p.epi_bufs == 2) {
-              if (local == 0) fetch(tile, 0);
-              const int next = tile + walk_step;
-              if (next < walk_end) fetch(next, eb ^ 1);         // lands while this tile is converted and stored
-            } else {
-              fetch(tile, 0);
-            }
-          }
+      fence_proxy_async();                             // generic-proxy smem writes -> visible to TMA
+      named_bar_sync(1 + wg, 128);
+      if (leader) {
+        for (int b = 0; b < nbox; ++b)
+          tma_store_2d(&tmC, epi_t + b * (kTileM * 128) + wg * 64 * 128, nbase + b * 64, m_tile * kTileM + wg * 64);
+        bulk_commit_group();
+      }
+      if (p.stats != nullptr) {
+        // Fused BN statistics: per-channel sum / sum of squares of the bf16-rounded outputs of this tile,
+        // read back from the staged tile (rows beyond M_total are exact zeros).  Accumulated in registers
+        // across the tiles of this CTA while it stays on the same channel block, then one fp64 atomic each.
+        if (st_ntile != n_tile) {
+          if (st_ntile >= 0) flush_stats();
+          st_ntile = n_tile;
         }
-        named_bar_sync(1, 256);
-        if (p.res != nullptr) {
-          // buffer b receives tiles b, b+2, b+4, ... (two buffers) or every tile (one buffer): k-th use -> parity k & 1
-          const uint32_t use = p.epi_bufs == 2 ? static_cast<uint32_t>(local >> 1) : static_cast<uint32_t>(local);
-          mbar_wait(&res_bar[eb], use & 1u);
-        }
-        mbar_wait(&tmem_full[acc], acc_phase);
-        tc_fence_after();
-        for (int c0 = half * 16; c0 < p.block_n; c0 += 32) {
-          uint32_t v[16];
-          tmem_ld16(taddr + c0, v);
-          tmem_ld_wait();
-          float f[16];
-#pragma unroll
-          for (int i = 0; i < 16; ++i) f[i] = __uint_as_float(v[i]);
-          if (p.bias != nullptr) {
-#pragma unroll
-            for (int i = 0; i < 16; ++i) f[i] += __ldg(p.bias + nbase + c0 + i);
-          }
-          uint8_t* box = epi + (c0 >> 6) * (kTileM * 128) + row * 128;
-          const int j0 = (c0 & 63) >> 3;  // 16B chunk index inside the 128B row
-          uint4* p0 = reinterpret_cast<uint4*>(box + (((j0) ^ (row & 7)) << 4));
-          uint4* p1 = reinterpret_cast<uint4*>(box + (((j0 + 1) ^ (row & 7)) << 4));
-          if (p.res != nullptr) {
-            const uint4 r0 = *p0, r1 = *p1;
-            const uint32_t rr[8] = {r0.x, r0.y, r0.z, r0.w, r1.x, r1.y, r1.z, r1.w};
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-              const float2 t = unpack_bf16x2(rr[i]);
-              f[2 * i] += t.x;
-              f[2 * i + 1] += t.y;
-            }
-          }
-          if (p.act == B200_ACT_RELU) {
-#pragma unroll
-            for (int i = 0; i < 16; ++i) f[i] = fmaxf(f[i], 0.f);
-          } else if (p.act == B200_ACT_RELU6) {
-#pragma unroll
-            for (int i = 0; i < 16; ++i) f[i] = fminf(fmaxf(f[i], 0.f), 6.f);
-          }
-          uint4 a, b;
-          a.x = pack_bf16x2(f[0], f[1]);   a.y = pack_bf16x2(f[2], f[3]);
-          a.z = pack_bf16x2(f[4], f[5]);   a.w = pack_bf16x2(f[6], f[7]);
-          b.x = pack_bf16x2(f[8], f[9]);   b.y = pack_bf16x2(f[10], f[11]);
-          b.z = pack_bf16x2(f[12], f[13]); b.w = pack_bf16x2(f[14], f[15]);
-          *p0 = a;
-          *p1 = b;
-        }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&tmem_empty[acc]);   // TMEM stage is free: the MMA warp may start tile+2
-        fence_proxy_async();                             // generic-proxy smem writes -> visible to TMA
-        named_bar_sync(1, 256);
-        if (leader) {
-          for (int b = 0; b < nbox; ++b)
-            tma_store_2d(&tmC, epi + b * (kTileM * 128), nbase + b * 64, m_tile * kTileM);
-          bulk_commit_group();
-        }
-        if (p.stats != nullptr) {
-          // Fused BN statistics: per-channel sum / sum of squares of the bf16-rounded outputs of this tile,
-          // read back from the staged tile (rows beyond M_total are exact zeros).  Accumulated in registers
-          // across the tiles of this CTA while it stays on the same channel block, then one fp64 atomic each.
-          if (st_ntile != n_tile) {
-            if (st_ntile >= 0) {
-              double* dst = p.stats + (blockIdx.x % kStatReplicas) * 2 * p.N_total + st_ntile * p.block_n + st_col;
-              atomicAdd(dst, (double)st_s1);
-              atomicAdd(dst + p.N_total, (double)st_s2);
-            }
-            st_ntile = n_tile; st_s1 = 0.f; st_s2 = 0.f;
-          }
-          const uint8_t* col = epi + (st_col >> 6) * (kTileM * 128) + (st_col & 7) * 2;
-          const int j = (st_col & 63) >> 3;
-          const int r_end = st_row0 + st_rows;
+        for (int u = 0; u < st_ncol; ++u) {
+          const int sc = st_col + 128 * u;
+          const uint8_t* col = epi_t + (sc >> 6) * (kTileM * 128) + (sc & 7) * 2;
+          const int j = (sc & 63) >> 3;
+          float s1 = 0.f, s2 = 0.f;
 #pragma unroll 8
-          for (int r = st_row0; r < r_end; ++r) {
+          for (int r = st_row0; r < st_row0 + st_rows; ++r) {
             const float vv = __bfloat162float(*reinterpret_cast<const __nv_bfloat16*>(col + r * 128 + ((j ^ (r & 7)) << 4)));
-            st_s1 += vv;
-            st_s2 = fmaf(vv, vv, st_s2);
+            s1 += vv;
+            s2 = fmaf(vv, vv, s2);
           }
+          st_s1[u] += s1;
+          st_s2[u] += s2;
         }
-        continue;
       }
-      mbar_wait(&tmem_full[acc], acc_phase);
-      tc_fence_after();
-      for (int c0 = half * 16; c0 < p.block_n; c0 += 32) {
-        uint32_t v0[16];
-        tmem_ld16(taddr + c0, v0);
-        tmem_ld_wait();
-        store_chunk16(p, v0, off, nbase + c0, row_ok && (nbase + c0 < p.N_total));
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tmem_empty[acc]);
+      continue;
     }
-    if (p.stats != nullptr && st_ntile >= 0) {
-      double* dst = p.stats + (blockIdx.x % kStatReplicas) * 2 * p.N_total + st_ntile * p.block_n + st_col;
-      atomicAdd(dst, (double)st_s1);
-      atomicAdd(dst + p.N_total, (double)st_s2);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int m = m_tile * kTileM + r_lo + 8 * h;
+      if (m >= p.M_total) continue;
+      const int img = m / IJ;
+      const int rem = m - img * IJ;
+      const int bi = rem / p.J;
+      const int bj = rem - bi * p.J;
+      const long long off = ((static_cast<long long>(img) * p.OH + (bi * p.os + p.oh0)) * p.OW + (bj * p.os + p.ow0)) *
+                            static_cast<long long>(p.ldo);
+#pragma unroll
+      for (int j = 0; j < 128; j += 4)
+        if (2 * j < p.block_n) store_pair(p, acc[j + 2 * h], acc[j + 2 * h + 1], off, nbase + 2 * j + c_lo);
     }
-    if (p.tma_store && warp == 2 && lane == 0) bulk_wait_group0();  // smem must outlive the last TMA store
   }
-  __syncwarp();
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, kTmemCols);
-  }
+  if (p.stats != nullptr && st_ntile >= 0) flush_stats();
+  if (p.tma_store && leader) bulk_wait_group0();  // smem must outlive the last TMA store
 }
 
 // ------------------------------------------------------------------------------------------------
 // wgrad: dw[k, tap, c] += sum_pix dy[pix, k] * x[pix @ tap, c]
 // A = dy tile, MN-major (rows of smem = pixels, 128/64/32B of k-channels); B = im2col(x) tile, MN-major.
+// A CTA owns 128 output channels (one k-tile) x boxes_per_cta channel boxes of x (at most 256 accumulator columns).
 struct WgradParams {
   int M_total;          // fwd output pixels N*P*Q
   int P, Q;
@@ -460,9 +364,8 @@ struct WgradParams {
   int bk;               // pixels per stage
   int c_chunks;         // ceil(C / ckB)
   int total_boxes;      // taps * c_chunks
-  int boxes_per_cta;    // <= 512 / (kt * ckB) and <= 8
-  int kt, k_groups;     // k-tiles (128 output channels each) accumulated side by side in TMEM by one CTA: the x tile is
-                        // fetched once for all of them (L2 -> SM delivery, not the tensor pipe, bounds these kernels)
+  int boxes_per_cta;    // boxes_per_cta * ckB <= 256 accumulator columns, <= 8
+  int kt, k_groups;     // kt == 1: one k-tile (128 output channels) per CTA
   int k_tiles, col_groups, splits;
   int blocks_per_split, total_blocks;  // in units of bk pixels
   int num_stages;
@@ -470,16 +373,13 @@ struct WgradParams {
   float* dw;
   int plain_x;           // 1: x is a dense [M_total, C] matrix (1x1 stride 1): tiled TMA instead of im2col
   float* partial;        // split-K partial tiles [tile][split][128][pitch] (nullptr: splits == 1, add into dw)
-  int pitch;             // kt * boxes_per_cta * ckB
-  int window;            // 0 dense; 128: k-tile t pairs with source channels [128t, 128t+128) only (kt == 1)
-  int S_filter;          // filter width: tap t = (r, s) = (t / S, t % S) gives the im2col offsets {s, r}.  Computed, not
-                         // read from a table: ptxas 12.9 (sm_100a) mis-split a 32-bit {off_w, off_h} word loaded through
-                         // the uniform datapath (LDCU + UPRMT on a stale register) -- wrong off_h for every tap row > 0
+  int pitch;             // boxes_per_cta * ckB
+  int window;            // 0 dense; 128: k-tile t pairs with source channels [128t, 128t+128) only
+  int S_filter;          // filter width: tap t = (r, s) = (t / S, t % S) gives the im2col offsets {s, r}
 };
 
-__device__ __forceinline__ void red_add_v4(float* addr, float a, float b, float c, float d) {
-  asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(addr), "f"(a), "f"(b), "f"(c), "f"(d)
-               : "memory");
+__device__ __forceinline__ void red_add_v2(float* addr, float a, float b) {
+  asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(addr), "f"(a), "f"(b) : "memory");
 }
 
 __global__ void __launch_bounds__(kThreads, 1)
@@ -488,8 +388,6 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_constan
   extern __shared__ uint8_t smem_raw[];
   __shared__ __align__(8) uint64_t full_bar[kMaxStages];
   __shared__ __align__(8) uint64_t empty_bar[kMaxStages];
-  __shared__ __align__(8) uint64_t acc_bar;
-  __shared__ uint32_t tmem_base_s;
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -499,22 +397,14 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_constan
   if (threadIdx.x == 0) {
     for (int s = 0; s < p.num_stages; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
+      mbar_init(&empty_bar[s], kConsumers / 32);
     }
-    mbar_init(&acc_bar, 1);
     fence_mbar_init();
     prefetch_tmap(&tmDy);
     prefetch_tmap(&tmX);
   }
-  if (warp == 1) {
-    tmem_alloc(&tmem_base_s, kTmemCols);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  pdl_wait();   // prologue above (barriers, TMEM, descriptor prefetch) overlaps the predecessor grid
-  const uint32_t tmem_base = tmem_base_s;
+  pdl_wait();   // prologue above (barriers, descriptor prefetch) overlaps the predecessor grid
 
   // work decomposition
   const int tiles = p.k_groups * p.col_groups;
@@ -522,187 +412,126 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_constan
   const int tile = blockIdx.x - split * tiles;
   const int k_group = tile % p.k_groups;
   const int cgroup = tile / p.k_groups;
-  const int k0 = k_group * p.kt * kTileM;
-  const int kt_valid = min(p.kt, p.k_tiles - k_group * p.kt);
+  const int k0 = k_group * kTileM;
   const int box0 = cgroup * p.boxes_per_cta;
   const int nboxes = min(p.boxes_per_cta, p.total_boxes - box0);
   const int blk_begin = split * p.blocks_per_split;
   const int blk_end = min(p.total_blocks, blk_begin + p.blocks_per_split);
   const int nblk = blk_end - blk_begin;
   const uint32_t a_tile = (kTileM / p.ckA) * p.boxA_bytes;   // one k-tile of dy: 128 channels x bk pixels
-  const uint32_t a_region = p.kt * a_tile;
+  if (nblk <= 0) return;
 
-  if (nblk > 0) {
-    if (warp == 0) {
-      if (lane == 0) {
-        int stage = 0;
-        uint32_t phase = 0;
-        const int PQ = p.P * p.Q;
-        // everything that does not depend on the pixel block is computed once: the producer thread's issue rate bounds
-        // the HBM-bound layers (one TMA request per 8 KB box)
-        int nA_j[4];
-        int nA_total = 0;
-        for (int j = 0; j < 4; ++j) {
-          nA_j[j] = j < kt_valid ? min(kTileM / p.ckA, (p.K_out - (k0 + j * kTileM) + p.ckA - 1) / p.ckA) : 0;
-          nA_total += nA_j[j];
-        }
-        int box_c[8];
-        uint16_t box_w[8], box_h[8];
-        for (int x = 0; x < 8; ++x) {
-          const int id = box0 + min(x, nboxes - 1);
-          const int t = id / p.c_chunks;
-          const int th = t / p.S_filter;
-          box_c[x] = (id - t * p.c_chunks) * p.ckB + (p.window ? k0 : 0);
-          box_w[x] = static_cast<uint16_t>(t - th * p.S_filter);
-          box_h[x] = static_cast<uint16_t>(th);
-        }
-        const uint32_t tx = nA_total * p.boxA_bytes + nboxes * p.boxB_bytes;
-        for (int b = blk_begin; b < blk_end; ++b) {
-          const int pix0 = b * p.bk;
-          mbar_wait(&empty_bar[stage], phase ^ 1u);
-          uint8_t* sa = smem + stage * p.stage_bytes;
-          uint8_t* sb = sa + a_region;
-          mbar_arrive_expect_tx(&full_bar[stage], tx);
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            const int kj = k0 + j * kTileM;
-            for (int a = 0; a < nA_j[j]; ++a)      // dy boxes actually present (K_out tail)
-              tma_load_2d(&tmDy, &full_bar[stage], sa + j * a_tile + a * p.boxA_bytes, kj + a * p.ckA, pix0);
-          }
-          if (p.plain_x) {
-#pragma unroll
-            for (int x = 0; x < 8; ++x)
-              if (x < nboxes) tma_load_2d(&tmX, &full_bar[stage], sb + x * p.boxB_bytes, box_c[x], pix0);
-          } else {
-            const int img = pix0 / PQ;
-            const int rem = pix0 - img * PQ;
-            const int pi = rem / p.Q;
-            const int pj = rem - pi * p.Q;
-            const int base_w = pj * p.trav + p.lower_w;
-            const int base_h = pi * p.trav + p.lower_h;
-#pragma unroll
-            for (int x = 0; x < 8; ++x)
-              if (x < nboxes)
-                tma_load_im2col_4d(&tmX, &full_bar[stage], sb + x * p.boxB_bytes, box_c[x], base_w, base_h, img, box_w[x],
-                                   box_h[x]);
-          }
-          if (++stage == p.num_stages) { stage = 0; phase ^= 1u; }
-        }
+  if (warp >= kProducerWarp) {
+    if (warp == kProducerWarp && lane == 0) {
+      int stage = 0;
+      uint32_t phase = 0;
+      const int PQ = p.P * p.Q;
+      // everything that does not depend on the pixel block is computed once: the producer thread's issue rate bounds
+      // the HBM-bound layers (one TMA request per 8 KB box)
+      const int nA = min(kTileM / p.ckA, (p.K_out - k0 + p.ckA - 1) / p.ckA);   // dy boxes present (K_out tail)
+      int box_c[8];
+      uint16_t box_w[8], box_h[8];
+      for (int x = 0; x < 8; ++x) {
+        const int id = box0 + min(x, nboxes - 1);
+        const int t = id / p.c_chunks;
+        const int th = t / p.S_filter;
+        box_c[x] = (id - t * p.c_chunks) * p.ckB + (p.window ? k0 : 0);
+        box_w[x] = static_cast<uint16_t>(t - th * p.S_filter);
+        box_h[x] = static_cast<uint16_t>(th);
       }
-    } else if (warp == 1) {
-      if (lane == 0) {
-        int stage = 0;
-        uint32_t phase = 0;
-        const uint64_t protoA = make_smem_desc(0, p.boxA_bytes, 8 * p.ckA * 2, layout_type_for_row_bytes(p.ckA * 2));
-        const uint64_t protoB = make_smem_desc(0, p.boxB_bytes, 8 * p.ckB * 2, layout_type_for_row_bytes(p.ckB * 2));
-        const uint32_t kincA = (16u * p.ckA * 2) >> 4, kincB = (16u * p.ckB * 2) >> 4;  // 16 pixel rows per K step
-        const int boxes_per_mma = min(8, 256 / p.ckB);
-        const int ksteps = p.bk / 16;
-        // the issuing thread is latency-bound per instruction: the (k-tile, box group) list of one stage -- descriptor
-        // offsets, TMEM column, instruction descriptor -- is built once
-        // slot (j, gi): k-tile j, box group gi (at most 2 groups of boxes_per_mma boxes); statically indexed -> registers
-        uint32_t g_da[8], g_db[8], g_tm[8], g_id[8];
-        bool g_on[8];
+      const uint32_t tx = nA * p.boxA_bytes + nboxes * p.boxB_bytes;
+      for (int b = blk_begin; b < blk_end; ++b) {
+        const int pix0 = b * p.bk;
+        mbar_wait(&empty_bar[stage], phase ^ 1u);
+        uint8_t* sa = smem + stage * p.stage_bytes;
+        uint8_t* sb = sa + a_tile;
+        mbar_arrive_expect_tx(&full_bar[stage], tx);
+        for (int a = 0; a < nA; ++a)
+          tma_load_2d(&tmDy, &full_bar[stage], sa + a * p.boxA_bytes, k0 + a * p.ckA, pix0);
+        if (p.plain_x) {
 #pragma unroll
-        for (int j = 0; j < 4; ++j)
-#pragma unroll
-          for (int gi = 0; gi < 2; ++gi) {
-            const int g0 = gi * boxes_per_mma;
-            const int nb = min(boxes_per_mma, nboxes - g0);
-            g_on[j * 2 + gi] = j < kt_valid && g0 < nboxes;
-            g_da[j * 2 + gi] = (j * a_tile) >> 4;
-            g_db[j * 2 + gi] = (a_region + g0 * p.boxB_bytes) >> 4;
-            g_tm[j * 2 + gi] = tmem_base + (j * p.boxes_per_cta + g0) * p.ckB;
-            g_id[j * 2 + gi] = make_idesc_bf16(kTileM, max(nb, 1) * p.ckB, 1, 1);
-          }
-        for (int b = 0; b < nblk; ++b) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint32_t a_addr = smem_u32(smem + stage * p.stage_bytes);
-          const uint64_t da_s = protoA + (a_addr >> 4), db_s = protoB + (a_addr >> 4);
-          const uint32_t first = b != 0 ? 1u : 0u;
-#pragma unroll
-          for (int g = 0; g < 8; ++g) {
-            if (!g_on[g]) continue;
-            const uint64_t da0 = da_s + g_da[g], db0 = db_s + g_db[g];
-            const uint32_t d_tmem = g_tm[g], idesc = g_id[g];
-            if (ksteps == 4) {
-              umma_bf16(d_tmem, da0, db0, idesc, first);
-              umma_bf16(d_tmem, da0 + kincA, db0 + kincB, idesc, 1u);
-              umma_bf16(d_tmem, da0 + 2 * kincA, db0 + 2 * kincB, idesc, 1u);
-              umma_bf16(d_tmem, da0 + 3 * kincA, db0 + 3 * kincB, idesc, 1u);
-            } else {
-              for (int k = 0; k < ksteps; ++k)
-                umma_bf16(d_tmem, da0 + k * kincA, db0 + k * kincB, idesc, (b | k) != 0 ? 1u : 0u);
-            }
-          }
-          umma_commit(&empty_bar[stage]);
-          if (b == nblk - 1) umma_commit(&acc_bar);
-          if (++stage == p.num_stages) { stage = 0; phase ^= 1u; }
-        }
-      }
-    } else {
-      const int q = warp & 3;
-      mbar_wait(&acc_bar, 0);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + (static_cast<uint32_t>(q * 32) << 16);
-      for (int j = 0; j < kt_valid; ++j) {
-        const int k = k0 + j * kTileM + q * 32 + lane;
-        const bool row_ok = k < p.K_out;
-        const int col_j = j * p.boxes_per_cta * p.ckB;
-        if (p.partial != nullptr) {
-          // split-K: plain stores of this CTA's fp32 tile; conv_wgrad_reduce_kernel sums the splits into dw
-          float* dst = p.partial + ((static_cast<long long>(tile) * p.splits + split) * kTileM + (q * 32 + lane)) * p.pitch +
-                       col_j;
-          const int ncols = nboxes * p.ckB;
-          for (int c0 = 0; c0 < ncols; c0 += 16) {
-            uint32_t v[16];
-            tmem_ld16(taddr + col_j + c0, v);
-            tmem_ld_wait();
-            if (row_ok) {
-#pragma unroll
-              for (int i = 0; i < 4; ++i)
-                *reinterpret_cast<float4*>(dst + c0 + 4 * i) =
-                    make_float4(__uint_as_float(v[4 * i]), __uint_as_float(v[4 * i + 1]), __uint_as_float(v[4 * i + 2]),
-                                __uint_as_float(v[4 * i + 3]));
-            }
-          }
+          for (int x = 0; x < 8; ++x)
+            if (x < nboxes) tma_load_2d(&tmX, &full_bar[stage], sb + x * p.boxB_bytes, box_c[x], pix0);
         } else {
-          for (int x = 0; x < nboxes; ++x) {
-            const int id = box0 + x;
-            const int t = id / p.c_chunks;
-            const int cc = id - t * p.c_chunks;
-            const int tap = t;
-            const int cbase = cc * p.ckB;
-            float* dst = p.dw + (static_cast<long long>(k) * p.taps_total + tap) * p.C + cbase;
-            for (int c0 = 0; c0 < p.ckB; c0 += 16) {
-              uint32_t v[16];
-              tmem_ld16(taddr + col_j + x * p.ckB + c0, v);
-              tmem_ld_wait();
-              if (row_ok) {
-                if (cbase + c0 + 16 <= p.C && (p.C & 3) == 0) {
+          const int img = pix0 / PQ;
+          const int rem = pix0 - img * PQ;
+          const int pi = rem / p.Q;
+          const int pj = rem - pi * p.Q;
+          const int base_w = pj * p.trav + p.lower_w;
+          const int base_h = pi * p.trav + p.lower_h;
 #pragma unroll
-                  for (int i = 0; i < 4; ++i)
-                    red_add_v4(dst + c0 + 4 * i, __uint_as_float(v[4 * i]), __uint_as_float(v[4 * i + 1]),
-                               __uint_as_float(v[4 * i + 2]), __uint_as_float(v[4 * i + 3]));
-                } else {
+          for (int x = 0; x < 8; ++x)
+            if (x < nboxes)
+              tma_load_im2col_4d(&tmX, &full_bar[stage], sb + x * p.boxB_bytes, box_c[x], base_w, base_h, img, box_w[x],
+                                 box_h[x]);
+        }
+        if (++stage == p.num_stages) { stage = 0; phase ^= 1u; }
+      }
+    }
+    return;
+  }
+
+  // ---- consumers: warpgroup wg computes output channels [k0 + 64 wg, k0 + 64 wg + 64) x all boxes of the CTA
+  const int wg = warp >> 2;
+  const bool wg_on = k0 + wg * 64 < p.K_out;
+  const int ncols = nboxes * p.ckB;
+  // A rows 64 wg.. start at dy box 64 wg / ckA; MN-major: LBO = box stride along M/N, SBO = 8 pixel rows
+  const uint64_t protoA = make_smem_desc(0, p.boxA_bytes, 8 * p.ckA * 2, layout_type_for_row_bytes(p.ckA * 2));
+  const uint64_t protoB = make_smem_desc(0, p.boxB_bytes, 8 * p.ckB * 2, layout_type_for_row_bytes(p.ckB * 2));
+  const uint32_t a_wg = (wg * (64 / p.ckA) * p.boxA_bytes) >> 4;
+  const uint32_t kincA = (16u * p.ckA * 2) >> 4, kincB = (16u * p.ckB * 2) >> 4;  // 16 pixel rows per K step
+  const int ksteps = p.bk / 16;
+  float acc[128];
+  wgmma_fence_acc(acc);
+  int stage = 0, prev = 0;
+  uint32_t phase = 0;
+  for (int b = 0; b < nblk; ++b) {
+    mbar_wait(&full_bar[stage], phase);
+    const uint32_t a_addr = smem_u32(smem + stage * p.stage_bytes);
+    if (wg_on) {
+      const uint64_t da = protoA + (a_addr >> 4) + a_wg, db = protoB + ((a_addr + a_tile) >> 4);
+      wgmma_fence();
+      for (int k = 0; k < ksteps; ++k)
+        wgmma_bf16<1, 1>(acc, ncols, da + k * kincA, db + k * kincB, (b | k) != 0 ? 1u : 0u);
+      wgmma_commit();
+      wgmma_wait<1>();
+    }
+    if (b > 0) release_stage(&empty_bar[prev], lane);
+    prev = stage;
+    if (++stage == p.num_stages) { stage = 0; phase ^= 1u; }
+  }
+  wgmma_wait<0>();
+  wgmma_fence_acc(acc);
+  release_stage(&empty_bar[prev], lane);
+  if (!wg_on) return;
+
+  const int r_lo = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // fragment rows r_lo, r_lo + 8 (output channels)
+  const int c_lo = 2 * (lane & 3);
 #pragma unroll
-                  for (int i = 0; i < 16; ++i)
-                    if (cbase + c0 + i < p.C) atomicAdd(dst + c0 + i, __uint_as_float(v[i]));
-                }
-              }
-            }
-          }
+  for (int h = 0; h < 2; ++h) {
+    const int k = k0 + r_lo + 8 * h;
+    if (k >= p.K_out) continue;
+    if (p.partial != nullptr) {
+      // split-K: plain stores of this CTA's fp32 tile; conv_wgrad_reduce_kernel sums the splits into dw
+      float* dst = p.partial + ((static_cast<long long>(tile) * p.splits + split) * kTileM + (r_lo + 8 * h)) * p.pitch;
+#pragma unroll
+      for (int j = 0; j < 128; j += 4)
+        if (2 * j < ncols)
+          *reinterpret_cast<float2*>(dst + 2 * j + c_lo) = make_float2(acc[j + 2 * h], acc[j + 2 * h + 1]);
+    } else {
+#pragma unroll
+      for (int j = 0; j < 128; j += 4) {
+        const int col = 2 * j + c_lo;
+        if (col < ncols) {
+          const int x = col / p.ckB;
+          const int id = box0 + x;
+          const int tap = id / p.c_chunks;
+          const int c = (id - tap * p.c_chunks) * p.ckB + (col - x * p.ckB);
+          if (c < p.C) red_add_v2(p.dw + (static_cast<long long>(k) * p.taps_total + tap) * p.C + c, acc[j + 2 * h],
+                                  acc[j + 2 * h + 1]);
         }
       }
     }
-  }
-  __syncwarp();
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, kTmemCols);
   }
 }
 
@@ -891,12 +720,11 @@ static int launch_igemm(const IgemmLaunch& L, cudaStream_t stream) {
   }
   // several n-tiles whose weights fit one at a time: a CTA owns an n-tile.  Worth it when the weights dominate the
   // L2->SM traffic of the round-robin walk (bytes ~ A * n_tiles + W * m_tiles vs A * n_tiles + W_tile * CTAs) and
-  // every CTA still gets a few m-tiles; needs >= 3 operand stages beside the resident weights and the staging tile
-  // (with two, l3 256->1024 did not gain although its L2->SM traffic fell 2.5x: pipeline depth matters as much).
+  // every CTA still gets a few m-tiles; needs >= 3 operand stages beside the resident weights and the staging tile.
   static const int own_mode = getenv("B200_IGEMM_OWN_NTILE") ? atoi(getenv("B200_IGEMM_OWN_NTILE")) : 1;
   int grid_own = 0;
   // B200_IGEMM_SMEM_KB: operand + staging budget (default 224 KB: three 48 KB stages for 256-wide tiles beside the 64 KB
-  // staging tile; with 200 KB they ran a TWO-stage pipeline -- l3/l4 1x1 layers 15-20 % slower, 0.35 ms/step)
+  // staging tile; 200 KB leaves only two)
   static const int budget_kb = getenv("B200_IGEMM_SMEM_KB") ? atoi(getenv("B200_IGEMM_SMEM_KB")) : 224;
   int budget = (budget_kb >= 96 && budget_kb <= 224 ? budget_kb : 224) * 1024;
   if (bstat_enabled && own_mode && !p.b_stationary && p.n_tiles > 1 && p.n_tiles <= 8 && !L.window &&
@@ -916,15 +744,10 @@ static int launch_igemm(const IgemmLaunch& L, cudaStream_t stream) {
       budget = kSmemBudgetMax;
     }
   }
-  // second staging tile (residual prefetched one tile ahead, store/convert overlap) when at least three operand
-  // stages remain.  B200_IGEMM_EPI2: 0 = never, 2 = every epilogue, default 1 = epilogues with a residual only --
-  // measured (profiles/r02_summary.md): residual epilogues gain up to 28 %, plain ones lose 0-8 % to the lost stage
-  static const int epi2_mode = getenv("B200_IGEMM_EPI2") ? atoi(getenv("B200_IGEMM_EPI2")) : 1;
-  p.epi_bufs = 1;
+  // a second staging tile when at least three operand stages remain beside it: a tile's epilogue then never waits for
+  // the previous tile's store to drain
+  p.epi_bufs = (p.tma_store && (budget - 2 * epi_bytes - bstat_bytes) / (int)stage >= 3) ? 2 : 1;
   p.epi_bytes = (uint32_t)epi_bytes;
-  if ((epi2_mode >= 2 || (epi2_mode == 1 && L.res != nullptr)) && p.tma_store &&
-      (budget - 2 * epi_bytes - bstat_bytes) / (int)stage >= 3)
-    p.epi_bufs = 2;
   const int epi_total = epi_bytes * p.epi_bufs;
   p.num_stages = (budget - epi_total - bstat_bytes) / (int)stage;
   if (p.num_stages > kMaxStages) p.num_stages = kMaxStages;
@@ -958,10 +781,10 @@ static int launch_igemm(const IgemmLaunch& L, cudaStream_t stream) {
   memset(&tmC, 0, sizeof(tmC));
   memset(&tmR, 0, sizeof(tmR));
   if (p.tma_store) {
-    rc = encode_tiled2(&tmC, L.out, L.ldo, (long long)p.M_total, 64, kTileM);
+    rc = encode_tiled2(&tmC, L.out, L.ldo, (long long)p.M_total, 64, kTileM / 2);   // one warpgroup's 64 rows
     if (rc) return rc;
     if (L.res != nullptr) {
-      rc = encode_tiled2(&tmR, L.res, L.ldo, (long long)p.M_total, 64, kTileM);
+      rc = encode_tiled2(&tmR, L.res, L.ldo, (long long)p.M_total, 64, kTileM / 2);
       if (rc) return rc;
     }
   }
@@ -974,7 +797,7 @@ static int launch_igemm(const IgemmLaunch& L, cudaStream_t stream) {
     fprintf(stderr, "[igemm] M=%d C=%d N=%d taps=%d block_n=%d n_tiles=%d stages=%d bstat=%d own=%d epi_bufs=%d grid=%d smem=%d\n",
             p.M_total, L.SC, L.Nout, L.ntaps, p.block_n, p.n_tiles, p.num_stages, p.b_stationary, p.own_ntile, p.epi_bufs,
             grid, smem_bytes);
-  b200::launch(conv_igemm_kernel, grid, kIgemmThreads, smem_bytes, stream, tmA, tmB, tmC, tmR, p);
+  b200::launch(conv_igemm_kernel, grid, kThreads, smem_bytes, stream, tmA, tmB, tmC, tmR, p);
   B200_CHECK_LAUNCH("conv_igemm_kernel");
   return B200_OK;
 }
@@ -1015,14 +838,6 @@ extern "C" int b200_conv_fprop(const b200_conv_desc* d, const void* x, const voi
                        (ep && ep->bn_stats_workspace) ? reinterpret_cast<double*>(ep->bn_stats_workspace) : nullptr,
                        (cudaStream_t)stream, d->window);
   }
-  if (d->R == 1 && d->S == 1 && d->stride == 1 && d->pad_h == 0 && d->pad_w == 0 && d->x_pixel_stride == 0 && !d->window &&
-      (!ep || !ep->out_fp32) && !(ep && ep->bias && ep->bn_stats_workspace) &&
-      pair_eligible((long long)d->N * d->H * d->W, d->C, d->K)) {   // opt-in CTA-pair kernel (conv_pair.cu)
-    return launch_pair(x, w, y, ep ? ep->residual : nullptr, ep ? ep->bias : nullptr, (long long)d->N * d->H * d->W, d->C,
-                       d->K, ep ? ep->act : 0,
-                       (ep && ep->bn_stats_workspace) ? reinterpret_cast<double*>(ep->bn_stats_workspace) : nullptr,
-                       (cudaStream_t)stream);
-  }
   IgemmLaunch L;
   memset(&L, 0, sizeof(L));
   L.src = x; L.Nimg = d->N; L.SH = d->H; L.SW = d->W; L.SC = d->C;
@@ -1058,10 +873,6 @@ extern "C" int b200_conv_dgrad(const b200_conv_desc* d, const void* dy, const vo
       (d->window == 0 || d->window == 64) && halo_eligible(d->H, d->W, d->K, d->C, 3, 3, 1)) {
     return launch_halo(dy, wt, dx, residual, nullptr, d->N, d->H, d->W, d->K, d->C, 3, 3, 1, 1, 0, nullptr, stream,
                        d->window);
-  }
-  if (d->R == 1 && d->S == 1 && st == 1 && d->pad_h == 0 && d->pad_w == 0 && !d->window &&
-      pair_eligible((long long)d->N * d->H * d->W, d->K, d->C)) {   // opt-in CTA-pair kernel: dx = dy * wt^T
-    return launch_pair(dy, wt, dx, residual, nullptr, (long long)d->N * d->H * d->W, d->K, d->C, 0, nullptr, stream);
   }
   // dx[h,w] = sum_{r,s : (h+pad-r) % st == 0} dy[(h+pad-r)/st, (w+pad-s)/st] * w[r,s]
   // one launch per residue class (h % st, w % st); each class is a stride-1 correlation over dy.
@@ -1139,8 +950,7 @@ extern "C" int b200_conv_wgrad(const b200_conv_desc* d, const void* x, const voi
       d->Q == d->W + 2 * d->pad_w - d->S + 1 && d->x_pixel_stride == 0 &&
       (d->window == 0 || d->window == 128) && halo_wgrad_eligible(d->P, d->Q, d->C, d->K, d->R, d->S, d->pad_h)) {
     // partial tiles of the halo kernel must fit the split-K workspace (units * splits <= SMs, or one split)
-    const int cw = d->C == 16 ? 16 : 32;
-    const int units = ((d->window ? d->window : d->C) / cw) * ((d->K + kTileM - 1) / kTileM);
+    const int units = ((d->window ? d->window : d->C) / 16) * ((d->K + kTileM - 1) / kTileM);   // 16-channel x chunks
     if (units <= sm_count() + 8)
       return launch_halo_wgrad(x, dy, dw, workspace, workspace_bytes, d->N, d->P, d->Q, d->C, d->K, d->R, d->S, d->pad_h,
                                stream, d->window);
@@ -1162,27 +972,18 @@ extern "C" int b200_conv_wgrad(const b200_conv_desc* d, const void* x, const voi
   p.k_tiles = (d->K + kTileM - 1) / kTileM;
   p.boxA_bytes = p.bk * p.ckA * 2;
   p.boxB_bytes = p.bk * p.ckB * 2;
-  // Tile shape: kt k-tiles x bpc channel boxes per CTA (kt * bpc * ckB <= 512 TMEM columns).  The kernels are bound by
-  // operand delivery from L2, so pick the shape that fetches the fewest bytes per MMA flop:
-  //   bytes per stage = kt * (dy tile) + bpc * (x box),  flops per stage ~ kt * bpc.
-  static const int kt_cap = getenv("B200_WGRAD_KT") ? atoi(getenv("B200_WGRAD_KT")) : 4;
-  double best = 1e30;
-  p.kt = 1; p.boxes_per_cta = 1;
-  for (int kt = 1; kt <= 4 && kt <= p.k_tiles && kt <= (d->window ? 1 : kt_cap); kt *= 2) {
-    int bpc = 512 / (kt * p.ckB);
-    if (bpc > 8) bpc = 8;
-    if (bpc > p.total_boxes) bpc = p.total_boxes;
-    if (bpc < 1) continue;
-    const double a_bytes = (double)kt * (kTileM / p.ckA) * p.boxA_bytes, b_bytes = (double)bpc * p.boxB_bytes;
-    if (a_bytes + b_bytes > 96.0 * 1024) continue;                       // at least two stages in shared memory
-    const double cost = (a_bytes + b_bytes) / ((double)kt * bpc * p.ckB);
-    if (cost < best * 0.999) { best = cost; p.kt = kt; p.boxes_per_cta = bpc; }
-  }
+  // Tile shape: one k-tile (128 output channels, the two consumer warpgroups) x bpc channel boxes of x per CTA, with
+  // bpc * ckB <= 256 accumulator columns (128 fp32 registers per consumer thread).  The x tile is fetched once for
+  // all 128 output channels.
+  p.kt = 1;
+  p.boxes_per_cta = 256 / p.ckB;
+  if (p.boxes_per_cta > 8) p.boxes_per_cta = 8;
+  if (p.boxes_per_cta > p.total_boxes) p.boxes_per_cta = p.total_boxes;
   p.k_groups = (p.k_tiles + p.kt - 1) / p.kt;
   p.col_groups = (p.total_boxes + p.boxes_per_cta - 1) / p.boxes_per_cta;
   p.total_blocks = (p.M_total + p.bk - 1) / p.bk;
   const int tiles = p.k_groups * p.col_groups;
-  int splits = sm_count() / tiles;  // one wave: a CTA owns the whole TMEM, two cannot share an SM
+  int splits = sm_count() / tiles;  // one wave: a CTA takes most of an SM's shared memory, two cannot share one
   if (splits > p.total_blocks) splits = p.total_blocks;
   if (splits < 1) splits = 1;
   p.blocks_per_split = (p.total_blocks + splits - 1) / splits;

@@ -1,27 +1,27 @@
-// Stride-1 RxS convolutions (3x3 pad 1 fprop/dgrad; the 4x4 pad 0 space-to-depth stem) as a "shift GEMM" on tcgen05
-// tensor cores.
+// Stride-1 RxS convolutions (3x3 pad 1 fprop/dgrad; the 4x4 pad 0 space-to-depth stem) as a "shift GEMM" on Hopper
+// tensor cores (wgmma).
 //
 // The im2col kernel (conv.cu) re-fetches the activation tile once per filter tap: 9 TMA loads of the same
 // pixels, shifted.  Here a tile is RT full image rows; its zero-padded halo box [(RT+2) x (W+2) pixels x 64 ch]
 // is loaded ONCE per 64-channel block (tiled 4D TMA, out-of-bounds = padding), and the nine taps are nine views of
-// that one shared-memory buffer: the UMMA descriptor start address is simply advanced by (r*(W+2)+s) pixel rows
-// (row-shifted 128B-swizzle descriptors are valid because the swizzle is a function of the absolute smem address;
-// measured with tools/shift_probe.cu).  The 128 accumulator rows are "virtual pixels" of the padded row pitch
-// W+2; the two halo columns per row are computed and discarded (2/(W+2) of the MMA work).
+// that one shared-memory buffer: the wgmma descriptor start address is simply advanced by (r*(W+2)+s) pixel rows
+// (row-shifted swizzled descriptors are valid because the swizzle is a function of the absolute smem address).
+// The 128 accumulator rows are "virtual pixels" of the padded row pitch W+2; the two halo columns per row are
+// computed and discarded (2/(W+2) of the MMA work).
 // Activation traffic from L2 drops ~9x -> ~1.3x; weights stream through a separate ring.
 //
 // Pixel rows are 128 B (64-channel chunks, 128B swizzle) or, for the 16-channel stem, 32 B (32B swizzle, one K=16
 // MMA per tap).  When all weight slices of a CTA fit in shared memory (64x64 3x3, the stem) they are loaded once
 // ("stationary") instead of streaming through the ring with every tile.
 //
-// Same warp roles / TMEM double buffering / TMA-store epilogue / fused BN statistics as conv_igemm_kernel.
+// Same warp roles / TMA-store epilogue / fused BN statistics as conv_igemm_kernel.
 #include "common.cuh"
 #include "host.h"
 #include <stdlib.h>
 
 namespace b200 {
 
-constexpr int kHThreads = 320;
+constexpr int kHThreads = 384;   // two consumer warpgroups + the producer warpgroup (warp 8 issues the TMA)
 constexpr int kHTileM = 128;
 constexpr int kHMaxA = 6, kHMaxB = 8;
 constexpr int kHMaxTaps = 16;
@@ -47,17 +47,16 @@ struct HaloParams {
   uint16_t b_tap[kHMaxTaps];  // weight tap slice used with it
 };
 
-// The MMA-issuing thread is latency-bound per instruction: descriptors are built once per operand buffer and
-// advanced by adding (byte offset >> 4) to the address field, with the tap / k-step loops fully unrolled.
-template <int NTAPS, int KSTEPS>
+// Descriptors are built once per operand buffer and advanced by adding (byte offset >> 4) to the address field, with
+// the tap / k-step loops fully unrolled.  BN = block_n (64, 128 or 256) sizes the accumulators exactly.
+template <int NTAPS, int KSTEPS, int BN>
 __global__ void __launch_bounds__(kHThreads, 1)
 conv_halo_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmB,
                  const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmR,
                  const __grid_constant__ HaloParams p) {
   extern __shared__ uint8_t smem_raw[];
   __shared__ __align__(8) uint64_t a_full[kHMaxA], a_empty[kHMaxA], b_full[kHMaxB], b_empty[kHMaxB];
-  __shared__ __align__(8) uint64_t tmem_full[2], tmem_empty[2], res_bar, bstat_bar;
-  __shared__ uint32_t tmem_base_s;
+  __shared__ __align__(8) uint64_t res_bar, bstat_bar;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const uint32_t raw_addr = smem_u32(smem_raw);
@@ -68,22 +67,16 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant_
   uint8_t* epi = sB + b_slots * p.b_bytes;
 
   if (threadIdx.x == 0) {
-    for (int i = 0; i < p.sa; ++i) { mbar_init(&a_full[i], 1); mbar_init(&a_empty[i], 1); }
-    for (int i = 0; i < kHMaxB; ++i) { mbar_init(&b_full[i], 1); mbar_init(&b_empty[i], 1); }
+    for (int i = 0; i < p.sa; ++i) { mbar_init(&a_full[i], 1); mbar_init(&a_empty[i], 8); }
+    for (int i = 0; i < kHMaxB; ++i) { mbar_init(&b_full[i], 1); mbar_init(&b_empty[i], 8); }
     mbar_init(&bstat_bar, 1);
-    mbar_init(&tmem_full[0], 1); mbar_init(&tmem_full[1], 1);
-    mbar_init(&tmem_empty[0], 8); mbar_init(&tmem_empty[1], 8);
     mbar_init(&res_bar, 1);
     fence_mbar_init();
     prefetch_tmap(&tmX); prefetch_tmap(&tmB); prefetch_tmap(&tmC);
     if (p.has_res) prefetch_tmap(&tmR);
   }
-  if (warp == 1) { tmem_alloc(&tmem_base_s, 512); tmem_relinquish(); }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  pdl_wait();   // prologue above (barriers, TMEM, descriptor prefetch) overlaps the predecessor grid
-  const uint32_t tmem_base = tmem_base_s;
+  pdl_wait();   // prologue above (barriers, descriptor prefetch) overlaps the predecessor grid
   // tile walk: dense -- tiles (m, n) round-robin over the CTAs; diagonal -- the CTA owns n-tile blockIdx.x % n_tiles and
   // walks the m-tiles with stride gridDim.x / n_tiles (the grid is a multiple of n_tiles)
   const int t_start = p.diag ? static_cast<int>(blockIdx.x) / p.n_tiles : static_cast<int>(blockIdx.x);
@@ -91,8 +84,8 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant_
   const int total_tiles = p.diag ? p.m_tiles : p.m_tiles * p.n_tiles;
   const int own_n = static_cast<int>(blockIdx.x) % p.n_tiles;
 
-  if (warp == 0) {
-    if (lane == 0) {
+  if (warp >= 8) {
+    if (warp == 8 && lane == 0) {
       int ia = 0, ib = 0; uint32_t pa = 0, pb = 0;
       const int cw = p.row_bytes >> 1;   // channels per chunk
       if (p.b_stationary && t_start < total_tiles) {
@@ -122,176 +115,161 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant_
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      int ia = 0, ib = 0; uint32_t pa = 0, pb = 0;
-      const uint32_t idesc = make_idesc_bf16(kHTileM, p.block_n, 0, 0);
-      const uint64_t proto = make_smem_desc(0, 16, 8u * p.row_bytes, layout_type_for_row_bytes(p.row_bytes));
-      uint32_t tap_inc[NTAPS];
-#pragma unroll
-      for (int t = 0; t < NTAPS; ++t) tap_inc[t] = (static_cast<uint32_t>(p.a_off[t]) * p.row_bytes) >> 4;
-      if (p.b_stationary && t_start < total_tiles) {
-        mbar_wait(&bstat_bar, 0);
-        tc_fence_after();
-      }
-      int local = 0;
-      for (int tile = t_start; tile < total_tiles; tile += t_step, ++local) {
-        const int acc = local & 1;
-        mbar_wait(&tmem_empty[acc], ((local >> 1) & 1u) ^ 1u);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * 256;
-        for (int cc = 0; cc < p.c_chunks; ++cc) {
-          mbar_wait(&a_full[ia], pa);
-          tc_fence_after();
-          const uint64_t da0 = proto + (smem_u32(sA + ia * p.a_bytes) >> 4);
-          if (p.b_stationary) {
-            const uint64_t db0 = proto + (smem_u32(sB + cc * NTAPS * p.b_bytes) >> 4);
-            const uint32_t b_inc = p.b_bytes >> 4;
-#pragma unroll
-            for (int t = 0; t < NTAPS; ++t) {
-#pragma unroll
-              for (int k = 0; k < KSTEPS; ++k)
-                umma_bf16(d_tmem, da0 + tap_inc[t] + 2 * k, db0 + t * b_inc + 2 * k, idesc,
-                          (t | k) != 0 ? 1u : (cc != 0 ? 1u : 0u));
-            }
-          } else {
-#pragma unroll
-            for (int t = 0; t < NTAPS; ++t) {
-              mbar_wait(&b_full[ib], pb);
-              tc_fence_after();
-              const uint64_t db0 = proto + (smem_u32(sB + ib * p.b_bytes) >> 4);
-#pragma unroll
-              for (int k = 0; k < KSTEPS; ++k)
-                umma_bf16(d_tmem, da0 + tap_inc[t] + 2 * k, db0 + 2 * k, idesc, (t | k) != 0 ? 1u : (cc != 0 ? 1u : 0u));
-              umma_commit(&b_empty[ib]);
-              if (++ib == p.sb) { ib = 0; pb ^= 1u; }
-            }
-          }
-          umma_commit(&a_empty[ia]);
-          if (++ia == p.sa) { ia = 0; pa ^= 1u; }
-        }
-        umma_commit(&tmem_full[acc]);
-      }
-    }
-  } else {
-    const int q = warp & 3;
-    const int half = (warp - 2) >> 2;
-    const bool leader = (warp == 2 && lane == 0);
-    const int v = q * 32 + lane;            // virtual pixel (accumulator row)
-    const int ry = v / p.Wp, cx = v - ry * p.Wp;
-    const int srow = ry * p.W + cx;         // row of the staged output tile [RT][W][64]
-    const int nbox = p.block_n >> 6;
-    const uint32_t box_bytes = static_cast<uint32_t>(p.RT * p.W) * 128u;
-    const uint32_t box_pitch = (box_bytes + 1023u) & ~1023u;
-    // fused BN statistics: this thread owns one output column and a row range of every tile
-    const int st_tid = threadIdx.x - 64;
-    const int st_col = st_tid % p.block_n;
-    const int st_rows = kHTileM / (256 / p.block_n);
-    const int st_row0 = (st_tid / p.block_n) * st_rows;
-    int st_ntile = -1;
-    float st_s1 = 0.f, st_s2 = 0.f;
-    int local = 0;
-    for (int tile = t_start; tile < total_tiles; tile += t_step, ++local) {
-      const int acc = local & 1;
-      const int m_tile = p.diag ? tile : tile / p.n_tiles, n_tile = p.diag ? own_n : tile - m_tile * p.n_tiles;
-      const int img = m_tile / p.tiles_per_img;
-      const int h0 = (m_tile - img * p.tiles_per_img) * p.RT;
-      const int nbase = n_tile * p.block_n;
-      const bool valid = (ry < p.RT) && (cx < p.W) && (h0 + ry < p.H);
-      if (leader && local > 0) bulk_wait_group_read0();
-      named_bar_sync(1, 256);
-      if (p.has_res) {
-        if (leader) {
-          mbar_arrive_expect_tx(&res_bar, static_cast<uint32_t>(nbox) * box_bytes);
-          for (int b = 0; b < nbox; ++b) tma_load_4d(&tmR, &res_bar, epi + b * box_pitch, nbase + b * 64, 0, h0, img);
-        }
-        mbar_wait(&res_bar, static_cast<uint32_t>(local & 1));
-      }
-      mbar_wait(&tmem_full[acc], (local >> 1) & 1u);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + acc * 256;
-      for (int c0 = half * 16; c0 < p.block_n; c0 += 32) {
-        uint32_t vv[16];
-        tmem_ld16(taddr + c0, vv);
-        tmem_ld_wait();
-        if (valid) {
-          float f[16];
-#pragma unroll
-          for (int i = 0; i < 16; ++i) f[i] = __uint_as_float(vv[i]);
-          if (p.bias != nullptr) {
-#pragma unroll
-            for (int i = 0; i < 16; ++i) f[i] += __ldg(p.bias + nbase + c0 + i);
-          }
-          uint8_t* row = epi + (c0 >> 6) * box_pitch + srow * 128;
-          const int j0 = (c0 & 63) >> 3;
-          uint4* p0 = reinterpret_cast<uint4*>(row + ((j0 ^ (srow & 7)) << 4));
-          uint4* p1 = reinterpret_cast<uint4*>(row + (((j0 + 1) ^ (srow & 7)) << 4));
-          if (p.has_res) {
-            const uint4 r0 = *p0, r1 = *p1;
-            const uint32_t rr[8] = {r0.x, r0.y, r0.z, r0.w, r1.x, r1.y, r1.z, r1.w};
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-              const float2 t2 = unpack_bf16x2(rr[i]);
-              f[2 * i] += t2.x;
-              f[2 * i + 1] += t2.y;
-            }
-          }
-          if (p.act == B200_ACT_RELU) {
-#pragma unroll
-            for (int i = 0; i < 16; ++i) f[i] = fmaxf(f[i], 0.f);
-          } else if (p.act == B200_ACT_RELU6) {
-#pragma unroll
-            for (int i = 0; i < 16; ++i) f[i] = fminf(fmaxf(f[i], 0.f), 6.f);
-          }
-          uint4 a, b;
-          a.x = pack_bf16x2(f[0], f[1]);   a.y = pack_bf16x2(f[2], f[3]);
-          a.z = pack_bf16x2(f[4], f[5]);   a.w = pack_bf16x2(f[6], f[7]);
-          b.x = pack_bf16x2(f[8], f[9]);   b.y = pack_bf16x2(f[10], f[11]);
-          b.z = pack_bf16x2(f[12], f[13]); b.w = pack_bf16x2(f[14], f[15]);
-          *p0 = a;
-          *p1 = b;
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tmem_empty[acc]);
-      fence_proxy_async();
-      named_bar_sync(1, 256);
-      if (leader) {
-        for (int b = 0; b < nbox; ++b) tma_store_4d(&tmC, epi + b * box_pitch, nbase + b * 64, 0, h0, img);
-        bulk_commit_group();
-      }
-      if (p.stats != nullptr) {
-        if (st_ntile != n_tile) {
-          if (st_ntile >= 0) {
-            double* dst = p.stats + (blockIdx.x % kHStatReplicas) * 2 * p.Kout + st_ntile * p.block_n + st_col;
-            atomicAdd(dst, (double)st_s1);
-            atomicAdd(dst + p.Kout, (double)st_s2);
-          }
-          st_ntile = n_tile; st_s1 = 0.f; st_s2 = 0.f;
-        }
-        const int vrows = min(p.RT, p.H - h0) * p.W;   // staged rows that belong to the image
-        const uint8_t* col = epi + (st_col >> 6) * box_pitch + (st_col & 7) * 2;
-        const int j = (st_col & 63) >> 3;
-        const int r_end = min(st_row0 + st_rows, vrows);
-        for (int r = st_row0; r < r_end; ++r) {
-          const float x = __bfloat162float(*reinterpret_cast<const __nv_bfloat16*>(col + r * 128 + ((j ^ (r & 7)) << 4)));
-          st_s1 += x;
-          st_s2 = fmaf(x, x, st_s2);
-        }
-      }
-    }
-    if (p.stats != nullptr && st_ntile >= 0) {
-      double* dst = p.stats + (blockIdx.x % kHStatReplicas) * 2 * p.Kout + st_ntile * p.block_n + st_col;
-      atomicAdd(dst, (double)st_s1);
-      atomicAdd(dst + p.Kout, (double)st_s2);
-    }
-    if (leader) bulk_wait_group0();
+    return;
   }
-  __syncwarp();
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) { tc_fence_after(); tmem_dealloc(tmem_base, 512); }
+
+  // ---- consumers: warpgroup wg computes accumulator rows (virtual pixels) [64 wg, 64 wg + 64) of every tile
+  const int wg = warp >> 2;
+  const int r_lo = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // fragment rows r_lo, r_lo + 8
+  const int c_lo = 2 * (lane & 3);
+  const bool leader = threadIdx.x == 0;
+  const uint64_t proto = make_smem_desc(0, 16, 8u * p.row_bytes, layout_type_for_row_bytes(p.row_bytes));
+  const uint32_t a_wg = (64u * wg * p.row_bytes) >> 4;
+  const int nbox = BN >> 6;
+  const uint32_t box_bytes = static_cast<uint32_t>(p.RT * p.W) * 128u;
+  const uint32_t box_pitch = (box_bytes + 1023u) & ~1023u;
+  int srow[2];
+  bool in_tile[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int v = r_lo + 8 * h;
+    const int ry = v / p.Wp, cx = v - ry * p.Wp;
+    srow[h] = ry * p.W + cx;            // row of the staged output tile [RT][W][64]
+    in_tile[h] = (ry < p.RT) && (cx < p.W);
+  }
+  // fused BN statistics: this thread owns one output column and a row range of every tile
+  const int st_col = threadIdx.x % BN;
+  const int st_rows = kHTileM / (256 / BN);
+  const int st_row0 = (threadIdx.x / BN) * st_rows;
+  int st_ntile = -1;
+  float st_s1 = 0.f, st_s2 = 0.f;
+  if (p.b_stationary && t_start < total_tiles) mbar_wait(&bstat_bar, 0);
+
+  float acc[BN / 2];
+  int ia = 0, ib = 0; uint32_t pa = 0, pb = 0;
+  int local = 0;
+  for (int tile = t_start; tile < total_tiles; tile += t_step, ++local) {
+    const int m_tile = p.diag ? tile : tile / p.n_tiles, n_tile = p.diag ? own_n : tile - m_tile * p.n_tiles;
+    const int img = m_tile / p.tiles_per_img;
+    const int h0 = (m_tile - img * p.tiles_per_img) * p.RT;
+    const int nbase = n_tile * BN;
+    // the staging tile is reused: the previous TMA store must have read it, every thread must be done with its
+    // statistics reads; then the residual tile is fetched into it while the MMAs run
+    if (leader && local > 0) bulk_wait_group_read0();
+    named_bar_sync(1, 256);
+    if (leader && p.has_res) {
+      fence_proxy_async();
+      mbar_arrive_expect_tx(&res_bar, static_cast<uint32_t>(nbox) * box_bytes);
+      for (int b = 0; b < nbox; ++b) tma_load_4d(&tmR, &res_bar, epi + b * box_pitch, nbase + b * 64, 0, h0, img);
+    }
+
+    // one commit group per tap (streamed weights: each tap frees a weight slot) or per channel block (resident weights);
+    // after wgmma_wait<1> all groups but the newest are complete, so the buffers whose last reader was the previous
+    // group are released then
+    wgmma_fence_acc(acc);
+    int rel_a = -1, rel_b = -1;
+    for (int cc = 0; cc < p.c_chunks; ++cc) {
+      mbar_wait(&a_full[ia], pa);
+      const uint64_t da0 = proto + (smem_u32(sA + ia * p.a_bytes) >> 4) + a_wg;
+#pragma unroll
+      for (int t = 0; t < NTAPS; ++t) {
+        uint64_t db0;
+        if (p.b_stationary) {
+          db0 = proto + (smem_u32(sB + (cc * NTAPS + t) * p.b_bytes) >> 4);
+        } else {
+          mbar_wait(&b_full[ib], pb);
+          db0 = proto + (smem_u32(sB + ib * p.b_bytes) >> 4);
+        }
+        const uint32_t tap_inc = (static_cast<uint32_t>(p.a_off[t]) * p.row_bytes) >> 4;
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < KSTEPS; ++k)
+          wgmma_bf16<0, 0>(acc, BN, da0 + tap_inc + 2 * k, db0 + 2 * k, (cc | t | k) != 0 ? 1u : 0u);
+        if (!p.b_stationary || t == NTAPS - 1) {
+          wgmma_commit();
+          wgmma_wait<1>();
+          if (rel_b >= 0) release_stage(&b_empty[rel_b], lane);
+          if (rel_a >= 0) release_stage(&a_empty[rel_a], lane);
+          rel_a = (t == NTAPS - 1) ? ia : -1;
+          rel_b = p.b_stationary ? -1 : ib;
+        }
+        if (!p.b_stationary && ++ib == p.sb) { ib = 0; pb ^= 1u; }
+      }
+      if (++ia == p.sa) { ia = 0; pa ^= 1u; }
+    }
+    wgmma_wait<0>();
+    wgmma_fence_acc(acc);
+    if (rel_b >= 0) release_stage(&b_empty[rel_b], lane);
+    if (rel_a >= 0) release_stage(&a_empty[rel_a], lane);
+
+    if (p.has_res) mbar_wait(&res_bar, static_cast<uint32_t>(local & 1));
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      if (!in_tile[h] || h0 + (r_lo + 8 * h) / p.Wp >= p.H) continue;
+      const int row = srow[h];
+#pragma unroll
+      for (int j = 0; j < BN / 2; j += 4) {
+        const int c = 2 * j + c_lo;
+        {
+          uint32_t* dst = reinterpret_cast<uint32_t*>(epi + (c >> 6) * box_pitch + row * 128 +
+                                                      ((((c & 63) >> 3) ^ (row & 7)) << 4) + (c & 7) * 2);
+          float v0 = acc[j + 2 * h], v1 = acc[j + 2 * h + 1];
+          if (p.bias != nullptr) { v0 += __ldg(p.bias + nbase + c); v1 += __ldg(p.bias + nbase + c + 1); }
+          if (p.has_res) {
+            const float2 t2 = unpack_bf16x2(*dst);
+            v0 += t2.x;
+            v1 += t2.y;
+          }
+          *dst = pack_bf16x2(apply_act(v0, p.act), apply_act(v1, p.act));
+        }
+      }
+    }
+    fence_proxy_async();
+    named_bar_sync(1, 256);
+    if (leader) {
+      for (int b = 0; b < nbox; ++b) tma_store_4d(&tmC, epi + b * box_pitch, nbase + b * 64, 0, h0, img);
+      bulk_commit_group();
+    }
+    if (p.stats != nullptr) {
+      if (st_ntile != n_tile) {
+        if (st_ntile >= 0) {
+          double* dst = p.stats + (blockIdx.x % kHStatReplicas) * 2 * p.Kout + st_ntile * BN + st_col;
+          atomicAdd(dst, (double)st_s1);
+          atomicAdd(dst + p.Kout, (double)st_s2);
+        }
+        st_ntile = n_tile; st_s1 = 0.f; st_s2 = 0.f;
+      }
+      const int vrows = min(p.RT, p.H - h0) * p.W;   // staged rows that belong to the image
+      const uint8_t* col = epi + (st_col >> 6) * box_pitch + (st_col & 7) * 2;
+      const int j = (st_col & 63) >> 3;
+      const int r_end = min(st_row0 + st_rows, vrows);
+      for (int r = st_row0; r < r_end; ++r) {
+        const float x = __bfloat162float(*reinterpret_cast<const __nv_bfloat16*>(col + r * 128 + ((j ^ (r & 7)) << 4)));
+        st_s1 += x;
+        st_s2 = fmaf(x, x, st_s2);
+      }
+    }
+  }
+  if (p.stats != nullptr && st_ntile >= 0) {
+    double* dst = p.stats + (blockIdx.x % kHStatReplicas) * 2 * p.Kout + st_ntile * BN + st_col;
+    atomicAdd(dst, (double)st_s1);
+    atomicAdd(dst + p.Kout, (double)st_s2);
+  }
+  if (leader) bulk_wait_group0();
+}
+
+typedef void (*HaloKernelFn)(const __grid_constant__ CUtensorMap, const __grid_constant__ CUtensorMap,
+                             const __grid_constant__ CUtensorMap, const __grid_constant__ CUtensorMap,
+                             const __grid_constant__ HaloParams);
+// 3x3 (9 taps, four 16-deep k-steps per 64-channel chunk) or the 4x4 stem (16 taps, one k-step per 16-channel pixel)
+static HaloKernelFn halo_kernel_for(int ntaps, int block_n) {
+  if (ntaps == 9)
+    return block_n == 64 ? conv_halo_kernel<9, 4, 64> : block_n == 128 ? conv_halo_kernel<9, 4, 128>
+         : block_n == 256 ? conv_halo_kernel<9, 4, 256> : nullptr;
+  if (ntaps == 16)
+    return block_n == 64 ? conv_halo_kernel<16, 1, 64> : block_n == 128 ? conv_halo_kernel<16, 1, 128>
+         : block_n == 256 ? conv_halo_kernel<16, 1, 256> : nullptr;
+  return nullptr;
 }
 
 static int enc4(CUtensorMap* tm, const void* base, int C, int W, int H, int N, int b0, int b1, int b2) {
@@ -420,8 +398,9 @@ int launch_halo(const void* src, const void* wmat, void* out, const void* res, c
     if (rc) return rc;
   }
   const int smem_bytes = p.sa * (int)p.a_bytes + b_region + (int)epi_bytes + 1024;
-  const void* kfn = (p.ntaps == 9) ? (const void*)conv_halo_kernel<9, 4> : (const void*)conv_halo_kernel<16, 1>;
-  cudaError_t e = cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes);
+  HaloKernelFn kfn = halo_kernel_for(p.ntaps, p.block_n);
+  B200_REQUIRE(kfn != nullptr, B200_ERR_UNSUPPORTED, "conv halo: %d taps with block_n %d unsupported", p.ntaps, p.block_n);
+  cudaError_t e = cudaFuncSetAttribute((const void*)kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes);
   B200_REQUIRE(e == cudaSuccess, B200_ERR_CUDA, "conv halo: smem attribute (%d bytes): %s", smem_bytes, cudaGetErrorString(e));
   const int total = p.m_tiles * p.n_tiles;
   int grid = total < sm_count() ? total : sm_count();
@@ -431,10 +410,7 @@ int launch_halo(const void* src, const void* wmat, void* out, const void* res, c
     if (per_n < 1) per_n = 1;
     grid = per_n * p.n_tiles;
   }
-  if (p.ntaps == 9)
-    b200::launch(conv_halo_kernel<9, 4>, grid, kHThreads, smem_bytes, stream, tmX, tmB, tmC, tmR, p);
-  else
-    b200::launch(conv_halo_kernel<16, 1>, grid, kHThreads, smem_bytes, stream, tmX, tmB, tmC, tmR, p);
+  b200::launch(kfn, grid, kHThreads, smem_bytes, stream, tmX, tmB, tmC, tmR, p);
   B200_CHECK_LAUNCH("conv_halo_kernel");
   return B200_OK;
 }
@@ -446,11 +422,12 @@ int launch_halo(const void* src, const void* wmat, void* out, const void* res, c
 // Both operands are MN-major (rows of shared memory = pixels = the GEMM K dimension).  A tile is RT output rows
 // in the padded pitch Wp: dy is loaded as [RT x Wp] pixels (the S-1 extra columns are out of bounds -> TMA writes
 // zeros), x as the [(RT+R-1) x Wp] halo, ONCE; the R*S taps are row-shifted views of that one x buffer, each
-// accumulating into its own TMEM column block [128 k x cw c].  With cw = 32 (3x3) the 9 taps use 288 of the 512
-// TMEM columns; the stem (16 taps x 16 channels) uses 256.  The im2col kernel re-fetched x once per tap.
+// accumulating into its own register block [128 k x cw c].  With cw = 16 the 9 taps of a 3x3 filter take 144
+// accumulator columns (72 registers per consumer thread), the stem's 16 taps 256.  The im2col kernel re-fetched x
+// once per tap.
 // One CTA owns a (k-tile, channel-chunk) unit and a contiguous range of pixel tiles (split-K over pixels); partial
 // fp32 tiles go to the workspace and conv_halo_wgrad_reduce_kernel adds them into dw in a fixed order.
-constexpr int kWThreads = 192;   // TMA warp, MMA warp, 4 epilogue warps
+constexpr int kWThreads = 384;   // two consumer warpgroups + the producer warpgroup (warp 8 issues the TMA)
 constexpr int kWMaxStages = 4;
 
 struct HaloWgradParams {
@@ -469,15 +446,15 @@ struct HaloWgradParams {
 
 // The S taps of one filter row are ONE MMA: their x views start one pixel row apart, so the descriptor's
 // leading-dimension stride (distance between swizzle atoms along N) is set to one pixel row and N = S * cw.  The
-// dy operand (4 KB per MMA) is then read from shared memory once per filter row instead of once per tap -- with
-// N = cw the kernel was bound by shared-memory bandwidth, not by the tensor pipe.
+// dy operand is then read from shared memory once per filter row instead of once per tap.
+// Consumer warpgroup wg owns output channels [k0 + 64 wg, k0 + 64 wg + 64): R accumulator blocks of S * cw columns.
 template <int R, int S>
 __global__ void __launch_bounds__(kWThreads, 1)
 conv_halo_wgrad_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_constant__ CUtensorMap tmX,
                        const __grid_constant__ HaloWgradParams p) {
+  constexpr int kCols = S * 16;   // accumulator columns of one filter row (cw = 16 channels per x chunk)
   extern __shared__ uint8_t smem_raw[];
-  __shared__ __align__(8) uint64_t full_bar[kWMaxStages], empty_bar[kWMaxStages], acc_bar;
-  __shared__ uint32_t tmem_base_s;
+  __shared__ __align__(8) uint64_t full_bar[kWMaxStages], empty_bar[kWMaxStages];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const uint32_t raw_addr = smem_u32(smem_raw);
   uint8_t* smem = smem_raw + (((raw_addr + 1023u) & ~1023u) - raw_addr);
@@ -491,19 +468,14 @@ conv_halo_wgrad_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_co
     for (int i = threadIdx.x; i < n16; i += kWThreads) z[i] = make_uint4(0u, 0u, 0u, 0u);
   }
   if (threadIdx.x == 0) {
-    for (int s = 0; s < p.stages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-    mbar_init(&acc_bar, 1);
+    for (int s = 0; s < p.stages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 8); }
     fence_mbar_init();
     prefetch_tmap(&tmDy);
     prefetch_tmap(&tmX);
   }
-  if (warp == 1) { tmem_alloc(&tmem_base_s, 512); tmem_relinquish(); }
   fence_proxy_async();
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  pdl_wait();   // prologue above (barriers, TMEM, descriptor prefetch) overlaps the predecessor grid
-  const uint32_t tmem_base = tmem_base_s;
+  pdl_wait();   // prologue above (barriers, descriptor prefetch) overlaps the predecessor grid
 
   const int split = blockIdx.x / p.units;
   const int unit = blockIdx.x - split * p.units;
@@ -514,73 +486,77 @@ conv_halo_wgrad_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_co
   const int t_end = min(p.m_tiles, t_begin + p.tiles_per_split);
   const int ntiles = t_end - t_begin;
   const int nA = min(2, (p.K_out - k0 + 63) / 64);
+  if (ntiles <= 0) return;
 
-  if (ntiles > 0) {
-    if (warp == 0) {
-      if (lane == 0) {
-        int stage = 0; uint32_t phase = 0;
-        const uint32_t tx = nA * p.a_box_bytes + p.x_box_bytes;
-        for (int tile = t_begin; tile < t_end; ++tile) {
-          const int img = tile / p.tiles_per_img;
-          const int h0 = (tile - img * p.tiles_per_img) * p.RT;
-          mbar_wait(&empty_bar[stage], phase ^ 1u);
-          uint8_t* sa = smem + stage * stage_bytes;
-          mbar_arrive_expect_tx(&full_bar[stage], tx);
-          for (int j = 0; j < nA; ++j) tma_load_4d(&tmDy, &full_bar[stage], sa + j * 16384, k0 + j * 64, 0, h0, img);
-          tma_load_4d(&tmX, &full_bar[stage], sa + p.a_bytes, cc * p.cw + (p.window ? k0 : 0), -p.pad, h0 - p.pad, img);
-          if (++stage == p.stages) { stage = 0; phase ^= 1u; }
-        }
-      }
-    } else if (warp == 1) {
-      if (lane == 0) {
-        int stage = 0; uint32_t phase = 0;
-        const uint32_t idesc = make_idesc_bf16(kHTileM, S * p.cw, 1, 1);
-        const uint64_t protoA = make_smem_desc(0, 16384, 1024, 2);
-        const uint64_t protoX = make_smem_desc(0, p.x_row_bytes, 8u * p.x_row_bytes, layout_type_for_row_bytes(p.x_row_bytes));
-        uint32_t row_inc[R];
-#pragma unroll
-        for (int r = 0; r < R; ++r) row_inc[r] = (static_cast<uint32_t>(p.x_off[r * S]) * p.x_row_bytes) >> 4;
-        const uint32_t kx_inc = (16u * p.x_row_bytes) >> 4;   // 16 pixel rows per K step
-        for (int i = 0; i < ntiles; ++i) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint32_t a_addr = smem_u32(smem + stage * stage_bytes);
-          const uint64_t da0 = protoA + (a_addr >> 4);
-          const uint64_t dx0 = protoX + ((a_addr + p.a_bytes) >> 4);
-#pragma unroll
-          for (int k = 0; k < 8; ++k) {
-            const uint32_t acc = (k != 0) ? 1u : (i != 0 ? 1u : 0u);
-#pragma unroll
-            for (int r = 0; r < R; ++r)
-              umma_bf16(tmem_base + r * S * p.cw, da0 + k * 128, dx0 + row_inc[r] + k * kx_inc, idesc, acc);
-          }
-          umma_commit(&empty_bar[stage]);
-          if (i == ntiles - 1) umma_commit(&acc_bar);
-          if (++stage == p.stages) { stage = 0; phase ^= 1u; }
-        }
-      }
-    } else {
-      const int q = warp & 3;
-      mbar_wait(&acc_bar, 0);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + (static_cast<uint32_t>(q * 32) << 16);
-      float* dst = p.partial + ((static_cast<long long>(unit) * p.splits + split) * kHTileM + (q * 32 + lane)) * p.ncols;
-      for (int c0 = 0; c0 < p.ncols; c0 += 16) {
-        uint32_t v[16];
-        tmem_ld16(taddr + c0, v);
-        tmem_ld_wait();
-#pragma unroll
-        for (int i = 0; i < 4; ++i)
-          *reinterpret_cast<float4*>(dst + c0 + 4 * i) =
-              make_float4(__uint_as_float(v[4 * i]), __uint_as_float(v[4 * i + 1]), __uint_as_float(v[4 * i + 2]),
-                          __uint_as_float(v[4 * i + 3]));
+  if (warp >= 8) {
+    if (warp == 8 && lane == 0) {
+      int stage = 0; uint32_t phase = 0;
+      const uint32_t tx = nA * p.a_box_bytes + p.x_box_bytes;
+      for (int tile = t_begin; tile < t_end; ++tile) {
+        const int img = tile / p.tiles_per_img;
+        const int h0 = (tile - img * p.tiles_per_img) * p.RT;
+        mbar_wait(&empty_bar[stage], phase ^ 1u);
+        uint8_t* sa = smem + stage * stage_bytes;
+        mbar_arrive_expect_tx(&full_bar[stage], tx);
+        for (int j = 0; j < nA; ++j) tma_load_4d(&tmDy, &full_bar[stage], sa + j * 16384, k0 + j * 64, 0, h0, img);
+        tma_load_4d(&tmX, &full_bar[stage], sa + p.a_bytes, cc * p.cw + (p.window ? k0 : 0), -p.pad, h0 - p.pad, img);
+        if (++stage == p.stages) { stage = 0; phase ^= 1u; }
       }
     }
+    return;
   }
-  __syncwarp();
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) { tc_fence_after(); tmem_dealloc(tmem_base, 512); }
+
+  const int wg = warp >> 2;
+  const bool wg_on = wg < nA;
+  // dy: one 64-channel box per warpgroup, MN-major, 128 B pixel rows; x: MN-major, LBO = one pixel row (the S taps)
+  const uint64_t protoA = make_smem_desc(0, 16384, 1024, 1);
+  const uint64_t protoX = make_smem_desc(0, p.x_row_bytes, 8u * p.x_row_bytes, layout_type_for_row_bytes(p.x_row_bytes));
+  uint32_t row_inc[R];
+#pragma unroll
+  for (int r = 0; r < R; ++r) row_inc[r] = (static_cast<uint32_t>(p.x_off[r * S]) * p.x_row_bytes) >> 4;
+  const uint32_t kx_inc = (16u * p.x_row_bytes) >> 4;   // 16 pixel rows per K step
+  float acc[R][kCols / 2];
+#pragma unroll
+  for (int r = 0; r < R; ++r) wgmma_fence_acc(acc[r]);
+  int stage = 0, prev = 0; uint32_t phase = 0;
+  for (int i = 0; i < ntiles; ++i) {
+    mbar_wait(&full_bar[stage], phase);
+    if (wg_on) {
+      const uint32_t a_addr = smem_u32(smem + stage * stage_bytes);
+      const uint64_t da0 = protoA + ((a_addr + wg * 16384) >> 4);
+      const uint64_t dx0 = protoX + ((a_addr + p.a_bytes) >> 4);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < 8; ++k) {
+        const uint32_t scale = (k != 0 || i != 0) ? 1u : 0u;
+#pragma unroll
+        for (int r = 0; r < R; ++r)
+          wgmma_bf16<1, 1>(acc[r], kCols, da0 + k * 128, dx0 + row_inc[r] + k * kx_inc, scale);
+      }
+      wgmma_commit();
+      wgmma_wait<1>();
+    }
+    if (i > 0) release_stage(&empty_bar[prev], lane);
+    prev = stage;
+    if (++stage == p.stages) { stage = 0; phase ^= 1u; }
+  }
+  wgmma_wait<0>();
+#pragma unroll
+  for (int r = 0; r < R; ++r) wgmma_fence_acc(acc[r]);
+  release_stage(&empty_bar[prev], lane);
+  if (!wg_on) return;
+
+  const int row = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // fragment rows row, row + 8 (output channels)
+  const int c_lo = 2 * (lane & 3);
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    float* dst = p.partial + ((static_cast<long long>(unit) * p.splits + split) * kHTileM + row + 8 * h) * p.ncols;
+#pragma unroll
+    for (int r = 0; r < R; ++r)
+#pragma unroll
+      for (int j = 0; j < kCols / 2; j += 4)
+        *reinterpret_cast<float2*>(dst + r * kCols + 2 * j + c_lo) = make_float2(acc[r][j + 2 * h], acc[r][j + 2 * h + 1]);
+  }
 }
 
 // dw[k][tap][c] += sum over splits of partial[unit(k_tile, cc)][split][k % 128][tap * cw + c % cw]
@@ -642,7 +618,7 @@ int launch_halo_wgrad(const void* x, const void* dy, float* dw, void* workspace,
                  "conv halo wgrad: window mode needs window == 128 and C == K, C %% 128 == 0 (C=%d K=%d)", C, K_out);
   p.N = N; p.H = H; p.W = W; p.K_out = K_out; p.C = C;
   p.ntaps = R * S; p.pad = pad;
-  p.cw = (C == 16) ? 16 : 32;
+  p.cw = 16;   // 16 channels per x chunk: R * S * 16 / 2 accumulator registers per consumer thread
   p.x_row_bytes = p.cw * 2;
   p.ncols = p.ntaps * p.cw;
   p.Wp = W + S - 1;

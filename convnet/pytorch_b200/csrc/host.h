@@ -35,15 +35,10 @@ bool halo_wgrad_eligible(int H, int W, int C, int K_out, int R, int S, int pad);
 int launch_halo_wgrad(const void* x, const void* dy, float* dw, void* workspace, size_t workspace_bytes, int N, int H,
                       int W, int C, int K_out, int R, int S, int pad, cudaStream_t stream, int window = 0);
 
-// conv_pair.cu: EXPERIMENTAL cta_group::2 GEMM for wide 1x1 / stride-1 layers (B200_IGEMM_PAIR=1)
-bool pair_eligible(long long M, int C, int Nout);
-int launch_pair(const void* a, const void* w, void* out, const void* res, const float* bias, long long M, int C, int Nout,
-                int act, double* stats, cudaStream_t stream);
-
 // Kernel launch with programmatic dependent launch (PDL): the grid may be scheduled while its stream predecessor is
 // still draining; every kernel launched through here executes pdl_wait() (griddepcontrol.wait, common.cuh) in all
 // threads before it touches global memory, which blocks until the predecessor grid has completed and its writes are
-// visible.  What overlaps is the launch latency, block scheduling and the smem/TMEM/barrier prologue -- ~560 kernel
+// visible.  What overlaps is the launch latency, block scheduling and the smem/barrier prologue -- ~560 kernel
 // boundaries per ResNet-50 step.  B200_PDL=0 launches without the attribute (pdl_wait() is then a no-op).
 bool pdl_enabled();
 template <typename... KArgs, typename... Args>

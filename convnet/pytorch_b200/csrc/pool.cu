@@ -143,7 +143,7 @@ __global__ void __launch_bounds__(256) maxpool_bwd_kernel(const __nv_bfloat16* _
 // Sliding-window versions (default): a thread owns one (image, output column, 8-channel vector) and walks down the
 // rows, keeping the window rows in registers (packed bf16) -- 6 loads per pooled output instead of 9, 2 instead of 8 per
 // input-gradient vector, no 64-bit index arithmetic.  These kernels are bound by load requests in flight, like the
-// BatchNorm ones (profiles/r02_summary.md); results are bit-identical to the kernels above.
+// BatchNorm ones; results are bit-identical to the kernels above.
 struct PoolSlide {
   int N, H, W, C, OH, OW;
   int TP;                 // pooled rows (fwd) / row pairs (bwd) per work item

@@ -1,6 +1,6 @@
 // Squeeze-and-excitation on the residual branch (reference models/modules/se.py:6-25, used by resnet_se / resnext_se,
 // models/resnet.py:112-113,159-160,434-436):   r' = r * sigmoid(W2 relu(W1 mean_hw(r) + b1) + b2).
-// The two tiny linear layers run on the tcgen05 1x1-conv kernels; this file holds the HBM-bound NHWC bf16 passes
+// The two tiny linear layers run on the wgmma 1x1-conv kernels; this file holds the HBM-bound NHWC bf16 passes
 // around them (pool, scale, and the two backward passes) plus a generic elementwise activation backward.
 //   forward : se_pool (read r) -> [MLP] -> se_scale_fwd (read r, write r')
 //   backward: se_bwd_reduce (read g, r: dlogit = sigma' * sum_hw g*r) -> [MLP backward] ->

@@ -3,12 +3,12 @@
 ``convert_b200(model)`` takes a model built by the registry (ordinary ``torch.nn`` layers, reference
 attribute names) and
   * moves every parameter into flat device arenas -- fp32 master ``p32``, fp32 gradient ``g32``, bf16
-    compute shadow ``p16`` -- conv weights physically [K][R*S][C] (the layout the tcgen05 kernels read)
+    compute shadow ``p16`` -- conv weights physically [K][R*S][C] (the layout the wgmma kernels read)
     while ``param.shape`` / ``state_dict()`` stay the reference's logical OIHW (SURVEY.md section 5,
     checkpoint row);
   * installs a runtime whose ``forward`` replaces ``model.forward`` (models/resnet.py:196-213 in the
     reference) by the kernel pipeline
-        conv (tcgen05 implicit GEMM) -> BN statistics -> BN apply + ReLU (+ residual) ...
+        conv (wgmma implicit GEMM) -> BN statistics -> BN apply + ReLU (+ residual) ...
     and whose backward (one autograd node for the whole net) runs BN backward, dgrad and wgrad kernels
     and writes parameter gradients straight into ``g32`` (``param.grad`` are views of it).
 Nothing here computes on the CPU or through cuDNN/cuBLAS: a missing library or an unsupported layer

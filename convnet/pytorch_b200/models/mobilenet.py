@@ -3,7 +3,7 @@ depthwise-separable units -- depthwise 3x3 (WITH bias, as in the reference, whos
 bias=True) -> BN -> ReLU -> 1x1 -> BN -> ReLU -- global average pooling and a linear classifier.  Module names
 (``features.{i}``, ``features.{i}.components.{j}``, ``fc``) match the reference so checkpoints interchange; weight decay
 skips the depthwise convolutions (models/mobilenet.py:23-36).  SURVEY.md section 8(f) row 4: a neighbour family that runs
-on the same kernels as MobileNet-v2 (depthwise CUDA-core kernels + tcgen05 1x1 convolutions)."""
+on the same kernels as MobileNet-v2 (depthwise CUDA-core kernels + wgmma 1x1 convolutions)."""
 import torch.nn as nn
 
 __all__ = ['mobilenet']

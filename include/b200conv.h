@@ -1,5 +1,5 @@
 /*
- * b200conv.h -- C ABI of libb200conv.so: the B200 (sm_100a) training hot path behind
+ * b200conv.h -- C ABI of libb200conv.so: the H100 (sm_90a) training hot path behind
  * eladhoffer/convNet.pytorch's trainer.Trainer loop and ResNet-family model factories.
  *
  * The reference has no FFI of its own (it is pure Python on top of torch.nn); every entry point
@@ -68,7 +68,7 @@ int b200_version(void);
 /* number of kernels launched by this library in this process (for bench.py's gpu_launches). */
 long long b200_launch_count(void);
 
-/* ---- convolution: implicit GEMM on tcgen05 tensor cores (csrc/conv.cu) ------------------------
+/* ---- convolution: implicit GEMM on wgmma tensor cores (csrc/conv.cu) ------------------------
  * replaces nn.Conv2d forward            (models/resnet.py:75-78,126-132,226-227; trainer.py:132)
  *          ConvolutionBackward0 (dgrad) (trainer.py:162 loss.backward())
  *          ConvolutionBackward0 (wgrad) (trainer.py:162)

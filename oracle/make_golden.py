@@ -1,5 +1,5 @@
-"""Generates tests/golden/* by running the UNMODIFIED reference (read-only at /root/reference) in this
-container.  Run once from the repo root:  python oracle/make_golden.py
+"""Generates tests/golden/* by running the UNMODIFIED reference (a checkout of eladhoffer/convNet.pytorch, read-only).
+Run once from the repo root:  B200_REFERENCE=<reference checkout> python oracle/make_golden.py
 The fixtures pin (a) the oracle restatement (oracle/ref_model.py), (b) the re-authored host code
 (models, regimes, trainer) and (c) -- through the GPU tests -- the CUDA pipeline.
 Nothing here is needed at test time: tests read only the committed fixtures.
@@ -12,11 +12,13 @@ from copy import deepcopy
 import numpy as np
 import torch
 
-REF = os.environ.get('B200_REFERENCE', '/root/reference')
+REF = os.environ.get('B200_REFERENCE', '')
 OUT = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), 'tests', 'golden')
 
 
 def import_reference():
+    if not os.path.isdir(REF):
+        raise SystemExit('set B200_REFERENCE to a checkout of eladhoffer/convNet.pytorch')
     sys.path.insert(0, REF)
     import models as ref_models            # noqa: E402
     import trainer as ref_trainer          # noqa: E402

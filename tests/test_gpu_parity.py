@@ -1,4 +1,4 @@
-"""Parity cases the round-1 review asked for (VERDICT.md "Next round" item 1), all through the C ABI:
+"""Parity cases of the training features around the step, all through the C ABI:
   * the sampled (Mix&Match, config C5) optimizer regime -- GradSmooth folded into the fused SGD kernel -- against the
     torch hook chain of the same regime;
   * Trainer.train with batch augmentation (duplicates D = 3, [B, D, C, H, W] inputs) and the sampled regime against

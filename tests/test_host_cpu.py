@@ -200,29 +200,3 @@ def test_evaluate_cli_cpu(tmp_path):
         del os.environ['B200_SYNTHETIC_LENGTH']
     assert abs(base['loss'] - absorbed['loss']) < 1e-4 * max(1.0, base['loss']) and base['prec1'] == absorbed['prec1']
     assert both['loss'] > 0 and 0 <= both['prec1'] <= 100
-
-
-def test_committed_profile_feeds_bench_traffic():
-    """bench.py reports roofline.traffic from profiles/r02_traffic.json (DRAM bytes per launch of the dominant kernel
-    class, produced by tools/summarize_launches.py from the committed ncu launch list): the file must carry the class
-    bench.py looks up, and the summariser must reproduce it from the committed CSV."""
-    import json
-    import subprocess
-    import sys
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    with open(os.path.join(root, 'profiles', 'r02_traffic.json')) as f:
-        tj = json.load(f)['classes']
-    for key in ('conv_fprop+dgrad', 'conv_wgrad', 'bn_apply', 'bn_bwd_dx', 'bn_bwd_reduce'):
-        assert tj[key]['launches'] > 0 and tj[key]['dram_read_bytes'] > 0, key
-    out_md, out_js = os.path.join('/tmp', 'r02_launches_check.md'), os.path.join('/tmp', 'r02_traffic_check.json')
-    r = subprocess.run([sys.executable, os.path.join(root, 'tools', 'summarize_launches.py'),
-                        os.path.join(root, 'profiles', 'r02_launches.csv'), out_md, 'check', out_js],
-                       capture_output=True, text=True, timeout=120)
-    assert r.returncode == 0, r.stderr[-500:]
-    with open(out_js) as f:
-        again = json.load(f)['classes']
-    assert again['conv_fprop+dgrad']['launches'] == tj['conv_fprop+dgrad']['launches']
-    assert abs(again['conv_fprop+dgrad']['dram_read_bytes'] - tj['conv_fprop+dgrad']['dram_read_bytes']) < 1.0
-    with open(out_md) as f:
-        assert 'b200::conv_igemm_kernel' in f.read()
-

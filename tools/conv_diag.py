@@ -1,4 +1,4 @@
-"""GPU diagnostic for the tcgen05 convolution kernels: runs ONE case (argv[1]) or lists cases.
+"""GPU diagnostic for the wgmma convolution kernels: runs ONE case (argv[1]) or lists cases.
 
 Each case compares fprop / dgrad / wgrad of libb200conv.so with an fp64 torch reference computed on
 bf16-rounded operands.  Driven case-by-case from tools/run_gpu_diag.sh so that a trapped kernel (sticky

@@ -1,4 +1,4 @@
-"""Per-tensor gradient comparison of the B200 pipeline against the bf16-emulating CPU oracle (diagnostic)."""
+"""Per-tensor gradient comparison of the kernel pipeline against the bf16-emulating CPU oracle (diagnostic)."""
 import sys, os, copy
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch

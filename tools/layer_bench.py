@@ -1,5 +1,5 @@
 """Per-layer timing of the conv kernels on ResNet-50 shapes (batch 256): CUDA-event median per launch, achieved
-TFLOP/s and algorithmic GB/s.  usage: layer_bench.py [filter] [--once]   (--once: one launch each, for ncu)"""
+TFLOP/s and algorithmic GB/s.  usage: layer_bench.py [filter] [--once]   (--once: one launch each)"""
 import sys, os, json
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch

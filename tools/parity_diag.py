@@ -1,5 +1,5 @@
 """Which tensors carry the gradient error?  usage: parity_diag.py <depth> <size> <batch> [oracle]
-Prints, for the B200 pipeline vs stock torch fp32 (and vs the bf16-storage CPU oracle with `oracle`), the tensors sorted
+Prints, for the kernel pipeline vs stock torch fp32 (and vs the bf16-storage CPU oracle with `oracle`), the tensors sorted
 by their share of the squared global gradient error."""
 import sys, os, copy
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
