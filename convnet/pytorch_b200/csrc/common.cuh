@@ -66,13 +66,16 @@ __device__ __forceinline__ uint64_t global_timer_ns() {
   asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));
   return t;
 }
+// Kept out of line: a trap instruction inlined after setmaxnreg makes ptxas allocate that code within the launch-bounds
+// register cap (168 for 384 threads) instead of the reallocated count, and the consumers spill.
+static __device__ __noinline__ void wait_timeout_trap() { __trap(); }
 // Bounded wait: a protocol bug becomes a trap (launch failure) after B200_WAIT_TIMEOUT_NS instead of a hung GPU.
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   if (mbar_try_wait(bar, parity)) return;
   const uint64_t t0 = global_timer_ns();
   uint32_t spins = 0;
   while (!mbar_try_wait(bar, parity)) {
-    if ((++spins & 0xFFu) == 0u && global_timer_ns() - t0 > B200_WAIT_TIMEOUT_NS) { __trap(); }
+    if ((++spins & 0xFFu) == 0u && global_timer_ns() - t0 > B200_WAIT_TIMEOUT_NS) wait_timeout_trap();
   }
 }
 
@@ -144,6 +147,17 @@ __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.a
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 template <int N>
 __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// Register reallocation of the 384-thread wgmma kernels (one producer warpgroup, two consumer warpgroups, 168 registers
+// per thread at launch): the producer, which only issues TMA, drops to 56 (the weight-gradient producer keeps its
+// per-box coordinate tables in registers) and the consumers grow to 224 (56 * 128 + 2 * 224 * 128 <= 65536).  Every
+// warp of a warpgroup must execute the call, before any of them exits.
+constexpr uint32_t kProducerRegs = 56, kConsumerRegs = 224;
+__device__ __forceinline__ void producer_setmaxnreg() {
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kProducerRegs));
+}
+__device__ __forceinline__ void consumer_setmaxnreg() {
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kConsumerRegs));
+}
 // Orders ordinary register accesses of the accumulators against the asynchronous MMAs that write them.
 template <int SZ>
 __device__ __forceinline__ void wgmma_fence_acc(float (&d)[SZ]) {

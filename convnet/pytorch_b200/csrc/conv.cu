@@ -6,14 +6,17 @@
 //
 // Operand tiles are staged by TMA (im2col mode for the activation side, tiled mode for weights / dy)
 // into 32/64/128B-swizzled shared memory and consumed by wgmma.mma_async with fp32 accumulators in registers.
-// Warp roles: warps 0..7 = two consumer warpgroups (rows 0-63 and 64-127 of a 128-row tile: MMA, then the epilogue),
-// warp 8 (of the third warpgroup) = TMA producer, which runs ahead through the stage ring while the consumers drain a tile.
+// Warp roles: warps 0..7 = two consumer warpgroups, warp 8 (of the third warpgroup) = TMA producer.  The implicit-GEMM
+// kernel runs the consumers ping-pong: each owns whole 128-row tiles, alternating with the other, so one warpgroup's
+// epilogue runs while the other's MMAs keep the tensor cores busy.  The weight-gradient kernel splits each tile's
+// output channels between them.
 //
 // Replaces cuDNN's convolution behind nn.Conv2d in the reference (models/resnet.py:75-78,126-132,
 // 226-227) and its autograd backward (trainer.py:162).
 #include "common.cuh"
 #include "host.h"
 #include <stdlib.h>
+#include <utility>
 
 namespace b200 {
 
@@ -53,11 +56,10 @@ struct IgemmParams {
   int own_ntile;         // 1 (with b_stationary): the CTA owns n-tile blockIdx.x % n_tiles -- its weight slices are loaded
                          // once -- and walks the m-tiles blockIdx.x / n_tiles, + gridDim.x / n_tiles, ... (the grid is a
                          // multiple of n_tiles).  Cuts the L2->SM re-streaming of the weights from once per tile to once
-                         // per CTA for layers whose per-n-tile weights fit in shared memory (K <= 256 at N-tile 256)
-  int window;            // > 0: block-diagonal convolution -- n-tile b (block_n == window) reads source channels
-                         // [window*b, window*b + window) only; the weight operand is [N_total][taps][window]
-  int epi_bufs;          // 1 or 2 output staging tiles: with 2, a tile's staging never waits for the previous tile's store
-  uint32_t epi_bytes;
+                         // per CTA for layers whose per-n-tile weights fit in shared memory beside the ring
+  int window;            // > 0: block-diagonal convolution -- output channels [window*b, window*b + window) read source
+                         // channels [window*b, window*b + window) only; the weight operand is [N_total][taps][window]
+  uint32_t epi_bytes;    // one warpgroup's output staging tile
   double* stats;         // fused BN statistics accumulators [kStatReplicas][2][N_total] (BN workspace) or nullptr
   void* out;
   const void* res;
@@ -106,6 +108,22 @@ __device__ __forceinline__ void store_pair(const IgemmParams& p, float v0, float
   }
 }
 
+// The MMAs of one operand stage for a warpgroup's 128-row tile: per 16-deep k-step, two m64 wgmmas (rows 0-63 and
+// 64-127) that share the B descriptor.  KS is the stage's k-steps (ck / 16); scale0 == 0 starts the accumulators.
+template <int KS, int SZ>
+__device__ __forceinline__ void igemm_stage_mma(float (&acc)[2][SZ], uint64_t da, uint64_t db, uint32_t a_half,
+                                                uint32_t scale0) {
+  wgmma_fence();
+#pragma unroll
+  for (int k = 0; k < KS; ++k) {
+    wgmma_bf16<0, 0>(acc[0], da + 2 * k, db + 2 * k, k != 0 ? 1u : scale0);
+    wgmma_bf16<0, 0>(acc[1], da + a_half + 2 * k, db + 2 * k, k != 0 ? 1u : scale0);
+  }
+  wgmma_commit();
+}
+
+// BN = block_n, the tile width: it sizes the accumulators exactly and fixes the wgmma shape at compile time.
+template <int BN>
 __global__ void __launch_bounds__(kThreads, 1)
 conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                   const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmR,
@@ -113,7 +131,7 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   extern __shared__ uint8_t smem_raw[];
   __shared__ __align__(8) uint64_t full_bar[kMaxStages];
   __shared__ __align__(8) uint64_t empty_bar[kMaxStages];
-  __shared__ __align__(8) uint64_t res_bar[2][2], bstat_bar;   // [warpgroup][staging buffer]
+  __shared__ __align__(8) uint64_t turn_bar[2], res_bar[2], bstat_bar;   // [warpgroup]
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -126,10 +144,13 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   if (threadIdx.x == 0) {
     for (int s = 0; s < p.num_stages; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], kConsumers / 32);
+      mbar_init(&empty_bar[s], 4);   // released by the four warps of the warpgroup that consumed it
     }
     mbar_init(&bstat_bar, 1);
-    for (int i = 0; i < 4; ++i) mbar_init(&res_bar[i >> 1][i & 1], 1);
+    for (int i = 0; i < 2; ++i) {
+      mbar_init(&res_bar[i], 1);
+      mbar_init(&turn_bar[i], 4);
+    }
     fence_mbar_init();
     prefetch_tmap(&tmA);
     prefetch_tmap(&tmB);
@@ -141,15 +162,15 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   __syncthreads();
   pdl_wait();   // prologue above (barriers, descriptor prefetch) overlaps the predecessor grid
 
-  const int total_tiles = p.m_tiles * p.n_tiles;
   const int k_iters = p.ntaps * p.c_chunks;
   // tile walk: round-robin over all (m, n) tiles, or -- owned n-tile -- over the m-tiles of one n-tile
   const int walk_first = p.own_ntile ? static_cast<int>(blockIdx.x) / p.n_tiles : static_cast<int>(blockIdx.x);
   const int walk_step = p.own_ntile ? static_cast<int>(gridDim.x) / p.n_tiles : static_cast<int>(gridDim.x);
-  const int walk_end = p.own_ntile ? p.m_tiles : total_tiles;
+  const int walk_end = p.own_ntile ? p.m_tiles : p.m_tiles * p.n_tiles;
   const int own_n = static_cast<int>(blockIdx.x) % p.n_tiles;
 
   if (warp >= kProducerWarp) {
+    producer_setmaxnreg();
     if (warp == kProducerWarp && lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
@@ -159,8 +180,9 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         for (int t = 0; t < p.ntaps; ++t)
           for (int cc = 0; cc < p.c_chunks; ++cc)
             tma_load_3d(&tmB, &bstat_bar, sBstat + (t * p.c_chunks + cc) * p.b_bytes, cc * p.ck, p.taps[t].b_tap,
-                        p.own_ntile ? own_n * p.block_n : 0);
+                        p.own_ntile ? own_n * BN : 0);
       }
+      // the ring is filled in tile order; the consumer warpgroups take the CTA's tiles alternately
       for (int tile = walk_first; tile < walk_end; tile += walk_step) {
         const int m_tile = p.own_ntile ? tile : tile / p.n_tiles;
         const int n_tile = p.own_ntile ? own_n : tile - m_tile * p.n_tiles;
@@ -171,6 +193,7 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         const int bj = rem - bi * p.J;
         const int base_w = bj * p.trav + p.lower_w;
         const int base_h = bi * p.trav + p.lower_h;
+        const int a_c0 = p.window ? (n_tile * BN / p.window) * p.window : 0;
         for (int t = 0; t < p.ntaps; ++t) {
           const TapEntry te = p.taps[t];
           for (int cc = 0; cc < p.c_chunks; ++cc) {
@@ -178,12 +201,12 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
             uint8_t* sa = smem + stage * stage_bytes;
             uint8_t* sb = sa + p.a_bytes;
             mbar_arrive_expect_tx(&full_bar[stage], p.b_stationary ? p.a_bytes : p.tx_bytes);
-            const int a_c = cc * p.ck + (p.window ? n_tile * p.window : 0);
+            const int a_c = a_c0 + cc * p.ck;
             if (p.plain_a)  // 1x1 / stride 1: the A operand is a dense [M, C] matrix -> tiled TMA (faster than im2col)
               tma_load_2d(&tmA, &full_bar[stage], sa, a_c, m0);
             else
               tma_load_im2col_4d(&tmA, &full_bar[stage], sa, a_c, base_w, base_h, img, te.off_w, te.off_h);
-            if (!p.b_stationary) tma_load_3d(&tmB, &full_bar[stage], sb, cc * p.ck, te.b_tap, n_tile * p.block_n);
+            if (!p.b_stationary) tma_load_3d(&tmB, &full_bar[stage], sb, cc * p.ck, te.b_tap, n_tile * BN);
             if (++stage == p.num_stages) { stage = 0; phase ^= 1u; }
           }
         }
@@ -191,162 +214,166 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     }
     return;
   }
+  consumer_setmaxnreg();
 
-  // ---- consumers: warpgroup wg computes rows [64 wg, 64 wg + 64) of every tile.  The two warpgroups share the operand
-  // ring but nothing else: each stages, stores and (optionally) reduces the statistics of its own 64 rows, so one
-  // warpgroup's epilogue overlaps the other's MMAs.
+  // ---- consumers, ping-pong: warpgroup wg computes the CTA's tiles local = wg, wg + 2, wg + 4, ... (128 rows x BN
+  // columns each).  It issues a tile's MMAs only after the other warpgroup has issued those of the tile before
+  // (turn_bar), so while one warpgroup runs its epilogue the other's MMAs run, and the two never compete for the tensor
+  // cores with the same tile phase.  Each warpgroup has its own staging tile, residual fetch and statistics.
   const int wg = warp >> 2;
-  const int wt = threadIdx.x & 127;                           // thread index inside the warpgroup
-  const int r_lo = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // this thread's fragment rows: r_lo and r_lo + 8
+  const int wt = threadIdx.x & 127;                  // thread index inside the warpgroup
+  const int r_lo = (warp & 3) * 16 + (lane >> 2);    // this thread's fragment rows of each 64-row half: r_lo, r_lo + 8
   const int c_lo = 2 * (lane & 3);
   const bool leader = wt == 0;
   const uint32_t row_bytes = p.ck * 2;
   const uint64_t proto = make_smem_desc(0, 16, 8 * row_bytes, layout_type_for_row_bytes(row_bytes));
-  const uint32_t a_wg = (64u * row_bytes * wg) >> 4;
+  const uint32_t a_half = (64u * row_bytes) >> 4;   // descriptor offset of rows 64-127 of the A tile
   const int ksteps = p.ck / 16;
   const uint32_t bstat_addr = smem_u32(sBstat);
-  const int nbox = p.block_n >> 6;
-  // fused-statistics bookkeeping: this thread owns columns st_col (+ 128 when block_n == 256), rows
-  // [st_row0, st_row0 + st_rows) of its warpgroup's half of each tile
-  const int st_col = wt % p.block_n;
-  const int st_ncol = p.block_n > 128 ? 2 : 1;
-  const int st_rows = 64 / (p.block_n > 128 ? 1 : 128 / p.block_n);
-  const int st_row0 = wg * 64 + (p.block_n > 128 ? 0 : (wt / p.block_n) * st_rows);
+  constexpr int nbox = BN / 64;
+  uint8_t* epi_w = epi + wg * p.epi_bytes;           // this warpgroup's staging tile: 64-column boxes of [128 rows][128 B]
+  // fused-statistics bookkeeping (BN = 64 or 128): this thread owns column st_col, rows [st_row0, st_row0 + st_rows)
+  // of each tile
+  const int st_col = wt % BN;
+  constexpr int st_rows = BN;
+  const int st_row0 = (wt / BN) * st_rows;
   int st_ntile = -1;
-  float st_s1[2] = {0.f, 0.f}, st_s2[2] = {0.f, 0.f};
+  float st_s1 = 0.f, st_s2 = 0.f;
   auto flush_stats = [&]() {
-    for (int u = 0; u < st_ncol; ++u) {
-      double* dst = p.stats + (blockIdx.x % kStatReplicas) * 2 * p.N_total + st_ntile * p.block_n + st_col + 128 * u;
-      atomicAdd(dst, (double)st_s1[u]);
-      atomicAdd(dst + p.N_total, (double)st_s2[u]);
-      st_s1[u] = 0.f; st_s2[u] = 0.f;
-    }
+    double* dst = p.stats + (blockIdx.x % kStatReplicas) * 2 * p.N_total + st_ntile * BN + st_col;
+    atomicAdd(dst, (double)st_s1);
+    atomicAdd(dst + p.N_total, (double)st_s2);
+    st_s1 = 0.f; st_s2 = 0.f;
   };
   const int IJ = p.I * p.J;
   if (p.b_stationary && walk_first < walk_end) mbar_wait(&bstat_bar, 0);
 
-  float acc[128];
-  int stage = 0;
-  uint32_t phase = 0;
+  float acc[2][BN / 2];
   int local = 0;
   for (int tile = walk_first; tile < walk_end; tile += walk_step, ++local) {
+    if ((local & 1) != wg) continue;
     const int m_tile = p.own_ntile ? tile : tile / p.n_tiles;
     const int n_tile = p.own_ntile ? own_n : tile - m_tile * p.n_tiles;
-    const int nbase = n_tile * p.block_n;
-    const int eb = p.epi_bufs == 2 ? (local & 1) : 0;
-    uint8_t* epi_t = epi + eb * p.epi_bytes;   // staging tile of this tile: 64-column boxes of [128 rows][128 B]
+    const int nbase = n_tile * BN;
+    const int mine = local >> 1;   // this warpgroup's tile count so far
     if (p.tma_store) {
-      // This warpgroup's rows of the staging tile are reused: its store of the tile that last used the buffer must
-      // have read them and its threads must be done with their statistics reads.  Then its half of the residual tile
-      // is fetched into them, landing while the MMAs run.
-      if (leader && local > 0) {
-        if (p.epi_bufs == 2) bulk_wait_group_read1();
-        else bulk_wait_group_read0();
-      }
+      // The staging tile is reused: this warpgroup's store of its previous tile must have read it and its threads must
+      // be done with their statistics reads.  Then the residual tile is fetched into it, landing while the MMAs run.
+      if (leader && mine > 0) bulk_wait_group_read0();
       named_bar_sync(1 + wg, 128);
       if (leader && p.res != nullptr) {
         fence_proxy_async();
-        mbar_arrive_expect_tx(&res_bar[wg][eb], static_cast<uint32_t>(nbox) * 64u * 128u);
+        mbar_arrive_expect_tx(&res_bar[wg], static_cast<uint32_t>(nbox) * kTileM * 128u);
         for (int b = 0; b < nbox; ++b)
-          tma_load_2d(&tmR, &res_bar[wg][eb], epi_t + b * (kTileM * 128) + wg * 64 * 128, nbase + b * 64,
-                      m_tile * kTileM + wg * 64);
+          tma_load_2d(&tmR, &res_bar[wg], epi_w + b * (kTileM * 128), nbase + b * 64, m_tile * kTileM);
       }
     }
 
-    wgmma_fence_acc(acc);
+    // ring position of this tile's first k-block: the producer filled k_iters stages for each earlier tile of the CTA
+    const int pos = local * k_iters;
+    int stage = pos % p.num_stages;
+    uint32_t phase = static_cast<uint32_t>(pos / p.num_stages) & 1u;
+    if (local > 0) mbar_wait(&turn_bar[wg], static_cast<uint32_t>((local - 1) >> 1) & 1u);
+    wgmma_fence_acc(acc[0]);
+    wgmma_fence_acc(acc[1]);
     int prev = 0;
     for (int it = 0; it < k_iters; ++it) {
       mbar_wait(&full_bar[stage], phase);
       const uint32_t a_addr = smem_u32(smem + stage * stage_bytes);
-      const uint64_t da = proto + (a_addr >> 4) + a_wg;
+      const uint64_t da = proto + (a_addr >> 4);
       const uint64_t db = proto + ((p.b_stationary ? bstat_addr + it * p.b_bytes : a_addr + p.a_bytes) >> 4);
-      wgmma_fence();
-      for (int k = 0; k < ksteps; ++k)
-        wgmma_bf16<0, 0>(acc, p.block_n, da + 2 * k, db + 2 * k, (it | k) != 0 ? 1u : 0u);
-      wgmma_commit();
+      const uint32_t scale0 = it != 0 ? 1u : 0u;
+      if (ksteps == 4) igemm_stage_mma<4>(acc, da, db, a_half, scale0);
+      else if (ksteps == 2) igemm_stage_mma<2>(acc, da, db, a_half, scale0);
+      else igemm_stage_mma<1>(acc, da, db, a_half, scale0);
       wgmma_wait<1>();                                    // the previous iteration's MMAs are done with their stage
       if (it > 0) release_stage(&empty_bar[prev], lane);
       prev = stage;
       if (++stage == p.num_stages) { stage = 0; phase ^= 1u; }
     }
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&turn_bar[wg ^ 1]);      // all MMAs of this tile are issued: the other warpgroup's turn
     wgmma_wait<0>();
-    wgmma_fence_acc(acc);
+    wgmma_fence_acc(acc[0]);
+    wgmma_fence_acc(acc[1]);
     release_stage(&empty_bar[prev], lane);
 
     if (p.tma_store) {
-      // Dense bf16 output: stage the tile in 128B-swizzled shared memory and write it with TMA (coalesced, clipped at
-      // the M tail); the residual was fetched into the same buffer.
-      if (p.res != nullptr)
-        mbar_wait(&res_bar[wg][eb], static_cast<uint32_t>((p.epi_bufs == 2 ? local >> 1 : local) & 1));
+      if constexpr (BN % 64 == 0) {
+        // Dense bf16 output: stage the tile in 128B-swizzled shared memory and write it with TMA (coalesced, clipped at
+        // the M tail); the residual was fetched into the same buffer.
+        if (p.res != nullptr) mbar_wait(&res_bar[wg], static_cast<uint32_t>(mine & 1));
 #pragma unroll
-      for (int j = 0; j < 128; j += 4) {
-        const int c = 2 * j + c_lo;
-        if (2 * j < p.block_n) {
+        for (int j = 0; j < BN / 2; j += 4) {
+          const int c = 2 * j + c_lo;
           float bias0 = 0.f, bias1 = 0.f;
           if (p.bias != nullptr) { bias0 = __ldg(p.bias + nbase + c); bias1 = __ldg(p.bias + nbase + c + 1); }
 #pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            const int row = r_lo + 8 * h;
-            uint32_t* dst = reinterpret_cast<uint32_t*>(epi_t + (c >> 6) * (kTileM * 128) + row * 128 +
-                                                        ((((c & 63) >> 3) ^ (row & 7)) << 4) + (c & 7) * 2);
-            float v0 = acc[j + 2 * h] + bias0, v1 = acc[j + 2 * h + 1] + bias1;
-            if (p.res != nullptr) {
-              const float2 t = unpack_bf16x2(*dst);
-              v0 += t.x;
-              v1 += t.y;
+          for (int mh = 0; mh < 2; ++mh)
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              const int row = mh * 64 + r_lo + 8 * h;
+              uint32_t* dst = reinterpret_cast<uint32_t*>(epi_w + (c >> 6) * (kTileM * 128) + row * 128 +
+                                                          ((((c & 63) >> 3) ^ (row & 7)) << 4) + (c & 7) * 2);
+              float v0 = acc[mh][j + 2 * h] + bias0, v1 = acc[mh][j + 2 * h + 1] + bias1;
+              if (p.res != nullptr) {
+                const float2 t = unpack_bf16x2(*dst);
+                v0 += t.x;
+                v1 += t.y;
+              }
+              *dst = pack_bf16x2(apply_act(v0, p.act), apply_act(v1, p.act));
             }
-            *dst = pack_bf16x2(apply_act(v0, p.act), apply_act(v1, p.act));
-          }
         }
-      }
-      fence_proxy_async();                             // generic-proxy smem writes -> visible to TMA
-      named_bar_sync(1 + wg, 128);
-      if (leader) {
-        for (int b = 0; b < nbox; ++b)
-          tma_store_2d(&tmC, epi_t + b * (kTileM * 128) + wg * 64 * 128, nbase + b * 64, m_tile * kTileM + wg * 64);
-        bulk_commit_group();
-      }
-      if (p.stats != nullptr) {
-        // Fused BN statistics: per-channel sum / sum of squares of the bf16-rounded outputs of this tile,
-        // read back from the staged tile (rows beyond M_total are exact zeros).  Accumulated in registers
-        // across the tiles of this CTA while it stays on the same channel block, then one fp64 atomic each.
-        if (st_ntile != n_tile) {
-          if (st_ntile >= 0) flush_stats();
-          st_ntile = n_tile;
+        fence_proxy_async();                             // generic-proxy smem writes -> visible to TMA
+        named_bar_sync(1 + wg, 128);
+        if (leader) {
+          for (int b = 0; b < nbox; ++b)
+            tma_store_2d(&tmC, epi_w + b * (kTileM * 128), nbase + b * 64, m_tile * kTileM);
+          bulk_commit_group();
         }
-        for (int u = 0; u < st_ncol; ++u) {
-          const int sc = st_col + 128 * u;
-          const uint8_t* col = epi_t + (sc >> 6) * (kTileM * 128) + (sc & 7) * 2;
-          const int j = (sc & 63) >> 3;
-          float s1 = 0.f, s2 = 0.f;
+        if constexpr (BN == 64 || BN == 128) {
+          if (p.stats != nullptr) {
+            // Fused BN statistics: per-channel sum / sum of squares of the bf16-rounded outputs of this tile, read
+            // back from the staged tile (rows beyond M_total are exact zeros).  Accumulated in registers across the
+            // warpgroup's tiles while it stays on the same channel block, then one fp64 atomic each.
+            if (st_ntile != n_tile) {
+              if (st_ntile >= 0) flush_stats();
+              st_ntile = n_tile;
+            }
+            const uint8_t* col = epi_w + (st_col >> 6) * (kTileM * 128) + (st_col & 7) * 2;
+            const int j = (st_col & 63) >> 3;
+            float s1 = 0.f, s2 = 0.f;
 #pragma unroll 8
-          for (int r = st_row0; r < st_row0 + st_rows; ++r) {
-            const float vv = __bfloat162float(*reinterpret_cast<const __nv_bfloat16*>(col + r * 128 + ((j ^ (r & 7)) << 4)));
-            s1 += vv;
-            s2 = fmaf(vv, vv, s2);
+            for (int r = st_row0; r < st_row0 + st_rows; ++r) {
+              const float vv = __bfloat162float(*reinterpret_cast<const __nv_bfloat16*>(col + r * 128 + ((j ^ (r & 7)) << 4)));
+              s1 += vv;
+              s2 = fmaf(vv, vv, s2);
+            }
+            st_s1 += s1;
+            st_s2 += s2;
           }
-          st_s1[u] += s1;
-          st_s2[u] += s2;
         }
       }
       continue;
     }
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int m = m_tile * kTileM + r_lo + 8 * h;
-      if (m >= p.M_total) continue;
-      const int img = m / IJ;
-      const int rem = m - img * IJ;
-      const int bi = rem / p.J;
-      const int bj = rem - bi * p.J;
-      const long long off = ((static_cast<long long>(img) * p.OH + (bi * p.os + p.oh0)) * p.OW + (bj * p.os + p.ow0)) *
-                            static_cast<long long>(p.ldo);
+    for (int mh = 0; mh < 2; ++mh)
 #pragma unroll
-      for (int j = 0; j < 128; j += 4)
-        if (2 * j < p.block_n) store_pair(p, acc[j + 2 * h], acc[j + 2 * h + 1], off, nbase + 2 * j + c_lo);
-    }
+      for (int h = 0; h < 2; ++h) {
+        const int m = m_tile * kTileM + mh * 64 + r_lo + 8 * h;
+        if (m >= p.M_total) continue;
+        const int img = m / IJ;
+        const int rem = m - img * IJ;
+        const int bi = rem / p.J;
+        const int bj = rem - bi * p.J;
+        const long long off = ((static_cast<long long>(img) * p.OH + (bi * p.os + p.oh0)) * p.OW + (bj * p.os + p.ow0)) *
+                              static_cast<long long>(p.ldo);
+#pragma unroll
+        for (int j = 0; j < BN / 2; j += 4) store_pair(p, acc[mh][j + 2 * h], acc[mh][j + 2 * h + 1], off, nbase + 2 * j + c_lo);
+      }
   }
-  if (p.stats != nullptr && st_ntile >= 0) flush_stats();
+  if constexpr (BN == 64 || BN == 128)
+    if (p.stats != nullptr && st_ntile >= 0) flush_stats();
   if (p.tma_store && leader) bulk_wait_group0();  // smem must outlive the last TMA store
 }
 
@@ -354,6 +381,7 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
 // wgrad: dw[k, tap, c] += sum_pix dy[pix, k] * x[pix @ tap, c]
 // A = dy tile, MN-major (rows of smem = pixels, 128/64/32B of k-channels); B = im2col(x) tile, MN-major.
 // A CTA owns 128 output channels (one k-tile) x boxes_per_cta channel boxes of x (at most 256 accumulator columns).
+constexpr int kBk = 64;   // pixels per wgrad stage: four 16-deep k-steps
 struct WgradParams {
   int M_total;          // fwd output pixels N*P*Q
   int P, Q;
@@ -382,6 +410,10 @@ __device__ __forceinline__ void red_add_v2(float* addr, float a, float b) {
   asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(addr), "f"(a), "f"(b) : "memory");
 }
 
+// NC = boxes_per_cta * ckB, the accumulator width: the last column group may hold fewer boxes (ncols < NC); its
+// missing columns are computed from whatever the stage holds and never stored.  The grid is one wave (splits fill the
+// SMs), so those CTAs take no longer than the full-width ones beside them.
+template <int NC>
 __global__ void __launch_bounds__(kThreads, 1)
 conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_constant__ CUtensorMap tmX,
                   const __grid_constant__ WgradParams p) {
@@ -422,6 +454,7 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_constan
   if (nblk <= 0) return;
 
   if (warp >= kProducerWarp) {
+    producer_setmaxnreg();
     if (warp == kProducerWarp && lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
@@ -471,6 +504,8 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_constan
     return;
   }
 
+  consumer_setmaxnreg();
+
   // ---- consumers: warpgroup wg computes output channels [k0 + 64 wg, k0 + 64 wg + 64) x all boxes of the CTA
   const int wg = warp >> 2;
   const bool wg_on = k0 + wg * 64 < p.K_out;
@@ -480,8 +515,7 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_constan
   const uint64_t protoB = make_smem_desc(0, p.boxB_bytes, 8 * p.ckB * 2, layout_type_for_row_bytes(p.ckB * 2));
   const uint32_t a_wg = (wg * (64 / p.ckA) * p.boxA_bytes) >> 4;
   const uint32_t kincA = (16u * p.ckA * 2) >> 4, kincB = (16u * p.ckB * 2) >> 4;  // 16 pixel rows per K step
-  const int ksteps = p.bk / 16;
-  float acc[128];
+  float acc[NC / 2];
   wgmma_fence_acc(acc);
   int stage = 0, prev = 0;
   uint32_t phase = 0;
@@ -491,8 +525,9 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_constan
     if (wg_on) {
       const uint64_t da = protoA + (a_addr >> 4) + a_wg, db = protoB + ((a_addr + a_tile) >> 4);
       wgmma_fence();
-      for (int k = 0; k < ksteps; ++k)
-        wgmma_bf16<1, 1>(acc, ncols, da + k * kincA, db + k * kincB, (b | k) != 0 ? 1u : 0u);
+#pragma unroll
+      for (int k = 0; k < kBk / 16; ++k)
+        wgmma_bf16<1, 1>(acc, da + k * kincA, db + k * kincB, (b | k) != 0 ? 1u : 0u);
       wgmma_commit();
       wgmma_wait<1>();
     }
@@ -515,12 +550,12 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_constan
       // split-K: plain stores of this CTA's fp32 tile; conv_wgrad_reduce_kernel sums the splits into dw
       float* dst = p.partial + ((static_cast<long long>(tile) * p.splits + split) * kTileM + (r_lo + 8 * h)) * p.pitch;
 #pragma unroll
-      for (int j = 0; j < 128; j += 4)
+      for (int j = 0; j < NC / 2; j += 4)
         if (2 * j < ncols)
           *reinterpret_cast<float2*>(dst + 2 * j + c_lo) = make_float2(acc[j + 2 * h], acc[j + 2 * h + 1]);
     } else {
 #pragma unroll
-      for (int j = 0; j < 128; j += 4) {
+      for (int j = 0; j < NC / 2; j += 4) {
         const int col = 2 * j + c_lo;
         if (col < ncols) {
           const int x = col / p.ckB;
@@ -675,6 +710,18 @@ struct IgemmLaunch {
   int window;
 };
 
+// The instantiations of a kernel templated on its tile width (16 * (I + 1) for I in Is), indexed by width.
+template <int... Is>
+static auto igemm_kernel_for(int block_n, std::integer_sequence<int, Is...>) {
+  static constexpr decltype(&conv_igemm_kernel<16>) table[] = {&conv_igemm_kernel<16 * (Is + 1)>...};
+  return table[block_n / 16 - 1];
+}
+template <int... Is>
+static auto wgrad_kernel_for(int ncols, std::integer_sequence<int, Is...>) {
+  static constexpr decltype(&conv_wgrad_kernel<16>) table[] = {&conv_wgrad_kernel<16 * (Is + 1)>...};
+  return table[ncols / 16 - 1];
+}
+
 static int launch_igemm(const IgemmLaunch& L, cudaStream_t stream) {
   B200_REQUIRE(L.SC % 8 == 0, B200_ERR_UNSUPPORTED, "igemm: source channels (%d) must be a multiple of 8", L.SC);
   B200_REQUIRE(L.ntaps >= 1 && L.ntaps <= kMaxTaps, B200_ERR_UNSUPPORTED, "igemm: %d taps unsupported", L.ntaps);
@@ -684,17 +731,24 @@ static int launch_igemm(const IgemmLaunch& L, cudaStream_t stream) {
   B200_REQUIRE(p.M_total > 0, B200_ERR_INVALID, "igemm: empty problem");
   p.I = L.I; p.J = L.J; p.trav = L.trav; p.lower_w = L.lower_w; p.lower_h = L.lower_h;
   p.N_total = L.Nout;
-  p.n_tiles = (L.Nout + 255) / 256;
-  p.block_n = (((L.Nout + p.n_tiles - 1) / p.n_tiles) + 15) / 16 * 16;
+  // n-tiles of at most 128 columns (a warpgroup's 128 x block_n tile is block_n accumulator registers per thread):
+  // 128 or 64 wide when that divides Nout, which keeps the TMA-store epilogue and computes no padding columns;
+  // otherwise the fewest equal tiles, rounded up to 16 columns
+  p.block_n = L.Nout % 128 == 0 ? 128 : (L.Nout % 64 == 0 ? 64 : 0);
+  if (p.block_n == 0) {
+    const int nt = (L.Nout + 127) / 128;
+    p.block_n = (((L.Nout + nt - 1) / nt) + 15) / 16 * 16;
+  }
+  p.n_tiles = (L.Nout + p.block_n - 1) / p.block_n;
   p.m_tiles = (p.M_total + kTileM - 1) / kTileM;
   p.ck = pick_ck(L.SC);
   p.c_chunks = (L.SC + p.ck - 1) / p.ck;
   p.window = L.window;
-  if (L.window) {   // block-diagonal: one n-tile per window, its K loop covers the window's channels only
+  if (L.window) {   // block-diagonal: one or two n-tiles per window, the K loop covers the window's channels only
     B200_REQUIRE(L.window % 64 == 0 && L.window <= 256 && L.SC == L.Nout && L.Nout % L.window == 0, B200_ERR_UNSUPPORTED,
                  "igemm: window %d needs C == K (C=%d K=%d), K %% window == 0", L.window, L.SC, L.Nout);
-    p.n_tiles = L.Nout / L.window;
-    p.block_n = L.window;
+    p.block_n = L.window <= 128 ? L.window : L.window / 2;
+    p.n_tiles = L.Nout / p.block_n;
     p.ck = 64;
     p.c_chunks = L.window / 64;
   }
@@ -708,7 +762,8 @@ static int launch_igemm(const IgemmLaunch& L, cudaStream_t stream) {
   // dense bf16 outputs with 64-channel granularity go out through shared memory + TMA store
   p.tma_store = (L.os == 1 && !L.out_fp32 && (p.block_n % 64) == 0 && (L.Nout % p.block_n) == 0 && L.ldo == L.Nout &&
                  L.OH == L.I && L.OW == L.J && L.oh0 == 0 && L.ow0 == 0) ? 1 : 0;
-  const int epi_bytes = p.tma_store ? kTileM * p.block_n * 2 : 0;
+  const int epi_bytes = p.tma_store ? kTileM * p.block_n * 2 : 0;   // per consumer warpgroup
+  const int epi_total = 2 * epi_bytes;
   // small 1x1 layers (all weight slices <= 64 KB): keep the weights resident, stream only the activations
   static const bool bstat_enabled = !(getenv("B200_IGEMM_BSTAT") && atoi(getenv("B200_IGEMM_BSTAT")) == 0);
   const int b_all = L.ntaps * p.c_chunks * (int)p.b_bytes;
@@ -723,10 +778,6 @@ static int launch_igemm(const IgemmLaunch& L, cudaStream_t stream) {
   // every CTA still gets a few m-tiles; needs >= 3 operand stages beside the resident weights and the staging tile.
   static const int own_mode = getenv("B200_IGEMM_OWN_NTILE") ? atoi(getenv("B200_IGEMM_OWN_NTILE")) : 1;
   int grid_own = 0;
-  // B200_IGEMM_SMEM_KB: operand + staging budget (default 224 KB: three 48 KB stages for 256-wide tiles beside the 64 KB
-  // staging tile; 200 KB leaves only two)
-  static const int budget_kb = getenv("B200_IGEMM_SMEM_KB") ? atoi(getenv("B200_IGEMM_SMEM_KB")) : 224;
-  int budget = (budget_kb >= 96 && budget_kb <= 224 ? budget_kb : 224) * 1024;
   if (bstat_enabled && own_mode && !p.b_stationary && p.n_tiles > 1 && p.n_tiles <= 8 && !L.window &&
       (p.a_bytes % 1024) == 0 && (p.b_bytes % 1024) == 0 && (L.Nout % p.block_n) == 0) {
     const int ctas = sm_count() / p.n_tiles;
@@ -734,29 +785,24 @@ static int launch_igemm(const IgemmLaunch& L, cudaStream_t stream) {
     const long long w_all = (long long)b_all * p.n_tiles;
     const long long rr_bytes = a_all * p.n_tiles + w_all * p.m_tiles;
     const long long own_bytes = a_all * p.n_tiles + (long long)b_all * ctas * p.n_tiles;
-    const int stages_left = (kSmemBudgetMax - epi_bytes - b_all) / (int)p.a_bytes;
+    const int stages_left = (kSmemBudgetMax - epi_total - b_all) / (int)p.a_bytes;
     if (ctas >= 1 && p.m_tiles >= 4 * ctas && stages_left >= 3 && own_bytes * 4 <= rr_bytes * 3) {
       p.b_stationary = 1;
       p.own_ntile = 1;
       bstat_bytes = b_all;
       stage = p.a_bytes;
       grid_own = ctas * p.n_tiles;
-      budget = kSmemBudgetMax;
     }
   }
-  // a second staging tile when at least three operand stages remain beside it: a tile's epilogue then never waits for
-  // the previous tile's store to drain
-  p.epi_bufs = (p.tma_store && (budget - 2 * epi_bytes - bstat_bytes) / (int)stage >= 3) ? 2 : 1;
   p.epi_bytes = (uint32_t)epi_bytes;
-  const int epi_total = epi_bytes * p.epi_bufs;
-  p.num_stages = (budget - epi_total - bstat_bytes) / (int)stage;
+  p.num_stages = (kSmemBudgetMax - epi_total - bstat_bytes) / (int)stage;
   if (p.num_stages > kMaxStages) p.num_stages = kMaxStages;
   if (p.num_stages < 2) p.num_stages = 2;
   p.OH = L.OH; p.OW = L.OW; p.os = L.os; p.oh0 = L.oh0; p.ow0 = L.ow0; p.ldo = L.ldo;
   p.act = L.act; p.out_fp32 = L.out_fp32; p.out = L.out; p.res = L.res; p.bias = L.bias;
   p.stats = L.stats;
   if (L.stats != nullptr)
-    B200_REQUIRE(p.tma_store && (256 % p.block_n) == 0 && L.res == nullptr && L.bias == nullptr && L.act == 0,
+    B200_REQUIRE(p.tma_store && (128 % p.block_n) == 0 && L.res == nullptr && L.bias == nullptr && L.act == 0,
                  B200_ERR_UNSUPPORTED, "conv_fprop: fused BN statistics need a dense bf16 output with K %% 64 == 0 "
                  "(block_n=%d) and no bias/residual/activation", p.block_n);
   for (int t = 0; t < L.ntaps; ++t) p.taps[t] = L.taps[t];
@@ -781,23 +827,26 @@ static int launch_igemm(const IgemmLaunch& L, cudaStream_t stream) {
   memset(&tmC, 0, sizeof(tmC));
   memset(&tmR, 0, sizeof(tmR));
   if (p.tma_store) {
-    rc = encode_tiled2(&tmC, L.out, L.ldo, (long long)p.M_total, 64, kTileM / 2);   // one warpgroup's 64 rows
+    rc = encode_tiled2(&tmC, L.out, L.ldo, (long long)p.M_total, 64, kTileM);
     if (rc) return rc;
     if (L.res != nullptr) {
-      rc = encode_tiled2(&tmR, L.res, L.ldo, (long long)p.M_total, 64, kTileM / 2);
+      rc = encode_tiled2(&tmR, L.res, L.ldo, (long long)p.M_total, 64, kTileM);
       if (rc) return rc;
     }
   }
   const int smem_bytes = p.num_stages * (int)stage + bstat_bytes + epi_total + 1024;
-  rc = set_smem_attr((const void*)conv_igemm_kernel, smem_bytes);
+  const auto kfn = igemm_kernel_for(p.block_n, std::make_integer_sequence<int, 8>{});
+  rc = set_smem_attr((const void*)kfn, smem_bytes);
   if (rc) return rc;
+  // With fewer tiles than SMs a CTA gets one tile and its second consumer warpgroup idles: the tiles are spread over
+  // all SMs rather than paired up on half of them.
   const int total_tiles = p.m_tiles * p.n_tiles;
   const int grid = grid_own ? grid_own : (total_tiles < sm_count() ? total_tiles : sm_count());
   if (getenv("B200_IGEMM_DEBUG"))
-    fprintf(stderr, "[igemm] M=%d C=%d N=%d taps=%d block_n=%d n_tiles=%d stages=%d bstat=%d own=%d epi_bufs=%d grid=%d smem=%d\n",
-            p.M_total, L.SC, L.Nout, L.ntaps, p.block_n, p.n_tiles, p.num_stages, p.b_stationary, p.own_ntile, p.epi_bufs,
-            grid, smem_bytes);
-  b200::launch(conv_igemm_kernel, grid, kThreads, smem_bytes, stream, tmA, tmB, tmC, tmR, p);
+    fprintf(stderr, "[igemm] M=%d C=%d N=%d taps=%d block_n=%d n_tiles=%d stages=%d bstat=%d own=%d grid=%d smem=%d\n",
+            p.M_total, L.SC, L.Nout, L.ntaps, p.block_n, p.n_tiles, p.num_stages, p.b_stationary, p.own_ntile, grid,
+            smem_bytes);
+  b200::launch(kfn, grid, kThreads, smem_bytes, stream, tmA, tmB, tmC, tmR, p);
   B200_CHECK_LAUNCH("conv_igemm_kernel");
   return B200_OK;
 }
@@ -966,7 +1015,7 @@ extern "C" int b200_conv_wgrad(const b200_conv_desc* d, const void* x, const voi
   p.window = d->window;
   p.ckA = pick_ck(d->K);
   p.ckB = pick_ck(Cw);
-  p.bk = 64;  // pixels per TMA box: fewer, larger TMA requests per byte (32-pixel boxes were request-rate bound)
+  p.bk = kBk;  // pixels per TMA box: fewer, larger TMA requests per byte (32-pixel boxes were request-rate bound)
   p.c_chunks = (Cw + p.ckB - 1) / p.ckB;
   p.total_boxes = p.taps_total * p.c_chunks;
   p.k_tiles = (d->K + kTileM - 1) / kTileM;
@@ -1026,10 +1075,11 @@ extern "C" int b200_conv_wgrad(const b200_conv_desc* d, const void* x, const voi
                        d->stride, d->x_pixel_stride, d->x_row_stride, d->x_image_stride);
   if (rc) return rc;
   const int smem_bytes = p.num_stages * (int)p.stage_bytes + 1024;
-  rc = set_smem_attr((const void*)conv_wgrad_kernel, smem_bytes);
+  const auto kfn = wgrad_kernel_for(p.pitch, std::make_integer_sequence<int, 16>{});
+  rc = set_smem_attr((const void*)kfn, smem_bytes);
   if (rc) return rc;
   const int grid = tiles * p.splits;
-  b200::launch(conv_wgrad_kernel, grid, kThreads, smem_bytes, stream, tmDy, tmX, p);
+  b200::launch(kfn, grid, kThreads, smem_bytes, stream, tmDy, tmX, p);
   B200_CHECK_LAUNCH("conv_wgrad_kernel");
   if (p.partial != nullptr) {
     const long long total = static_cast<long long>(d->K) * p.taps_total * (Cw / 4);

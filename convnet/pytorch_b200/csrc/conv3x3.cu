@@ -85,6 +85,7 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant_
   const int own_n = static_cast<int>(blockIdx.x) % p.n_tiles;
 
   if (warp >= 8) {
+    producer_setmaxnreg();
     if (warp == 8 && lane == 0) {
       int ia = 0, ib = 0; uint32_t pa = 0, pb = 0;
       const int cw = p.row_bytes >> 1;   // channels per chunk
@@ -117,6 +118,7 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant_
     }
     return;
   }
+  consumer_setmaxnreg();
 
   // ---- consumers: warpgroup wg computes accumulator rows (virtual pixels) [64 wg, 64 wg + 64) of every tile
   const int wg = warp >> 2;
@@ -184,7 +186,7 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant_
         wgmma_fence();
 #pragma unroll
         for (int k = 0; k < KSTEPS; ++k)
-          wgmma_bf16<0, 0>(acc, BN, da0 + tap_inc + 2 * k, db0 + 2 * k, (cc | t | k) != 0 ? 1u : 0u);
+          wgmma_bf16<0, 0>(acc, da0 + tap_inc + 2 * k, db0 + 2 * k, (cc | t | k) != 0 ? 1u : 0u);
         if (!p.b_stationary || t == NTAPS - 1) {
           wgmma_commit();
           wgmma_wait<1>();
@@ -489,6 +491,7 @@ conv_halo_wgrad_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_co
   if (ntiles <= 0) return;
 
   if (warp >= 8) {
+    producer_setmaxnreg();
     if (warp == 8 && lane == 0) {
       int stage = 0; uint32_t phase = 0;
       const uint32_t tx = nA * p.a_box_bytes + p.x_box_bytes;
@@ -505,6 +508,7 @@ conv_halo_wgrad_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_co
     }
     return;
   }
+  consumer_setmaxnreg();
 
   const int wg = warp >> 2;
   const bool wg_on = wg < nA;
@@ -531,7 +535,7 @@ conv_halo_wgrad_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_co
         const uint32_t scale = (k != 0 || i != 0) ? 1u : 0u;
 #pragma unroll
         for (int r = 0; r < R; ++r)
-          wgmma_bf16<1, 1>(acc[r], kCols, da0 + k * 128, dx0 + row_inc[r] + k * kx_inc, scale);
+          wgmma_bf16<1, 1>(acc[r], da0 + k * 128, dx0 + row_inc[r] + k * kx_inc, scale);
       }
       wgmma_commit();
       wgmma_wait<1>();

@@ -108,7 +108,9 @@ def make_desc(N, H, W, C, K, R, S, stride, pad, P=None, Q=None, x_strides=(0, 0,
 
 # ------------------------------------------------------------------------------------ convolution
 def can_fuse_bn_stats(K):
-    """b200_conv_fprop can accumulate BN statistics in its epilogue when the output tile is 64/128/256 wide."""
+    """b200_conv_fprop can accumulate BN statistics in its epilogue for this K on every path it may take.  The halo
+    kernel (3x3 stride 1, conv3x3.cu) splits K into equal 64/128/256-wide tiles and is the stricter of the two; the
+    implicit-GEMM kernel (conv.cu) accepts any K % 64 == 0."""
     n_tiles = (K + 255) // 256
     block_n = ((K + n_tiles - 1) // n_tiles + 15) // 16 * 16
     return K % 64 == 0 and K % block_n == 0 and 256 % block_n == 0
