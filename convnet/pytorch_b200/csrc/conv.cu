@@ -842,10 +842,17 @@ static int launch_igemm(const IgemmLaunch& L, cudaStream_t stream) {
   // all SMs rather than paired up on half of them.
   const int total_tiles = p.m_tiles * p.n_tiles;
   const int grid = grid_own ? grid_own : (total_tiles < sm_count() ? total_tiles : sm_count());
-  if (getenv("B200_IGEMM_DEBUG"))
-    fprintf(stderr, "[igemm] M=%d C=%d N=%d taps=%d block_n=%d n_tiles=%d stages=%d bstat=%d own=%d grid=%d smem=%d\n",
-            p.M_total, L.SC, L.Nout, L.ntaps, p.block_n, p.n_tiles, p.num_stages, p.b_stationary, p.own_ntile, grid,
-            smem_bytes);
+  if (getenv("B200_IGEMM_DEBUG")) {
+    // max_tiles: tiles of the busiest CTA (its warpgroups take them alternately, so >= 2 means warpgroup 1 computes)
+    const int max_tiles = p.own_ntile ? (p.m_tiles + grid / p.n_tiles - 1) / (grid / p.n_tiles)
+                                      : (total_tiles + grid - 1) / grid;
+    fprintf(stderr, "[igemm] M=%d C=%d N=%d taps=%d os=%d block_n=%d n_tiles=%d m_tiles=%d ck=%d k_iters=%d stages=%d "
+            "tma_store=%d plain_a=%d bstat=%d own=%d out_fp32=%d bias=%d res=%d act=%d stats=%d grid=%d max_tiles=%d "
+            "smem=%d\n",
+            p.M_total, L.SC, L.Nout, L.ntaps, L.os, p.block_n, p.n_tiles, p.m_tiles, p.ck, L.ntaps * p.c_chunks,
+            p.num_stages, p.tma_store, p.plain_a, p.b_stationary, p.own_ntile, p.out_fp32, L.bias != nullptr,
+            L.res != nullptr, p.act, L.stats != nullptr, grid, max_tiles, smem_bytes);
+  }
   b200::launch(kfn, grid, kThreads, smem_bytes, stream, tmA, tmB, tmC, tmR, p);
   B200_CHECK_LAUNCH("conv_igemm_kernel");
   return B200_OK;
@@ -1056,11 +1063,6 @@ extern "C" int b200_conv_wgrad(const b200_conv_desc* d, const void* x, const voi
     p.partial = static_cast<float*>(workspace);
   }
   p.S_filter = d->S;
-  if (getenv("B200_WGRAD_DEBUG"))
-    fprintf(stderr, "wgrad cfg: K=%d C=%d taps=%d ckA=%d ckB=%d kt=%d bpc=%d k_groups=%d col_groups=%d splits=%d bps=%d "
-            "stages=%d stage=%u pitch=%d partial=%d\n", d->K, d->C, p.taps_total, p.ckA, p.ckB, p.kt, p.boxes_per_cta,
-            p.k_groups, p.col_groups, p.splits, p.blocks_per_split, p.num_stages, p.stage_bytes, p.pitch,
-            p.partial != nullptr);
   CUtensorMap tmDy, tmX;
   rc = encode_tiled2(&tmDy, dy, d->K, (long long)p.M_total, p.ckA, p.bk);
   if (rc) return rc;
@@ -1068,6 +1070,12 @@ extern "C" int b200_conv_wgrad(const b200_conv_desc* d, const void* x, const voi
   const int upper_h = p.lower_h + (d->P - 1) * d->stride + 1 - d->H;
   p.plain_x = (d->R == 1 && d->S == 1 && d->stride == 1 && d->pad_h == 0 && d->pad_w == 0 && d->P == d->H &&
                d->Q == d->W && d->x_pixel_stride == 0) ? 1 : 0;
+  if (getenv("B200_WGRAD_DEBUG"))
+    fprintf(stderr, "[wgrad] K=%d C=%d taps=%d stride=%d ckA=%d ckB=%d kt=%d bpc=%d k_groups=%d col_groups=%d splits=%d "
+            "bps=%d stages=%d stage=%u nc=%d nboxes_last=%d plain_x=%d partial=%d\n", d->K, d->C, p.taps_total,
+            d->stride, p.ckA, p.ckB, p.kt, p.boxes_per_cta, p.k_groups, p.col_groups, p.splits, p.blocks_per_split,
+            p.num_stages, p.stage_bytes, p.pitch, p.total_boxes - (p.col_groups - 1) * p.boxes_per_cta, p.plain_x,
+            p.partial != nullptr);
   if (p.plain_x)
     rc = encode_tiled2(&tmX, x, d->C, (long long)p.M_total, p.ckB, p.bk);
   else

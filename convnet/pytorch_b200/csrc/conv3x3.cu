@@ -412,6 +412,11 @@ int launch_halo(const void* src, const void* wmat, void* out, const void* res, c
     if (per_n < 1) per_n = 1;
     grid = per_n * p.n_tiles;
   }
+  if (getenv("B200_HALO_DEBUG"))
+    fprintf(stderr, "[halo] dir=%d N=%d H=%d W=%d C=%d K=%d taps=%d block_n=%d n_tiles=%d m_tiles=%d bstat=%d diag=%d "
+            "sa=%d sb=%d bias=%d res=%d act=%d stats=%d grid=%d\n", dir, N, H, W, Cs, Nout, p.ntaps, p.block_n,
+            p.n_tiles, p.m_tiles, p.b_stationary, p.diag, p.sa, p.sb, bias != nullptr, res != nullptr, act,
+            stats != nullptr, grid);
   b200::launch(kfn, grid, kHThreads, smem_bytes, stream, tmX, tmB, tmC, tmR, p);
   B200_CHECK_LAUNCH("conv_halo_kernel");
   return B200_OK;
@@ -668,6 +673,10 @@ int launch_halo_wgrad(const void* x, const void* dy, float* dw, void* workspace,
   cudaError_t e = cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes);
   B200_REQUIRE(e == cudaSuccess, B200_ERR_CUDA, "conv halo wgrad: smem attribute (%d bytes): %s", smem_bytes,
                cudaGetErrorString(e));
+  if (getenv("B200_HALO_DEBUG"))
+    fprintf(stderr, "[halo_wgrad] N=%d H=%d W=%d C=%d K=%d taps=%d k_tiles=%d c_chunks=%d m_tiles=%d units=%d "
+            "splits=%d tiles_per_split=%d stages=%d grid=%d\n", N, H, W, C, K_out, p.ntaps, p.k_tiles, p.c_chunks,
+            p.m_tiles, p.units, p.splits, p.tiles_per_split, p.stages, p.units * p.splits);
   if (p.ntaps == 9)
     b200::launch(conv_halo_wgrad_kernel<3, 3>, p.units * p.splits, kWThreads, smem_bytes, stream, tmDy, tmX, p);
   else

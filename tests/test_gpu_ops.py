@@ -442,6 +442,9 @@ _CONV_CASE_NAMES = [
     'halo_8_256', 'halo_stem', 'halo_stem_67',
     # owned-n-tile (weight-stationary) walk of the igemm kernel
     'own_256_1024', 'own_1024_256', 'own_128_512_res',
+    # small and ragged shapes of the diagnostic table (the 16-channel ones are in test_gpu_conv_sweep.py)
+    'p1_64_64_m128', 'p1_128_256', 'p1_256_64_odd', 'c3_64_64', 'c3s2_64_128', 'c3_32_32', 'p1_512_2048_7',
+    'p1_256_128_ragged', 'p1_512_512_res', 'p1_256_1024_14',
 ]
 
 
