@@ -1,7 +1,7 @@
 // Fused softmax cross-entropy forward + backward (one block per sample) and the bias-gradient column
 // sum.  Replaces utils/cross_entropy.py:14-67 of the reference: F.cross_entropy when smooth_eps == 0
 // (:20-24) and the label-smoothing formula loss = -((1-eps-eps/C)*lsm[target] + (eps/C)*sum(lsm)) (:48-52),
-// reduction='mean'.
+// reduction='mean'; and the soft-target loss of MixUp / CutMix (utils/mixup.py:37-45 with :53-54 of cross_entropy.py).
 #include "common.cuh"
 #include "host.h"
 #include <math_constants.h>
@@ -25,12 +25,17 @@ __device__ __forceinline__ float block_reduce(float v, bool is_max, float* sh) {
   return r;
 }
 
+// MIX: soft target q = lam*onehot(t) + (1-lam)*onehot(t2) with t2 = target[perm[b]] (MixUp / CutMix); eps is 0 then.
+// A template parameter, so that the plain instantiation keeps its code.
+template <bool MIX>
 __global__ void __launch_bounds__(kCeThreads) softmax_ce_kernel(const float* __restrict__ logits,
                                                                 const long long* __restrict__ target, int B,
                                                                 int classes, int ld, float eps, float grad_scale,
                                                                 const float* __restrict__ grad_scale_dev,
                                                                 float* __restrict__ row_loss,
-                                                                __nv_bfloat16* __restrict__ dlogits) {
+                                                                __nv_bfloat16* __restrict__ dlogits,
+                                                                const long long* __restrict__ perm,
+                                                                const float* __restrict__ lam_dev) {
   pdl_wait();
   // row_loss layout: [0, B) per-sample loss, [B, 2B) number of classes scoring strictly above the target class
   // (rank of the target: top-1 <=> 0, top-5 <=> < 5 -- utils/meters.py:59-72 of the reference, ties aside)
@@ -52,6 +57,8 @@ __global__ void __launch_bounds__(kCeThreads) softmax_ce_kernel(const float* __r
   const int t = (int)target[b];
   const float eps_sum = eps / (float)classes;
   const float eps_nll = 1.f - eps_sum - eps;
+  const int t2 = MIX ? (int)target[perm[b]] : t;
+  const float lam = MIX ? __ldg(lam_dev) : 1.f, oml = 1.f - lam;
   if (row_loss != nullptr) {
     const float xt = row[t];
     float above = 0.f;
@@ -59,17 +66,24 @@ __global__ void __launch_bounds__(kCeThreads) softmax_ce_kernel(const float* __r
     above = block_reduce(above, false, sh);
     if (threadIdx.x == 0) {
       // sum_c lsm[c] = sx - classes*lse
-      row_loss[b] = -(eps_nll * (xt - lse) + eps_sum * (sx - (float)classes * lse));
+      if (MIX)
+        row_loss[b] = -(lam * (xt - lse) + oml * (row[t2] - lse));
+      else
+        row_loss[b] = -(eps_nll * (xt - lse) + eps_sum * (sx - (float)classes * lse));
       row_loss[B + b] = above;
     }
   }
   if (dlogits != nullptr) {
     const float gs = grad_scale * (grad_scale_dev != nullptr ? __ldg(grad_scale_dev) : 1.f) / (float)B;
     // d/dx_c of li: (eps_nll + classes*eps_sum) * softmax_c - eps_nll*[c==t] - eps_sum
-    const float wsm = eps_nll + (float)classes * eps_sum;
+    const float wsm = MIX ? lam + oml : eps_nll + (float)classes * eps_sum;
     for (int c = threadIdx.x; c < classes; c += kCeThreads) {
       const float sm = expf(row[c] - lse);
-      float g = wsm * sm - eps_sum - (c == t ? eps_nll : 0.f);
+      float g;
+      if (MIX)
+        g = wsm * sm - (c == t ? lam : 0.f) - (c == t2 ? oml : 0.f);
+      else
+        g = wsm * sm - eps_sum - (c == t ? eps_nll : 0.f);
       dlogits[(long long)b * ld + c] = __float2bfloat16(g * gs);
     }
     for (int c = classes + threadIdx.x; c < ld; c += kCeThreads) dlogits[(long long)b * ld + c] = __float2bfloat16(0.f);
@@ -121,8 +135,28 @@ extern "C" int b200_softmax_ce(const float* logits, const long long* target, int
   B200_REQUIRE((loss == nullptr) == (row_loss == nullptr), B200_ERR_INVALID,
                "softmax_ce: loss and row_loss must be given together");
   B200_REQUIRE(loss != nullptr || dlogits_bf16 != nullptr, B200_ERR_INVALID, "softmax_ce: nothing to compute");
-  b200::launch(softmax_ce_kernel, B, kCeThreads, 0, (cudaStream_t)stream, logits, target, B, classes, ld, smooth_eps, grad_scale,
-                                                              grad_scale_dev, row_loss, (__nv_bfloat16*)dlogits_bf16);
+  b200::launch(softmax_ce_kernel<false>, B, kCeThreads, 0, (cudaStream_t)stream, logits, target, B, classes, ld, smooth_eps,
+               grad_scale, grad_scale_dev, row_loss, (__nv_bfloat16*)dlogits_bf16, (const long long*)nullptr,
+               (const float*)nullptr);
+  B200_CHECK_LAUNCH("softmax_ce_kernel");
+  if (loss != nullptr) {
+    b200::launch(ce_mean_kernel, 1, kCeThreads, 0, (cudaStream_t)stream, row_loss, B, loss);
+    B200_CHECK_LAUNCH("ce_mean_kernel");
+  }
+  return B200_OK;
+}
+
+extern "C" int b200_softmax_ce_mix(const float* logits, const long long* target, const long long* perm,
+                                   const float* lam_dev, int B, int classes, int ld, float grad_scale,
+                                   const float* grad_scale_dev, float* loss, float* row_loss, void* dlogits_bf16,
+                                   b200_stream_t stream) {
+  B200_REQUIRE(logits && target && perm && lam_dev && B > 0 && classes > 0 && ld >= classes, B200_ERR_INVALID,
+               "softmax_ce_mix: bad argument");
+  B200_REQUIRE((loss == nullptr) == (row_loss == nullptr), B200_ERR_INVALID,
+               "softmax_ce_mix: loss and row_loss must be given together");
+  B200_REQUIRE(loss != nullptr || dlogits_bf16 != nullptr, B200_ERR_INVALID, "softmax_ce_mix: nothing to compute");
+  b200::launch(softmax_ce_kernel<true>, B, kCeThreads, 0, (cudaStream_t)stream, logits, target, B, classes, ld, 0.f,
+               grad_scale, grad_scale_dev, row_loss, (__nv_bfloat16*)dlogits_bf16, perm, lam_dev);
   B200_CHECK_LAUNCH("softmax_ce_kernel");
   if (loss != nullptr) {
     b200::launch(ce_mean_kernel, 1, kCeThreads, 0, (cudaStream_t)stream, row_loss, B, loss);

@@ -8,9 +8,38 @@
 
 namespace b200 {
 
+// Optional input mixing (MixUp / CutMix of the reference's utils/mixup.py:19-26,57-90, applied at trainer.py:119-135).
+// MIX is a template parameter so that the plain instantiation compiles to exactly the code it had without mixing.
+//   MIX == 1 (MixUp):  v = lambda * x[n] + (1 - lambda) * x[perm[n]], two fp32 products and one fp32 sum (no FMA
+//                      contraction: the reference's torch expression, bit for bit), then the single bf16 rounding.
+//   MIX == 2 (CutMix): pixel (r, c) of sample n comes from sample perm[n] inside the box [r0, r1) x [c0, c1), else
+//                      from n; in the space-to-depth layouts every one of the four sub-pixels decides on its own.
+// The parameter block lives in device memory so that a captured CUDA graph reads each step's values.
+constexpr int kMixNone = 0, kMixUp = 1, kMixCut = 2;
+
+template <int MIX>
+__device__ __forceinline__ float mix_pick(float a, float b, float lam) {
+  return MIX == kMixUp ? __fadd_rn(__fmul_rn(lam, a), __fmul_rn(__fsub_rn(1.f, lam), b)) : a;
+}
+
+__device__ __forceinline__ bool in_box(const b200_mix_params& p, int r, int c) {
+  return r >= p.r0 && r < p.r1 && c >= p.c0 && c < p.c1;
+}
+
+// source image of the element at pixel (r, c): x[n], or x[perm[n]] where CutMix pastes its box
+template <int MIX, typename T>
+__device__ __forceinline__ const T* mix_src(const T* xi, const T* xm, const b200_mix_params& p, int r, int c) {
+  return (MIX == kMixCut && in_box(p, r, c)) ? xm : xi;
+}
+
+template <int MIX>
 __global__ void __launch_bounds__(256) input_prep_kernel(const float* __restrict__ x, int N, int C, int H, int W,
-                                                         int Cpad, int mode, __nv_bfloat16* __restrict__ out) {
+                                                         int Cpad, int mode, __nv_bfloat16* __restrict__ out,
+                                                         const long long* __restrict__ perm,
+                                                         const b200_mix_params* __restrict__ mixp) {
   pdl_wait();
+  b200_mix_params mp = {};
+  if (MIX != kMixNone) mp = *mixp;
   // one thread per output pixel; Cpad is a multiple of 8
   const int brd = mode == 2 ? 2 : 0;                       // low border of the padded space-to-depth layout
   const int OH = mode == 0 ? H : H / 2 + (mode == 2 ? 3 : 0), OW = mode == 0 ? W : W / 2 + (mode == 2 ? 3 : 0);
@@ -24,6 +53,7 @@ __global__ void __launch_bounds__(256) input_prep_kernel(const float* __restrict
     __nv_bfloat16* o = out + idx * Cpad;
     const bool inside = mode != 2 || (i >= 0 && j >= 0 && i < H / 2 && j < W / 2);
     const float* xi = x + (long long)n * C * plane;
+    const float* xm = MIX != kMixNone ? x + __ldg(perm + n) * C * plane : xi;
     for (int c0 = 0; c0 < Cpad; c0 += 8) {
       float f[8];
 #pragma unroll
@@ -31,12 +61,26 @@ __global__ void __launch_bounds__(256) input_prep_kernel(const float* __restrict
         const int ch = c0 + e;
         float val = 0.f;
         if (mode == 0) {
-          if (ch < C) val = __ldg(xi + (long long)ch * plane + (long long)i * W + j);
+          if (ch < C) {
+            if (MIX == kMixNone) {
+              val = __ldg(xi + (long long)ch * plane + (long long)i * W + j);
+            } else {
+              const long long off = (long long)ch * plane + (long long)i * W + j;
+              val = __ldg(mix_src<MIX>(xi, xm, mp, i, j) + off);
+              if (MIX == kMixUp) val = mix_pick<MIX>(val, __ldg(xm + off), mp.lam);
+            }
+          }
         } else {
           const int sub = ch / C, c = ch - sub * C;  // sub = dy*2+dx
           if (sub < 4 && inside) {
             const int dy = sub >> 1, dx = sub & 1;
-            val = __ldg(xi + (long long)c * plane + (long long)(2 * i + dy) * W + (2 * j + dx));
+            if (MIX == kMixNone) {
+              val = __ldg(xi + (long long)c * plane + (long long)(2 * i + dy) * W + (2 * j + dx));
+            } else {
+              const long long off = (long long)c * plane + (long long)(2 * i + dy) * W + (2 * j + dx);
+              val = __ldg(mix_src<MIX>(xi, xm, mp, 2 * i + dy, 2 * j + dx) + off);
+              if (MIX == kMixUp) val = mix_pick<MIX>(val, __ldg(xm + off), mp.lam);
+            }
           }
         }
         f[e] = val;
@@ -53,10 +97,15 @@ __global__ void __launch_bounds__(256) input_prep_kernel(const float* __restrict
 // value = u8 * scale[c] + bias[c]  (scale = 1 / (255 * std), bias = -mean / std: ToTensor + Normalize of the reference's
 // preprocess.py:20-24).  4x fewer host->device bytes than the fp32 NCHW batch and no separate normalisation pass.
 struct U8Norm { float scale[4], bias[4]; };
+template <int MIX>
 __global__ void __launch_bounds__(256) input_prep_u8_kernel(const uint8_t* __restrict__ x, int N, int C, int H, int W,
                                                             int Cpad, int mode, U8Norm nm,
-                                                            __nv_bfloat16* __restrict__ out) {
+                                                            __nv_bfloat16* __restrict__ out,
+                                                            const long long* __restrict__ perm,
+                                                            const b200_mix_params* __restrict__ mixp) {
   pdl_wait();
+  b200_mix_params mp = {};
+  if (MIX != kMixNone) mp = *mixp;
   const int brd = mode == 2 ? 2 : 0;
   const int OH = mode == 0 ? H : H / 2 + (mode == 2 ? 3 : 0), OW = mode == 0 ? W : W / 2 + (mode == 2 ? 3 : 0);
   const long long total = (long long)N * OH * OW;
@@ -68,19 +117,37 @@ __global__ void __launch_bounds__(256) input_prep_u8_kernel(const uint8_t* __res
     __nv_bfloat16* o = out + idx * Cpad;
     const bool inside = mode != 2 || (i >= 0 && j >= 0 && i < H / 2 && j < W / 2);
     const uint8_t* xi = x + (long long)n * H * W * C;
+    const uint8_t* xm = MIX != kMixNone ? x + __ldg(perm + n) * H * W * C : xi;
     for (int c0 = 0; c0 < Cpad; c0 += 8) {
       float f[8];
 #pragma unroll
       for (int e = 0; e < 8; ++e) {
         const int ch = c0 + e;
         float val = 0.f;
+        // each source is normalised on its own (the fp32 batch the reference mixes), then mixed
         if (mode == 0) {
-          if (ch < C) val = fmaf((float)__ldg(xi + ((long long)i * W + j) * C + ch), nm.scale[ch], nm.bias[ch]);
+          if (ch < C) {
+            if (MIX == kMixNone) {
+              val = fmaf((float)__ldg(xi + ((long long)i * W + j) * C + ch), nm.scale[ch], nm.bias[ch]);
+            } else {
+              const long long off = ((long long)i * W + j) * C + ch;
+              val = fmaf((float)__ldg(mix_src<MIX>(xi, xm, mp, i, j) + off), nm.scale[ch], nm.bias[ch]);
+              if (MIX == kMixUp)
+                val = mix_pick<MIX>(val, fmaf((float)__ldg(xm + off), nm.scale[ch], nm.bias[ch]), mp.lam);
+            }
+          }
         } else {
           const int sub = ch / C, c = ch - sub * C;  // sub = dy*2+dx
           if (sub < 4 && inside) {
             const int dy = sub >> 1, dx = sub & 1;
-            val = fmaf((float)__ldg(xi + ((long long)(2 * i + dy) * W + (2 * j + dx)) * C + c), nm.scale[c], nm.bias[c]);
+            if (MIX == kMixNone) {
+              val = fmaf((float)__ldg(xi + ((long long)(2 * i + dy) * W + (2 * j + dx)) * C + c), nm.scale[c], nm.bias[c]);
+            } else {
+              const long long off = ((long long)(2 * i + dy) * W + (2 * j + dx)) * C + c;
+              val = fmaf((float)__ldg(mix_src<MIX>(xi, xm, mp, 2 * i + dy, 2 * j + dx) + off), nm.scale[c], nm.bias[c]);
+              if (MIX == kMixUp)
+                val = mix_pick<MIX>(val, fmaf((float)__ldg(xm + off), nm.scale[c], nm.bias[c]), mp.lam);
+            }
           }
         }
         f[e] = val;
@@ -210,8 +277,8 @@ static inline int grid_cap(long long total, int threads) {
 
 using namespace b200;
 
-extern "C" int b200_input_prep(const float* x, int N, int C, int H, int W, int Cpad, int mode, void* out,
-                               b200_stream_t stream) {
+static int input_prep_impl(const float* x, int N, int C, int H, int W, int Cpad, int mode, const long long* perm,
+                           const b200_mix_params* params, int kind, void* out, b200_stream_t stream) {
   B200_REQUIRE(x && out && N > 0 && C > 0 && H > 0 && W > 0, B200_ERR_INVALID, "input_prep: bad argument");
   B200_REQUIRE(Cpad % 8 == 0, B200_ERR_UNSUPPORTED, "input_prep: Cpad=%d must be a multiple of 8", Cpad);
   if (mode == 0) {
@@ -222,15 +289,26 @@ extern "C" int b200_input_prep(const float* x, int N, int C, int H, int W, int C
   } else {
     B200_REQUIRE(false, B200_ERR_INVALID, "input_prep: unknown mode %d", mode);
   }
+  B200_REQUIRE(kind >= B200_MIX_NONE && kind <= B200_MIX_CUTMIX, B200_ERR_INVALID, "input_prep: unknown mix kind %d", kind);
+  B200_REQUIRE(kind == B200_MIX_NONE || (perm && params), B200_ERR_INVALID, "input_prep: mixing needs perm and params");
   const long long total = (long long)N * (mode == 0 ? (long long)H * W : (long long)(H / 2 + (mode == 2 ? 3 : 0)) * (W / 2 + (mode == 2 ? 3 : 0)));
-  b200::launch(input_prep_kernel, grid_cap(total, 256), 256, 0, (cudaStream_t)stream, x, N, C, H, W, Cpad, mode,
-                                                                          (__nv_bfloat16*)out);
+  const int grid = grid_cap(total, 256);
+  if (kind == B200_MIX_MIXUP)
+    b200::launch(input_prep_kernel<kMixUp>, grid, 256, 0, (cudaStream_t)stream, x, N, C, H, W, Cpad, mode,
+                 (__nv_bfloat16*)out, perm, params);
+  else if (kind == B200_MIX_CUTMIX)
+    b200::launch(input_prep_kernel<kMixCut>, grid, 256, 0, (cudaStream_t)stream, x, N, C, H, W, Cpad, mode,
+                 (__nv_bfloat16*)out, perm, params);
+  else
+    b200::launch(input_prep_kernel<kMixNone>, grid, 256, 0, (cudaStream_t)stream, x, N, C, H, W, Cpad, mode,
+                 (__nv_bfloat16*)out, (const long long*)nullptr, (const b200_mix_params*)nullptr);
   B200_CHECK_LAUNCH("input_prep_kernel");
   return B200_OK;
 }
 
-extern "C" int b200_input_prep_u8(const uint8_t* x_nhwc, int N, int C, int H, int W, int Cpad, int mode,
-                                  const float* scale_host, const float* bias_host, void* out, b200_stream_t stream) {
+static int input_prep_u8_impl(const uint8_t* x_nhwc, int N, int C, int H, int W, int Cpad, int mode,
+                              const float* scale_host, const float* bias_host, const long long* perm,
+                              const b200_mix_params* params, int kind, void* out, b200_stream_t stream) {
   B200_REQUIRE(x_nhwc && out && scale_host && bias_host && N > 0 && C > 0 && C <= 4 && H > 0 && W > 0,
                B200_ERR_INVALID, "input_prep_u8: bad argument (C must be 1..4)");
   B200_REQUIRE(Cpad % 8 == 0 && Cpad >= C, B200_ERR_INVALID, "input_prep_u8: Cpad must be a multiple of 8 and >= C");
@@ -238,6 +316,9 @@ extern "C" int b200_input_prep_u8(const uint8_t* x_nhwc, int N, int C, int H, in
   if (mode != 0)
     B200_REQUIRE(H % 2 == 0 && W % 2 == 0 && 4 * C <= Cpad, B200_ERR_UNSUPPORTED,
                  "input_prep_u8: space-to-depth needs even H, W and 4*C <= Cpad");
+  B200_REQUIRE(kind >= B200_MIX_NONE && kind <= B200_MIX_CUTMIX, B200_ERR_INVALID, "input_prep_u8: unknown mix kind %d",
+               kind);
+  B200_REQUIRE(kind == B200_MIX_NONE || (perm && params), B200_ERR_INVALID, "input_prep_u8: mixing needs perm and params");
   U8Norm nm;
   for (int c = 0; c < 4; ++c) { nm.scale[c] = c < C ? scale_host[c] : 0.f; nm.bias[c] = c < C ? bias_host[c] : 0.f; }
   const int OH = mode == 0 ? H : H / 2 + (mode == 2 ? 3 : 0), OW = mode == 0 ? W : W / 2 + (mode == 2 ? 3 : 0);
@@ -245,10 +326,39 @@ extern "C" int b200_input_prep_u8(const uint8_t* x_nhwc, int N, int C, int H, in
   long long blocks = (total + 255) / 256;
   const long long cap = (long long)sm_count() * 16;
   if (blocks > cap) blocks = cap;
-  b200::launch(input_prep_u8_kernel, (int)blocks, 256, 0, (cudaStream_t)stream, x_nhwc, N, C, H, W, Cpad, mode, nm,
-                                                                       (__nv_bfloat16*)out);
+  if (kind == B200_MIX_MIXUP)
+    b200::launch(input_prep_u8_kernel<kMixUp>, (int)blocks, 256, 0, (cudaStream_t)stream, x_nhwc, N, C, H, W, Cpad,
+                 mode, nm, (__nv_bfloat16*)out, perm, params);
+  else if (kind == B200_MIX_CUTMIX)
+    b200::launch(input_prep_u8_kernel<kMixCut>, (int)blocks, 256, 0, (cudaStream_t)stream, x_nhwc, N, C, H, W, Cpad,
+                 mode, nm, (__nv_bfloat16*)out, perm, params);
+  else
+    b200::launch(input_prep_u8_kernel<kMixNone>, (int)blocks, 256, 0, (cudaStream_t)stream, x_nhwc, N, C, H, W, Cpad,
+                 mode, nm, (__nv_bfloat16*)out, (const long long*)nullptr, (const b200_mix_params*)nullptr);
   B200_CHECK_LAUNCH("input_prep_u8_kernel");
   return B200_OK;
+}
+
+extern "C" int b200_input_prep(const float* x, int N, int C, int H, int W, int Cpad, int mode, void* out,
+                               b200_stream_t stream) {
+  return input_prep_impl(x, N, C, H, W, Cpad, mode, nullptr, nullptr, B200_MIX_NONE, out, stream);
+}
+
+extern "C" int b200_input_prep_mix(const float* x, int N, int C, int H, int W, int Cpad, int mode, const long long* perm,
+                                   const b200_mix_params* params, int kind, void* out, b200_stream_t stream) {
+  return input_prep_impl(x, N, C, H, W, Cpad, mode, perm, params, kind, out, stream);
+}
+
+extern "C" int b200_input_prep_u8(const uint8_t* x_nhwc, int N, int C, int H, int W, int Cpad, int mode,
+                                  const float* scale_host, const float* bias_host, void* out, b200_stream_t stream) {
+  return input_prep_u8_impl(x_nhwc, N, C, H, W, Cpad, mode, scale_host, bias_host, nullptr, nullptr, B200_MIX_NONE, out,
+                            stream);
+}
+
+extern "C" int b200_input_prep_u8_mix(const uint8_t* x_nhwc, int N, int C, int H, int W, int Cpad, int mode,
+                                      const float* scale_host, const float* bias_host, const long long* perm,
+                                      const b200_mix_params* params, int kind, void* out, b200_stream_t stream) {
+  return input_prep_u8_impl(x_nhwc, N, C, H, W, Cpad, mode, scale_host, bias_host, perm, params, kind, out, stream);
 }
 
 extern "C" int b200_weight_transpose(const void* src, void* dst, int K, int T, int C, b200_stream_t stream) {

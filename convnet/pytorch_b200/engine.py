@@ -332,17 +332,19 @@ class Runtime(object):
     input_mean = (0.485, 0.456, 0.406)
     input_std = (0.229, 0.224, 0.225)
 
-    def _input(self, x):
-        """-> (tensor, relayout function, (N, C, H, W))"""
+    def _input(self, x, mix=None):
+        """-> (tensor, relayout function, (N, C, H, W)).  ``mix`` (ops.Mix): MixUp / CutMix applied by the relayout
+        kernel itself (the reference mixes the fp32 batch before the forward pass, trainer.py:119-135)."""
         if x.dtype == torch.uint8:
             if x.dim() != 4 or x.shape[-1] > 4:
                 raise B200Error('uint8 network inputs must be NHWC [N, H, W, C<=4]; got %s' % (tuple(x.shape),))
             N, H, W, C = x.shape
             mean = getattr(self.model, 'input_mean', self.input_mean)
             std = getattr(self.model, 'input_std', self.input_std)
-            return x.contiguous(), (lambda t, cpad, **kw: ops.input_prep_u8(t, cpad, mean[:C], std[:C], **kw)), (N, C, H, W)
+            return x.contiguous(), (lambda t, cpad, **kw: ops.input_prep_u8(t, cpad, mean[:C], std[:C], mix=mix, **kw)), \
+                (N, C, H, W)
         N, C, H, W = x.shape
-        return x.float().contiguous(), ops.input_prep, (N, C, H, W)
+        return x.float().contiguous(), (lambda t, cpad, **kw: ops.input_prep(t, cpad, mix=mix, **kw)), (N, C, H, W)
 
     # ---- inference: BatchNorm folded into the convolution (reference utils/absorb_bn.py:18-48) ----------------
     # w' = w * gamma/sqrt(var+eps) per output channel, b' = beta - mean*gamma/sqrt(var+eps): one kernel computes
@@ -617,24 +619,28 @@ class Runtime(object):
         logits, _ = self.run_forward(x, training, False)
         return logits
 
-    def run_forward(self, x, training, want_tape):
+    def run_forward(self, x, training, want_tape, mix=None):
         raise NotImplementedError
 
     def run_backward(self, tape, dlogits, dl_bf16=None):
         raise NotImplementedError
 
-    def train_step(self, x, target, smooth_eps=0.0, upstream=None):
+    def train_step(self, x, target, smooth_eps=0.0, upstream=None, mix=None):
         """forward + mean softmax cross-entropy (label smoothing ``smooth_eps``) + backward of one batch as a straight
         sequence of library calls -- no autograd graph, no autograd worker thread, no ATen kernels: what Trainer runs
         (and captures into a CUDA graph) when the criterion is the plain CrossEntropyLoss of the reference
         (trainer.py:132-162 with utils/cross_entropy.py:20-24,46-52).  ``upstream``: optional 0-dim fp32 device tensor
         multiplied into the gradients (loss scale x grad scale).  Gradients accumulate into the arena.
+        ``mix`` (ops.Mix): MixUp / CutMix of the batch (trainer.py:119-135 with utils/mixup.py of the reference) -- the
+        relayout kernel mixes the input and the loss is the soft-target cross-entropy against lam*onehot(target) +
+        (1-lam)*onehot(target[perm]); ``smooth_eps`` is then ignored, as the reference's cross_entropy ignores it for
+        soft targets (utils/cross_entropy.py:38-54).  Top-1 / top-5 still count against ``target``.
         Returns (logits, stats): logits detached, stats = fp32[3] device tensor {mean loss, top-1 %, top-5 %}."""
         if x.device.type != 'cuda':
             raise B200Error('B200 runtime needs CUDA inputs (no CPU fallback); got %s' % x.device)
         if target.dtype != torch.int64 or target.dim() != 1 or target.shape[0] != x.shape[0] or not target.is_cuda:
             raise B200Error('train_step: target must be a CUDA int64 vector with one class index per sample')
-        logits, tape = self.run_forward(x, True, True)
+        logits, tape = self.run_forward(x, True, True, mix=mix)
         pad = tape['head']['logits_pad']
         dev = pad.device
         stats = torch.empty(3, device=dev, dtype=torch.float32)
@@ -643,8 +649,12 @@ class Runtime(object):
         up = None
         if upstream is not None:
             up = upstream.reshape(1)
-        ops.softmax_ce(pad, target.contiguous(), self.classes, smooth_eps, loss=stats, row_loss=rows, dlogits=dl,
-                       grad_scale_dev=up)
+        if mix is not None:
+            ops.softmax_ce_mix(pad, target.contiguous(), mix, self.classes, loss=stats, row_loss=rows, dlogits=dl,
+                               grad_scale_dev=up)
+        else:
+            ops.softmax_ce(pad, target.contiguous(), self.classes, smooth_eps, loss=stats, row_loss=rows, dlogits=dl,
+                           grad_scale_dev=up)
         self.arena.rebind_grads()
         self.arena.grads_zero = False
         self.run_backward(tape, logits, dl_bf16=dl)
@@ -764,8 +774,8 @@ class ResNetRuntime(Runtime):
         self._head_build(m.fc)
 
     # ---- stem ---------------------------------------------------------------------------------------
-    def _stem_fwd(self, x, training):
-        x, prep, (N, Cin, H, W) = self._input(x)
+    def _stem_fwd(self, x, training, mix=None):
+        x, prep, (N, Cin, H, W) = self._input(x, mix)
         K = self.stem_conv.out_channels
         st = {}
         if self.imagenet_stem:
@@ -882,11 +892,11 @@ class ResNetRuntime(Runtime):
         return self._conv_bwd(u, dz, residual=skip)
 
     # ---- whole network ------------------------------------------------------------------------------
-    def run_forward(self, x, training, want_tape):
+    def run_forward(self, x, training, want_tape, mix=None):
         self._want_tape = want_tape
         if training:
             self.arena.version += 1          # running statistics change: folded inference weights become stale
-        h, stem = self._stem_fwd(x, training)
+        h, stem = self._stem_fwd(x, training, mix)
         saved = []
         for spec in self.blocks:
             h, s = self._block_fwd(spec, h, training)
@@ -972,8 +982,8 @@ class MobileNetRuntime(Runtime):
             return ops.dwconv_dgrad(dz, u.conv.w16, u.desc) if need_dx else None
         return self._conv_bwd(u, dz, need_dx=need_dx, residual=residual)
 
-    def _stem_fwd(self, x, training):
-        x, prep, (N, Cin, H, W) = self._input(x)
+    def _stem_fwd(self, x, training, mix=None):
+        x, prep, (N, Cin, H, W) = self._input(x, mix)
         K = self.stem_conv.out_channels
         xs = prep(x, 16, s2d=False)
         ws = torch.zeros((K, 9, 16), device=self.device, dtype=torch.bfloat16)
@@ -998,11 +1008,11 @@ class MobileNetRuntime(Runtime):
             self.stem_g32.view(K, 9, Cin).add_(dws[:, :, :Cin])
         self._wgrad_async(stem_wgrad, u.x, dz)
 
-    def run_forward(self, x, training, want_tape):
+    def run_forward(self, x, training, want_tape, mix=None):
         self._want_tape = want_tape
         if training:
             self.arena.version += 1
-        h, stem = self._stem_fwd(x, training)
+        h, stem = self._stem_fwd(x, training, mix)
         saved = []
         for spec in self.blocks:
             xin, units = h, []

@@ -52,6 +52,7 @@ def build_parser():
     a('-j', '--workers', default=8, type=int, metavar='N', help='number of data loading workers')
     a('-b', '--batch-size', default=256, type=int, metavar='N', help='mini-batch size')
     a('--label-smoothing', default=0, type=float, help='label smoothing coefficient')
+    a('--mixup', default=None, type=float, help='mixup alpha coefficient - accepted for CLI parity, unused in evaluation')
     a('--duplicates', default=1, type=int, help='number of augmentations over single example')
     a('--augment', action='store_true', default=False, help='perform augmentations')
     a('--calibrate-bn', action='store_true', default=False, help='calibrate bn stats')
@@ -137,7 +138,7 @@ def main_worker(args):
     criterion = getattr(model, 'criterion', CrossEntropyLoss)(**loss_params)
     criterion.to(args.device)
     trainer = Trainer(model, criterion, device_ids=args.device_ids, device=args.device, dtype=dtype,
-                      print_freq=args.print_freq)
+                      mixup=args.mixup, print_freq=args.print_freq)
     common = {'datasets_path': args.datasets_dir, 'name': args.dataset, 'input_size': args.input_size,
               'batch_size': args.batch_size, 'num_workers': args.workers, 'pin_memory': cuda, 'drop_last': False}
     val_data = DataRegime(None, defaults=dict(common, split='val', augment=args.augment, shuffle=False,

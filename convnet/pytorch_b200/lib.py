@@ -12,6 +12,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("B200_LIB_PATH") or os.path.join(_HERE, "libb200conv.so")   # override: A/B builds in tools/
 
 ACT_NONE, ACT_RELU, ACT_RELU6 = 0, 1, 2
+MIX_NONE, MIX_MIXUP, MIX_CUTMIX = 0, 1, 2      # B200_MIX_* (input mixing of b200_input_prep_mix)
 
 
 class B200Error(RuntimeError):
@@ -60,6 +61,9 @@ SIGNATURES = {
     "b200_input_prep": [_vp, _i, _i, _i, _i, _i, _i, _vp, _vp],
     "b200_input_prep_u8": [_vp, _i, _i, _i, _i, _i, _i, ctypes.POINTER(ctypes.c_float), ctypes.POINTER(ctypes.c_float),
                            _vp, _vp],
+    "b200_input_prep_mix": [_vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _i, _vp, _vp],
+    "b200_input_prep_u8_mix": [_vp, _i, _i, _i, _i, _i, _i, ctypes.POINTER(ctypes.c_float),
+                               ctypes.POINTER(ctypes.c_float), _vp, _vp, _i, _vp, _vp],
     "b200_weight_transpose": [_vp, _vp, _i, _i, _i, _vp],
     "b200_weight_transpose_batched": [_vp, _vp, _vp, _i, _i, _vp],
     "b200_stem_weight_to_s2d": [_vp, _i, _i, _i, _vp, _vp],
@@ -73,6 +77,7 @@ SIGNATURES = {
     "b200_se_bwd_dx": [_vp, _vp, _vp, _i, _i, _i, _vp, _vp],
     "b200_act_bwd": [_vp, _vp, _ll, _i, _vp, _vp],
     "b200_softmax_ce": [_vp, _vp, _i, _i, _i, _f, _f, _vp, _vp, _vp, _vp, _vp],
+    "b200_softmax_ce_mix": [_vp, _vp, _vp, _vp, _i, _i, _i, _f, _vp, _vp, _vp, _vp, _vp],
     "b200_colsum_bf16": [_vp, _i, _i, _vp, _vp],
     "b200_fused_sgd": [_vp, _vp, _vp, _vp, _ll, _ll, _f, _f, _f, _f, _f, _vp, _i, _i, _vp],
     "b200_sumsq": [_vp, _ll, _vp, _vp, _vp],

@@ -63,8 +63,9 @@ def build_parser():
     a('--save-all', action='store_true', default=False, help='save checkpoint for every epoch')
     a('--label-smoothing', default=0, type=float, help='label smoothing coefficient')
     a('--sync-bn', action='store_true', default=False, help='synchronize batch-norm statistics across ranks')
-    a('--mixup', default=None, type=float, help='mixup alpha coefficient (not supported)')
-    a('--cutmix', default=None, type=float, help='cutmix alpha coefficient (not supported)')
+    a('--mixup', default=None, type=float, help='mixup alpha coefficient - default None')
+    a('--cutmix', default=None, type=float,
+      help='cutmix alpha coefficient - default None (with --mixup as well: CutMix with the --mixup alpha)')
     a('--duplicates', default=1, type=int, help='number of augmentations over single example')
     a('--chunk-batch', default=1, type=int, help='chunk batch size for multiple passes (training)')
     a('--cutout', action='store_true', default=False, help='cutout augmentations (ignored for synthetic data)')

@@ -394,36 +394,88 @@ def act_bwd(dy, y, act):
 
 
 # ------------------------------------------------------------------------------------ layout / casts
-def input_prep(x_nchw, cpad, s2d=False, border=False):
-    """NCHW fp32 -> NHWC bf16 (channels zero-padded to cpad) or its 2x2 space-to-depth form (optionally with
-    the physical zero border of mode 2: +2 low / +1 high in H and W)."""
-    _chk(x_nchw, torch.float32, "x")
-    N, C, H, W = x_nchw.shape
+class Mix(object):
+    """Device-side draws of one MixUp / CutMix step for the mixing kernels: ``perm`` int64 [N], ``params`` the
+    b200_mix_params block (int32 [5] on the device: lambda as fp32 bits, then r0, r1, c0, c1), ``kind`` MIX_MIXUP or
+    MIX_CUTMIX.  The kernels read perm and params at run time, so a captured graph follows new values in place."""
+    __slots__ = ('perm', 'params', 'kind')
+
+    def __init__(self, perm, params, kind):
+        self.perm, self.params, self.kind = perm, params, int(kind)
+
+    @property
+    def lam(self):
+        """fp32 [1] device view of lambda (the first field of the parameter block)."""
+        return self.params[:1].view(torch.float32)
+
+
+def _check_mix(mix, n):
+    _chk(mix.perm, torch.int64, "perm"); _chk(mix.params, torch.int32, "mix params")
+    if mix.perm.numel() != n or mix.params.numel() < 5 or mix.kind not in (_l.MIX_MIXUP, _l.MIX_CUTMIX):
+        raise _l.B200Error("mix: perm must have one entry per sample, params 5 int32, kind MIXUP or CUTMIX")
+
+
+def _prep_out(N, H, W, cpad, s2d, border, device, out):
     if s2d and border:
         shape = (N, H // 2 + 3, W // 2 + 3, cpad)
     else:
         shape = (N, H // 2, W // 2, cpad) if s2d else (N, H, W, cpad)
-    out = torch.empty(shape, device=x_nchw.device, dtype=bf16)
-    with _T('input_prep', 0, 4 * x_nchw.numel() + 2 * out.numel()):
-        _l.check(_l.load().b200_input_prep(x_nchw.data_ptr(), N, C, H, W, cpad, (2 if border else 1) if s2d else 0, out.data_ptr(),
-                                           _stream()), "b200_input_prep")
+    if out is None:
+        return torch.empty(shape, device=device, dtype=bf16)
+    _chk(out, bf16, "out")
+    if tuple(out.shape) != shape:
+        raise _l.B200Error("input_prep: out has shape %s, expected %s" % (tuple(out.shape), shape))
     return out
 
 
-def input_prep_u8(x_nhwc_u8, cpad, mean, std, s2d=False, border=False):
+def input_prep(x_nchw, cpad, s2d=False, border=False, mix=None, out=None):
+    """NCHW fp32 -> NHWC bf16 (channels zero-padded to cpad) or its 2x2 space-to-depth form (optionally with
+    the physical zero border of mode 2: +2 low / +1 high in H and W).  ``mix`` (a Mix): MixUp / CutMix in the pass."""
+    _chk(x_nchw, torch.float32, "x")
+    N, C, H, W = x_nchw.shape
+    out = _prep_out(N, H, W, cpad, s2d, border, x_nchw.device, out)
+    mode = (2 if border else 1) if s2d else 0
+    if mix is None:
+        with _T('input_prep', 0, 4 * x_nchw.numel() + 2 * out.numel()):
+            _l.check(_l.load().b200_input_prep(x_nchw.data_ptr(), N, C, H, W, cpad, mode, out.data_ptr(),
+                                               _stream()), "b200_input_prep")
+        return out
+    _check_mix(mix, N)
+    reads = 2 if mix.kind == _l.MIX_MIXUP else 1
+    with _T('input_prep', 0, 4 * reads * x_nchw.numel() + 2 * out.numel()):
+        _l.check(_l.load().b200_input_prep_mix(x_nchw.data_ptr(), N, C, H, W, cpad, mode, mix.perm.data_ptr(),
+                                               mix.params.data_ptr(), mix.kind, out.data_ptr(), _stream()),
+                 "b200_input_prep_mix")
+    return out
+
+
+def u8_norm_coeffs(mean, std):
+    """fp32 scale / bias of the uint8 normalisation: value = u8 * scale + bias = (u8/255 - mean)/std."""
+    scale = [1.0 / (255.0 * float(s)) for s in std]
+    bias = [-float(m) / float(s) for m, s in zip(mean, std)]
+    return scale, bias
+
+
+def input_prep_u8(x_nhwc_u8, cpad, mean, std, s2d=False, border=False, mix=None, out=None):
     """uint8 NHWC [N,H,W,C] -> the layouts of input_prep, normalised as (u8/255 - mean)/std in the same pass."""
     _chk(x_nhwc_u8, torch.uint8, "x")
     N, H, W, C = x_nhwc_u8.shape
-    if s2d and border:
-        shape = (N, H // 2 + 3, W // 2 + 3, cpad)
-    else:
-        shape = (N, H // 2, W // 2, cpad) if s2d else (N, H, W, cpad)
-    out = torch.empty(shape, device=x_nhwc_u8.device, dtype=bf16)
-    scale = (ctypes.c_float * C)(*[1.0 / (255.0 * float(s)) for s in std])
-    bias = (ctypes.c_float * C)(*[-float(m) / float(s) for m, s in zip(mean, std)])
-    with _T('input_prep', 0, x_nhwc_u8.numel() + 2 * out.numel()):
-        _l.check(_l.load().b200_input_prep_u8(x_nhwc_u8.data_ptr(), N, C, H, W, cpad, (2 if border else 1) if s2d else 0,
-                                              scale, bias, out.data_ptr(), _stream()), "b200_input_prep_u8")
+    out = _prep_out(N, H, W, cpad, s2d, border, x_nhwc_u8.device, out)
+    sc, bi = u8_norm_coeffs(mean, std)
+    scale = (ctypes.c_float * C)(*sc)
+    bias = (ctypes.c_float * C)(*bi)
+    mode = (2 if border else 1) if s2d else 0
+    if mix is None:
+        with _T('input_prep', 0, x_nhwc_u8.numel() + 2 * out.numel()):
+            _l.check(_l.load().b200_input_prep_u8(x_nhwc_u8.data_ptr(), N, C, H, W, cpad, mode, scale, bias,
+                                                  out.data_ptr(), _stream()), "b200_input_prep_u8")
+        return out
+    _check_mix(mix, N)
+    reads = 2 if mix.kind == _l.MIX_MIXUP else 1
+    with _T('input_prep', 0, reads * x_nhwc_u8.numel() + 2 * out.numel()):
+        _l.check(_l.load().b200_input_prep_u8_mix(x_nhwc_u8.data_ptr(), N, C, H, W, cpad, mode, scale, bias,
+                                                  mix.perm.data_ptr(), mix.params.data_ptr(), mix.kind, out.data_ptr(),
+                                                  _stream()), "b200_input_prep_u8_mix")
     return out
 
 
@@ -511,6 +563,24 @@ def softmax_ce(logits, target, classes, smooth_eps, loss=None, row_loss=None, dl
                                            float(smooth_eps or 0.0), float(grad_scale), _l.ptr(grad_scale_dev),
                                            _l.ptr(loss), _l.ptr(row_loss), _l.ptr(dlogits), _stream()),
                  "b200_softmax_ce")
+
+
+def softmax_ce_mix(logits, target, mix, classes, loss=None, row_loss=None, dlogits=None, grad_scale=1.0,
+                   grad_scale_dev=None):
+    """softmax_ce with the soft MixUp / CutMix target lam*onehot(t) + (1-lam)*onehot(t[perm]); ``mix`` is an ops.Mix
+    (perm and lambda are read on the device).  Top-1 / top-5 count against ``target`` itself; no label smoothing."""
+    if loss is not None and (loss.numel() < 3 or row_loss is None or row_loss.numel() < 2 * logits.shape[0]):
+        raise _l.B200Error("softmax_ce_mix: loss needs 3 floats and row_loss 2*B floats")
+    B, ld = logits.shape
+    _chk(logits, torch.float32, "logits"); _chk(target, torch.int64, "target"); _chk(dlogits, bf16, "dlogits")
+    _chk(loss, torch.float32, "loss"); _chk(row_loss, torch.float32, "row_loss")
+    _chk(grad_scale_dev, torch.float32, "grad_scale_dev")
+    _check_mix(mix, B)
+    with _T('softmax_ce', 0, 4 * logits.numel()):
+        _l.check(_l.load().b200_softmax_ce_mix(logits.data_ptr(), target.data_ptr(), mix.perm.data_ptr(),
+                                               mix.lam.data_ptr(), B, int(classes), int(ld), float(grad_scale),
+                                               _l.ptr(grad_scale_dev), _l.ptr(loss), _l.ptr(row_loss), _l.ptr(dlogits),
+                                               _stream()), "b200_softmax_ce_mix")
 
 
 def colsum_bf16(m, out):

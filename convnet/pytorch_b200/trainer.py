@@ -14,18 +14,25 @@ does the bf16/NHWC conversion), gradients land in the flat arena, the data-paral
 NCCL all-reduce of that arena (no DistributedDataParallel wrapper, no per-forward buffer broadcast --
 SURVEY.md section 2.3 C1/C2), and the per-tensor unscale / clip loops of the reference
 (trainer.py:165-172) are folded into the fused optimizer kernel.
+
+MixUp / CutMix (``mixup`` / ``cutmix``, trainer.py:44-51,119-138): drawn on the host per training chunk by
+utils/mixup.py; on the fused B200 path the input relayout and loss kernels do the mixing (see ``_upload_mix``).
 """
 import logging
 import os
+import random
 import time
 
+import numpy as np
 import torch
 import torch.nn as nn
 import torch.distributed as dist
 from torch.nn.utils import clip_grad_norm_
 
+from .lib import B200Error, MIX_CUTMIX, MIX_MIXUP
 from .utils import regularization
 from .utils.meters import AverageMeter, accuracy
+from .utils.mixup import CutMix, MixUp
 
 _METERS = ('step', 'data', 'loss', 'prec1', 'prec5')
 
@@ -51,6 +58,17 @@ def _average_duplicates(outputs, target, batch_first=True):
     if batch_first:
         return outputs.view(bsz, -1, *outputs.shape[1:]).mean(dim=1)
     return outputs.view(-1, bsz, *outputs.shape[1:]).mean(dim=0)
+
+
+def _mixup(mixup_modules, alpha, batch_size):
+    """One module of ``mixup_modules`` draws this chunk's mixing (trainer.py:44-51 of the reference): Python's
+    random.sample picks it -- called even for a single candidate, so the Python generator advances as in the
+    reference -- then torch.randperm and numpy's beta draw inside ``sample``."""
+    for m in mixup_modules:
+        m.reset()
+    layer = random.sample(mixup_modules, 1)[0]
+    layer.sample(alpha, batch_size)
+    return layer
 
 
 def _cuda_prefetch(loader, device, dtype):
@@ -106,8 +124,6 @@ class Trainer(object):
     def __init__(self, model, criterion, optimizer=None, device_ids=[0], device='cuda', dtype=torch.float,
                  distributed=False, local_rank=-1, adapt_grad_norm=None, mixup=None, cutmix=None,
                  loss_scale=1., grad_clip=-1, print_freq=100):
-        if mixup is not None or cutmix is not None:
-            raise NotImplementedError('mixup / cutmix are outside the B200 hot path (SURVEY.md section 2, #18)')
         self._model = model
         self.criterion = criterion
         self.epoch = 0
@@ -119,6 +135,12 @@ class Trainer(object):
         self.local_rank = local_rank
         self.print_freq = print_freq
         self.grad_clip = grad_clip
+        # input mixing (trainer.py:119-135 of the reference).  With both set the reference builds a CutMix whose alpha
+        # is taken from ``mixup`` (mix_val = mixup or cutmix): reproduced as is
+        self.mixup = mixup
+        self.cutmix = cutmix
+        self.last_mix = None                   # the MixUp / CutMix module of the latest training chunk (its draws)
+        self._mix_dev, self._mix_ring, self._mix_turn = {}, {}, 0
         self.grad_scale = None
         self.loss_scale = loss_scale
         self.adapt_grad_norm = adapt_grad_norm
@@ -235,15 +257,19 @@ class Trainer(object):
             self._graph_static_ok = ok
         return self._graph_static_ok
 
-    def graphed_forward_backward(self, inputs, target):
+    def graphed_forward_backward(self, inputs, target, mix=None):
         """Forward + criterion + backward of one device-resident batch through a captured CUDA graph.
         Returns (logits, loss, stats) -- detached device tensors; stats = fp32[3] {loss, top-1 %, top-5 %} when the fused
         loss kernel computed them, else None -- or None when this call has to run eagerly (warm-up steps of
-        a new shape, unsupported configuration).  Gradients land in the arena exactly as in the eager path."""
+        a new shape, unsupported configuration).  Gradients land in the arena exactly as in the eager path.
+        ``mix`` (ops.Mix, from _upload_mix): the step mixes its input; the graph reads the permutation, lambda and box
+        from their persistent device buffers, so every replay uses the values uploaded for that step."""
         if not self._graph_eligible() or not inputs.is_cuda:
             return None
-        # loss / gradient scales are NOT part of the key: they reach the kernels through a device scalar
-        key = (tuple(inputs.shape), inputs.dtype, tuple(target.shape), target.dtype, self._model.training)
+        # loss / gradient scales are NOT part of the key: they reach the kernels through a device scalar; neither are
+        # the mixing draws (device buffers) -- only the kind of mixing
+        key = (tuple(inputs.shape), inputs.dtype, tuple(target.shape), target.dtype, self._model.training,
+               mix.kind if mix is not None else 0)
         st = self._graphs.get(key)
         if st is None:
             st = self._graphs[key] = {'seen': 0, 'graph': None}
@@ -252,7 +278,7 @@ class Trainer(object):
             if st['seen'] <= 2:
                 return None                       # eager warm-up (library handles, allocator, autotuned state)
             try:
-                self._capture(st, inputs, target)
+                self._capture(st, inputs, target, mix)
             except Exception as e:  # noqa: BLE001  -- keep training eagerly if capture is impossible here
                 if self.b200.grad_bucket_hook is not None:
                     # NCCL inside the capture is the likely culprit: fall back to ONE flat all-reduce after the graph
@@ -273,7 +299,7 @@ class Trainer(object):
         self.graph_replayed_launches += st['launches']
         return st['out'].detach(), st['loss'].detach(), st['stats']
 
-    def _capture(self, st, inputs, target):
+    def _capture(self, st, inputs, target, mix=None):
         from . import lib
         x_s, y_s = torch.empty_like(inputs), torch.empty_like(target)
         x_s.copy_(inputs)
@@ -297,7 +323,7 @@ class Trainer(object):
         with torch.cuda.graph(graph, pool=self._graph_pool, stream=self._capture_stream, capture_error_mode=mode):
             stats = None
             if eps is not None:            # the whole step is library calls: nothing of autograd inside the graph
-                out, stats = self.b200.train_step(x_s, y_s, eps, up)
+                out, stats = self.b200.train_step(x_s, y_s, eps, up, mix=mix)
                 loss = stats[0]
             else:
                 out = self.model(x_s)
@@ -373,13 +399,21 @@ class Trainer(object):
 
         chunks = zip(inputs_batch.chunk(chunk_batch, dim=0), target_batch.chunk(chunk_batch, dim=0))
         for i, (inputs, target) in enumerate(chunks):
+            is_u8 = inputs.dtype == torch.uint8
             target = target.to(self.device, non_blocking=True)
             if self.b200 is not None and inputs.dtype == torch.uint8:
                 inputs = inputs.to(self.device, non_blocking=True)
             else:
                 inputs = inputs.to(self.device, dtype=self._input_dtype(), non_blocking=True)
-            if training and chunk_batch == 1 and not average_output:
-                replayed = self.graphed_forward_backward(inputs, target)
+            mixer = None
+            if training and (self.mixup is not None or self.cutmix is not None):
+                mixer = self._draw_mix(inputs.size(0), average_output)
+            fused = training and self.b200 is not None and chunk_batch == 1 and not average_output and inputs.is_cuda \
+                and self._hooks_static() and self._plain_ce_eps() is not None \
+                and target.dtype == torch.long and target.dim() == 1
+            mix = self._upload_mix(mixer, inputs) if (mixer is not None and fused) else None
+            if training and chunk_batch == 1 and not average_output and (mixer is None or mix is not None):
+                replayed = self.graphed_forward_backward(inputs, target, mix)
                 if replayed is not None:
                     outputs.append(replayed[0])
                     if replayed[2] is not None:
@@ -387,15 +421,20 @@ class Trainer(object):
                     else:
                         total_loss += float(replayed[1])
                     continue
-            if training and self.b200 is not None and chunk_batch == 1 and not average_output and inputs.is_cuda \
-                    and self._hooks_static() and self._plain_ce_eps() is not None \
-                    and target.dtype == torch.long and target.dim() == 1:
+            if fused:
                 # eager form of the captured step (warm-up iterations of a new shape, B200_CUDA_GRAPH=0)
                 self.optimizer.pre_forward()
-                output, stats = self.b200.train_step(inputs, target, self._plain_ce_eps(), self._upstream())
+                output, stats = self.b200.train_step(inputs, target, self._plain_ce_eps(), self._upstream(), mix=mix)
                 outputs.append(output)
                 self.optimizer.pre_backward()
                 continue
+            if mixer is not None:
+                # generic path (chunked batches, other criteria): the reference's fp32 mixing of the batch on its device
+                # and the soft target through the criterion
+                if is_u8:
+                    raise B200Error('mixup / cutmix of a uint8 batch needs the fused path (chunk_batch=1, plain '
+                                    'CrossEntropyLoss, a converted model); normalise the batch to fp32 otherwise')
+                inputs = mixer(inputs.clone() if isinstance(mixer, CutMix) else inputs)   # the caller's batch stays intact
             if training:
                 self.optimizer.pre_forward()
             output = self.model(inputs)
@@ -404,6 +443,8 @@ class Trainer(object):
                     output = [_average_duplicates(o, target) if o is not None else None for o in output]
                 else:
                     output = _average_duplicates(output, target)
+            if mixer is not None:
+                target = mixer.mix_target(target, (output[0] if isinstance(output, (list, tuple)) else output).size(-1))
             loss = self.criterion(output, target)
             if chunk_batch > 1:
                 loss = loss / chunk_batch
@@ -445,6 +486,57 @@ class Trainer(object):
             self.training_steps += 1
 
         return (outputs[0] if len(outputs) == 1 else torch.cat(outputs, dim=0)), (stats if stats is not None else total_loss), grad
+
+    # ------------------------------------------------------------------ input mixing (MixUp / CutMix)
+    def _draw_mix(self, batch_size, average_output=False):
+        """This chunk's mixing draws, made on the host in the reference's order (trainer.py:119-131): random.sample,
+        torch.randperm, numpy beta (and, for CutMix, the box centre when the batch is mixed).  Returns the module."""
+        if average_output:
+            # the permutation would run over the B*D duplicated rows while the averaged output and the target have B
+            # rows: the reference fails in mix_target here
+            raise NotImplementedError('mixup / cutmix with average_output: the mixing permutation covers the B*D '
+                                      'duplicated inputs but the averaged outputs and targets have B rows')
+        input_mixup = CutMix() if self.cutmix else MixUp()
+        # ResNet(mixup=True) intermediate mixing layers are not supported, so the input mixer is the only candidate
+        self.last_mix = _mixup([input_mixup], self.mixup or self.cutmix, batch_size)
+        return self.last_mix
+
+    _MIX_RING = 4
+
+    def _upload_mix(self, mixer, inputs):
+        """-> ops.Mix over persistent device buffers holding this step's permutation and {lambda, r0, r1, c0, c1}.
+        One int64 device buffer per batch size: [perm (B) | parameter block (3 words)]; a CUDA graph captured with it
+        reads whatever the latest upload wrote.  The host side stages through a small ring of pinned buffers (an event
+        guards each slot until its copy has run) and issues ONE non-blocking copy on the current stream, which orders
+        it after the previous step's kernels: no host synchronisation per step."""
+        from . import ops
+        B = inputs.size(0)
+        H, W = (inputs.shape[1], inputs.shape[2]) if inputs.dtype == torch.uint8 else (inputs.shape[-2], inputs.shape[-1])
+        if isinstance(mixer, CutMix):
+            kind, box = MIX_CUTMIX, mixer.draw_box(H, W)     # the reference draws the box when the batch is mixed
+        else:
+            kind, box = MIX_MIXUP, (0, 0, 0, 0)
+        dev = self._mix_dev.get(B)
+        if dev is None:
+            dev = self._mix_dev[B] = torch.zeros(B + 3, dtype=torch.int64, device=inputs.device)
+        ring = self._mix_ring.setdefault(B, [])
+        k = self._mix_turn % self._MIX_RING
+        self._mix_turn += 1
+        if len(ring) <= k:
+            ring.append([torch.zeros(B + 3, dtype=torch.int64).pin_memory(), None])
+        host, ev = ring[k]
+        if ev is not None:
+            ev.synchronize()                           # the copy that last read this slot has run (long ago)
+        h = host.numpy()
+        h[:B] = mixer.mix_index.numpy()
+        blk = h[B:].view(np.int32)
+        blk[0:1].view(np.float32)[0] = mixer.mix_values.numpy()[0]
+        blk[1:5] = box
+        dev.copy_(host, non_blocking=True)
+        ev = torch.cuda.Event()
+        ev.record()
+        ring[k][1] = ev
+        return ops.Mix(dev[:B], dev[B:].view(torch.int32), kind)
 
     # ------------------------------------------------------------------ epoch loop
     def forward(self, data_loader, num_steps=None, training=False, average_output=False, chunk_batch=1):

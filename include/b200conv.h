@@ -5,6 +5,7 @@
  * The reference has no FFI of its own (it is pure Python on top of torch.nn); every entry point
  * below replaces one implicit torch/cuDNN/ATen operator the reference invokes, cited per function
  * as reference file:line (paths under the reference tree).  INTEGRATION.md shows the ctypes stubs.
+ * 47 entry points.
  *
  * Conventions
  *  - every function returns 0 on success or a negative B200_ERR_* code; b200_last_error() gives text.
@@ -167,6 +168,28 @@ int b200_input_prep(const float* x_nchw, int N, int C, int H, int W, int Cpad, i
  * preprocess.py:20-24 fused into the relayout (SURVEY.md section 8(f) row 2).  scale_host / bias_host: HOST arrays [C]. */
 int b200_input_prep_u8(const uint8_t* x_nhwc, int N, int C, int H, int W, int Cpad, int mode, const float* scale_host,
                        const float* bias_host, void* out, b200_stream_t stream);
+/* The same relayouts with the reference Trainer's input mixing (utils/mixup.py:19-26,57-90; trainer.py:119-135) done in
+ * the pass.  perm: device int64 [N], the partner sample of each sample.  params: DEVICE parameter block, read by the
+ * kernel at run time so that a captured CUDA graph picks up each step's values.  kind:
+ *   B200_MIX_NONE   -- exactly b200_input_prep / b200_input_prep_u8 (perm and params may be NULL);
+ *   B200_MIX_MIXUP  -- v = lam*x[n] + (1-lam)*x[perm[n]] with two fp32 products and one fp32 sum (no FMA), then one
+ *                      rounding to bf16 (bit-exact against the reference's fp32 expression);
+ *   B200_MIX_CUTMIX -- pixel (r, c) of sample n is taken from sample perm[n] when r0 <= r < r1 and c0 <= c < c1, else
+ *                      from n; in modes 1/2 each of the four sub-pixels of a 2x2 cell decides on its own.
+ * uint8 input: each source pixel is normalised (u8*scale+bias, one fmaf) before it is mixed.  The zero border of
+ * mode 2 and the channel padding stay zero. */
+#define B200_MIX_NONE 0
+#define B200_MIX_MIXUP 1
+#define B200_MIX_CUTMIX 2
+typedef struct {
+  float lam;          /* MixUp weight of the sample itself; CutMix: 1 - box area / image area (the loss reads it) */
+  int r0, r1, c0, c1; /* CutMix box: rows [r0, r1) x columns [c0, c1) */
+} b200_mix_params;
+int b200_input_prep_mix(const float* x_nchw, int N, int C, int H, int W, int Cpad, int mode, const long long* perm,
+                        const b200_mix_params* params, int kind, void* out, b200_stream_t stream);
+int b200_input_prep_u8_mix(const uint8_t* x_nhwc, int N, int C, int H, int W, int Cpad, int mode, const float* scale_host,
+                           const float* bias_host, const long long* perm, const b200_mix_params* params, int kind,
+                           void* out, b200_stream_t stream);
 /* bf16 [K][T][C] -> bf16 [C][T][K] (dgrad weight layout), multi-tensor: n tensors described by
  * device arrays. */
 int b200_weight_transpose(const void* src, void* dst, int K, int T, int C, b200_stream_t stream);
@@ -214,6 +237,15 @@ int b200_act_bwd(const void* dy, const void* y, long long n, int act, void* dx, 
 int b200_softmax_ce(const float* logits, const long long* target, int B, int classes, int ld, float smooth_eps,
                     float grad_scale, const float* grad_scale_dev, float* loss, float* row_loss, void* dlogits_bf16,
                     b200_stream_t stream);
+/* soft-target form for MixUp / CutMix (the reference's mix_target + cross_entropy with a float target,
+ * utils/mixup.py:37-45, utils/cross_entropy.py:53-54): q = lam*onehot(target[b]) + (1-lam)*onehot(target[perm[b]]),
+ * lam = *lam_dev (device: b200_mix_params.lam).  Row loss -(lam*lsm[t] + (1-lam)*lsm[t2]), gradient
+ * (lam + (1-lam))*softmax - lam*[c==t] - (1-lam)*[c==t2].  The top-1 / top-5 ranks use target[b] (the meters of the
+ * reference read the original target, trainer.py:224).  No smoothing argument: the reference drops label smoothing
+ * for soft targets.  Other arguments as b200_softmax_ce. */
+int b200_softmax_ce_mix(const float* logits, const long long* target, const long long* perm, const float* lam_dev, int B,
+                        int classes, int ld, float grad_scale, const float* grad_scale_dev, float* loss, float* row_loss,
+                        void* dlogits_bf16, b200_stream_t stream);
 /* column sums of a bf16 [B][K] matrix accumulated into fp32 out[K] (fc bias gradient) */
 int b200_colsum_bf16(const void* m, int B, int K, float* out, b200_stream_t stream);
 
