@@ -97,12 +97,21 @@ __global__ void __launch_bounds__(256) input_prep_kernel(const float* __restrict
 // value = u8 * scale[c] + bias[c]  (scale = 1 / (255 * std), bias = -mean / std: ToTensor + Normalize of the reference's
 // preprocess.py:20-24).  4x fewer host->device bytes than the fp32 NCHW batch and no separate normalisation pass.
 struct U8Norm { float scale[4], bias[4]; };
-template <int MIX>
+
+// Batch augmentation (AUG, mode 0 only): output row n of N = B*D rows is copy n % D of image n / D after the
+// reference's RandomCrop(padding) + RandomHorizontalFlip + ToTensor + Normalize + Cutout (preprocess.py:44-54,185-227).
+// params[n] = {oy, ox, flip, y1, y2, x1, x2, ...} (int16, holes boxes); lut[c][u] = Normalize(ToTensor(u)) in fp32, as
+// torchvision computes it; a cut element is v * 0 (the reference multiplies by its mask: a signed zero).  Any values in
+// params are memory-safe: a source pixel is read only when it lies inside image n / D, else the pad value 0 is used.
+struct U8Aug { const int16_t* params; const float* lut; int D, pad, holes; };
+
+template <int MIX, bool AUG = false>
 __global__ void __launch_bounds__(256) input_prep_u8_kernel(const uint8_t* __restrict__ x, int N, int C, int H, int W,
                                                             int Cpad, int mode, U8Norm nm,
                                                             __nv_bfloat16* __restrict__ out,
                                                             const long long* __restrict__ perm,
-                                                            const b200_mix_params* __restrict__ mixp) {
+                                                            const b200_mix_params* __restrict__ mixp, U8Aug ag) {
+  static_assert(!AUG || MIX == kMixNone, "batch augmentation is not combined with mixing");
   pdl_wait();
   b200_mix_params mp = {};
   if (MIX != kMixNone) mp = *mixp;
@@ -115,6 +124,36 @@ __global__ void __launch_bounds__(256) input_prep_u8_kernel(const uint8_t* __res
     const int i = (int)((idx / OW) % OH) - brd;
     const int n = (int)(idx / ((long long)OW * OH));
     __nv_bfloat16* o = out + idx * Cpad;
+    if (AUG) {
+      const int16_t* pr = ag.params + (long long)n * (3 + 4 * ag.holes);
+      const int cs = __ldg(pr + 2) != 0 ? W - 1 - j : j;
+      const int sy = i + __ldg(pr + 0) - ag.pad, sx = cs + __ldg(pr + 1) - ag.pad;
+      const bool ok = sy >= 0 && sy < H && sx >= 0 && sx < W;
+      bool cut = false;
+      for (int h = 0; h < ag.holes; ++h) {
+        const int16_t* b = pr + 3 + 4 * h;
+        cut |= i >= __ldg(b + 0) && i < __ldg(b + 1) && j >= __ldg(b + 2) && j < __ldg(b + 3);
+      }
+      const uint8_t* src = x + ((long long)(n / ag.D) * H * W + (ok ? (long long)sy * W + sx : 0)) * C;
+      for (int c0 = 0; c0 < Cpad; c0 += 8) {
+        float f[8];
+#pragma unroll
+        for (int e = 0; e < 8; ++e) {
+          const int ch = c0 + e;
+          float val = 0.f;
+          if (ch < C) {
+            val = __ldg(ag.lut + ch * 256 + (ok ? __ldg(src + ch) : 0));
+            if (cut) val = __fmul_rn(val, 0.f);
+          }
+          f[e] = val;
+        }
+        uint4 u;
+        u.x = pack_bf16x2(f[0], f[1]); u.y = pack_bf16x2(f[2], f[3]);
+        u.z = pack_bf16x2(f[4], f[5]); u.w = pack_bf16x2(f[6], f[7]);
+        *reinterpret_cast<uint4*>(o + c0) = u;
+      }
+      continue;
+    }
     const bool inside = mode != 2 || (i >= 0 && j >= 0 && i < H / 2 && j < W / 2);
     const uint8_t* xi = x + (long long)n * H * W * C;
     const uint8_t* xm = MIX != kMixNone ? x + __ldg(perm + n) * H * W * C : xi;
@@ -328,14 +367,32 @@ static int input_prep_u8_impl(const uint8_t* x_nhwc, int N, int C, int H, int W,
   if (blocks > cap) blocks = cap;
   if (kind == B200_MIX_MIXUP)
     b200::launch(input_prep_u8_kernel<kMixUp>, (int)blocks, 256, 0, (cudaStream_t)stream, x_nhwc, N, C, H, W, Cpad,
-                 mode, nm, (__nv_bfloat16*)out, perm, params);
+                 mode, nm, (__nv_bfloat16*)out, perm, params, U8Aug{});
   else if (kind == B200_MIX_CUTMIX)
     b200::launch(input_prep_u8_kernel<kMixCut>, (int)blocks, 256, 0, (cudaStream_t)stream, x_nhwc, N, C, H, W, Cpad,
-                 mode, nm, (__nv_bfloat16*)out, perm, params);
+                 mode, nm, (__nv_bfloat16*)out, perm, params, U8Aug{});
   else
     b200::launch(input_prep_u8_kernel<kMixNone>, (int)blocks, 256, 0, (cudaStream_t)stream, x_nhwc, N, C, H, W, Cpad,
-                 mode, nm, (__nv_bfloat16*)out, (const long long*)nullptr, (const b200_mix_params*)nullptr);
+                 mode, nm, (__nv_bfloat16*)out, (const long long*)nullptr, (const b200_mix_params*)nullptr, U8Aug{});
   B200_CHECK_LAUNCH("input_prep_u8_kernel");
+  return B200_OK;
+}
+
+extern "C" int b200_input_prep_u8_aug(const uint8_t* x_nhwc, int N, int D, int C, int H, int W, int Cpad, int pad,
+                                      const float* lut, const int16_t* params, int holes, void* out,
+                                      b200_stream_t stream) {
+  B200_REQUIRE(x_nhwc && out && lut && params && N > 0 && D > 0 && C > 0 && C <= 4 && H > 0 && W > 0,
+               B200_ERR_INVALID, "input_prep_u8_aug: bad argument (C must be 1..4)");
+  B200_REQUIRE(Cpad % 8 == 0 && Cpad >= C, B200_ERR_INVALID, "input_prep_u8_aug: Cpad must be a multiple of 8 and >= C");
+  B200_REQUIRE(pad >= 0 && holes >= 0 && holes <= 64, B200_ERR_INVALID, "input_prep_u8_aug: pad=%d holes=%d out of range",
+               pad, holes);
+  B200_REQUIRE((long long)N * D <= 0x7fffffffLL, B200_ERR_UNSUPPORTED, "input_prep_u8_aug: N*D too large");
+  const U8Norm nm = {};
+  const long long total = (long long)N * D * H * W;
+  b200::launch(input_prep_u8_kernel<kMixNone, true>, grid_cap(total, 256), 256, 0, (cudaStream_t)stream, x_nhwc,
+               N * D, C, H, W, Cpad, 0, nm, (__nv_bfloat16*)out, (const long long*)nullptr,
+               (const b200_mix_params*)nullptr, U8Aug{params, lut, D, pad, holes});
+  B200_CHECK_LAUNCH("input_prep_u8_aug_kernel");
   return B200_OK;
 }
 

@@ -8,8 +8,14 @@ Datasets: the north-star configurations are synthetic, so ``synthetic_*`` names 
 (the reference has no synthetic option and needs downloads -- SURVEY.md section 8c shim 5):
   synthetic_cifar10 / synthetic_cifar100 : N(0,1) 3x32x32 tensors, 10 / 100 classes
   synthetic_imagenet                     : N(0,1) 3xSxS tensors (S = input_size, default 224), 1000 classes
-Real datasets (cifar10, cifar100, imagenet folders) go through torchvision if it is importable; the PIL
-augmentation stack of the reference (preprocess.py, autoaugment.py) is out of scope (SURVEY.md section 2).
+Real datasets (cifar10, cifar100, imagenet folders) go through torchvision if it is importable; the basic PIL
+augmentation stack of the reference (preprocess.py) is reproduced with Cutout, AutoAugment and colour jitter /
+Lighting are out of scope (SURVEY.md section 2).
+
+Batch augmentation on the device (transform key ``device_augment``, CIFAR-style training only): the loader yields
+(utils.augment.AugmentedBatch of the B uint8 NHWC images and their per-copy draws, target repeated to B*D) and the
+stem relayout kernel writes the B*D augmented copies.  Real cifar10 / cifar100 read the dataset's uint8 ``.data``;
+synthetic_cifar* use a pool of uniform uint8 images.
 """
 import os
 from copy import deepcopy
@@ -19,6 +25,7 @@ import torch
 from torch.utils.data import Dataset, Subset
 from torch.utils.data.distributed import DistributedSampler
 
+from .utils.augment import AugmentCollate, BatchAugment, Cutout
 from .utils.regime import Regime
 
 
@@ -46,6 +53,21 @@ class SyntheticImages(Dataset):
         return img, int(self.labels[idx])
 
 
+class U8Images(Dataset):
+    """(uint8 HWC image, label) samples for device augmentation: ``images`` uint8 [P, H, W, C] (indexed modulo P, so a
+    small synthetic pool stands for a long dataset), ``labels`` one per sample."""
+
+    def __init__(self, images, labels):
+        self.images = torch.as_tensor(images)
+        self.labels = torch.as_tensor(labels, dtype=torch.long)
+
+    def __len__(self):
+        return len(self.labels)
+
+    def __getitem__(self, idx):
+        return self.images[idx % len(self.images)], int(self.labels[idx])
+
+
 _IMAGE_STATS = {'mean': [0.485, 0.456, 0.406], 'std': [0.229, 0.224, 0.225]}   # preprocess.py:7-8 of the reference
 
 
@@ -53,12 +75,12 @@ def real_dataset_transform(transform_name='imagenet', input_size=None, scale_siz
                            cutout=None, autoaugment=False, padding=None, duplicates=1, num_crops=1):
     """The basic transform stacks the reference's ``get_transform`` selects for real image datasets
     (preprocess.py:114-161): random-resized-crop + flip (imagenet, train), pad-4 random crop + flip (cifar, train),
-    resize + centre crop (evaluation), then ToTensor + Normalize.  The research augmentations -- AutoAugment, Cutout,
-    Lighting/colour jitter, multi-crop evaluation -- are outside this repo's scope (SURVEY.md section 2, rows 14-15)
-    and raise instead of being silently dropped."""
+    resize + centre crop (evaluation), then ToTensor + Normalize, then Cutout when ``cutout`` = {'holes', 'length'}
+    (preprocess.py:159-160).  AutoAugment, Lighting/colour jitter and multi-crop evaluation are outside this repo's
+    scope (SURVEY.md section 2, rows 14-15) and raise instead of being silently dropped."""
     import torchvision.transforms as T
-    if autoaugment or cutout is not None or num_crops != 1:
-        raise NotImplementedError('autoaugment / cutout / multi-crop evaluation are outside the B200 hot path '
+    if autoaugment or num_crops != 1:
+        raise NotImplementedError('autoaugment / multi-crop evaluation are outside the B200 hot path '
                                   '(reference preprocess.py, autoaugment.py); use the reference data pipeline')
     stats = normalize or _IMAGE_STATS
     tail = [T.ToTensor(), T.Normalize(**stats)]
@@ -85,6 +107,8 @@ def real_dataset_transform(transform_name='imagenet', input_size=None, scale_siz
             head = ([T.Resize(scale_size)] if scale_size != input_size else []) + [T.CenterCrop(input_size)]
     else:
         raise NotImplementedError('no transform for dataset family %r' % transform_name)
+    if cutout is not None:
+        tail.append(Cutout(**cutout))
     fn = T.Compose(head + tail)
     if duplicates > 1:   # batch augmentation: D independent draws of the transform per sample (preprocess.py:105-112)
         return T.Lambda(lambda img: torch.stack([fn(img) for _ in range(duplicates)], dim=0))
@@ -123,11 +147,53 @@ def get_dataset(name, split='train', transform=None, target_transform=None, down
     raise ValueError('unknown dataset %r' % name)
 
 
+def device_augment_spec(transform_name='cifar10', input_size=None, scale_size=None, normalize=None, augment=True,
+                        cutout=None, autoaugment=False, padding=None, duplicates=1, num_crops=1, device_augment=True):
+    """The BatchAugment of a ``device_augment`` transform setting: the CIFAR training transform of
+    real_dataset_transform (pad-4 random crop + flip + ToTensor + Normalize [+ Cutout]) with its duplicates.  The
+    settings it cannot reproduce raise."""
+    if 'cifar' not in (transform_name or ''):
+        raise NotImplementedError('device_augment reproduces the CIFAR training transform only (RandomResizedCrop of '
+                                  'imagenet needs decoded variable-size images); got transform %r' % transform_name)
+    if not augment:
+        raise ValueError('device_augment is a training transform (augment=True); evaluation loaders do not take it')
+    if autoaugment or num_crops != 1:
+        raise NotImplementedError('device_augment does not reproduce autoaugment / multi-crop')
+    if scale_size is not None and input_size is not None and scale_size != input_size:
+        raise NotImplementedError('device_augment does not resize: scale_size %s != input_size %s'
+                                  % (scale_size, input_size))
+    return BatchAugment(padding=padding or 4, flip=True, cutout=cutout, duplicates=duplicates or 1,
+                        normalize=normalize or _IMAGE_STATS)
+
+
+def u8_dataset(name, input_size=None, split='train', download=True, datasets_path='~/Datasets', synthetic_length=None,
+               **_):
+    """uint8 NHWC samples for device augmentation: the dataset's own uint8 array (cifar10 / cifar100), or a pool of
+    256 uniform uint8 images for synthetic_cifar*."""
+    train = split == 'train'
+    if name in ('synthetic_cifar10', 'synthetic_cifar100'):
+        size, classes, n_train, n_val = _SYNTHETIC[name]
+        size = input_size or size
+        length = synthetic_length or int(os.environ.get('B200_SYNTHETIC_LENGTH', n_train if train else n_val))
+        g = torch.Generator().manual_seed(0 if train else 1)
+        images = torch.randint(0, 256, (min(256, length), size, size, 3), generator=g, dtype=torch.uint8)
+        return U8Images(images, torch.randint(0, classes, (length,), generator=g))
+    if name in ('cifar10', 'cifar100'):
+        import torchvision.datasets as tvd
+        if input_size not in (None, 32):
+            raise NotImplementedError('device_augment does not resize: %s images are 32x32, input_size %s'
+                                      % (name, input_size))
+        cls = tvd.CIFAR10 if name == 'cifar10' else tvd.CIFAR100
+        ds = cls(root=os.path.join(os.path.expanduser(datasets_path), name), train=train, download=download)
+        return U8Images(ds.data, ds.targets)
+    raise NotImplementedError('device_augment supports cifar10, cifar100 and synthetic_cifar*; got %r' % name)
+
+
 _DATA_ARGS = {'name', 'split', 'transform', 'target_transform', 'download', 'datasets_path', 'synthetic_length'}
 _DATALOADER_ARGS = {'batch_size', 'shuffle', 'sampler', 'batch_sampler', 'num_workers', 'collate_fn', 'pin_memory',
                     'drop_last', 'timeout', 'worker_init_fn'}
 _TRANSFORM_ARGS = {'transform_name', 'input_size', 'scale_size', 'normalize', 'augment', 'cutout', 'duplicates',
-                   'num_crops', 'autoaugment'}
+                   'num_crops', 'autoaugment', 'device_augment'}
 _OTHER_ARGS = {'distributed'}
 
 
@@ -157,15 +223,21 @@ class DataRegime(object):
                 setting.update(override_settings)
             data_kwargs = dict(setting['data'])
             name = data_kwargs.get('name', '')
-            if name in _SYNTHETIC:  # the "transform" of a synthetic dataset is just its geometry
+            collate = None
+            if setting['transform'].get('device_augment'):
+                spec = device_augment_spec(**setting['transform'])
+                self._data = u8_dataset(input_size=setting['transform'].get('input_size'), **data_kwargs)
+                collate = AugmentCollate(spec)
+            elif name in _SYNTHETIC:  # the "transform" of a synthetic dataset is just its geometry
                 data_kwargs['input_size'] = setting['transform'].get('input_size')
                 data_kwargs['duplicates'] = setting['transform'].get('duplicates') or 1
             elif data_kwargs.get('transform') is None:
                 # real images: build the transform the regime asks for (reference data.py:101-102) -- never fall back
                 # to a bare ToTensor(), which would train on unnormalised, unaugmented, variable-size images
-                tf = {k: v for k, v in setting['transform'].items() if v is not None}
+                tf = {k: v for k, v in setting['transform'].items() if v is not None and k != 'device_augment'}
                 data_kwargs['transform'] = real_dataset_transform(**tf)
-            self._data = get_dataset(**data_kwargs)
+            if collate is None:
+                self._data = get_dataset(**data_kwargs)
             if subset_indices is not None:
                 self._data = Subset(self._data, subset_indices)
             loader_kwargs = dict(setting['loader'])
@@ -174,6 +246,11 @@ class DataRegime(object):
             if setting['other'].get('distributed', False):
                 loader_kwargs['sampler'] = DistributedSampler(self._data)
                 loader_kwargs['shuffle'] = None
+                loader_kwargs['pin_memory'] = False
+            if collate is not None:
+                loader_kwargs['collate_fn'] = collate
+                # a pin-memory thread may not allocate pinned memory while the Trainer captures a step graph (global
+                # capture mode); the batch is ~1/130 of the fp32 one, so its pageable copy costs little
                 loader_kwargs['pin_memory'] = False
             self._sampler = loader_kwargs.get('sampler', None)
             self._loader = torch.utils.data.DataLoader(self._data, **loader_kwargs)

@@ -332,17 +332,30 @@ class Runtime(object):
     input_mean = (0.485, 0.456, 0.406)
     input_std = (0.229, 0.224, 0.225)
 
-    def _input(self, x, mix=None):
+    def _input(self, x, mix=None, aug=None):
         """-> (tensor, relayout function, (N, C, H, W)).  ``mix`` (ops.Mix): MixUp / CutMix applied by the relayout
-        kernel itself (the reference mixes the fp32 batch before the forward pass, trainer.py:119-135)."""
+        kernel itself (the reference mixes the fp32 batch before the forward pass, trainer.py:119-135).  ``aug``
+        (ops.Aug): x holds the B un-augmented uint8 images and the relayout writes their B*D augmented copies."""
         if x.dtype == torch.uint8:
             if x.dim() != 4 or x.shape[-1] > 4:
                 raise B200Error('uint8 network inputs must be NHWC [N, H, W, C<=4]; got %s' % (tuple(x.shape),))
             N, H, W, C = x.shape
+            if aug is not None:
+                if mix is not None:
+                    raise B200Error('batch augmentation on the device is not combined with MixUp / CutMix')
+
+                def prep_aug(t, cpad, s2d=False, border=False, **kw):
+                    if s2d:
+                        raise B200Error('batch augmentation on the device needs the CIFAR-style 3x3 stem '
+                                        '(the space-to-depth stem layouts are not supported)')
+                    return ops.input_prep_u8_aug(t, cpad, aug, **kw)
+                return x.contiguous(), prep_aug, (N * aug.duplicates, C, H, W)
             mean = getattr(self.model, 'input_mean', self.input_mean)
             std = getattr(self.model, 'input_std', self.input_std)
             return x.contiguous(), (lambda t, cpad, **kw: ops.input_prep_u8(t, cpad, mean[:C], std[:C], mix=mix, **kw)), \
                 (N, C, H, W)
+        if aug is not None:
+            raise B200Error('batch augmentation on the device needs the uint8 NHWC images; got %s' % (x.dtype,))
         N, C, H, W = x.shape
         return x.float().contiguous(), (lambda t, cpad, **kw: ops.input_prep(t, cpad, mix=mix, **kw)), (N, C, H, W)
 
@@ -619,13 +632,13 @@ class Runtime(object):
         logits, _ = self.run_forward(x, training, False)
         return logits
 
-    def run_forward(self, x, training, want_tape, mix=None):
+    def run_forward(self, x, training, want_tape, mix=None, aug=None):
         raise NotImplementedError
 
     def run_backward(self, tape, dlogits, dl_bf16=None):
         raise NotImplementedError
 
-    def train_step(self, x, target, smooth_eps=0.0, upstream=None, mix=None):
+    def train_step(self, x, target, smooth_eps=0.0, upstream=None, mix=None, aug=None):
         """forward + mean softmax cross-entropy (label smoothing ``smooth_eps``) + backward of one batch as a straight
         sequence of library calls -- no autograd graph, no autograd worker thread, no ATen kernels: what Trainer runs
         (and captures into a CUDA graph) when the criterion is the plain CrossEntropyLoss of the reference
@@ -635,12 +648,15 @@ class Runtime(object):
         relayout kernel mixes the input and the loss is the soft-target cross-entropy against lam*onehot(target) +
         (1-lam)*onehot(target[perm]); ``smooth_eps`` is then ignored, as the reference's cross_entropy ignores it for
         soft targets (utils/cross_entropy.py:38-54).  Top-1 / top-5 still count against ``target``.
+        ``aug`` (ops.Aug): x is the uint8 NHWC batch of B images and the step trains on its B*D augmented copies
+        (row b*D + d); ``target`` then has B*D entries.
         Returns (logits, stats): logits detached, stats = fp32[3] device tensor {mean loss, top-1 %, top-5 %}."""
         if x.device.type != 'cuda':
             raise B200Error('B200 runtime needs CUDA inputs (no CPU fallback); got %s' % x.device)
-        if target.dtype != torch.int64 or target.dim() != 1 or target.shape[0] != x.shape[0] or not target.is_cuda:
+        n_rows = x.shape[0] * (aug.duplicates if aug is not None else 1)
+        if target.dtype != torch.int64 or target.dim() != 1 or target.shape[0] != n_rows or not target.is_cuda:
             raise B200Error('train_step: target must be a CUDA int64 vector with one class index per sample')
-        logits, tape = self.run_forward(x, True, True, mix=mix)
+        logits, tape = self.run_forward(x, True, True, mix=mix, aug=aug)
         pad = tape['head']['logits_pad']
         dev = pad.device
         stats = torch.empty(3, device=dev, dtype=torch.float32)
@@ -774,8 +790,8 @@ class ResNetRuntime(Runtime):
         self._head_build(m.fc)
 
     # ---- stem ---------------------------------------------------------------------------------------
-    def _stem_fwd(self, x, training, mix=None):
-        x, prep, (N, Cin, H, W) = self._input(x, mix)
+    def _stem_fwd(self, x, training, mix=None, aug=None):
+        x, prep, (N, Cin, H, W) = self._input(x, mix, aug)
         K = self.stem_conv.out_channels
         st = {}
         if self.imagenet_stem:
@@ -892,11 +908,11 @@ class ResNetRuntime(Runtime):
         return self._conv_bwd(u, dz, residual=skip)
 
     # ---- whole network ------------------------------------------------------------------------------
-    def run_forward(self, x, training, want_tape, mix=None):
+    def run_forward(self, x, training, want_tape, mix=None, aug=None):
         self._want_tape = want_tape
         if training:
             self.arena.version += 1          # running statistics change: folded inference weights become stale
-        h, stem = self._stem_fwd(x, training, mix)
+        h, stem = self._stem_fwd(x, training, mix, aug)
         saved = []
         for spec in self.blocks:
             h, s = self._block_fwd(spec, h, training)
@@ -982,8 +998,8 @@ class MobileNetRuntime(Runtime):
             return ops.dwconv_dgrad(dz, u.conv.w16, u.desc) if need_dx else None
         return self._conv_bwd(u, dz, need_dx=need_dx, residual=residual)
 
-    def _stem_fwd(self, x, training, mix=None):
-        x, prep, (N, Cin, H, W) = self._input(x, mix)
+    def _stem_fwd(self, x, training, mix=None, aug=None):
+        x, prep, (N, Cin, H, W) = self._input(x, mix, aug)
         K = self.stem_conv.out_channels
         xs = prep(x, 16, s2d=False)
         ws = torch.zeros((K, 9, 16), device=self.device, dtype=torch.bfloat16)
@@ -1008,11 +1024,11 @@ class MobileNetRuntime(Runtime):
             self.stem_g32.view(K, 9, Cin).add_(dws[:, :, :Cin])
         self._wgrad_async(stem_wgrad, u.x, dz)
 
-    def run_forward(self, x, training, want_tape, mix=None):
+    def run_forward(self, x, training, want_tape, mix=None, aug=None):
         self._want_tape = want_tape
         if training:
             self.arena.version += 1
-        h, stem = self._stem_fwd(x, training, mix)
+        h, stem = self._stem_fwd(x, training, mix, aug)
         saved = []
         for spec in self.blocks:
             xin, units = h, []

@@ -6,7 +6,8 @@
         --dataset synthetic_imagenet --dtype bfloat16 -b 256                         # config C2 (B200 path)
 
 Additions over the reference: ``--dtype bfloat16`` (compute type of the B200 kernels; parameters stay fp32
-masters in the arena), ``synthetic_*`` datasets, ``--b200 {auto,on,off}`` (auto: on for CUDA devices), and
+masters in the arena), ``synthetic_*`` datasets, ``--b200 {auto,on,off}`` (auto: on for CUDA devices),
+``--device-augment`` (batch augmentation of the CIFAR transform done in the input relayout kernel), and
 rank/world are read from the torchrun environment when ``--local_rank`` is not given.
 """
 import argparse
@@ -68,7 +69,11 @@ def build_parser():
       help='cutmix alpha coefficient - default None (with --mixup as well: CutMix with the --mixup alpha)')
     a('--duplicates', default=1, type=int, help='number of augmentations over single example')
     a('--chunk-batch', default=1, type=int, help='chunk batch size for multiple passes (training)')
-    a('--cutout', action='store_true', default=False, help='cutout augmentations (ignored for synthetic data)')
+    a('--cutout', action='store_true', default=False,
+      help='cutout augmentations (ignored for synthetic data unless --device-augment)')
+    a('--device-augment', action='store_true', default=False,
+      help='CIFAR training: ship uint8 images and per-copy draws, and crop / flip / cutout the --duplicates copies '
+           'inside the input relayout on the GPU')
     a('--autoaugment', action='store_true', default=False, help='autoaugment policies (ignored for synthetic data)')
     a('--grad-clip', default=-1, type=float, help='maximum grad norm value, -1 for none')
     a('--loss-scale', default=1, type=float, help='loss scale for mixed precision training')
@@ -233,7 +238,8 @@ def main_worker(args):
                       'input_size': args.input_size, 'batch_size': args.batch_size, 'shuffle': True,
                       'num_workers': args.workers, 'pin_memory': True, 'drop_last': True,
                       'distributed': args.distributed, 'duplicates': args.duplicates,
-                      'autoaugment': args.autoaugment, 'cutout': {'holes': 1, 'length': 16} if args.cutout else None}
+                      'autoaugment': args.autoaugment, 'cutout': {'holes': 1, 'length': 16} if args.cutout else None,
+                      'device_augment': args.device_augment}
     if hasattr(model, 'sampled_data_regime'):
         probs, configs = zip(*model.sampled_data_regime)
         train_data = SampledDataRegime([DataRegime(None, defaults={**train_defaults, **cfg}) for cfg in configs],

@@ -479,6 +479,38 @@ def input_prep_u8(x_nhwc_u8, cpad, mean, std, s2d=False, border=False, mix=None,
     return out
 
 
+class Aug(object):
+    """Device-side draws of one batch-augmentation step (utils/augment.py): ``params`` int16 [N*D, 3 + 4*holes] rows
+    {oy, ox, flip, y1, y2, x1, x2, ...}, ``lut`` fp32 [C, 256] (ToTensor + Normalize of each uint8 value), ``duplicates``
+    D, ``pad`` the crop padding.  The kernel reads params at run time, so a captured graph follows new draws in place."""
+    __slots__ = ('params', 'lut', 'duplicates', 'pad')
+
+    def __init__(self, params, lut, duplicates, pad):
+        self.params, self.lut, self.duplicates, self.pad = params, lut, int(duplicates), int(pad)
+
+    @property
+    def holes(self):
+        return (self.params.shape[-1] - 3) // 4
+
+
+def input_prep_u8_aug(x_nhwc_u8, cpad, aug, out=None):
+    """uint8 NHWC [N,H,W,C] -> bf16 NHWC [N*D, H, W, cpad]: the D augmented copies of every image (crop, flip, Cutout)
+    normalised through aug.lut, row n*D + d = copy d of image n."""
+    _chk(x_nhwc_u8, torch.uint8, "x"); _chk(aug.params, torch.int16, "aug params"); _chk(aug.lut, torch.float32, "lut")
+    N, H, W, C = x_nhwc_u8.shape
+    D = aug.duplicates
+    if aug.params.dim() != 2 or aug.params.shape[0] != N * D or (aug.params.shape[1] - 3) % 4 != 0 \
+            or tuple(aug.lut.shape) != (C, 256):
+        raise _l.B200Error("input_prep_u8_aug: params must be int16 [N*D, 3+4*holes] and lut fp32 [C, 256]; got %s, %s"
+                           % (tuple(aug.params.shape), tuple(aug.lut.shape)))
+    out = _prep_out(N * D, H, W, cpad, False, False, x_nhwc_u8.device, out)
+    with _T('input_prep', 0, x_nhwc_u8.numel() + 2 * aug.params.numel() + 2 * out.numel()):
+        _l.check(_l.load().b200_input_prep_u8_aug(x_nhwc_u8.data_ptr(), N, D, C, H, W, cpad, aug.pad,
+                                                  aug.lut.data_ptr(), aug.params.data_ptr(), aug.holes,
+                                                  out.data_ptr(), _stream()), "b200_input_prep_u8_aug")
+    return out
+
+
 def weight_transpose(w, out=None):
     """bf16 [K,T,C] -> [C,T,K]."""
     K, T, C = w.shape

@@ -17,6 +17,10 @@ SURVEY.md section 2.3 C1/C2), and the per-tensor unscale / clip loops of the ref
 
 MixUp / CutMix (``mixup`` / ``cutmix``, trainer.py:44-51,119-138): drawn on the host per training chunk by
 utils/mixup.py; on the fused B200 path the input relayout and loss kernels do the mixing (see ``_upload_mix``).
+
+Batch augmentation on the device (a loader yielding utils.augment.AugmentedBatch, data.py ``device_augment``): on the
+fused B200 path the stem relayout kernel writes the B*D augmented copies from the uint8 images and their draws; every
+other path trains on ``AugmentedBatch.apply()``, the same fp32 batch.  The meters count B*D samples.
 """
 import logging
 import os
@@ -31,6 +35,7 @@ from torch.nn.utils import clip_grad_norm_
 
 from .lib import B200Error, MIX_CUTMIX, MIX_MIXUP
 from .utils import regularization
+from .utils.augment import AugmentedBatch
 from .utils.meters import AverageMeter, accuracy
 from .utils.mixup import CutMix, MixUp
 
@@ -77,31 +82,39 @@ def _cuda_prefetch(loader, device, dtype):
     The copies land in a ring of three persistent device buffers per (shape, dtype): no caching-allocator traffic per
     step (a fresh 154 MB tensor per batch that is handed across streams made the allocator stall now and then)."""
     copy_stream = torch.cuda.Stream(device=device)
-    ring = {}          # (shape, dtype) of x and y -> [[x_buf, y_buf, consumed_event or None], ...]
+    ring = {}          # (shape, dtype) of x and y -> [[x_buf, y_buf, consumed_event or None, draws_buf], ...]
     turn = {}
 
     def stage(inputs, target):
-        x_dtype = inputs.dtype if inputs.dtype == torch.uint8 else dtype     # uint8 image batches stay uint8
-        key = (tuple(inputs.shape), x_dtype, tuple(target.shape), target.dtype)
+        # an AugmentedBatch: its uint8 images and its draw table travel together, in the same slot
+        spec = inputs.spec if isinstance(inputs, AugmentedBatch) else None
+        draws = inputs.params if spec is not None else None
+        x = inputs.images if spec is not None else inputs
+        x_dtype = x.dtype if x.dtype == torch.uint8 else dtype     # uint8 image batches stay uint8
+        key = (tuple(x.shape), x_dtype, tuple(target.shape), target.dtype,
+               tuple(draws.shape) if draws is not None else None)
         slots = ring.setdefault(key, [])
         k = turn.get(key, 0)
         turn[key] = (k + 1) % 3
         if len(slots) <= k:
-            slots.append([torch.empty(inputs.shape, device=device, dtype=x_dtype),
-                          torch.empty(target.shape, device=device, dtype=target.dtype), None])
+            slots.append([torch.empty(x.shape, device=device, dtype=x_dtype),
+                          torch.empty(target.shape, device=device, dtype=target.dtype), None,
+                          torch.empty(draws.shape, device=device, dtype=draws.dtype) if draws is not None else None])
         slot = slots[k]
         with torch.cuda.stream(copy_stream):
             if slot[2] is not None:
                 copy_stream.wait_event(slot[2])            # the step that read this slot has been enqueued AND has run
-            slot[0].copy_(inputs, non_blocking=True)
+            slot[0].copy_(x, non_blocking=True)
             slot[1].copy_(target, non_blocking=True)
+            if draws is not None:
+                slot[3].copy_(draws, non_blocking=True)
             ready = torch.cuda.Event()
             ready.record(copy_stream)
-        return slot, ready
+        return slot, ready, spec
 
-    def hand_over(slot, ready):
+    def hand_over(slot, ready, spec):
         torch.cuda.current_stream(device).wait_event(ready)
-        return slot[0], slot[1]
+        return (slot[0] if spec is None else AugmentedBatch(slot[0], slot[3], spec)), slot[1]
 
     def release(slot):
         ev = torch.cuda.Event()
@@ -141,6 +154,7 @@ class Trainer(object):
         self.cutmix = cutmix
         self.last_mix = None                   # the MixUp / CutMix module of the latest training chunk (its draws)
         self._mix_dev, self._mix_ring, self._mix_turn = {}, {}, 0
+        self._aug_luts = {}                    # (normalisation, C, device) -> fp32 [C, 256] device LUT of AugmentedBatch
         self.grad_scale = None
         self.loss_scale = loss_scale
         self.adapt_grad_norm = adapt_grad_norm
@@ -257,19 +271,22 @@ class Trainer(object):
             self._graph_static_ok = ok
         return self._graph_static_ok
 
-    def graphed_forward_backward(self, inputs, target, mix=None):
+    def graphed_forward_backward(self, inputs, target, mix=None, aug=None):
         """Forward + criterion + backward of one device-resident batch through a captured CUDA graph.
         Returns (logits, loss, stats) -- detached device tensors; stats = fp32[3] {loss, top-1 %, top-5 %} when the fused
         loss kernel computed them, else None -- or None when this call has to run eagerly (warm-up steps of
         a new shape, unsupported configuration).  Gradients land in the arena exactly as in the eager path.
         ``mix`` (ops.Mix, from _upload_mix): the step mixes its input; the graph reads the permutation, lambda and box
-        from their persistent device buffers, so every replay uses the values uploaded for that step."""
+        from their persistent device buffers, so every replay uses the values uploaded for that step.
+        ``aug`` (ops.Aug, from _device_aug): the step augments its uint8 images on the device; the graph reads the draws
+        from a static buffer refreshed like the input, so every replay uses that step's draws."""
         if not self._graph_eligible() or not inputs.is_cuda:
             return None
         # loss / gradient scales are NOT part of the key: they reach the kernels through a device scalar; neither are
         # the mixing draws (device buffers) -- only the kind of mixing
         key = (tuple(inputs.shape), inputs.dtype, tuple(target.shape), target.dtype, self._model.training,
-               mix.kind if mix is not None else 0)
+               mix.kind if mix is not None else 0,
+               (tuple(aug.params.shape), aug.duplicates, aug.pad, aug.lut.data_ptr()) if aug is not None else None)
         st = self._graphs.get(key)
         if st is None:
             st = self._graphs[key] = {'seen': 0, 'graph': None}
@@ -278,7 +295,7 @@ class Trainer(object):
             if st['seen'] <= 2:
                 return None                       # eager warm-up (library handles, allocator, autotuned state)
             try:
-                self._capture(st, inputs, target, mix)
+                self._capture(st, inputs, target, mix, aug)
             except Exception as e:  # noqa: BLE001  -- keep training eagerly if capture is impossible here
                 if self.b200.grad_bucket_hook is not None:
                     # NCCL inside the capture is the likely culprit: fall back to ONE flat all-reduce after the graph
@@ -293,17 +310,20 @@ class Trainer(object):
                 return None
         st['x'].copy_(inputs, non_blocking=True)
         st['y'].copy_(target, non_blocking=True)
+        if aug is not None:
+            st['aug'].copy_(aug.params, non_blocking=True)
         self._upstream()                          # refresh the device scalar if a scale changed
         st['graph'].replay()
         self.graph_replays += 1
         self.graph_replayed_launches += st['launches']
         return st['out'].detach(), st['loss'].detach(), st['stats']
 
-    def _capture(self, st, inputs, target, mix=None):
-        from . import lib
+    def _capture(self, st, inputs, target, mix=None, aug=None):
+        from . import lib, ops
         x_s, y_s = torch.empty_like(inputs), torch.empty_like(target)
         x_s.copy_(inputs)
         y_s.copy_(target)
+        aug_s = ops.Aug(aug.params.clone(), aug.lut, aug.duplicates, aug.pad) if aug is not None else None
         if self._graph_pool is None:
             self._graph_pool = torch.cuda.graph_pool_handle()
         graph = torch.cuda.CUDAGraph()
@@ -323,13 +343,14 @@ class Trainer(object):
         with torch.cuda.graph(graph, pool=self._graph_pool, stream=self._capture_stream, capture_error_mode=mode):
             stats = None
             if eps is not None:            # the whole step is library calls: nothing of autograd inside the graph
-                out, stats = self.b200.train_step(x_s, y_s, eps, up, mix=mix)
+                out, stats = self.b200.train_step(x_s, y_s, eps, up, mix=mix, aug=aug_s)
                 loss = stats[0]
             else:
                 out = self.model(x_s)
                 loss = self.criterion(out, y_s)
                 torch.autograd.backward(loss, grad_tensors=[up])
-        st.update(graph=graph, x=x_s, y=y_s, out=out, loss=loss, stats=stats, launches=lib.launch_count() - n0)
+        st.update(graph=graph, x=x_s, y=y_s, aug=aug_s.params if aug_s is not None else None, out=out, loss=loss,
+                  stats=stats, launches=lib.launch_count() - n0)
 
     def release_graphs(self):
         """Drop every captured step (call before tearing the process group down: graphs that captured NCCL all-reduces
@@ -396,6 +417,15 @@ class Trainer(object):
         if training:
             self.optimizer.zero_grad()
             self.optimizer.update(self.epoch, self.training_steps)
+        aug = None
+        if isinstance(inputs_batch, AugmentedBatch):
+            if training and self.b200 is not None and chunk_batch == 1 and not average_output \
+                    and 'cuda' in str(self.device) and self._hooks_static() and self._plain_ce_eps() is not None \
+                    and target_batch.dtype == torch.long and target_batch.dim() == 1:
+                aug = self._device_aug(inputs_batch)
+                inputs_batch = inputs_batch.images
+            else:
+                inputs_batch = inputs_batch.apply()     # the same fp32 batch the fused relayout would compute
 
         chunks = zip(inputs_batch.chunk(chunk_batch, dim=0), target_batch.chunk(chunk_batch, dim=0))
         for i, (inputs, target) in enumerate(chunks):
@@ -412,8 +442,10 @@ class Trainer(object):
                 and self._hooks_static() and self._plain_ce_eps() is not None \
                 and target.dtype == torch.long and target.dim() == 1
             mix = self._upload_mix(mixer, inputs) if (mixer is not None and fused) else None
+            if aug is not None and not fused:
+                raise B200Error('batch augmentation on the device: the fused training step is not available here')
             if training and chunk_batch == 1 and not average_output and (mixer is None or mix is not None):
-                replayed = self.graphed_forward_backward(inputs, target, mix)
+                replayed = self.graphed_forward_backward(inputs, target, mix, aug)
                 if replayed is not None:
                     outputs.append(replayed[0])
                     if replayed[2] is not None:
@@ -424,7 +456,8 @@ class Trainer(object):
             if fused:
                 # eager form of the captured step (warm-up iterations of a new shape, B200_CUDA_GRAPH=0)
                 self.optimizer.pre_forward()
-                output, stats = self.b200.train_step(inputs, target, self._plain_ce_eps(), self._upstream(), mix=mix)
+                output, stats = self.b200.train_step(inputs, target, self._plain_ce_eps(), self._upstream(), mix=mix,
+                                                     aug=aug)
                 outputs.append(output)
                 self.optimizer.pre_backward()
                 continue
@@ -538,6 +571,31 @@ class Trainer(object):
         ring[k][1] = ev
         return ops.Mix(dev[:B], dev[B:].view(torch.int32), kind)
 
+    # ------------------------------------------------------------------ batch augmentation on the device
+    def _device_aug(self, batch):
+        """-> ops.Aug over the batch's draws on the training device and a persistent device LUT of its normalisation
+        (one per statistics, channel count and device, so that a captured graph keeps reading a live tensor)."""
+        from . import ops
+        spec = batch.spec
+        device = torch.device(self.device)
+        C = batch.images.shape[-1]
+        key = (tuple(spec.normalize['mean']), tuple(spec.normalize['std']), C, str(device))
+        lut = self._aug_luts.get(key)
+        if lut is None:
+            lut = self._aug_luts[key] = spec.lut(C).to(device)
+        params = batch.params.to(device, non_blocking=True).reshape(-1, batch.params.shape[-1])
+        return ops.Aug(params, lut, spec.duplicates, spec.padding)
+
+    def _check_device_augment(self, training, average_output):
+        if average_output:
+            raise NotImplementedError('batch augmentation on the device with average_output: the outputs would be '
+                                      'averaged over the duplicates; use the [B, D, C, H, W] loader instead')
+        if training and (self.mixup is not None or self.cutmix is not None):
+            raise NotImplementedError('batch augmentation on the device is not combined with mixup / cutmix')
+        if training and self.adapt_grad_norm is not None:
+            raise NotImplementedError('batch augmentation on the device with adapt_grad_norm: the per-copy gradient '
+                                      'norms need the [B, D, C, H, W] batch; use the host-side loader instead')
+
     # ------------------------------------------------------------------ epoch loop
     def forward(self, data_loader, num_steps=None, training=False, average_output=False, chunk_batch=1):
         meters = {name: AverageMeter() for name in _METERS}
@@ -574,7 +632,9 @@ class Trainer(object):
                 meters['prec5'].update(float(v[2]), n)
 
         for i, (inputs, target) in enumerate(batches):
-            duplicates = inputs.dim() > 4  # B x D x C x H x W
+            if isinstance(inputs, AugmentedBatch):
+                self._check_device_augment(training, average_output)
+            duplicates = not isinstance(inputs, AugmentedBatch) and inputs.dim() > 4  # B x D x C x H x W
             if training and duplicates and self.adapt_grad_norm is not None and i % self.adapt_grad_norm == 0:
                 per_copy = sum(float(self._grad_norm(inputs.select(1, j), target)) for j in range(inputs.size(1)))
                 per_copy /= inputs.size(1)
@@ -588,7 +648,7 @@ class Trainer(object):
                                                      expand_target=not average_output)
             output, loss, grad = self._step(inputs, target, training=training, average_output=average_output,
                                             chunk_batch=chunk_batch)
-            n = inputs.size(0)
+            n = inputs.rows if isinstance(inputs, AugmentedBatch) else inputs.size(0)
             if torch.is_tensor(loss):              # fused statistics: asynchronous read-back
                 if pinned is None:
                     pinned = torch.empty((ring, 3), dtype=torch.float32).pin_memory()

@@ -190,6 +190,18 @@ int b200_input_prep_mix(const float* x_nchw, int N, int C, int H, int W, int Cpa
 int b200_input_prep_u8_mix(const uint8_t* x_nhwc, int N, int C, int H, int W, int Cpad, int mode, const float* scale_host,
                            const float* bias_host, const long long* perm, const b200_mix_params* params, int kind,
                            void* out, b200_stream_t stream);
+/* Batch augmentation (the reference's --duplicates with RandomCrop(padding) + RandomHorizontalFlip + ToTensor + Normalize
+ * [+ Cutout], preprocess.py:44-54,105-112,159-161,185-227) fused into the mode-0 relayout: uint8 NHWC images
+ * x_nhwc [N][H][W][C] (C <= 4) -> out bf16 [N*D][H][W][Cpad].  Output row n' is copy n' % D of image n' / D with the
+ * DEVICE draw row params[n'] = int16 {oy, ox, flip, y1, y2, x1, x2, ...} (3 + 4*holes entries per row):
+ *   c' = flip ? W-1-c : c,  sy = r + oy - pad,  sx = c' + ox - pad,
+ *   u  = (0 <= sy < H && 0 <= sx < W) ? x[n'/D][sy][sx][ch] : 0,   v = lut[ch][u]  (DEVICE fp32 [C][256]),
+ *   v  = v * 0.f when y1 <= r < y2 and x1 <= c < x2 for any box, then one rounding to bf16.
+ * With lut[ch][u] = ((float)u / 255 - mean[ch]) / std[ch] in fp32 (torchvision's ToTensor + Normalize) the output is
+ * b200_input_prep of the reference's augmented fp32 batch, bit for bit.  Any draw values are memory-safe; the kernel
+ * reads them at run time, so a captured CUDA graph follows each step's draws. */
+int b200_input_prep_u8_aug(const uint8_t* x_nhwc, int N, int D, int C, int H, int W, int Cpad, int pad, const float* lut,
+                           const int16_t* params, int holes, void* out, b200_stream_t stream);
 /* bf16 [K][T][C] -> bf16 [C][T][K] (dgrad weight layout), multi-tensor: n tensors described by
  * device arrays. */
 int b200_weight_transpose(const void* src, void* dst, int K, int T, int C, b200_stream_t stream);
