@@ -14,7 +14,6 @@
 // The workspace must be zero before first use and must not be shared by concurrent streams.
 #include "common.cuh"
 #include "host.h"
-#include <stdlib.h>
 
 namespace b200 {
 
@@ -40,9 +39,8 @@ static inline int reduce_blocks(long long M, int C, const RowMap& rm, int reside
   long long want = (iters + 7) / 8;          // >= 8 row-iterations per block
   long long cap = 1200000LL / (2 * C);       // bound the number of fp64 atomics (blocks * 2C)
   if (cap < sm_count()) cap = sm_count();
-  static const int env_per_sm = getenv("B200_BN_REDUCE_BLOCKS_PER_SM") ? atoi(getenv("B200_BN_REDUCE_BLOCKS_PER_SM")) : 0;
-  const int per_sm = env_per_sm > 0 ? env_per_sm : resident_per_sm;   // one full wave of fat blocks, no tail wave
-  if (cap > per_sm * sm_count()) cap = per_sm * sm_count();
+  // one full wave of fat blocks, no tail wave
+  if (cap > resident_per_sm * sm_count()) cap = resident_per_sm * sm_count();
   if (want > cap) want = cap;
   if (want < 1) want = 1;
   return (int)want;
@@ -51,8 +49,7 @@ static inline int reduce_blocks(long long M, int C, const RowMap& rm, int reside
 static inline int partial_blocks(long long M, const RowMap& rm, int resident_per_sm) {
   long long iters = (M + rm.rows_per_iter - 1) / rm.rows_per_iter;
   long long want = (iters + 3) / 4;
-  static const int env_per_sm = getenv("B200_BN_REDUCE_BLOCKS_PER_SM") ? atoi(getenv("B200_BN_REDUCE_BLOCKS_PER_SM")) : 0;
-  long long cap = (long long)(env_per_sm > 0 ? env_per_sm : resident_per_sm) * sm_count();
+  long long cap = (long long)resident_per_sm * sm_count();
   if (cap > kMaxPartialBlocks) cap = kMaxPartialBlocks;
   if (want > cap) want = cap;
   if (want < 1) want = 1;
@@ -137,7 +134,6 @@ __global__ void __launch_bounds__(kBnThreads) bn_stats_kernel(
     const float* __restrict__ gamma, const float* __restrict__ beta, float eps, float momentum, float* running_mean,
     float* running_var, long long* num_batches_tracked, float* mean, float* invstd, float* scale, float* shift,
     double* accum, unsigned* ticket) {
-  pdl_wait();
   const int t = threadIdx.x;
   const bool active = t < rows_per_iter * cv;
   const int r0 = t / cv, v = t - r0 * cv;
@@ -212,7 +208,6 @@ __global__ void __launch_bounds__(kBnThreads) bn_finalize_kernel(
     long long M, int C, const float* __restrict__ gamma, const float* __restrict__ beta, float eps, float momentum,
     float* running_mean, float* running_var, long long* num_batches_tracked, float* mean, float* invstd, float* scale,
     float* shift, double* accum) {
-  pdl_wait();
   // 16 lanes per channel, one per accumulator replica (a serial loop over the replicas was a chain of L2 round
   // trips in a kernel that sits on the critical path between the convolution and the BN apply)
   static_assert(kReplicas == 16, "lane mapping below assumes 16 replicas");
@@ -258,13 +253,11 @@ __global__ void __launch_bounds__(kBnThreads) bn_finalize_kernel(
     *num_batches_tracked += 1;
 }
 __global__ void bn_bump_kernel(long long* nbt) {
-  pdl_wait();
   *nbt += 1;
 }
 
 __global__ void bn_eval_coeffs_kernel(int C, const float* gamma, const float* beta, const float* rm, const float* rv,
                                       float eps, float* scale, float* shift) {
-  pdl_wait();
   const int c = blockIdx.x * blockDim.x + threadIdx.x;
   if (c >= C) return;
   const float istd = rsqrtf(rv[c] + eps);
@@ -299,7 +292,6 @@ __global__ void __launch_bounds__(kBnThreads) bn_apply_kernel(
     const float* __restrict__ scale, const float* __restrict__ shift, const __nv_bfloat16* __restrict__ res,
     const float* __restrict__ scale2, const float* __restrict__ shift2, int act, __nv_bfloat16* __restrict__ y,
     uint8_t* __restrict__ act_mask) {
-  pdl_wait();
   const int t = threadIdx.x;
   if (t >= rows_per_iter * cv) return;
   const int r0 = t / cv, v = t - r0 * cv;
@@ -380,69 +372,14 @@ __device__ __forceinline__ void loadfv(const float* p, float (&f)[VEC]) {
   }
 }
 
-// Gradient arriving at a pre-pool pixel of a 3x3 / stride 2 / pad 1 max pool, gathered from the POOLED gradient dp
-// [N, OH, OW, C] through the argmax bytes (pool.cu) -- the stem's BN backward reads dp + one byte per pooled element
-// instead of a materialised [N, H, W, C] gradient tensor (saves the max-pool backward kernel: one write and two reads
-// of the largest activation of the network).  A pixel lies in at most 2 x 2 windows; fp32 sum, no rounding.
-struct PoolGeom {
-  int H, W, OH, OW;
-};
-template <int VEC>
-__device__ __forceinline__ void pool_gather(const __nv_bfloat16* __restrict__ dp, const uint8_t* __restrict__ amax,
-                                            long long row, long long col, int C, const PoolGeom& pg, float (&g)[VEC]) {
-  const unsigned r32 = (unsigned)row;                 // the host checks N*H*W < 2^31: 32-bit div/mod
-  const int w = (int)(r32 % (unsigned)pg.W);
-  const unsigned t = r32 / (unsigned)pg.W;
-  const int h = (int)(t % (unsigned)pg.H);
-  const long long n = t / (unsigned)pg.H;
-  const int p_lo = h >> 1, q_lo = w >> 1;
-  uint32_t ab[4][VEC / 4];
-  uint32_t gr[4][VEC / 2];
-  int want[4];
-  bool ok[4];
-#pragma unroll
-  for (int j = 0; j < 4; ++j) {
-    const int p = p_lo + (j >> 1), q = q_lo + (j & 1);
-    ok[j] = p <= ((h + 1) >> 1) && q <= ((w + 1) >> 1) && p < pg.OH && q < pg.OW;
-    want[j] = (h - (2 * p - 1)) * 3 + (w - (2 * q - 1));
-    if (ok[j]) {
-      const long long o = ((n * pg.OH + p) * pg.OW + q) * C + col;
-      if constexpr (VEC == 8) {
-        const uint2 a = __ldg(reinterpret_cast<const uint2*>(amax + o));
-        const uint4 d = __ldg(reinterpret_cast<const uint4*>(dp + o));
-        ab[j][0] = a.x; ab[j][1] = a.y;
-        gr[j][0] = d.x; gr[j][1] = d.y; gr[j][2] = d.z; gr[j][3] = d.w;
-      } else {
-        ab[j][0] = __ldg(reinterpret_cast<const uint32_t*>(amax + o));
-        const uint2 d = __ldg(reinterpret_cast<const uint2*>(dp + o));
-        gr[j][0] = d.x; gr[j][1] = d.y;
-      }
-    }
-  }
-#pragma unroll
-  for (int i = 0; i < VEC; ++i) g[i] = 0.f;
-#pragma unroll
-  for (int j = 0; j < 4; ++j) {
-    if (!ok[j]) continue;
-#pragma unroll
-    for (int i = 0; i < VEC; ++i) {
-      const int b = (ab[j][i >> 2] >> (8 * (i & 3))) & 0xff;
-      const float2 g2 = unpack_bf16x2(gr[j][i >> 1]);
-      if (b == want[j]) g[i] += (i & 1) ? g2.y : g2.x;
-    }
-  }
-}
-
 // ---- backward reduce: dbeta = sum g, dgamma = sum g * xhat ------------------------------------------
-// SRC: activation argument 0 recomputed from z, 1 = y, 2 = mask bits; 3 = like 0, with the gradient gathered from a
-// max-pooled gradient (dy = dp, amask = argmax bytes, pool_gather above)
+// SRC: activation argument 0 recomputed from z, 1 = y, 2 = mask bits
 template <int VEC, int ROWS, int MINB, int SRC>
 __global__ void __launch_bounds__(kBnThreads, MINB) bn_bwd_reduce_kernel(
     const __nv_bfloat16* __restrict__ dy, const __nv_bfloat16* __restrict__ y, const uint8_t* __restrict__ amask,
     const __nv_bfloat16* __restrict__ z, long long M, int C, int cv, int rows_per_iter, int act,
     const float* __restrict__ mean, const float* __restrict__ invstd, const float* __restrict__ gamma,
-    const float* __restrict__ beta, float* __restrict__ partial, const PoolGeom pg) {
-  pdl_wait();
+    const float* __restrict__ beta, float* __restrict__ partial) {
   const int t = threadIdx.x;
   const bool active = t < rows_per_iter * cv;
   const int r0 = t / cv, v = t - r0 * cv;
@@ -457,7 +394,7 @@ __global__ void __launch_bounds__(kBnThreads, MINB) bn_bwd_reduce_kernel(
   if (active) {
     float mu[VEC], sc[VEC], sh[VEC];
     loadfv<VEC>(mean + v * VEC, mu);
-    if ((SRC == 0 || SRC == 3) && act != B200_ACT_NONE) {
+    if (SRC == 0 && act != B200_ACT_NONE) {
       float is[VEC];
       loadfv<VEC>(invstd + v * VEC, is);
       if (gamma) loadfv<VEC>(gamma + v * VEC, sc);
@@ -481,7 +418,7 @@ __global__ void __launch_bounds__(kBnThreads, MINB) bn_bwd_reduce_kernel(
         const long long rr = r + (long long)u * rstep;
         ok[u] = rr < row_end;
         if (ok[u]) {
-          if (SRC != 3) rd[u] = ldv(dy + rr * C + col, (RawVec<VEC>*)nullptr);
+          rd[u] = ldv(dy + rr * C + col, (RawVec<VEC>*)nullptr);
           rz[u] = ldv(z + rr * C + col, (RawVec<VEC>*)nullptr);
           if (SRC == 1) ry[u] = ldv(y + rr * C + col, (RawVec<VEC>*)nullptr);
         }
@@ -490,8 +427,7 @@ __global__ void __launch_bounds__(kBnThreads, MINB) bn_bwd_reduce_kernel(
       for (int u = 0; u < ROWS; ++u) {
         if (!ok[u]) continue;
         float da[VEC], za[VEC], ya[VEC];
-        if (SRC == 3) pool_gather<VEC>(dy, amask, r + (long long)u * rstep, col, C, pg, da);
-        else unpackv(rd[u], da);
+        unpackv(rd[u], da);
         unpackv(rz[u], za);
         if (SRC == 1) unpackv(ry[u], ya);
 #pragma unroll
@@ -531,7 +467,6 @@ __global__ void __launch_bounds__(kBnThreads, MINB) bn_bwd_reduce_kernel(
 __global__ void __launch_bounds__(kBnThreads) bn_bwd_reduce_final_kernel(const float* __restrict__ partial, int nblocks,
                                                                           int C, float* __restrict__ sums,
                                                                           float* dgamma_acc, float* dbeta_acc) {
-  pdl_wait();
   __shared__ double red[64][5];
   const int lane_o = threadIdx.x & 3, grp = threadIdx.x >> 2;
   const int o = blockIdx.x * 4 + lane_o;
@@ -568,8 +503,7 @@ __global__ void __launch_bounds__(kBnThreads, MINB) bn_bwd_dx_kernel(
     const __nv_bfloat16* __restrict__ z, long long M, int C, int cv, int rows_per_iter, int act,
     const float* __restrict__ mean, const float* __restrict__ invstd, const float* __restrict__ gamma,
     const float* __restrict__ beta, const float* __restrict__ sums, __nv_bfloat16* __restrict__ dz,
-    __nv_bfloat16* __restrict__ g_out, const PoolGeom pg) {
-  pdl_wait();
+    __nv_bfloat16* __restrict__ g_out) {
   const int t = threadIdx.x;
   if (t >= rows_per_iter * cv) return;
   const int r0 = t / cv, v = t - r0 * cv;
@@ -611,7 +545,7 @@ __global__ void __launch_bounds__(kBnThreads, MINB) bn_bwd_dx_kernel(
       const long long rr = r + (long long)u * rstep;
       ok[u] = rr < row_end;
       if (ok[u]) {
-        if (SRC != 3) rd[u] = ldv(dy + rr * C + col, (RawVec<VEC>*)nullptr);
+        rd[u] = ldv(dy + rr * C + col, (RawVec<VEC>*)nullptr);
         rz[u] = ldv(z + rr * C + col, (RawVec<VEC>*)nullptr);
         if (SRC == 1) ry[u] = ldv(y + rr * C + col, (RawVec<VEC>*)nullptr);
       }
@@ -621,8 +555,7 @@ __global__ void __launch_bounds__(kBnThreads, MINB) bn_bwd_dx_kernel(
       if (!ok[u]) continue;
       const long long rr = r + (long long)u * rstep;
       float da[VEC], za[VEC], ya[VEC];
-      if (SRC == 3) pool_gather<VEC>(dy, amask, rr, col, C, pg, da);
-      else unpackv(rd[u], da);
+      unpackv(rd[u], da);
       unpackv(rz[u], za);
       if (SRC == 1) unpackv(ry[u], ya);
 #pragma unroll
@@ -647,11 +580,6 @@ static inline RowMap make_rowmap_v(int C) {
   return m;
 }
 
-// tuning knob (measured with tools/bn_bench.py): rows in flight per thread x resident blocks per SM
-static int bwd_variant() {
-  static const int v = getenv("B200_BN_BWD_VARIANT") ? atoi(getenv("B200_BN_BWD_VARIANT")) : 0;
-  return v;
-}
 static int check_c(int C, const char* who) {
   B200_REQUIRE(C > 0 && C % 8 == 0 && C <= kBnMaxC, B200_ERR_UNSUPPORTED,
                "%s: C=%d must be a multiple of 8 and <= %d", who, C, kBnMaxC);
@@ -737,26 +665,26 @@ extern "C" int b200_bn_apply(const void* z, long long M, int C, const float* sca
   return B200_OK;
 }
 
-// pooled: dy is the gradient of a 3x3/s2/p1 max pool's OUTPUT and act_mask holds the argmax bytes (SRC 3)
-static int bn_bwd_reduce_impl(const void* dy, const void* y, const uint8_t* act_mask, const void* z, long long M, int C,
-                              int act, const float* mean, const float* invstd, const float* gamma, const float* beta,
-                              float* sums, float* dgamma_acc, float* dbeta_acc, float* workspace, b200_stream_t stream_,
-                              bool pooled, const PoolGeom pg) {
+// Launch shape of the backward kernels (VEC channels per thread, ROWS rows in flight per thread, MINB resident blocks
+// per SM): (4, 4, 4) up to C = 1024, (8, 2, 3) above.
+extern "C" int b200_bn_bwd_reduce(const void* dy, const void* y, const uint8_t* act_mask, const void* z, long long M,
+                                  int C, int act,
+                                  const float* mean, const float* invstd, const float* gamma, const float* beta,
+                                  float* sums, float* dgamma_acc, float* dbeta_acc, float* workspace,
+                                  b200_stream_t stream_) {
   int rc = check_c(C, "bn_bwd_reduce");
   if (rc) return rc;
   B200_REQUIRE(dy && z && mean && invstd && sums && workspace && M > 0, B200_ERR_INVALID, "bn_bwd_reduce: bad argument");
   // activation-argument source: 2 = mask bits, 1 = y, 0 = recomputed from z (or no activation)
-  const int src = pooled ? 3 : ((act == B200_ACT_NONE) ? 0 : (act_mask != nullptr ? 2 : (y != nullptr ? 1 : 0)));
+  const int src = (act == B200_ACT_NONE) ? 0 : (act_mask != nullptr ? 2 : (y != nullptr ? 1 : 0));
 #define B200_RED_ARGS(VEC)                                                                                     \
   (const __nv_bfloat16*)dy, (const __nv_bfloat16*)y, act_mask, (const __nv_bfloat16*)z, M, C, rm.cv,           \
-      rm.rows_per_iter, act, mean, invstd, gamma, beta, partial, pg
+      rm.rows_per_iter, act, mean, invstd, gamma, beta, partial
 #define B200_LAUNCH_RED(VEC, ROWS, MINB)                                                                       \
   do {                                                                                                         \
     const RowMap rm = make_rowmap_v<VEC>(C);                                                                   \
     blocks = partial_blocks(M, rm, MINB);                                                                      \
-    if (src == 3)                                                                                              \
-      b200::launch(bn_bwd_reduce_kernel<VEC, ROWS, MINB, 3>, blocks, kBnThreads, 0, stream, B200_RED_ARGS(VEC));         \
-    else if (src == 2)                                                                                         \
+    if (src == 2)                                                                                              \
       b200::launch(bn_bwd_reduce_kernel<VEC, ROWS, MINB, 2>, blocks, kBnThreads, 0, stream, B200_RED_ARGS(VEC));         \
     else if (src == 1)                                                                                         \
       b200::launch(bn_bwd_reduce_kernel<VEC, ROWS, MINB, 1>, blocks, kBnThreads, 0, stream, B200_RED_ARGS(VEC));         \
@@ -766,18 +694,10 @@ static int bn_bwd_reduce_impl(const void* dy, const void* y, const uint8_t* act_
   cudaStream_t stream = (cudaStream_t)stream_;
   float* partial = workspace + kAccumFloats;
   int blocks = 0;
-  if (pooled) {                 // the gather needs registers: two rows in flight instead of four
-    B200_LAUNCH_RED(4, 2, 4);
-  } else if (C > 1024) {
+  if (C > 1024)
     B200_LAUNCH_RED(8, 2, 3);
-  } else {
-    switch (bwd_variant()) {
-      case 1: B200_LAUNCH_RED(4, 2, 5); break;
-      case 2: B200_LAUNCH_RED(4, 8, 3); break;
-      case 3: B200_LAUNCH_RED(8, 2, 3); break;
-      default: B200_LAUNCH_RED(4, 4, 4); break;
-    }
-  }
+  else
+    B200_LAUNCH_RED(4, 4, 4);
 #undef B200_LAUNCH_RED
 #undef B200_RED_ARGS
   B200_CHECK_LAUNCH("bn_bwd_reduce_kernel");
@@ -787,90 +707,34 @@ static int bn_bwd_reduce_impl(const void* dy, const void* y, const uint8_t* act_
   return B200_OK;
 }
 
-extern "C" int b200_bn_bwd_reduce(const void* dy, const void* y, const uint8_t* act_mask, const void* z, long long M,
-                                  int C, int act,
-                                  const float* mean, const float* invstd, const float* gamma, const float* beta,
-                                  float* sums, float* dgamma_acc, float* dbeta_acc, float* workspace,
-                                  b200_stream_t stream_) {
-  return bn_bwd_reduce_impl(dy, y, act_mask, z, M, C, act, mean, invstd, gamma, beta, sums, dgamma_acc, dbeta_acc,
-                            workspace, stream_, false, PoolGeom{0, 0, 0, 0});
-}
-
-static int pooled_geom(int N, int H, int W, int C, const void* dp, const uint8_t* argmax, PoolGeom* pg) {
-  B200_REQUIRE(N > 0 && H > 1 && W > 1 && dp && argmax, B200_ERR_INVALID, "bn_bwd (pooled): bad argument");
-  B200_REQUIRE(C % 8 == 0, B200_ERR_UNSUPPORTED, "bn_bwd (pooled): C=%d must be a multiple of 8", C);
-  B200_REQUIRE((long long)N * H * W < (1LL << 31), B200_ERR_UNSUPPORTED, "bn_bwd (pooled): tensor too large");
-  pg->H = H; pg->W = W; pg->OH = (H - 1) / 2 + 1; pg->OW = (W - 1) / 2 + 1;
-  return B200_OK;
-}
-
-extern "C" int b200_bn_bwd_reduce_pooled(const void* dp, const uint8_t* argmax, const void* z, int N, int H, int W, int C,
-                                         int act, const float* mean, const float* invstd, const float* gamma,
-                                         const float* beta, float* sums, float* dgamma_acc, float* dbeta_acc,
-                                         float* workspace, b200_stream_t stream_) {
-  PoolGeom pg;
-  int rc = pooled_geom(N, H, W, C, dp, argmax, &pg);
-  if (rc) return rc;
-  return bn_bwd_reduce_impl(dp, nullptr, argmax, z, (long long)N * H * W, C, act, mean, invstd, gamma, beta, sums,
-                            dgamma_acc, dbeta_acc, workspace, stream_, true, pg);
-}
-
-static int bn_bwd_dx_impl(const void* dy, const void* y, const uint8_t* act_mask, const void* z, long long M, int C,
-                          int act, const float* mean, const float* invstd, const float* gamma, const float* beta,
-                          const float* sums, void* dz, void* g_out, b200_stream_t stream_, bool pooled,
-                          const PoolGeom pg) {
+extern "C" int b200_bn_bwd_dx(const void* dy, const void* y, const uint8_t* act_mask, const void* z, long long M, int C,
+                              int act,
+                              const float* mean, const float* invstd, const float* gamma, const float* beta,
+                              const float* sums, void* dz, void* g_out, b200_stream_t stream_) {
   int rc = check_c(C, "bn_bwd_dx");
   if (rc) return rc;
   B200_REQUIRE(dy && z && mean && invstd && sums && dz && M > 0, B200_ERR_INVALID, "bn_bwd_dx: bad argument");
-  const int src = pooled ? 3 : ((act == B200_ACT_NONE) ? 0 : (act_mask != nullptr ? 2 : (y != nullptr ? 1 : 0)));
+  const int src = (act == B200_ACT_NONE) ? 0 : (act_mask != nullptr ? 2 : (y != nullptr ? 1 : 0));
 #define B200_DX_ARGS(VEC)                                                                                    \
   (const __nv_bfloat16*)dy, (const __nv_bfloat16*)y, act_mask, (const __nv_bfloat16*)z, M, C, rm.cv,         \
-      rm.rows_per_iter, act, mean, invstd, gamma, beta, sums, (__nv_bfloat16*)dz, (__nv_bfloat16*)g_out, pg
+      rm.rows_per_iter, act, mean, invstd, gamma, beta, sums, (__nv_bfloat16*)dz, (__nv_bfloat16*)g_out
 #define B200_LAUNCH_DX(VEC, ROWS, MINB)                                                                      \
   do {                                                                                                       \
     const RowMap rm = make_rowmap_v<VEC>(C);                                                                 \
     const int blocks = stream_blocks(M, rm);                                                                 \
-    if (src == 3)                                                                                            \
-      b200::launch(bn_bwd_dx_kernel<VEC, ROWS, MINB, 3>, blocks, kBnThreads, 0, (cudaStream_t)stream_, B200_DX_ARGS(VEC)); \
-    else if (src == 2)                                                                                       \
+    if (src == 2)                                                                                            \
       b200::launch(bn_bwd_dx_kernel<VEC, ROWS, MINB, 2>, blocks, kBnThreads, 0, (cudaStream_t)stream_, B200_DX_ARGS(VEC)); \
     else if (src == 1)                                                                                       \
       b200::launch(bn_bwd_dx_kernel<VEC, ROWS, MINB, 1>, blocks, kBnThreads, 0, (cudaStream_t)stream_, B200_DX_ARGS(VEC)); \
     else                                                                                                     \
       b200::launch(bn_bwd_dx_kernel<VEC, ROWS, MINB, 0>, blocks, kBnThreads, 0, (cudaStream_t)stream_, B200_DX_ARGS(VEC)); \
   } while (0)
-  if (pooled) {
-    B200_LAUNCH_DX(4, 2, 4);
-  } else if (C > 1024) {
+  if (C > 1024)
     B200_LAUNCH_DX(8, 2, 3);
-  } else {
-    switch (bwd_variant()) {
-      case 1: B200_LAUNCH_DX(4, 2, 5); break;
-      case 2: B200_LAUNCH_DX(4, 8, 3); break;
-      case 3: B200_LAUNCH_DX(8, 2, 3); break;
-      default: B200_LAUNCH_DX(4, 4, 4); break;
-    }
-  }
+  else
+    B200_LAUNCH_DX(4, 4, 4);
 #undef B200_LAUNCH_DX
 #undef B200_DX_ARGS
   B200_CHECK_LAUNCH("bn_bwd_dx_kernel");
   return B200_OK;
-}
-
-extern "C" int b200_bn_bwd_dx(const void* dy, const void* y, const uint8_t* act_mask, const void* z, long long M, int C,
-                              int act,
-                              const float* mean, const float* invstd, const float* gamma, const float* beta,
-                              const float* sums, void* dz, void* g_out, b200_stream_t stream_) {
-  return bn_bwd_dx_impl(dy, y, act_mask, z, M, C, act, mean, invstd, gamma, beta, sums, dz, g_out, stream_, false,
-                        PoolGeom{0, 0, 0, 0});
-}
-
-extern "C" int b200_bn_bwd_dx_pooled(const void* dp, const uint8_t* argmax, const void* z, int N, int H, int W, int C,
-                                     int act, const float* mean, const float* invstd, const float* gamma,
-                                     const float* beta, const float* sums, void* dz, b200_stream_t stream_) {
-  PoolGeom pg;
-  int rc = pooled_geom(N, H, W, C, dp, argmax, &pg);
-  if (rc) return rc;
-  return bn_bwd_dx_impl(dp, nullptr, argmax, z, (long long)N * H * W, C, act, mean, invstd, gamma, beta, sums, dz,
-                        nullptr, stream_, true, pg);
 }

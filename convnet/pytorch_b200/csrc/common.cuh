@@ -126,16 +126,6 @@ __device__ __forceinline__ void bulk_commit_group() { asm volatile("cp.async.bul
 __device__ __forceinline__ void bulk_wait_group_read0() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
 __device__ __forceinline__ void bulk_wait_group_read1() { asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory"); }
 __device__ __forceinline__ void bulk_wait_group0() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
-// programmatic dependent launch (host.h: b200::launch): block until the stream predecessor grid has completed and its
-// memory is visible, then allow the stream SUCCESSOR to be scheduled (its blocks park in their own pdl_wait until this
-// grid has completed; the trigger only takes effect once every block of this grid has started, so look-ahead is one
-// kernel deep and never competes with unscheduled blocks of the running grid).  Both are no-ops for a launch without
-// the attribute.  EVERY thread of every kernel calls this before its first global access, so completion of a grid
-// implies completion of all its predecessors.
-__device__ __forceinline__ void pdl_wait() {
-  asm volatile("griddepcontrol.wait;" ::: "memory");
-  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-}
 __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }

@@ -160,7 +160,6 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     }
   }
   __syncthreads();
-  pdl_wait();   // prologue above (barriers, descriptor prefetch) overlaps the predecessor grid
 
   const int k_iters = p.ntaps * p.c_chunks;
   // tile walk: round-robin over all (m, n) tiles, or -- owned n-tile -- over the m-tiles of one n-tile
@@ -436,7 +435,6 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_constan
     prefetch_tmap(&tmX);
   }
   __syncthreads();
-  pdl_wait();   // prologue above (barriers, descriptor prefetch) overlaps the predecessor grid
 
   // work decomposition
   const int tiles = p.k_groups * p.col_groups;
@@ -577,7 +575,6 @@ __global__ void __launch_bounds__(256) conv_wgrad_reduce_kernel(const float* __r
                                                                 int K_out, int taps, int C, int ckB, int c_chunks,
                                                                 int boxes_per_cta, int kt, int k_groups, int splits,
                                                                 int pitch) {
-  pdl_wait();
   __shared__ float4 red[8][32];
   const int c4n = C >> 2;
   const long long total = static_cast<long long>(K_out) * taps * c4n;
@@ -716,9 +713,14 @@ static auto igemm_kernel_for(int block_n, std::integer_sequence<int, Is...>) {
   static constexpr decltype(&conv_igemm_kernel<16>) table[] = {&conv_igemm_kernel<16 * (Is + 1)>...};
   return table[block_n / 16 - 1];
 }
-template <int... Is>
-static auto wgrad_kernel_for(int ncols, std::integer_sequence<int, Is...>) {
-  static constexpr decltype(&conv_wgrad_kernel<16>) table[] = {&conv_wgrad_kernel<16 * (Is + 1)>...};
+// The weight-gradient widths b200_conv_wgrad reaches: boxes_per_cta * ckB with ckB in {16, 32, 64} and
+// boxes_per_cta <= min(8, 256 / ckB), i.e. 16..128 in steps of 16 and 160, 192, 224, 256.
+static auto wgrad_kernel_for(int ncols) {
+  static constexpr decltype(&conv_wgrad_kernel<16>) table[] = {
+      &conv_wgrad_kernel<16>,  &conv_wgrad_kernel<32>,  &conv_wgrad_kernel<48>,  &conv_wgrad_kernel<64>,
+      &conv_wgrad_kernel<80>,  &conv_wgrad_kernel<96>,  &conv_wgrad_kernel<112>, &conv_wgrad_kernel<128>,
+      nullptr,                 &conv_wgrad_kernel<160>, nullptr,                 &conv_wgrad_kernel<192>,
+      nullptr,                 &conv_wgrad_kernel<224>, nullptr,                 &conv_wgrad_kernel<256>};
   return table[ncols / 16 - 1];
 }
 
@@ -765,10 +767,9 @@ static int launch_igemm(const IgemmLaunch& L, cudaStream_t stream) {
   const int epi_bytes = p.tma_store ? kTileM * p.block_n * 2 : 0;   // per consumer warpgroup
   const int epi_total = 2 * epi_bytes;
   // small 1x1 layers (all weight slices <= 64 KB): keep the weights resident, stream only the activations
-  static const bool bstat_enabled = !(getenv("B200_IGEMM_BSTAT") && atoi(getenv("B200_IGEMM_BSTAT")) == 0);
   const int b_all = L.ntaps * p.c_chunks * (int)p.b_bytes;
   int bstat_bytes = 0;
-  if (bstat_enabled && p.n_tiles == 1 && !L.window && (p.a_bytes % 1024) == 0 && (p.b_bytes % 1024) == 0 && b_all <= 64 * 1024) {
+  if (p.n_tiles == 1 && !L.window && (p.a_bytes % 1024) == 0 && (p.b_bytes % 1024) == 0 && b_all <= 64 * 1024) {
     p.b_stationary = 1;
     bstat_bytes = b_all;
     stage = p.a_bytes;
@@ -776,9 +777,8 @@ static int launch_igemm(const IgemmLaunch& L, cudaStream_t stream) {
   // several n-tiles whose weights fit one at a time: a CTA owns an n-tile.  Worth it when the weights dominate the
   // L2->SM traffic of the round-robin walk (bytes ~ A * n_tiles + W * m_tiles vs A * n_tiles + W_tile * CTAs) and
   // every CTA still gets a few m-tiles; needs >= 3 operand stages beside the resident weights and the staging tile.
-  static const int own_mode = getenv("B200_IGEMM_OWN_NTILE") ? atoi(getenv("B200_IGEMM_OWN_NTILE")) : 1;
   int grid_own = 0;
-  if (bstat_enabled && own_mode && !p.b_stationary && p.n_tiles > 1 && p.n_tiles <= 8 && !L.window &&
+  if (!p.b_stationary && p.n_tiles > 1 && p.n_tiles <= 8 && !L.window &&
       (p.a_bytes % 1024) == 0 && (p.b_bytes % 1024) == 0 && (L.Nout % p.block_n) == 0) {
     const int ctas = sm_count() / p.n_tiles;
     const long long a_all = (long long)p.M_total * L.SC * 2 * L.ntaps;
@@ -1083,7 +1083,7 @@ extern "C" int b200_conv_wgrad(const b200_conv_desc* d, const void* x, const voi
                        d->stride, d->x_pixel_stride, d->x_row_stride, d->x_image_stride);
   if (rc) return rc;
   const int smem_bytes = p.num_stages * (int)p.stage_bytes + 1024;
-  const auto kfn = wgrad_kernel_for(p.pitch, std::make_integer_sequence<int, 16>{});
+  const auto kfn = wgrad_kernel_for(p.pitch);
   rc = set_smem_attr((const void*)kfn, smem_bytes);
   if (rc) return rc;
   const int grid = tiles * p.splits;

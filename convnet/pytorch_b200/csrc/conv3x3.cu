@@ -76,7 +76,6 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant_
     if (p.has_res) prefetch_tmap(&tmR);
   }
   __syncthreads();
-  pdl_wait();   // prologue above (barriers, descriptor prefetch) overlaps the predecessor grid
   // tile walk: dense -- tiles (m, n) round-robin over the CTAs; diagonal -- the CTA owns n-tile blockIdx.x % n_tiles and
   // walks the m-tiles with stride gridDim.x / n_tiles (the grid is a multiple of n_tiles)
   const int t_start = p.diag ? static_cast<int>(blockIdx.x) / p.n_tiles : static_cast<int>(blockIdx.x);
@@ -289,15 +288,9 @@ static int enc4(CUtensorMap* tm, const void* base, int C, int W, int H, int N, i
   return B200_OK;
 }
 
-static bool halo_enabled() {
-  static const bool enabled = !(getenv("B200_HALO") && atoi(getenv("B200_HALO")) == 0);
-  return enabled;
-}
-
 // Geometry shared by the fprop/dgrad and wgrad halo kernels: stride-1 RxS taps over an H x W OUTPUT map.
 // Supported: 3x3 pad 1 with 64-channel source chunks, and the 4x4 pad 0 stem with a 16-channel source.
 bool halo_geometry_ok(int H, int W, int Cs, int R, int S, int pad) {
-  if (!halo_enabled()) return false;
   const bool k3 = (R == 3 && S == 3 && pad == 1 && Cs % 64 == 0);
   const bool k4 = (R == 4 && S == 4 && pad == 0 && Cs == 16);
   if (!k3 && !k4) return false;
@@ -482,7 +475,6 @@ conv_halo_wgrad_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_co
   }
   fence_proxy_async();
   __syncthreads();
-  pdl_wait();   // prologue above (barriers, descriptor prefetch) overlaps the predecessor grid
 
   const int split = blockIdx.x / p.units;
   const int unit = blockIdx.x - split * p.units;
@@ -573,7 +565,6 @@ conv_halo_wgrad_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_co
 __global__ void __launch_bounds__(256) conv_halo_wgrad_reduce_kernel(const float* __restrict__ partial,
                                                                      float* __restrict__ dw, int K_out, int ntaps, int C,
                                                                      int cw, int k_tiles, int splits, int ncols) {
-  pdl_wait();
   __shared__ float4 red[8][32];
   const int c4n = C >> 2;
   const long long total = static_cast<long long>(K_out) * ntaps * c4n;
@@ -612,8 +603,7 @@ __global__ void __launch_bounds__(256) conv_halo_wgrad_reduce_kernel(const float
 }
 
 bool halo_wgrad_eligible(int H, int W, int C, int K_out, int R, int S, int pad) {
-  static const bool enabled = !(getenv("B200_HALO_WGRAD") && atoi(getenv("B200_HALO_WGRAD")) == 0);
-  if (!enabled || !halo_geometry_ok(H, W, C, R, S, pad)) return false;
+  if (!halo_geometry_ok(H, W, C, R, S, pad)) return false;
   return K_out % 64 == 0;
 }
 

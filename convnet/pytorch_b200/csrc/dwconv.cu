@@ -5,7 +5,6 @@
 // and its autograd backward.  Weight layout: [R*S][C] (bf16 for fprop/dgrad, fp32 gradient).
 #include "common.cuh"
 #include "host.h"
-#include <stdlib.h>
 
 namespace b200 {
 
@@ -24,7 +23,6 @@ __device__ __forceinline__ void dst8(__nv_bfloat16* p, const float (&f)[8]) {
 __global__ void __launch_bounds__(256) dw_fprop_kernel(const __nv_bfloat16* __restrict__ x,
                                                        const __nv_bfloat16* __restrict__ w, b200_conv_desc d,
                                                        __nv_bfloat16* __restrict__ y) {
-  pdl_wait();
   const int cv = d.C >> 3;
   const long long total = (long long)d.N * d.P * d.Q * cv;
   for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
@@ -57,7 +55,6 @@ __global__ void __launch_bounds__(256) dw_fprop_kernel(const __nv_bfloat16* __re
 __global__ void __launch_bounds__(256) dw_dgrad_kernel(const __nv_bfloat16* __restrict__ dy,
                                                        const __nv_bfloat16* __restrict__ w, b200_conv_desc d,
                                                        __nv_bfloat16* __restrict__ dx) {
-  pdl_wait();
   const int cv = d.C >> 3;
   const long long total = (long long)d.N * d.H * d.W * cv;
   for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
@@ -100,7 +97,6 @@ __global__ void __launch_bounds__(kDwThreads) dw_wgrad_partial_kernel(const __nv
                                                                       const __nv_bfloat16* __restrict__ dy,
                                                                       b200_conv_desc d, int cv, int rows_per_iter,
                                                                       float* __restrict__ partial) {
-  pdl_wait();
   __shared__ float red[kDwThreads][9];
   const int t = threadIdx.x;
   const bool active = t < rows_per_iter * cv;
@@ -157,7 +153,6 @@ __global__ void __launch_bounds__(kDwThreads) dw_wgrad_partial_kernel(const __nv
 // blocks) was a chain of L2 round trips, 0.3 ms per layer.
 __global__ void __launch_bounds__(256) dw_wgrad_final_kernel(const float* __restrict__ partial, int nblocks, int n,
                                                              float* __restrict__ dw) {
-  pdl_wait();
   __shared__ double red[64][5];
   const int lane_o = threadIdx.x & 3, grp = threadIdx.x >> 2;
   const int o = blockIdx.x * 4 + lane_o;
@@ -212,7 +207,6 @@ template <int STRIDE>
 __global__ void __launch_bounds__(128) dw3x3_fprop_kernel(const __nv_bfloat16* __restrict__ x,
                                                           const __nv_bfloat16* __restrict__ w, const Dw3 g, int flip,
                                                           __nv_bfloat16* __restrict__ y) {
-  pdl_wait();
   const unsigned cv = (unsigned)g.C >> 3;
   const unsigned chunks = (unsigned)(g.P + g.TP - 1) / (unsigned)g.TP;
   const unsigned total = (unsigned)g.N * chunks * (unsigned)g.Q * cv;
@@ -279,7 +273,6 @@ __global__ void __launch_bounds__(128) dw3x3_fprop_kernel(const __nv_bfloat16* _
 __global__ void __launch_bounds__(128) dw3x3_dgrad_s2_kernel(const __nv_bfloat16* __restrict__ dy,
                                                              const __nv_bfloat16* __restrict__ w, const Dw3 g,
                                                              __nv_bfloat16* __restrict__ dx) {
-  pdl_wait();
   const unsigned cv = (unsigned)g.C >> 3;
   const int J = (g.H + 1) >> 1;                                   // row pairs of dx
   const unsigned chunks = (unsigned)(J + g.TP - 1) / (unsigned)g.TP;
@@ -340,7 +333,6 @@ __global__ void __launch_bounds__(kDwThreads) dw3x3_wgrad_partial_kernel(const _
                                                                          const __nv_bfloat16* __restrict__ dy,
                                                                          const Dw3 g, int cv, int rows_per_iter,
                                                                          float* __restrict__ partial) {
-  pdl_wait();
   __shared__ float red[kDwThreads][9];
   const int t = threadIdx.x;
   const bool active = t < rows_per_iter * cv;
@@ -417,8 +409,7 @@ __global__ void __launch_bounds__(kDwThreads) dw3x3_wgrad_partial_kernel(const _
 
 // the specialised path covers 3x3, pad 1, stride 1 or 2 (all of MobileNet); anything else runs the generic kernels
 static inline bool dw3_ok(const b200_conv_desc* d) {
-  static const bool on = !(getenv("B200_DW3X3") && atoi(getenv("B200_DW3X3")) == 0);
-  return on && d->R == 3 && d->S == 3 && d->pad_h == 1 && d->pad_w == 1 && (d->stride == 1 || d->stride == 2) &&
+  return d->R == 3 && d->S == 3 && d->pad_h == 1 && d->pad_w == 1 && (d->stride == 1 || d->stride == 2) &&
          d->P == (d->H - 1) / d->stride + 1 && d->Q == (d->W - 1) / d->stride + 1 &&
          (long long)d->N * d->H * d->W * (d->C / 8) < (1LL << 31);
 }

@@ -1,6 +1,5 @@
 // C-ABI plumbing: error text, launch counter, driver entry points.
 #include "host.h"
-#include <stdlib.h>
 #include <atomic>
 #include <mutex>
 #include <string.h>
@@ -49,15 +48,8 @@ EncodeIm2colFn encode_im2col_fn() {
   return fn;
 }
 
-bool pdl_enabled() {
-  static const bool on = getenv("B200_PDL") ? atoi(getenv("B200_PDL")) != 0 : false;
-  return on;
-}
-
 int wgrad_reduce_warps(int splits) {
-  static const int env = getenv("B200_WGRAD_REDUCE_WARPS") ? atoi(getenv("B200_WGRAD_REDUCE_WARPS")) : 0;
-  int w = env > 0 ? env : 8;
-  if (w > 8) w = 8;
+  int w = 8;
   while (w > 1 && w > splits) w >>= 1;   // no idle warps when there are only a few splits
   return w;
 }

@@ -35,25 +35,10 @@ bool halo_wgrad_eligible(int H, int W, int C, int K_out, int R, int S, int pad);
 int launch_halo_wgrad(const void* x, const void* dy, float* dw, void* workspace, size_t workspace_bytes, int N, int H,
                       int W, int C, int K_out, int R, int S, int pad, cudaStream_t stream, int window = 0);
 
-// Kernel launch with programmatic dependent launch (PDL): the grid may be scheduled while its stream predecessor is
-// still draining; every kernel launched through here executes pdl_wait() (griddepcontrol.wait, common.cuh) in all
-// threads before it touches global memory, which blocks until the predecessor grid has completed and its writes are
-// visible.  What overlaps is the launch latency, block scheduling and the smem/barrier prologue -- ~560 kernel
-// boundaries per ResNet-50 step.  B200_PDL=0 launches without the attribute (pdl_wait() is then a no-op).
-bool pdl_enabled();
+// Kernel launch; each argument is converted to the kernel's parameter type.
 template <typename... KArgs, typename... Args>
 inline void launch(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream, Args&&... args) {
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = grid;
-  cfg.blockDim = block;
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = pdl_enabled() ? 1 : 0;
-  cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);   // errors surface in B200_CHECK_LAUNCH
+  kernel<<<grid, block, smem, stream>>>(static_cast<KArgs>(args)...);   // errors surface in B200_CHECK_LAUNCH
 }
 
 // warps of a split-K reduce block that share the loop over the splits (1..8)

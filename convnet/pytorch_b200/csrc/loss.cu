@@ -36,7 +36,6 @@ __global__ void __launch_bounds__(kCeThreads) softmax_ce_kernel(const float* __r
                                                                 __nv_bfloat16* __restrict__ dlogits,
                                                                 const long long* __restrict__ perm,
                                                                 const float* __restrict__ lam_dev) {
-  pdl_wait();
   // row_loss layout: [0, B) per-sample loss, [B, 2B) number of classes scoring strictly above the target class
   // (rank of the target: top-1 <=> 0, top-5 <=> < 5 -- utils/meters.py:59-72 of the reference, ties aside)
   __shared__ float sh[kCeThreads / 32];
@@ -94,7 +93,6 @@ __global__ void __launch_bounds__(kCeThreads) softmax_ce_kernel(const float* __r
 // order (bit-reproducible, no atomics, no pre-zeroed output)
 __global__ void __launch_bounds__(kCeThreads) ce_mean_kernel(const float* __restrict__ row_loss, int B,
                                                              float* __restrict__ loss) {
-  pdl_wait();
   __shared__ float sh[kCeThreads / 32];
   float s = 0.f, t1 = 0.f, t5 = 0.f;
   for (int b = threadIdx.x; b < B; b += kCeThreads) {
@@ -115,7 +113,6 @@ __global__ void __launch_bounds__(kCeThreads) ce_mean_kernel(const float* __rest
 
 __global__ void __launch_bounds__(256) colsum_bf16_kernel(const __nv_bfloat16* __restrict__ m, int B, int K,
                                                           float* __restrict__ out) {
-  pdl_wait();
   const int k = blockIdx.x * blockDim.x + threadIdx.x;
   if (k >= K) return;
   float s = 0.f;

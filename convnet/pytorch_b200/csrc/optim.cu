@@ -16,7 +16,6 @@ __global__ void __launch_bounds__(256) fused_sgd_kernel(float* __restrict__ p32,
                                                         long long n, long long wd_count, float lr, float momentum,
                                                         float dampening, float wd, float inv_scale,
                                                         const float* __restrict__ clip_coef, int first_step) {
-  pdl_wait();
   const float gs = inv_scale * (clip_coef != nullptr ? __ldg(clip_coef) : 1.f);
   const long long n4 = n >> 2;
   const long long stride = (long long)gridDim.x * blockDim.x;
@@ -65,7 +64,6 @@ __global__ void __launch_bounds__(256) fused_sgd_kernel(float* __restrict__ p32,
 constexpr int kSumsqBlocks = 592;
 __global__ void __launch_bounds__(256) sumsq_partial_kernel(const float* __restrict__ g, long long n,
                                                             float* __restrict__ partial) {
-  pdl_wait();
   __shared__ float sh[8];
   float acc = 0.f;
   const long long n4 = n >> 2;
@@ -86,7 +84,6 @@ __global__ void __launch_bounds__(256) sumsq_partial_kernel(const float* __restr
   }
 }
 __global__ void sumsq_final_kernel(const float* __restrict__ partial, int nb, float* out) {
-  pdl_wait();
   __shared__ double sh[8];
   double acc = 0.0;
   for (int i = threadIdx.x; i < nb; i += blockDim.x) acc += (double)partial[i];
@@ -103,7 +100,6 @@ __global__ void sumsq_final_kernel(const float* __restrict__ partial, int nb, fl
 
 __global__ void grad_coef_kernel(const float* sumsq, float inv_scale, int mode, float max_norm, float momentum,
                                  float* state, float* coef_out, float* norm_out) {
-  pdl_wait();
   const float norm = sqrtf(*sumsq) * inv_scale;
   float coef = 1.f;
   if (mode == 0) {

@@ -5,7 +5,6 @@
 #include "common.cuh"
 #include "host.h"
 #include <math_constants.h>
-#include <stdlib.h>
 
 namespace b200 {
 
@@ -29,7 +28,6 @@ __global__ void __launch_bounds__(256) maxpool_fwd_kernel(const __nv_bfloat16* _
                                                           int C, int OH, int OW, const float* __restrict__ scale,
                                                           const float* __restrict__ shift, int act,
                                                           __nv_bfloat16* __restrict__ y, uint8_t* __restrict__ amax) {
-  pdl_wait();
   const int cv = C >> 3;
   // 32-bit index arithmetic (the host checks N*H*W*C/8 < 2^31): 64-bit div/mod cost more than the loads
   const unsigned total = (unsigned)N * OH * OW * cv;
@@ -92,166 +90,14 @@ __global__ void __launch_bounds__(256) maxpool_fwd_kernel(const __nv_bfloat16* _
   }
 }
 
-__global__ void __launch_bounds__(256) maxpool_bwd_kernel(const __nv_bfloat16* __restrict__ dy,
-                                                          const uint8_t* __restrict__ amax, int N, int H, int W, int C,
-                                                          int OH, int OW, __nv_bfloat16* __restrict__ dx) {
-  pdl_wait();
-  const int cv = C >> 3;
-  const unsigned total = (unsigned)N * H * W * cv;
-  for (unsigned idx = blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += gridDim.x * blockDim.x) {
-    const int v = (int)(idx % (unsigned)cv);
-    unsigned pix = idx / (unsigned)cv;
-    const int w = (int)(pix % (unsigned)W); pix /= (unsigned)W;
-    const int h = (int)(pix % (unsigned)H);
-    const int n = (int)(pix / (unsigned)H);
-    float acc[8];
-#pragma unroll
-    for (int i = 0; i < 8; ++i) acc[i] = 0.f;
-    // windows containing h: 2p-1 <= h <= 2p+1 (at most 2 x 2 of them); all loads are issued before they are used
-    const int p_lo = h / 2, q_lo = w / 2;
-    uint2 pk[4];
-    uint4 gr[4];
-    int want[4];
-    bool ok[4];
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const int p = p_lo + (j >> 1), q = q_lo + (j & 1);
-      ok[j] = p <= (h + 1) / 2 && q <= (w + 1) / 2 && p < OH && q < OW;
-      want[j] = (h - (2 * p - 1)) * 3 + (w - (2 * q - 1));
-      if (ok[j]) {
-        const long long o = (((long long)n * OH + p) * OW + q) * C + v * 8;
-        pk[j] = *reinterpret_cast<const uint2*>(amax + o);
-        gr[j] = *reinterpret_cast<const uint4*>(dy + o);
-      }
-    }
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      if (!ok[j]) continue;
-      const uint32_t gw[4] = {gr[j].x, gr[j].y, gr[j].z, gr[j].w};
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        const int b = (i < 4 ? (pk[j].x >> (8 * i)) : (pk[j].y >> (8 * (i - 4)))) & 0xff;
-        const float2 g2 = unpack_bf16x2(gw[i >> 1]);
-        if (b == want[j]) acc[i] += (i & 1) ? g2.y : g2.x;
-      }
-    }
-    st8(dx + (((long long)n * H + h) * W + w) * C + v * 8, acc);
-  }
-}
-
 // ------------------------------------------------------------------------------------------------
-// Sliding-window versions (default): a thread owns one (image, output column, 8-channel vector) and walks down the
-// rows, keeping the window rows in registers (packed bf16) -- 6 loads per pooled output instead of 9, 2 instead of 8 per
-// input-gradient vector, no 64-bit index arithmetic.  These kernels are bound by load requests in flight, like the
-// BatchNorm ones; results are bit-identical to the kernels above.
+// Sliding-window backward: the pooled gradient rows stay in registers -- 2 loads instead of 8 per input-gradient
+// vector, no 64-bit index arithmetic.  The kernel is bound by load requests in flight, like the BatchNorm ones.
 struct PoolSlide {
   int N, H, W, C, OH, OW;
-  int TP;                 // pooled rows (fwd) / row pairs (bwd) per work item
+  int TP;                 // row pairs per work item
 };
 __device__ __forceinline__ uint4 pool_ldg(const void* p) { return __ldg(reinterpret_cast<const uint4*>(p)); }
-
-template <bool AFFINE>
-__global__ void __launch_bounds__(128) maxpool_fwd_slide_kernel(const __nv_bfloat16* __restrict__ x, const PoolSlide g,
-                                                                const float* __restrict__ scale,
-                                                                const float* __restrict__ shift, int act,
-                                                                __nv_bfloat16* __restrict__ y,
-                                                                uint8_t* __restrict__ amax) {
-  pdl_wait();
-  const unsigned cv = (unsigned)g.C >> 3;
-  const unsigned chunks = (unsigned)(g.OH + g.TP - 1) / (unsigned)g.TP;
-  const unsigned total = (unsigned)g.N * chunks * (unsigned)g.OW * cv;
-  const unsigned step = gridDim.x * blockDim.x;            // a multiple of cv (host): the channel vector is per thread
-  unsigned idx = blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= total) return;
-  const unsigned v = idx % cv;
-  float sc[8], sh[8];
-  if (AFFINE) {
-#pragma unroll
-    for (int i = 0; i < 8; i += 4) {
-      const float4 a = __ldg(reinterpret_cast<const float4*>(scale + v * 8 + i));
-      const float4 b = __ldg(reinterpret_cast<const float4*>(shift + v * 8 + i));
-      sc[i] = a.x; sc[i + 1] = a.y; sc[i + 2] = a.z; sc[i + 3] = a.w;
-      sh[i] = b.x; sh[i + 1] = b.y; sh[i + 2] = b.z; sh[i + 3] = b.w;
-    }
-  }
-  for (; idx < total; idx += step) {
-    unsigned t = idx / cv;
-    const int q = (int)(t % (unsigned)g.OW); t /= (unsigned)g.OW;
-    const int ch = (int)(t % chunks);
-    const int n = (int)(t / chunks);
-    const int p0 = ch * g.TP, p1 = min(g.OH, p0 + g.TP);
-    const int c0 = 2 * q - 1;
-    const bool okc[3] = {c0 >= 0, true, c0 + 2 < g.W};
-    const __nv_bfloat16* xn = x + (size_t)n * g.H * g.W * g.C + v * 8;
-    // one window row: three packed vectors (already act(x*scale+shift) rounded to bf16 in the fused variant)
-    auto load_row = [&](int h, uint4 (&row)[3]) {
-      if (h < 0 || h >= g.H) return;                          // invalid rows are skipped by the scan below
-      const __nv_bfloat16* r = xn + ((size_t)h * g.W + c0) * g.C;
-#pragma unroll
-      for (int c = 0; c < 3; ++c) {
-        if (!okc[c]) continue;
-        uint4 u = pool_ldg(r + c * g.C);
-        if (AFFINE) {
-          float f[8];
-          const float2 a = unpack_bf16x2(u.x), b = unpack_bf16x2(u.y), cc = unpack_bf16x2(u.z), d = unpack_bf16x2(u.w);
-          f[0] = a.x; f[1] = a.y; f[2] = b.x; f[3] = b.y; f[4] = cc.x; f[5] = cc.y; f[6] = d.x; f[7] = d.y;
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            float o = fmaf(f[i], sc[i], sh[i]);
-            if (act == B200_ACT_RELU) o = fmaxf(o, 0.f);
-            else if (act == B200_ACT_RELU6) o = fminf(fmaxf(o, 0.f), 6.f);
-            f[i] = o;
-          }
-          u.x = pack_bf16x2(f[0], f[1]); u.y = pack_bf16x2(f[2], f[3]);
-          u.z = pack_bf16x2(f[4], f[5]); u.w = pack_bf16x2(f[6], f[7]);
-        }
-        row[c] = u;
-      }
-    };
-    uint4 win[3][3];
-    int h = 2 * p0 - 1;
-    load_row(h, win[0]);
-    size_t o = (((size_t)n * g.OH + p0) * g.OW + q) * g.C + v * 8;
-    for (int p = p0; p < p1; ++p) {
-      load_row(h + 1, win[1]);
-      load_row(h + 2, win[2]);
-      float best[8];
-      int bidx[8];
-      const int first = (h < 0 ? 3 : 0) + (okc[0] ? 0 : 1);   // first valid position in scan order
-#pragma unroll
-      for (int i = 0; i < 8; ++i) { best[i] = -CUDART_INF_F; bidx[i] = first; }
-#pragma unroll
-      for (int r = 0; r < 3; ++r) {
-        const int hh = h + r;
-        if (hh < 0 || hh >= g.H) continue;
-#pragma unroll
-        for (int c = 0; c < 3; ++c) {
-          if (!okc[c]) continue;
-          const uint4 u = win[r][c];
-          float f[8];
-          const float2 a = unpack_bf16x2(u.x), b = unpack_bf16x2(u.y), cc = unpack_bf16x2(u.z), d = unpack_bf16x2(u.w);
-          f[0] = a.x; f[1] = a.y; f[2] = b.x; f[3] = b.y; f[4] = cc.x; f[5] = cc.y; f[6] = d.x; f[7] = d.y;
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            // first occurrence wins on ties (strict >), NaN propagates, like ATen's max_pool2d
-            if (f[i] > best[i] || f[i] != f[i]) { best[i] = f[i]; bidx[i] = r * 3 + c; }
-          }
-        }
-      }
-      st8(y + o, best);
-      if (amax != nullptr) {
-        uint2 pk;
-        pk.x = bidx[0] | (bidx[1] << 8) | (bidx[2] << 16) | (bidx[3] << 24);
-        pk.y = bidx[4] | (bidx[5] << 8) | (bidx[6] << 16) | (bidx[7] << 24);
-        *reinterpret_cast<uint2*>(amax + o) = pk;
-      }
-      o += (size_t)g.OW * g.C;
-#pragma unroll
-      for (int c = 0; c < 3; ++c) win[0][c] = win[2][c];
-      h += 2;
-    }
-  }
-}
 
 // backward: a thread owns one INPUT column (n, w, v) and walks the row pairs (2j, 2j + 1); pooled rows j and j + 1 are
 // the only ones whose windows contain them.  Column slots: even w lies in window q = w/2 only (local column 1), odd w
@@ -259,7 +105,6 @@ __global__ void __launch_bounds__(128) maxpool_fwd_slide_kernel(const __nv_bfloa
 __global__ void __launch_bounds__(128) maxpool_bwd_slide_kernel(const __nv_bfloat16* __restrict__ dy,
                                                                 const uint8_t* __restrict__ amax, const PoolSlide g,
                                                                 __nv_bfloat16* __restrict__ dx) {
-  pdl_wait();
   const unsigned cv = (unsigned)g.C >> 3;
   const int J = (g.H + 1) >> 1;
   const unsigned chunks = (unsigned)(J + g.TP - 1) / (unsigned)g.TP;
@@ -304,7 +149,7 @@ __global__ void __launch_bounds__(128) maxpool_bwd_slide_kernel(const __nv_bfloa
       float e[8], o[8];
 #pragma unroll
       for (int i = 0; i < 8; ++i) { e[i] = 0.f; o[i] = 0.f; }
-      // accumulation order = window order (p, q) ascending, as in the gather kernel above (fp32 sums, same rounding)
+      // accumulation order = window order (p, q) ascending (fp32 sums)
       if (odd) {
         add_if(cgb, cmb, 3 + sb, e); add_if(cga, cma, 3 + sa, e);        // row 2j    : local row 1 of pooled row j
         add_if(cgb, cmb, 6 + sb, o); add_if(cga, cma, 6 + sa, o);        // row 2j + 1: local row 2 of pooled row j
@@ -325,14 +170,8 @@ __global__ void __launch_bounds__(128) maxpool_bwd_slide_kernel(const __nv_bfloa
 static inline PoolSlide pool_slide_geom(int N, int H, int W, int C, int OH, int OW, int rows) {
   PoolSlide g;
   g.N = N; g.H = H; g.W = W; g.C = C; g.OH = OH; g.OW = OW;
-  g.TP = rows < 14 ? rows : 14;       // 112 -> 56 pooled rows: four chunks of 14
+  g.TP = rows < 14 ? rows : 14;       // 112 rows -> 56 row pairs: four chunks of 14
   return g;
-}
-// B200_POOL_SLIDE: 0 = gather kernels only, 1 (default) = sliding-window BACKWARD (0.29 -> 0.21 ms on the ResNet-50 stem),
-// 2 = sliding-window forward too (measured slower than the gather kernel: 0.38 vs 0.29 ms -- 117 registers per thread)
-static inline int pool_slide_mode() {
-  static const int mode = getenv("B200_POOL_SLIDE") ? atoi(getenv("B200_POOL_SLIDE")) : 1;
-  return mode;
 }
 static inline int pool_slide_grid(long long items, int cv) {
   long long b = (items + 127) / 128;
@@ -344,7 +183,6 @@ static inline int pool_slide_grid(long long items, int cv) {
 
 __global__ void __launch_bounds__(256) avgpool_fwd_kernel(const __nv_bfloat16* __restrict__ x, int N, int HW, int C,
                                                           __nv_bfloat16* __restrict__ y) {
-  pdl_wait();
   const int cv = C >> 3;
   const int idx = blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= N * cv) return;
@@ -367,7 +205,6 @@ __global__ void __launch_bounds__(256) avgpool_fwd_kernel(const __nv_bfloat16* _
 
 __global__ void __launch_bounds__(256) avgpool_bwd_kernel(const __nv_bfloat16* __restrict__ dy, int N, int HW, int C,
                                                           __nv_bfloat16* __restrict__ dx) {
-  pdl_wait();
   const int cv = C >> 3;
   const long long total = (long long)N * HW * cv;
   const float inv = 1.f / (float)HW;
@@ -402,14 +239,6 @@ extern "C" int b200_maxpool3x3s2_fwd(const void* x, int N, int H, int W, int C, 
   B200_REQUIRE(C % 8 == 0, B200_ERR_UNSUPPORTED, "maxpool_fwd: C=%d must be a multiple of 8", C);
   B200_REQUIRE((long long)N * H * W * (C / 8) < (1LL << 31), B200_ERR_UNSUPPORTED, "maxpool_fwd: tensor too large");
   const int OH = (H + 2 - 3) / 2 + 1, OW = (W + 2 - 3) / 2 + 1;
-  if (pool_slide_mode() >= 2) {
-    const PoolSlide g = pool_slide_geom(N, H, W, C, OH, OW, OH);
-    const long long items = (long long)N * ((OH + g.TP - 1) / g.TP) * OW * (C / 8);
-    b200::launch(maxpool_fwd_slide_kernel<false>, pool_slide_grid(items, C / 8), 128, 0, (cudaStream_t)stream,
-                 (const __nv_bfloat16*)x, g, nullptr, nullptr, 0, (__nv_bfloat16*)y, argmax);
-    B200_CHECK_LAUNCH("maxpool_fwd_slide_kernel");
-    return B200_OK;
-  }
   const long long total = (long long)N * OH * OW * (C / 8);
   b200::launch(maxpool_fwd_kernel<false>, grid_for(total, 256), 256, 0, (cudaStream_t)stream, (const __nv_bfloat16*)x, N, H,
                W, C, OH, OW, nullptr, nullptr, 0, (__nv_bfloat16*)y, argmax);
@@ -423,14 +252,6 @@ extern "C" int b200_bn_apply_maxpool3x3s2(const void* z, int N, int H, int W, in
   B200_REQUIRE(C % 8 == 0, B200_ERR_UNSUPPORTED, "bn_apply_maxpool: C=%d must be a multiple of 8", C);
   B200_REQUIRE((long long)N * H * W * (C / 8) < (1LL << 31), B200_ERR_UNSUPPORTED, "bn_apply_maxpool: tensor too large");
   const int OH = (H + 2 - 3) / 2 + 1, OW = (W + 2 - 3) / 2 + 1;
-  if (pool_slide_mode() >= 2) {
-    const PoolSlide g = pool_slide_geom(N, H, W, C, OH, OW, OH);
-    const long long items = (long long)N * ((OH + g.TP - 1) / g.TP) * OW * (C / 8);
-    b200::launch(maxpool_fwd_slide_kernel<true>, pool_slide_grid(items, C / 8), 128, 0, (cudaStream_t)stream,
-                 (const __nv_bfloat16*)z, g, scale, shift, act, (__nv_bfloat16*)y, argmax);
-    B200_CHECK_LAUNCH("maxpool_fwd_slide_kernel<affine>");
-    return B200_OK;
-  }
   const long long total = (long long)N * OH * OW * (C / 8);
   b200::launch(maxpool_fwd_kernel<true>, grid_for(total, 256), 256, 0, (cudaStream_t)stream, (const __nv_bfloat16*)z, N, H,
                W, C, OH, OW, scale, shift, act, (__nv_bfloat16*)y, argmax);
@@ -444,19 +265,12 @@ extern "C" int b200_maxpool3x3s2_bwd(const void* dy, const uint8_t* argmax, int 
   B200_REQUIRE(C % 8 == 0, B200_ERR_UNSUPPORTED, "maxpool_bwd: C=%d must be a multiple of 8", C);
   B200_REQUIRE((long long)N * H * W * (C / 8) < (1LL << 31), B200_ERR_UNSUPPORTED, "maxpool_bwd: tensor too large");
   const int OH = (H + 2 - 3) / 2 + 1, OW = (W + 2 - 3) / 2 + 1;
-  if (pool_slide_mode() >= 1) {
-    const int J = (H + 1) / 2;
-    const PoolSlide g = pool_slide_geom(N, H, W, C, OH, OW, J);
-    const long long items = (long long)N * ((J + g.TP - 1) / g.TP) * W * (C / 8);
-    b200::launch(maxpool_bwd_slide_kernel, pool_slide_grid(items, C / 8), 128, 0, (cudaStream_t)stream,
-                 (const __nv_bfloat16*)dy, argmax, g, (__nv_bfloat16*)dx);
-    B200_CHECK_LAUNCH("maxpool_bwd_slide_kernel");
-    return B200_OK;
-  }
-  const long long total = (long long)N * H * W * (C / 8);
-  b200::launch(maxpool_bwd_kernel, grid_for(total, 256), 256, 0, (cudaStream_t)stream, (const __nv_bfloat16*)dy, argmax, N, H, W,
-                                                                           C, OH, OW, (__nv_bfloat16*)dx);
-  B200_CHECK_LAUNCH("maxpool_bwd_kernel");
+  const int J = (H + 1) / 2;
+  const PoolSlide g = pool_slide_geom(N, H, W, C, OH, OW, J);
+  const long long items = (long long)N * ((J + g.TP - 1) / g.TP) * W * (C / 8);
+  b200::launch(maxpool_bwd_slide_kernel, pool_slide_grid(items, C / 8), 128, 0, (cudaStream_t)stream,
+               (const __nv_bfloat16*)dy, argmax, g, (__nv_bfloat16*)dx);
+  B200_CHECK_LAUNCH("maxpool_bwd_slide_kernel");
   return B200_OK;
 }
 

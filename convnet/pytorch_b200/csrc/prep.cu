@@ -37,7 +37,6 @@ __global__ void __launch_bounds__(256) input_prep_kernel(const float* __restrict
                                                          int Cpad, int mode, __nv_bfloat16* __restrict__ out,
                                                          const long long* __restrict__ perm,
                                                          const b200_mix_params* __restrict__ mixp) {
-  pdl_wait();
   b200_mix_params mp = {};
   if (MIX != kMixNone) mp = *mixp;
   // one thread per output pixel; Cpad is a multiple of 8
@@ -112,7 +111,6 @@ __global__ void __launch_bounds__(256) input_prep_u8_kernel(const uint8_t* __res
                                                             const long long* __restrict__ perm,
                                                             const b200_mix_params* __restrict__ mixp, U8Aug ag) {
   static_assert(!AUG || MIX == kMixNone, "batch augmentation is not combined with mixing");
-  pdl_wait();
   b200_mix_params mp = {};
   if (MIX != kMixNone) mp = *mixp;
   const int brd = mode == 2 ? 2 : 0;
@@ -202,7 +200,6 @@ __global__ void __launch_bounds__(256) input_prep_u8_kernel(const uint8_t* __res
 // bf16 [K][T][C] -> [C][T][K]; one 32x32 tile per block, blockIdx.z = tap
 __global__ void __launch_bounds__(256) weight_transpose_kernel(const __nv_bfloat16* __restrict__ src,
                                                                __nv_bfloat16* __restrict__ dst, int K, int T, int C) {
-  pdl_wait();
   __shared__ __nv_bfloat16 tile[32][33];
   const int t = blockIdx.z;
   const int c0 = blockIdx.x * 32, k0 = blockIdx.y * 32;
@@ -224,7 +221,6 @@ __global__ void __launch_bounds__(256) weight_transpose_kernel(const __nv_bfloat
 __global__ void __launch_bounds__(256) weight_transpose_batched_kernel(const __nv_bfloat16* __restrict__ src_base,
                                                                        __nv_bfloat16* __restrict__ dst_base,
                                                                        const int* __restrict__ jobs, int njobs) {
-  pdl_wait();
   __shared__ __nv_bfloat16 tile[32][33];
   int lo = 0, hi = njobs - 1;
   const int g = blockIdx.x;
@@ -257,7 +253,6 @@ __global__ void __launch_bounds__(256) weight_transpose_batched_kernel(const __n
 // r = 2*ah + bh - 1, s = 2*aw + bw - 1 (out-of-range -> 0)
 __global__ void stem_w_to_s2d_kernel(const float* __restrict__ w, int K, int C, int Cpad,
                                      __nv_bfloat16* __restrict__ out) {
-  pdl_wait();
   const int total = K * 16 * Cpad;
   for (int idx = blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += gridDim.x * blockDim.x) {
     const int ch = idx % Cpad;
@@ -276,7 +271,6 @@ __global__ void stem_w_to_s2d_kernel(const float* __restrict__ w, int K, int C, 
 // reverse gather for the gradient: dw[K][7][7][C] += dw_s2d[K][16][Cpad]
 __global__ void stem_wgrad_from_s2d_kernel(const float* __restrict__ dws, int K, int C, int Cpad,
                                            float* __restrict__ dw) {
-  pdl_wait();
   const int total = K * 49 * C;
   for (int idx = blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += gridDim.x * blockDim.x) {
     const int c = idx % C;
@@ -290,7 +284,6 @@ __global__ void stem_wgrad_from_s2d_kernel(const float* __restrict__ dws, int K,
 
 __global__ void __launch_bounds__(256) cast_f32_bf16_kernel(const float* __restrict__ src,
                                                             __nv_bfloat16* __restrict__ dst, long long n) {
-  pdl_wait();
   const long long n4 = n >> 2;
   const long long stride = (long long)gridDim.x * blockDim.x;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += stride) {
@@ -473,7 +466,6 @@ extern "C" int b200_cast_f32_to_bf16(const float* src, void* dst, long long n, b
 namespace b200 {
 __global__ void __launch_bounds__(256) group_pack_kernel(const float* __restrict__ wg, int K, int T, int C, int groups,
                                                          int Wd, int transpose, __nv_bfloat16* __restrict__ out) {
-  pdl_wait();
   const int cg = C / groups, kg = K / groups;
   const int rows = transpose ? C : K;
   const long long total = (long long)rows * T * Wd;
@@ -494,7 +486,6 @@ __global__ void __launch_bounds__(256) group_pack_kernel(const float* __restrict
 }
 __global__ void __launch_bounds__(256) group_unpack_kernel(const float* __restrict__ dw_win, int K, int T, int C,
                                                            int groups, int Wd, float* __restrict__ dwg) {
-  pdl_wait();
   const int cg = C / groups, kg = K / groups;
   const long long total = (long long)K * T * cg;
   for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < total;

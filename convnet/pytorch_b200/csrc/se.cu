@@ -31,7 +31,6 @@ __global__ void __launch_bounds__(256) se_reduce_kernel(const __nv_bfloat16* __r
                                                         const __nv_bfloat16* __restrict__ b,
                                                         const float* __restrict__ logit, int HW, int C,
                                                         __nv_bfloat16* __restrict__ out) {
-  pdl_wait();
   __shared__ float red[32][65];
   const int n = blockIdx.x, slab = blockIdx.y;
   const int v = threadIdx.x & 7, lane = threadIdx.x >> 3;      // 8 vectors of 8 channels, 32 row lanes
@@ -82,7 +81,6 @@ __global__ void __launch_bounds__(256) se_scale_kernel(const __nv_bfloat16* __re
                                                        const float* __restrict__ logit,
                                                        const __nv_bfloat16* __restrict__ dmean, long long total_vec,
                                                        int HW, int C, __nv_bfloat16* __restrict__ out) {
-  pdl_wait();
   const int cv = C >> 3;
   const float inv = 1.f / (float)HW;
   for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < total_vec;
@@ -113,7 +111,6 @@ __global__ void __launch_bounds__(256) se_scale_kernel(const __nv_bfloat16* __re
 __global__ void __launch_bounds__(256) act_bwd_kernel(const __nv_bfloat16* __restrict__ dy,
                                                       const __nv_bfloat16* __restrict__ y, long long nvec, int act,
                                                       __nv_bfloat16* __restrict__ dx) {
-  pdl_wait();
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < nvec; i += (long long)gridDim.x * blockDim.x) {
     float g[8], f[8];
     se_ld8(dy + i * 8, g);

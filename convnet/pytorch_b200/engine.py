@@ -14,8 +14,6 @@ attribute names) and
 Nothing here computes on the CPU or through cuDNN/cuBLAS: a missing library or an unsupported layer
 raises ``B200Error``.
 """
-import os
-
 import torch
 import torch.nn as nn
 
@@ -23,21 +21,7 @@ from . import ops
 from .lib import B200Error, ACT_NONE, ACT_RELU, ACT_RELU6
 
 _ALIGN = 64  # elements; keeps every slot 128B-aligned in the bf16 shadow (TMA needs 16B)
-WIDE_STEM = os.environ.get('B200_WIDE_STEM', '1') != '0'  # overlapping-pixel TMA view for the ImageNet stem
-HALO_STEM = os.environ.get('B200_HALO_STEM', '1') != '0'  # stem fprop on the halo kernel (dense 4x4 description)
-HALO_STEM_WGRAD = os.environ.get('B200_HALO_STEM_WGRAD', '1') != '0'
-WGRAD_STREAM = os.environ.get('B200_WGRAD_STREAM', '1') != '0'   # weight gradients on a second CUDA stream
-FOLD_BN_EVAL = os.environ.get('B200_FOLD_BN_EVAL', '1') != '0'   # inference: BN folded into conv weights + epilogue bias
-BATCHED_TRANSPOSE = os.environ.get('B200_BATCHED_TRANSPOSE', '1') != '0'  # one launch for all dgrad weight layouts
-# 1-bit activation masks for residual joins, packed in row-quad words: the BN backward kernels read 1 bit instead of the
-# bf16 output per element with ONE extra load per thread and iteration (measured: -0.74 ms/step on ResNet-50)
-BN_ACT_MASK = os.environ.get('B200_BN_ACT_MASK', '1') != '0'
-FUSE_BN_STATS = os.environ.get('B200_FUSE_BN_STATS', '1') != '0'  # BN statistics in the conv epilogue
-# stem bn1+relu+maxpool: 0 = three kernels, 1 (default) = one forward pass (the 112x112 activation is never written),
-# backward through maxpool_bwd + the plain BN kernels; 2 = also the BN backward kernels gather the pooled gradient
-# through the argmax bytes (no materialised pre-pool gradient) -- measured SLOWER (+0.4 ms: the kernels are bound by
-# load requests in flight and the gather replaces one streaming load by 4.5 cached ones)
-FUSE_STEM_POOL = int(os.environ.get('B200_FUSE_STEM_POOL', '1'))
+FOLD_BN_EVAL = True   # inference: BN folded into conv weights + epilogue bias (tests turn it off to compare)
 
 
 def _round_up(n, m):
@@ -279,7 +263,7 @@ class Runtime(object):
         self._anchor = self.arena.slots[0].param
         self._max_c = max([m.num_features for m in model.modules() if isinstance(m, nn.BatchNorm2d)] + [8])
         self._ws = torch.zeros(ops.bn_workspace_floats(self._max_c), device=device, dtype=torch.float32)
-        self._wg_stream = torch.cuda.Stream(device=device) if WGRAD_STREAM else None
+        self._wg_stream = torch.cuda.Stream(device=device)   # weight gradients on a second CUDA stream
         self._wg_keep = []
         self._fold_cache = {}
         self._want_tape = True
@@ -287,7 +271,7 @@ class Runtime(object):
         self.grad_bucket_hook = None # Trainer (data parallel): .bucket(lo, hi, wg_stream) when g32[lo:hi) is complete,
                                      # .finish() at the end of the backward pass
         self._bucket_hi = None
-        self._bucket_min = int(os.environ.get('B200_BUCKET_MIN_ELEMS', 1 << 20))
+        self._bucket_min = 1 << 20
         # SyncBatchNorm (main.py:190-191 of the reference: nn.SyncBatchNorm.convert_sync_batchnorm): with sync_bn set
         # (engine.enable_sync_batchnorm) the per-channel sum / sum^2 accumulated by the conv epilogue are all-reduced over
         # the ranks before the statistics are finalised, and d gamma / d beta sums before the BN input gradient
@@ -304,7 +288,7 @@ class Runtime(object):
         unit."""
         self._p16t, self._wt_jobs, self._wt_tiles = None, None, 0
         convs = [c for c in self.arena.convs if c.kind == 'conv' and c.groups == 1]
-        if not BATCHED_TRANSPOSE or not convs:
+        if not convs:
             return
         self._p16t = torch.empty_like(self.arena.p16)
         spec = []
@@ -404,9 +388,10 @@ class Runtime(object):
         u.w = conv.kernel_weights()
         self._conv_and_coeffs(u, x, u.w, training)
         # a join (something is added before the activation) cannot recompute act'(.) from z alone: keep one bit per
-        # element instead of re-reading the bf16 output in both backward kernels
+        # element instead of re-reading the bf16 output in both backward kernels (row-quad words, one extra load per
+        # thread and iteration; -0.74 ms/step on ResNet-50)
         u.mask = None
-        if BN_ACT_MASK and tape and training and act != ACT_NONE and (other is not None or residual is not None):
+        if tape and training and act != ACT_NONE and (other is not None or residual is not None):
             u.mask = torch.empty(ops.bn_act_mask_bytes(u.z.numel() // u.z.shape[-1], u.z.shape[-1]), device=self.device,
                                  dtype=torch.uint8)
         if other is not None:
@@ -419,7 +404,7 @@ class Runtime(object):
     def _conv_and_coeffs(self, u, x, w16, training):
         """z = conv(x) and the BN coefficients; in training the statistics are accumulated by the conv epilogue
         itself whenever the output width allows it (saves one full read of z)."""
-        if training and FUSE_BN_STATS and ops.can_fuse_bn_stats(u.desc.K):
+        if training and ops.can_fuse_bn_stats(u.desc.K):
             u.z = ops.conv_fprop(x, w16, u.desc, bn_stats_ws=self._ws)
             self._bn_coeffs(u, training, fused=True)
         else:
@@ -565,7 +550,7 @@ class Runtime(object):
         if conv.groups > 1:
             wt = conv.dgrad_weights()
         else:
-            wt = conv.wt if (conv.wt is not None and self._wt_jobs is not None) else ops.weight_transpose(u.w)
+            wt = conv.wt
         return ops.conv_dgrad(dz, wt, u.desc, residual=residual)
 
     # ---- classifier head: global average pool -> (dropout) -> linear as a 1x1 conv on a 1x1 map ----------
@@ -798,23 +783,16 @@ class ResNetRuntime(Runtime):
             ws = torch.empty((K, 16, 16), device=self.device, dtype=torch.bfloat16)
             ops.stem_weight_to_s2d(self.stem_w32, K, Cin, 16, ws)
             Hs, Ws = H // 2, W // 2
-            if WIDE_STEM:
-                # 7x7/s2 -> space-to-depth 4x4/s1 on 16 channels -> 4x1 on "wide pixels": 4 neighbouring 32-byte
-                # pixels of the zero-bordered tensor are read as ONE 64-channel (128 B) pixel, so every tap row is a
-                # full 128B-swizzle TMA tile (4 loads per tile instead of 16 quarter-width ones).
-                xs = prep(x, 16, s2d=True, border=True)                # [N, Hs+3, Ws+3, 16], data at (+2,+2)
-                desc = ops.make_desc(N, Hs + 3, Ws, 64, K, 4, 1, 1, 0, P=Hs, Q=Ws,
-                                     x_strides=(16, (Ws + 3) * 16, (Hs + 3) * (Ws + 3) * 16), algo_macs=K * 49 * Cin)
-                st['wgrad_desc'] = desc
-                if HALO_STEM and Ws + 3 <= 128:
-                    # same bordered tensor described as the dense 4x4 / pad-0 convolution it is: the library runs it
-                    # on the halo kernel (one 32-byte-row tile load per output row, weights stationary in smem)
-                    desc = ops.make_desc(N, Hs + 3, Ws + 3, 16, K, 4, 4, 1, 0, P=Hs, Q=Ws, algo_macs=K * 49 * Cin)
-                    if HALO_STEM_WGRAD:
-                        st['wgrad_desc'] = desc
-            else:
-                xs = prep(x, 16, s2d=True)                             # [N, H/2, W/2, 16]
-                desc = ops.make_desc(N, Hs, Ws, 16, K, 4, 4, 1, 2, P=Hs, Q=Ws, algo_macs=K * 49 * Cin)
+            # 7x7/s2 -> space-to-depth 4x4/s1 on 16 channels -> 4x1 on "wide pixels": 4 neighbouring 32-byte
+            # pixels of the zero-bordered tensor are read as ONE 64-channel (128 B) pixel, so every tap row is a
+            # full 128B-swizzle TMA tile (4 loads per tile instead of 16 quarter-width ones).
+            xs = prep(x, 16, s2d=True, border=True)                # [N, Hs+3, Ws+3, 16], data at (+2,+2)
+            desc = ops.make_desc(N, Hs + 3, Ws, 64, K, 4, 1, 1, 0, P=Hs, Q=Ws,
+                                 x_strides=(16, (Ws + 3) * 16, (Hs + 3) * (Ws + 3) * 16), algo_macs=K * 49 * Cin)
+            if Ws + 3 <= 128:
+                # same bordered tensor described as the dense 4x4 / pad-0 convolution it is: the library runs it
+                # on the halo kernel (one 32-byte-row tile load per output row, weights stationary in smem)
+                desc = ops.make_desc(N, Hs + 3, Ws + 3, 16, K, 4, 4, 1, 0, P=Hs, Q=Ws, algo_macs=K * 49 * Cin)
         else:
             xs = prep(x, 16, s2d=False)
             ws = torch.zeros((K, 9, 16), device=self.device, dtype=torch.bfloat16)
@@ -824,35 +802,26 @@ class ResNetRuntime(Runtime):
         u.conv, u.bn, u.act, u.x, u.desc = None, self.stem_bn, ACT_RELU, xs, desc
         self._conv_and_coeffs(u, xs, ws, training)
         st['unit'] = u
-        if self.has_maxpool and FUSE_STEM_POOL:
+        if self.has_maxpool:
             # bn1 -> relu -> maxpool in one pass: the [N, 112, 112, 64] activation is never written
             u.y = None
             out, st['argmax'] = ops.bn_apply_maxpool(u.z, u.scale, u.shift, ACT_RELU)
         else:
             u.y = ops.bn_apply(u.z, u.scale, u.shift, ACT_RELU)
             out = u.y
-            if self.has_maxpool:
-                out, st['argmax'] = ops.maxpool_fwd(u.y)
         st['cin'] = Cin
         return out, st
 
     def _stem_bwd(self, st, dy):
         u = st['unit']
-        if self.has_maxpool and u.y is None and FUSE_STEM_POOL >= 2:
-            # the BN backward kernels gather the pre-pool gradient from dy through the argmax bytes
-            bn = u.bn
-            dz = ops.bn_bwd_pooled(dy, st['argmax'], u.z, ACT_RELU, u.mean, u.invstd, bn.gamma, bn.beta, u.sums,
-                                   bn.dgamma, bn.dbeta, self._ws,
-                                   sums_hook=self._sync_bn_sums if self.sync_bn_world > 1 else None)
-        else:
-            if self.has_maxpool:
-                dy = ops.maxpool_bwd(dy, st['argmax'], tuple(u.z.shape))
-            dz, _ = self._bn_bwd(u, dy, None, ACT_RELU)   # mask recomputed from z: the activation is not needed
+        if self.has_maxpool:
+            dy = ops.maxpool_bwd(dy, st['argmax'], tuple(u.z.shape))
+        dz, _ = self._bn_bwd(u, dy, None, ACT_RELU)   # mask recomputed from z: the activation is not needed
         K, Cin = self.stem_conv.out_channels, st['cin']
         def stem_wgrad():   # every wgrad shares the split-K workspace: all of them go through _wgrad_async
             if self.imagenet_stem:
                 dws = torch.zeros((K, 16, 16), device=self.device, dtype=torch.float32)
-                ops.conv_wgrad(u.x, dz, st.get('wgrad_desc', u.desc), dws)
+                ops.conv_wgrad(u.x, dz, u.desc, dws)
                 ops.stem_wgrad_from_s2d(dws, K, Cin, 16, self.stem_g32)
             else:
                 dws = torch.zeros((K, 9, 16), device=self.device, dtype=torch.float32)
@@ -1098,8 +1067,6 @@ def enable_sync_batchnorm(model, process_group=None):
         raise B200Error('enable_sync_batchnorm needs a model converted by convert_b200')
     if not (dist.is_available() and dist.is_initialized()):
         raise B200Error('enable_sync_batchnorm needs an initialised process group')
-    if not FUSE_BN_STATS:
-        raise B200Error('SyncBatchNorm needs B200_FUSE_BN_STATS=1 (statistics accumulated by the conv epilogue)')
     rt.sync_bn_group = process_group
     rt.sync_bn_world = dist.get_world_size(process_group)
     return model

@@ -54,8 +54,6 @@ SIGNATURES = {
     "b200_maxpool3x3s2_fwd": [_vp, _i, _i, _i, _i, _vp, _vp, _vp],
     "b200_maxpool3x3s2_bwd": [_vp, _vp, _i, _i, _i, _i, _vp, _vp],
     "b200_bn_apply_maxpool3x3s2": [_vp, _i, _i, _i, _i, _vp, _vp, _i, _vp, _vp, _vp],
-    "b200_bn_bwd_reduce_pooled": [_vp, _vp, _vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp],
-    "b200_bn_bwd_dx_pooled": [_vp, _vp, _vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp],
     "b200_avgpool_fwd": [_vp, _i, _i, _i, _vp, _vp],
     "b200_avgpool_bwd": [_vp, _i, _i, _i, _vp, _vp],
     "b200_input_prep": [_vp, _i, _i, _i, _i, _i, _i, _vp, _vp],

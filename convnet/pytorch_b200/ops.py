@@ -309,30 +309,6 @@ def bn_apply_maxpool(z, scale, shift, act=ACT_RELU, want_argmax=True):
     return y, am
 
 
-def bn_bwd_pooled(dp, argmax, z, act, mean, invstd, gamma, beta, sums, dgamma_acc, dbeta_acc, workspace, dz=None,
-                  sums_hook=None):
-    """BatchNorm(+activation) backward whose incoming gradient is the gradient of the max-pooled tensor: both kernels
-    gather it through the argmax bytes (no materialised pre-pool gradient).  sums_hook(sums) runs between the two
-    kernels (SyncBatchNorm all-reduce).  Returns dz."""
-    N, H, W, C = z.shape
-    _chk(dp, bf16, "dp"); _chk(z, bf16, "z"); _chk(argmax, torch.uint8, "argmax")
-    if dz is None:
-        dz = torch.empty_like(z)
-    lib = _l.load()
-    with _T('bn_bwd_reduce', 0, 2 * z.numel() + 3 * dp.numel()):
-        _l.check(lib.b200_bn_bwd_reduce_pooled(dp.data_ptr(), argmax.data_ptr(), z.data_ptr(), N, H, W, C, int(act),
-                                               mean.data_ptr(), invstd.data_ptr(), _l.ptr(gamma), _l.ptr(beta),
-                                               sums.data_ptr(), _l.ptr(dgamma_acc), _l.ptr(dbeta_acc),
-                                               workspace.data_ptr(), _stream()), "b200_bn_bwd_reduce_pooled")
-    if sums_hook is not None:
-        sums_hook(sums)
-    with _T('bn_bwd_dx', 0, 4 * z.numel() + 3 * dp.numel()):
-        _l.check(lib.b200_bn_bwd_dx_pooled(dp.data_ptr(), argmax.data_ptr(), z.data_ptr(), N, H, W, C, int(act),
-                                           mean.data_ptr(), invstd.data_ptr(), _l.ptr(gamma), _l.ptr(beta),
-                                           sums.data_ptr(), dz.data_ptr(), _stream()), "b200_bn_bwd_dx_pooled")
-    return dz
-
-
 def avgpool_fwd(x):
     N, H, W, C = x.shape
     y = torch.empty((N, 1, 1, C), device=x.device, dtype=bf16)

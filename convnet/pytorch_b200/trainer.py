@@ -23,7 +23,6 @@ fused B200 path the stem relayout kernel writes the B*D augmented copies from th
 other path trains on ``AugmentedBatch.apply()``, the same fp32 batch.  The meters count B*D samples.
 """
 import logging
-import os
 import random
 import time
 
@@ -160,7 +159,7 @@ class Trainer(object):
         self.adapt_grad_norm = adapt_grad_norm
         self.b200 = getattr(model, '_b200', None)
         self._graphs, self._graph_pool, self._graph_broken, self._graph_static_ok = {}, None, False, None
-        self.use_graphs = os.environ.get('B200_CUDA_GRAPH', '1') != '0'
+        self.use_graphs = True
         self.graph_replays = 0                 # bench.py: launches replayed from graphs are not counted by the library
         self.graph_replayed_launches = 0
         self.world_size = dist.get_world_size() if (distributed and dist.is_initialized()) else 1
@@ -172,8 +171,7 @@ class Trainer(object):
                 optimizer.fold_zero_grad(True)     # the fused SGD pass also clears the gradient arena
             if distributed and self.world_size > 1:
                 self._broadcast_initial_state()
-                if os.environ.get('B200_AR_OVERLAP', '1') != '0':
-                    self.b200.grad_bucket_hook = Trainer._GradBuckets(self.b200.arena, self.b200.device)
+                self.b200.grad_bucket_hook = Trainer._GradBuckets(self.b200.arena, self.b200.device)
         elif distributed:
             if device_ids and 'cuda' in str(device):
                 self.model = nn.parallel.DistributedDataParallel(model, device_ids=device_ids,
@@ -195,10 +193,11 @@ class Trainer(object):
         arena.sync_shadow()
 
     def _allreduce_gradients(self):
-        """Sum of the gradient arena over the ranks (the 1/world factor is folded into the SGD kernel).  With the
-        bucketed path (default) the reduction already ran inside the backward pass -- NCCL all-reduces of arena ranges
-        on a communication stream, launched as soon as a range is final and overlapped with the remaining backward
-        kernels (inside the captured graph they are graph nodes) -- and nothing is left to do here."""
+        """Sum of the gradient arena over the ranks (the 1/world factor is folded into the SGD kernel).  Normally the
+        reduction already ran inside the backward pass -- NCCL all-reduces of arena ranges on a communication stream,
+        launched as soon as a range is final and overlapped with the remaining backward kernels (inside the captured
+        graph they are graph nodes) -- and nothing is left to do here; the flat all-reduce below serves runs whose
+        capture with in-graph all-reduces failed."""
         if self.b200 is None or self.world_size <= 1 or self.b200.grad_bucket_hook is not None:
             return
         from . import ops
@@ -338,8 +337,7 @@ class Trainer(object):
         # dgrad of the next unit) and a side-stream weight gradient become ready together the block scheduler starts the
         # critical one first and the wgrad CTAs fill in beside the HBM-bound BN kernels that follow
         if getattr(self, '_capture_stream', None) is None:
-            prio = -1 if os.environ.get('B200_MAIN_PRIORITY', '1') != '0' else 0
-            self._capture_stream = torch.cuda.Stream(device=x_s.device, priority=prio)
+            self._capture_stream = torch.cuda.Stream(device=x_s.device, priority=-1)
         with torch.cuda.graph(graph, pool=self._graph_pool, stream=self._capture_stream, capture_error_mode=mode):
             stats = None
             if eps is not None:            # the whole step is library calls: nothing of autograd inside the graph
@@ -454,7 +452,7 @@ class Trainer(object):
                         total_loss += float(replayed[1])
                     continue
             if fused:
-                # eager form of the captured step (warm-up iterations of a new shape, B200_CUDA_GRAPH=0)
+                # eager form of the captured step (warm-up iterations of a new shape, use_graphs off)
                 self.optimizer.pre_forward()
                 output, stats = self.b200.train_step(inputs, target, self._plain_ce_eps(), self._upstream(), mix=mix,
                                                      aug=aug)

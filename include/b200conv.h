@@ -5,7 +5,7 @@
  * The reference has no FFI of its own (it is pure Python on top of torch.nn); every entry point
  * below replaces one implicit torch/cuDNN/ATen operator the reference invokes, cited per function
  * as reference file:line (paths under the reference tree).  INTEGRATION.md shows the ctypes stubs.
- * 47 entry points.
+ * 46 entry points.
  *
  * Conventions
  *  - every function returns 0 on success or a negative B200_ERR_* code; b200_last_error() gives text.
@@ -137,21 +137,11 @@ int b200_bn_bwd_dx(const void* dy, const void* y, const uint8_t* act_mask, const
  * replaces nn.MaxPool2d(3,2,1) (models/resnet.py:230) and nn.AdaptiveAvgPool2d(1) (resnet.py:241) */
 int b200_maxpool3x3s2_fwd(const void* x, int N, int H, int W, int C, void* y, uint8_t* argmax, b200_stream_t stream);
 int b200_maxpool3x3s2_bwd(const void* dy, const uint8_t* argmax, int N, int H, int W, int C, void* dx, b200_stream_t stream);
-/* ImageNet stem tail bn1 -> relu -> maxpool (models/resnet.py:226-230) without materialising the [N,H,W,C] activation:
- * forward  y = maxpool3x3s2(bf16(act(z*scale+shift))) + argmax bytes, bit-identical to b200_bn_apply followed by
- *          b200_maxpool3x3s2_fwd;
- * backward the two BatchNorm kernels gather their incoming gradient from the POOLED gradient dp [N,OH,OW,C] through
- *          the argmax bytes (fp32 sum over the <= 4 windows of a pixel) instead of reading the output of
- *          b200_maxpool3x3s2_bwd; the activation mask is recomputed from z.  Arguments otherwise as the plain
- *          b200_bn_bwd_reduce / b200_bn_bwd_dx. */
+/* ImageNet stem tail bn1 -> relu -> maxpool forward (models/resnet.py:226-230) without materialising the [N,H,W,C]
+ * activation: y = maxpool3x3s2(bf16(act(z*scale+shift))) + argmax bytes, bit-identical to b200_bn_apply followed by
+ * b200_maxpool3x3s2_fwd. */
 int b200_bn_apply_maxpool3x3s2(const void* z, int N, int H, int W, int C, const float* scale, const float* shift,
                                int act, void* y, uint8_t* argmax, b200_stream_t stream);
-int b200_bn_bwd_reduce_pooled(const void* dp, const uint8_t* argmax, const void* z, int N, int H, int W, int C, int act,
-                              const float* mean, const float* invstd, const float* gamma, const float* beta,
-                              float* sums, float* dgamma_acc, float* dbeta_acc, float* workspace, b200_stream_t stream);
-int b200_bn_bwd_dx_pooled(const void* dp, const uint8_t* argmax, const void* z, int N, int H, int W, int C, int act,
-                          const float* mean, const float* invstd, const float* gamma, const float* beta,
-                          const float* sums, void* dz, b200_stream_t stream);
 int b200_avgpool_fwd(const void* x, int N, int HW, int C, void* y, b200_stream_t stream);
 int b200_avgpool_bwd(const void* dy, int N, int HW, int C, void* dx, b200_stream_t stream);
 

@@ -151,10 +151,10 @@ def test_maxpool(N, H, W, C):
 
 
 @pytest.mark.parametrize("N,H,W,C", [(4, 112, 112, 64), (3, 17, 23, 16), (2, 9, 8, 128)])
-def test_stem_bn_relu_maxpool_fused(N, H, W, C):
-    """ImageNet stem tail (models/resnet.py:226-230 of the reference: bn1 -> relu -> maxpool) as two fused passes:
-    forward bit-identical to bn_apply + maxpool_fwd; backward (BN kernels gathering the pooled gradient through the
-    argmax bytes) against fp64 autograd of the same function and against the unfused kernel chain."""
+def test_stem_bn_relu_maxpool_chain(N, H, W, C):
+    """ImageNet stem tail (models/resnet.py:226-230 of the reference: bn1 -> relu -> maxpool): the fused forward is
+    bit-identical to bn_apply + maxpool_fwd; the backward chain the engine runs (maxpool_bwd -> bn_bwd_reduce ->
+    bn_bwd_dx, ReLU mask recomputed from z) against fp64 autograd of the same function."""
     ops = _ops()
     g = torch.Generator().manual_seed(11)
     z = (torch.randn(N, H, W, C, generator=g) * 1.5 + 0.3).cuda().to(bf16)
@@ -170,15 +170,13 @@ def test_stem_bn_relu_maxpool_fused(N, H, W, C):
     assert torch.equal(p, p_ref) and torch.equal(am, am_ref)
 
     dp = torch.randn(p.shape, generator=g).cuda().to(bf16)
-    sums, dgam, dbet = torch.empty(2 * C).cuda(), torch.zeros(C).cuda(), torch.zeros(C).cuda()
-    dz = ops.bn_bwd_pooled(dp, am, z, 1, mean, invstd, gamma, beta, sums, dgam, dbet, ws)
-    # unfused chain (rounds the pre-pool gradient to bf16 in between)
     da = ops.maxpool_bwd(dp, am, (N, H, W, C))
-    sums_u, dg_u, db_u = torch.empty(2 * C).cuda(), torch.zeros(C).cuda(), torch.zeros(C).cuda()
-    ops.bn_bwd_reduce(da, None, z, 1, mean, invstd, gamma, beta, sums_u, dg_u, db_u, ws)
-    dz_u = ops.bn_bwd_dx(da, None, z, 1, mean, invstd, gamma, beta, sums_u)
+    sums, dgam, dbet = torch.empty(2 * C).cuda(), torch.zeros(C).cuda(), torch.zeros(C).cuda()
+    ops.bn_bwd_reduce(da, None, z, 1, mean, invstd, gamma, beta, sums, dgam, dbet, ws)
+    dz = ops.bn_bwd_dx(da, None, z, 1, mean, invstd, gamma, beta, sums)
     torch.cuda.synchronize()
-    # fp64 reference with the kernel's routing: gradient to the stored argmax element, ReLU mask on the fp32 argument
+    # fp64 reference with the kernel's routing: gradient to the stored argmax element, rounded to bf16 once (the
+    # materialised pre-pool gradient), ReLU mask on the fp32 argument
     zd = z.double().view(-1, C).requires_grad_(True)
     mu, var = zd.mean(0), zd.var(0, unbiased=False)
     xhat = (zd - mu) / torch.sqrt(var + 1e-5)
@@ -190,13 +188,13 @@ def test_stem_bn_relu_maxpool_fused(N, H, W, C):
     hh = 2 * p_i - 1 + am.long() // 3
     ww = 2 * q_i - 1 + am.long() % 3
     gd.index_put_((n_i, hh, ww, c_i), dp.double(), accumulate=True)
+    gd = gd.to(bf16).double()
     mask = ((z.float() * scale + shift) > 0).double()
     gd = (gd * mask).view(-1, C)
     dz_ref, = torch.autograd.grad(pre, zd, gd)
     tol = 1e-5 * math.sqrt(max(N * H * W, 1e4) / 1e4) * 10
     assert rel(dgam, (gd * xhat.detach()).sum(0)) < tol and rel(dbet, gd.sum(0)) < tol
     assert close_bf16(dz.view(-1, C), dz_ref)
-    assert rel(dg_u, dgam) < 1e-2 and rel(db_u, dbet) < 1e-2 and rel(dz_u.float(), dz.float()) < 1e-2
 
 
 def test_avgpool():

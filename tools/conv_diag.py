@@ -45,7 +45,7 @@ CASES = {
     "halo_stem_67": (3, 67, 67, 16, 64, 4, 4, 1, 0, {"no_dgrad": True}),
     "halo_56_128": (2, 56, 56, 128, 64, 3, 3, 1, 1, {}),
     "halo_8_256": (5, 8, 8, 256, 128, 3, 3, 1, 1, {}),
-    # wide 1x1 layers: the shapes the opt-in CTA-pair kernel (B200_IGEMM_PAIR=1) takes over; ragged M, residual + ReLU
+    # wide 1x1 layers: ragged M, residual + ReLU
     "p1_256_128_ragged": (3, 13, 13, 256, 128, 1, 1, 1, 0, {}),
     "p1_512_512_res": (2, 14, 14, 512, 512, 1, 1, 1, 0, {"residual": True, "act": 1}),
     "p1_256_1024_14": (4, 14, 14, 256, 1024, 1, 1, 1, 0, {}),
