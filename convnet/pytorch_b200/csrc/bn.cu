@@ -337,8 +337,9 @@ __global__ void __launch_bounds__(kBnThreads) bn_apply_kernel(
 // ---- backward kernels -----------------------------------------------------------------------------
 // Thread mapping: VEC channels per thread (VEC=4: 64-bit accesses, half the per-channel coefficient registers of
 // VEC=8, which is what keeps these 2-read(+1-write) streams at the occupancy of bn_apply; VEC=8 only for C > 1024).
-// g = dy * act'(.), where the activation argument is y when given, else recomputed as z*scale+shift (bit-identical
-// to the forward's fused multiply-add).
+// g = dy where act'(.) passes, else +0 (selected, not multiplied: dy * 0 would give -0 for negative dy, unlike the
+// mask-bit source and torch's threshold backward), where the activation argument is y when given, else recomputed as
+// z*scale+shift (bit-identical to the forward's fused multiply-add).
 template <int VEC> struct RawVec;
 template <> struct RawVec<4> { uint2 u; };
 template <> struct RawVec<8> { uint4 u; };
@@ -434,7 +435,7 @@ __global__ void __launch_bounds__(kBnThreads, MINB) bn_bwd_reduce_kernel(
         for (int i = 0; i < VEC; ++i) {
           float g = da[i];
           if (SRC == 2) g = ((rm >> (8 * u + i)) & 1ull) ? g : 0.f;
-          else if (act != B200_ACT_NONE) g *= act_mask(SRC == 1 ? ya[i] : fmaf(za[i], sc[i], sh[i]), act);
+          else if (act != B200_ACT_NONE && act_mask(SRC == 1 ? ya[i] : fmaf(za[i], sc[i], sh[i]), act) == 0.f) g = 0.f;
           acc[i] = fmaf(g, za[i] - mu[i], acc[i]);   // the 1/std factor is applied once per channel below
           acc[VEC + i] += g;
         }
@@ -562,7 +563,7 @@ __global__ void __launch_bounds__(kBnThreads, MINB) bn_bwd_dx_kernel(
       for (int i = 0; i < VEC; ++i) {
         float g = da[i];
         if (SRC == 2) g = ((rm >> (8 * u + i)) & 1ull) ? g : 0.f;
-        else if (act != B200_ACT_NONE) g *= act_mask(SRC == 1 ? ya[i] : fmaf(za[i], A[i], sh[i]), act);
+        else if (act != B200_ACT_NONE && act_mask(SRC == 1 ? ya[i] : fmaf(za[i], A[i], sh[i]), act) == 0.f) g = 0.f;
         da[i] = g;
         za[i] = A[i] * g + B[i] * za[i] + Cc[i];
       }

@@ -275,33 +275,43 @@ def bn_bwd_dx(dy, y, z, act, mean, invstd, gamma, beta, sums, dz=None, g_out=Non
 
 
 # ------------------------------------------------------------------------------------ pooling
-def maxpool_fwd(x, want_argmax=True):
+def _out(out, shape, dtype, device, name):
+    """a caller-supplied output (checked: dtype, contiguity, shape) or a new tensor"""
+    if out is None:
+        return torch.empty(shape, device=device, dtype=dtype)
+    _chk(out, dtype, name)
+    if tuple(out.shape) != tuple(shape):
+        raise _l.B200Error("%s has shape %s, expected %s" % (name, tuple(out.shape), tuple(shape)))
+    return out
+
+
+def maxpool_fwd(x, want_argmax=True, out=None, argmax_out=None):
     N, H, W, C = x.shape
     OH, OW = (H - 1) // 2 + 1, (W - 1) // 2 + 1
-    y = torch.empty((N, OH, OW, C), device=x.device, dtype=bf16)
-    am = torch.empty((N, OH, OW, C), device=x.device, dtype=torch.uint8) if want_argmax else None
+    y = _out(out, (N, OH, OW, C), bf16, x.device, "out")
+    am = _out(argmax_out, (N, OH, OW, C), torch.uint8, x.device, "argmax_out") if want_argmax else None
     with _T('maxpool_fwd', 0, 2 * x.numel() + 3 * y.numel()):
         _l.check(_l.load().b200_maxpool3x3s2_fwd(x.data_ptr(), N, H, W, C, y.data_ptr(), _l.ptr(am), _stream()),
                  "b200_maxpool3x3s2_fwd")
     return y, am
 
 
-def maxpool_bwd(dy, argmax, in_shape):
+def maxpool_bwd(dy, argmax, in_shape, out=None):
     N, H, W, C = in_shape
-    dx = torch.empty(in_shape, device=dy.device, dtype=bf16)
+    dx = _out(out, in_shape, bf16, dy.device, "out")
     with _T('maxpool_bwd', 0, 2 * dx.numel() + 3 * dy.numel()):
         _l.check(_l.load().b200_maxpool3x3s2_bwd(dy.data_ptr(), argmax.data_ptr(), N, H, W, C, dx.data_ptr(), _stream()),
                  "b200_maxpool3x3s2_bwd")
     return dx
 
 
-def bn_apply_maxpool(z, scale, shift, act=ACT_RELU, want_argmax=True):
+def bn_apply_maxpool(z, scale, shift, act=ACT_RELU, want_argmax=True, out=None, argmax_out=None):
     """maxpool3x3s2(bf16(act(z*scale+shift))) in one pass (the ImageNet stem tail); returns (pooled, argmax bytes)."""
     N, H, W, C = z.shape
     _chk(z, bf16, "z")
     OH, OW = (H - 1) // 2 + 1, (W - 1) // 2 + 1
-    y = torch.empty((N, OH, OW, C), device=z.device, dtype=bf16)
-    am = torch.empty((N, OH, OW, C), device=z.device, dtype=torch.uint8) if want_argmax else None
+    y = _out(out, (N, OH, OW, C), bf16, z.device, "out")
+    am = _out(argmax_out, (N, OH, OW, C), torch.uint8, z.device, "argmax_out") if want_argmax else None
     with _T('bn_apply', 0, 2 * z.numel() + 3 * y.numel()):
         _l.check(_l.load().b200_bn_apply_maxpool3x3s2(z.data_ptr(), N, H, W, C, scale.data_ptr(), shift.data_ptr(),
                                                       int(act), y.data_ptr(), _l.ptr(am), _stream()),
@@ -309,61 +319,61 @@ def bn_apply_maxpool(z, scale, shift, act=ACT_RELU, want_argmax=True):
     return y, am
 
 
-def avgpool_fwd(x):
+def avgpool_fwd(x, out=None):
     N, H, W, C = x.shape
-    y = torch.empty((N, 1, 1, C), device=x.device, dtype=bf16)
+    y = _out(out, (N, 1, 1, C), bf16, x.device, "out")
     with _T('avgpool', 0, 2 * x.numel()):
         _l.check(_l.load().b200_avgpool_fwd(x.data_ptr(), N, H * W, C, y.data_ptr(), _stream()), "b200_avgpool_fwd")
     return y
 
 
-def avgpool_bwd(dy, in_shape):
+def avgpool_bwd(dy, in_shape, out=None):
     N, H, W, C = in_shape
-    dx = torch.empty(in_shape, device=dy.device, dtype=bf16)
+    dx = _out(out, in_shape, bf16, dy.device, "out")
     with _T('avgpool', 0, 2 * dx.numel()):
         _l.check(_l.load().b200_avgpool_bwd(dy.data_ptr(), N, H * W, C, dx.data_ptr(), _stream()), "b200_avgpool_bwd")
     return dx
 
 
 # ------------------------------------------------------------------------------------ squeeze-and-excitation
-def se_pool(r):
+def se_pool(r, out=None):
     N, H, W, C = r.shape
-    out = torch.empty((N, 1, 1, C), device=r.device, dtype=bf16)
+    out = _out(out, (N, 1, 1, C), bf16, r.device, "out")
     with _T('se', 0, 2 * r.numel()):
         _l.check(_l.load().b200_se_pool(r.data_ptr(), N, H * W, C, out.data_ptr(), _stream()), "b200_se_pool")
     return out
 
 
-def se_scale_fwd(r, logit):
+def se_scale_fwd(r, logit, out=None):
     N, H, W, C = r.shape
     _chk(logit, torch.float32, "logit")
-    out = torch.empty_like(r)
+    out = _out(out, r.shape, bf16, r.device, "out")
     with _T('se', 0, 4 * r.numel()):
         _l.check(_l.load().b200_se_scale_fwd(r.data_ptr(), logit.data_ptr(), N, H * W, C, out.data_ptr(), _stream()),
                  "b200_se_scale_fwd")
     return out
 
 
-def se_bwd_reduce(g, r, logit):
+def se_bwd_reduce(g, r, logit, out=None):
     N, H, W, C = r.shape
-    out = torch.empty((N, 1, 1, C), device=r.device, dtype=bf16)
+    out = _out(out, (N, 1, 1, C), bf16, r.device, "out")
     with _T('se', 0, 4 * r.numel()):
         _l.check(_l.load().b200_se_bwd_reduce(g.data_ptr(), r.data_ptr(), logit.data_ptr(), N, H * W, C, out.data_ptr(),
                                               _stream()), "b200_se_bwd_reduce")
     return out
 
 
-def se_bwd_dx(g, logit, dmean):
+def se_bwd_dx(g, logit, dmean, out=None):
     N, H, W, C = g.shape
-    out = torch.empty_like(g)
+    out = _out(out, g.shape, bf16, g.device, "out")
     with _T('se', 0, 4 * g.numel()):
         _l.check(_l.load().b200_se_bwd_dx(g.data_ptr(), logit.data_ptr(), dmean.data_ptr(), N, H * W, C, out.data_ptr(),
                                           _stream()), "b200_se_bwd_dx")
     return out
 
 
-def act_bwd(dy, y, act):
-    out = torch.empty_like(dy)
+def act_bwd(dy, y, act, out=None):
+    out = _out(out, dy.shape, bf16, dy.device, "out")
     _l.check(_l.load().b200_act_bwd(dy.data_ptr(), y.data_ptr(), dy.numel(), int(act), out.data_ptr(), _stream()),
              "b200_act_bwd")
     return out
