@@ -1,0 +1,244 @@
+// RandomResizedCrop + RandomHorizontalFlip + ToTensor + Normalize of the ImageNet training transform (the reference's
+// inception_preprocess, preprocess.py:71-77) fused into the stem relayout: uint8 regions -> bf16 stem layouts.
+//
+// The resample is Pillow's ImagingResample with the BILINEAR filter on 8-bit channels, applied to the crop as if the
+// crop were the whole image (torchvision crops, then resizes): per axis, coefficients computed in double without
+// contraction, normalised by their sum, converted to 22-bit integers; a horizontal pass into a uint8 intermediate, then
+// a vertical pass over it, each accumulating in int32 from 2^21 and shifting right by 22 with a clamp to [0, 255].
+//
+// One block owns kRrcRows output rows of one copy and one thread owns one resampled column.  Each thread runs the
+// horizontal pass of its column over the intermediate rows the band needs and feeds every finished intermediate value
+// straight into its per-row vertical accumulators (registers), so the intermediate never leaves the thread.  Horizontal
+// coefficients sit in a per-thread shared-memory slab of kRrcTaps taps (rebuilt per row when a column has more taps, so
+// the scale is unbounded); vertical coefficients are computed per chunk of kRrcYChunk intermediate rows.  The grid
+// depends only on (B*D, OH) and there is no workspace: a captured CUDA graph replays with new tables and regions.
+#include "common.cuh"
+#include "host.h"
+
+namespace b200 {
+
+constexpr int kRrcRows = 8;      // output rows per block (even, so that space-to-depth row pairs stay in one block)
+constexpr int kRrcTaps = 16;     // horizontal taps per coefficient slab
+constexpr int kRrcYChunk = 32;   // intermediate rows per vertical-coefficient chunk
+constexpr int kRrcMaxOW = 512;   // one thread per output column
+
+struct RrcAxis { double scale, support, ss; int in; };
+
+__device__ __forceinline__ RrcAxis rrc_axis(int in, int out) {
+  RrcAxis a;
+  a.in = in;
+  a.scale = __ddiv_rn((double)in, (double)out);
+  const double fs = a.scale < 1.0 ? 1.0 : a.scale;
+  a.support = fs;                       // the bilinear filter's support (1.0) times the filter scale
+  a.ss = __ddiv_rn(1.0, fs);
+  return a;
+}
+
+// first source index and tap count of output index xx; center = (xx + 0.5) * scale
+__device__ __forceinline__ void rrc_bounds(const RrcAxis& a, int xx, double& center, int& xmin, int& cnt) {
+  center = __dmul_rn(__dadd_rn((double)xx, 0.5), a.scale);
+  int lo = __double2int_rz(__dadd_rn(__dsub_rn(center, a.support), 0.5));
+  int hi = __double2int_rz(__dadd_rn(__dadd_rn(center, a.support), 0.5));
+  if (lo < 0) lo = 0;
+  if (hi > a.in) hi = a.in;
+  xmin = lo;
+  cnt = hi - lo;
+}
+
+// un-normalised weight of source index x: tri((x - center + 0.5) * ss)
+__device__ __forceinline__ double rrc_tri(const RrcAxis& a, double center, int x) {
+  double t = __dmul_rn(__dadd_rn(__dsub_rn((double)x, center), 0.5), a.ss);
+  if (t < 0.0) t = -t;
+  return t < 1.0 ? __dsub_rn(1.0, t) : 0.0;
+}
+
+__device__ __forceinline__ double rrc_sum(const RrcAxis& a, double center, int xmin, int cnt) {
+  double ww = 0.0;
+  for (int x = 0; x < cnt; ++x) ww = __dadd_rn(ww, rrc_tri(a, center, xmin + x));
+  return ww;
+}
+
+__device__ __forceinline__ int rrc_coef(double w, double ww) {
+  const double k = ww != 0.0 ? __ddiv_rn(w, ww) : w;
+  return __double2int_rz(__dadd_rn(0.5, __dmul_rn(k, 4194304.0)));     // (int)(0.5 + k * 2^22)
+}
+
+__device__ __forceinline__ int rrc_clip8(int acc) {
+  const int v = acc >> 22;
+  return v < 0 ? 0 : (v > 255 ? 255 : v);
+}
+
+struct RrcRow { double center, ww; int ymin, cnt; };
+
+__global__ void __launch_bounds__(kRrcMaxOW) input_prep_rrc_kernel(
+    const uint8_t* __restrict__ regions, long long region_bytes, const long long* __restrict__ index,
+    const int* __restrict__ draws, int D, int C, int OH, int OW, int Cpad, int mode, const float* __restrict__ lut,
+    __nv_bfloat16* __restrict__ out) {
+  extern __shared__ __align__(16) unsigned char rrc_smem[];
+  int* ktab = reinterpret_cast<int*>(rrc_smem);                                  // [kRrcTaps][blockDim.x]
+  uint8_t* tile = rrc_smem + (size_t)kRrcTaps * blockDim.x * sizeof(int);        // [kRrcRows][OW][C], output columns
+  __shared__ RrcRow rows[kRrcRows];
+  __shared__ int vtab[kRrcRows * kRrcYChunk];
+
+  const int n = blockIdx.y;                     // output row n: copy n % D of image n / D
+  const int o0 = blockIdx.x * kRrcRows;
+  const int tb = min(kRrcRows, OH - o0);
+  const int xx = threadIdx.x;
+  const int nt = blockDim.x;
+
+  // the image's region and the copy's crop box, clamped: any table values read inside the region and the buffer
+  const long long* ix = index + (long long)(n / D) * 3;
+  const int* dr = draws + (long long)n * 5;
+  const long long off = min(max(__ldg(ix + 0), 0LL), region_bytes - 1);
+  const int rh = (int)min(max(__ldg(ix + 1), 1LL), 65535LL), rw = (int)min(max(__ldg(ix + 2), 1LL), 65535LL);
+  const int cy = min(max(__ldg(dr + 0), 0), rh - 1), cx = min(max(__ldg(dr + 1), 0), rw - 1);
+  const int ch = min(max(__ldg(dr + 2), 1), rh - cy), cw = min(max(__ldg(dr + 3), 1), rw - cx);
+  const bool flip = __ldg(dr + 4) != 0;
+
+  const RrcAxis ay = rrc_axis(ch, OH), ax = rrc_axis(cw, OW);
+  if (xx < tb) {
+    RrcRow r;
+    rrc_bounds(ay, o0 + xx, r.center, r.ymin, r.cnt);
+    r.ww = rrc_sum(ay, r.center, r.ymin, r.cnt);
+    rows[xx] = r;
+  }
+  double xc = 0.0, xww = 0.0;
+  int xmin = 0, xcnt = 0;
+  if (xx < OW) {
+    rrc_bounds(ax, xx, xc, xmin, xcnt);
+    xww = rrc_sum(ax, xc, xmin, xcnt);
+  }
+  __syncthreads();
+  int ybeg = rows[0].ymin, yend = rows[0].ymin + rows[0].cnt;
+  for (int r = 1; r < tb; ++r) {
+    ybeg = min(ybeg, rows[r].ymin);
+    yend = max(yend, rows[r].ymin + rows[r].cnt);
+  }
+
+  int acc[kRrcRows][4];
+#pragma unroll
+  for (int r = 0; r < kRrcRows; ++r)
+#pragma unroll
+    for (int c = 0; c < 4; ++c) acc[r][c] = 1 << 21;
+  int built = -1;                               // first tap of the slab this thread holds
+
+  for (int y0 = ybeg; y0 < yend; y0 += kRrcYChunk) {
+    __syncthreads();                            // the previous chunk's vertical coefficients are consumed
+    for (int e = threadIdx.x; e < kRrcRows * kRrcYChunk; e += nt) {
+      const int r = e / kRrcYChunk, t = y0 + e % kRrcYChunk;
+      int k = 0;
+      if (r < tb && t >= rows[r].ymin && t < rows[r].ymin + rows[r].cnt)
+        k = rrc_coef(rrc_tri(ay, rows[r].center, t), rows[r].ww);
+      vtab[e] = k;
+    }
+    __syncthreads();
+    if (xx >= OW) continue;
+    const int y1 = min(y0 + kRrcYChunk, yend);
+    for (int y = y0; y < y1; ++y) {
+      const long long row = off + ((long long)(cy + y) * rw + cx + xmin) * C;
+      int h[4] = {1 << 21, 1 << 21, 1 << 21, 1 << 21};
+      for (int t0 = 0; t0 < xcnt; t0 += kRrcTaps) {
+        const int te = min(kRrcTaps, xcnt - t0);
+        if (t0 != built) {
+          for (int t = 0; t < te; ++t) ktab[t * nt + xx] = rrc_coef(rrc_tri(ax, xc, xmin + t0 + t), xww);
+          built = t0;
+        }
+        for (int t = 0; t < te; ++t) {
+          const int k = ktab[t * nt + xx];
+          const long long p = row + (long long)(t0 + t) * C;
+#pragma unroll
+          for (int c = 0; c < 4; ++c)
+            if (c < C) h[c] += (int)__ldg(regions + min(p + c, region_bytes - 1)) * k;
+        }
+      }
+#pragma unroll
+      for (int c = 0; c < 4; ++c) h[c] = rrc_clip8(h[c]);
+#pragma unroll
+      for (int r = 0; r < kRrcRows; ++r) {
+        const int k = vtab[r * kRrcYChunk + (y - y0)];
+        if (k != 0) {
+#pragma unroll
+          for (int c = 0; c < 4; ++c) acc[r][c] += h[c] * k;
+        }
+      }
+    }
+  }
+
+  // flip mirrors the resampled column; the tile holds the band's bytes in output-column order
+  if (xx < OW) {
+    const int j = flip ? OW - 1 - xx : xx;
+#pragma unroll
+    for (int r = 0; r < kRrcRows; ++r)
+      if (r < tb)
+#pragma unroll
+        for (int c = 0; c < 4; ++c)
+          if (c < C) tile[((size_t)r * OW + j) * C + c] = (uint8_t)rrc_clip8(acc[r][c]);
+  }
+  __syncthreads();
+
+  // mode 0: [N][OH][OW][Cpad];  mode 2: [N][OH/2+3][OW/2+3][Cpad], data at (+2, +2), channel (dy*2+dx)*C + c.
+  // The first band also writes the top border rows, the last band the bottom one.
+  const bool s2d = mode == 2;
+  const int PH = s2d ? OH / 2 + 3 : OH, PW = s2d ? OW / 2 + 3 : OW, brd = s2d ? 2 : 0;
+  const int r_lo = s2d ? (o0 == 0 ? 0 : o0 / 2 + brd) : o0;
+  const int r_hi = s2d ? (o0 + tb == OH ? PH : (o0 + tb) / 2 + brd) : o0 + tb;
+  const int total = (r_hi - r_lo) * PW;
+  for (int p = threadIdx.x; p < total; p += nt) {
+    const int pr = r_lo + p / PW, pc = p % PW;
+    const int i = pr - brd, jj = pc - brd;
+    const bool inside = !s2d || (i >= 0 && i < OH / 2 && jj >= 0 && jj < OW / 2);
+    __nv_bfloat16* o = out + (((long long)n * PH + pr) * PW + pc) * Cpad;
+    for (int c0 = 0; c0 < Cpad; c0 += 8) {
+      float f[8];
+#pragma unroll
+      for (int e = 0; e < 8; ++e) {
+        const int chn = c0 + e;
+        const int sub = s2d ? chn / C : (chn < C ? 0 : 4), c = s2d ? chn - sub * C : chn;
+        float v = 0.f;
+        if (sub < 4 && inside) {
+          const int ty = s2d ? 2 * i + (sub >> 1) : i, tx = s2d ? 2 * jj + (sub & 1) : jj;
+          v = __ldg(lut + c * 256 + tile[((size_t)(ty - o0) * OW + tx) * C + c]);
+        }
+        f[e] = v;
+      }
+      uint4 u;
+      u.x = pack_bf16x2(f[0], f[1]); u.y = pack_bf16x2(f[2], f[3]);
+      u.z = pack_bf16x2(f[4], f[5]); u.w = pack_bf16x2(f[6], f[7]);
+      *reinterpret_cast<uint4*>(o + c0) = u;
+    }
+  }
+}
+
+}  // namespace b200
+
+using namespace b200;
+
+extern "C" int b200_input_prep_u8_rrc(const uint8_t* regions, long long region_bytes, const long long* index,
+                                      const int* draws, int B, int D, int C, int OH, int OW, int Cpad, int mode,
+                                      const float* lut, void* out, b200_stream_t stream) {
+  B200_REQUIRE(regions && index && draws && lut && out && region_bytes > 0 && B > 0 && D > 0 && C > 0 && C <= 4 &&
+                   OH > 0 && OW > 0,
+               B200_ERR_INVALID, "input_prep_u8_rrc: bad argument (C must be 1..4)");
+  B200_REQUIRE(OW <= kRrcMaxOW, B200_ERR_UNSUPPORTED, "input_prep_u8_rrc: OW=%d above %d", OW, kRrcMaxOW);
+  B200_REQUIRE((long long)B * D <= 65535LL, B200_ERR_UNSUPPORTED, "input_prep_u8_rrc: B*D=%lld above 65535",
+               (long long)B * D);
+  B200_REQUIRE(Cpad % 8 == 0, B200_ERR_INVALID, "input_prep_u8_rrc: Cpad=%d must be a multiple of 8", Cpad);
+  if (mode == 0) {
+    B200_REQUIRE(Cpad >= C, B200_ERR_INVALID, "input_prep_u8_rrc: Cpad < C");
+  } else if (mode == 2) {
+    B200_REQUIRE(OH % 2 == 0 && OW % 2 == 0 && Cpad >= 4 * C, B200_ERR_UNSUPPORTED,
+                 "input_prep_u8_rrc: space-to-depth needs even OH, OW and Cpad >= 4C");
+  } else {
+    B200_REQUIRE(false, B200_ERR_UNSUPPORTED, "input_prep_u8_rrc: mode %d (0 or 2 only)", mode);
+  }
+  const int threads = (OW + 31) / 32 * 32;
+  const size_t smem = (size_t)kRrcTaps * threads * sizeof(int) + (size_t)kRrcRows * OW * C;
+  const dim3 grid((OH + kRrcRows - 1) / kRrcRows, B * D);
+  cudaError_t e = cudaFuncSetAttribute(input_prep_rrc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  B200_REQUIRE(e == cudaSuccess, B200_ERR_CUDA, "input_prep_u8_rrc: smem attribute (%d bytes): %s", (int)smem,
+               cudaGetErrorString(e));
+  b200::launch(input_prep_rrc_kernel, grid, threads, smem, (cudaStream_t)stream, regions, region_bytes, index, draws,
+               D, C, OH, OW, Cpad, mode, lut, (__nv_bfloat16*)out);
+  B200_CHECK_LAUNCH("input_prep_rrc_kernel");
+  return B200_OK;
+}

@@ -16,6 +16,12 @@ Batch augmentation on the device (transform key ``device_augment``, CIFAR-style 
 (utils.augment.AugmentedBatch of the B uint8 NHWC images and their per-copy draws, target repeated to B*D) and the
 stem relayout kernel writes the B*D augmented copies.  Real cifar10 / cifar100 read the dataset's uint8 ``.data``;
 synthetic_cifar* use a pool of uniform uint8 images.
+
+RandomResizedCrop on the device (transform key ``device_resized_crop``, ImageNet-style training only): the workers
+decode and draw the reference's crop boxes and flips per image; the loader yields (utils.augment.ResizedCropBatch of
+the images' regions and draws, target repeated to B*D) and the stem relayout kernel resamples, flips and normalises.
+Real imagenet decodes with the reference's pil_loader (convert('RGB')); synthetic_imagenet uses a seeded pool of 64
+uniform uint8 images of 200-600 px.
 """
 import os
 from copy import deepcopy
@@ -25,7 +31,7 @@ import torch
 from torch.utils.data import Dataset, Subset
 from torch.utils.data.distributed import DistributedSampler
 
-from .utils.augment import AugmentCollate, BatchAugment, Cutout
+from .utils.augment import AugmentCollate, BatchAugment, Cutout, ResizedCrop, ResizedCropCollate
 from .utils.regime import Regime
 
 
@@ -148,7 +154,8 @@ def get_dataset(name, split='train', transform=None, target_transform=None, down
 
 
 def device_augment_spec(transform_name='cifar10', input_size=None, scale_size=None, normalize=None, augment=True,
-                        cutout=None, autoaugment=False, padding=None, duplicates=1, num_crops=1, device_augment=True):
+                        cutout=None, autoaugment=False, padding=None, duplicates=1, num_crops=1, device_augment=True,
+                        device_resized_crop=False):
     """The BatchAugment of a ``device_augment`` transform setting: the CIFAR training transform of
     real_dataset_transform (pad-4 random crop + flip + ToTensor + Normalize [+ Cutout]) with its duplicates.  The
     settings it cannot reproduce raise."""
@@ -189,11 +196,76 @@ def u8_dataset(name, input_size=None, split='train', download=True, datasets_pat
     raise NotImplementedError('device_augment supports cifar10, cifar100 and synthetic_cifar*; got %r' % name)
 
 
+def resized_crop_spec(transform_name='imagenet', input_size=None, scale_size=None, normalize=None, augment=True,
+                      cutout=None, autoaugment=False, padding=None, duplicates=1, num_crops=1, device_augment=False,
+                      device_resized_crop=True, interpolation='bilinear', color_jitter=None, lighting=None):
+    """The ResizedCrop of a ``device_resized_crop`` transform setting: the imagenet training transform of
+    real_dataset_transform (RandomResizedCrop(input_size) + flip + ToTensor + Normalize) with its duplicates.  The
+    settings it cannot reproduce raise."""
+    if 'imagenet' not in (transform_name or ''):
+        raise NotImplementedError('device_resized_crop reproduces the ImageNet training transform only; got transform '
+                                  '%r (CIFAR training: use device_augment)' % transform_name)
+    if not augment:
+        raise NotImplementedError('device_resized_crop is a training transform (augment=True); evaluation loaders do '
+                                  'not take it')
+    if device_augment:
+        raise NotImplementedError('device_resized_crop and device_augment are two different transforms; set one')
+    if cutout:
+        raise NotImplementedError('device_resized_crop does not apply Cutout')
+    if autoaugment or num_crops != 1:
+        raise NotImplementedError('device_resized_crop does not reproduce autoaugment / multi-crop')
+    if color_jitter or lighting:
+        raise NotImplementedError('device_resized_crop does not reproduce colour jitter / Lighting')
+    if str(interpolation).lower() != 'bilinear':
+        raise NotImplementedError('device_resized_crop resamples bilinearly only; got %r' % (interpolation,))
+    return ResizedCrop(input_size or 224, duplicates=duplicates or 1, normalize=normalize or _IMAGE_STATS)
+
+
+class DecodedImages(Dataset):
+    """(transform(PIL image), label) samples of ``images`` (PIL images, indexed modulo their count) and ``labels``."""
+
+    def __init__(self, images, labels, transform=None):
+        self.images, self.labels, self.transform = images, torch.as_tensor(labels, dtype=torch.long), transform
+
+    def __len__(self):
+        return len(self.labels)
+
+    def __getitem__(self, idx):
+        img = self.images[idx % len(self.images)]
+        return (self.transform(img) if self.transform is not None else img), int(self.labels[idx])
+
+
+def synthetic_imagenet_pool(n=64, lo=200, hi=600, seed=0):
+    """``n`` seeded uniform uint8 RGB PIL images with sides in [lo, hi]."""
+    from PIL import Image
+    g = torch.Generator().manual_seed(seed)
+    sizes = torch.randint(lo, hi + 1, (n, 2), generator=g)
+    return [Image.fromarray(torch.randint(0, 256, (int(h), int(w), 3), generator=g, dtype=torch.uint8).numpy(), 'RGB')
+            for h, w in sizes]
+
+
+def decoded_dataset(name, transform, split='train', datasets_path='~/Datasets', synthetic_length=None, **_):
+    """Decode-only samples for device_resized_crop: ImageFolder with the reference's pil_loader (convert('RGB')) for
+    imagenet, the seeded synthetic_imagenet_pool for synthetic_imagenet; ``transform`` (a ResizedCrop) draws."""
+    train = split == 'train'
+    if name == 'synthetic_imagenet':
+        _, classes, n_train, n_val = _SYNTHETIC[name]
+        length = synthetic_length or int(os.environ.get('B200_SYNTHETIC_LENGTH', n_train if train else n_val))
+        pool = synthetic_imagenet_pool(seed=0 if train else 1)
+        g = torch.Generator().manual_seed(2 if train else 3)
+        return DecodedImages(pool, torch.randint(0, classes, (length,), generator=g), transform)
+    if name == 'imagenet':
+        import torchvision.datasets as tvd
+        return tvd.ImageFolder(root=os.path.join(os.path.expanduser(datasets_path), name, 'train' if train else 'val'),
+                               transform=transform)
+    raise NotImplementedError('device_resized_crop supports imagenet and synthetic_imagenet; got %r' % name)
+
+
 _DATA_ARGS = {'name', 'split', 'transform', 'target_transform', 'download', 'datasets_path', 'synthetic_length'}
 _DATALOADER_ARGS = {'batch_size', 'shuffle', 'sampler', 'batch_sampler', 'num_workers', 'collate_fn', 'pin_memory',
                     'drop_last', 'timeout', 'worker_init_fn'}
 _TRANSFORM_ARGS = {'transform_name', 'input_size', 'scale_size', 'normalize', 'augment', 'cutout', 'duplicates',
-                   'num_crops', 'autoaugment', 'device_augment'}
+                   'num_crops', 'autoaugment', 'device_augment', 'device_resized_crop'}
 _OTHER_ARGS = {'distributed'}
 
 
@@ -224,7 +296,11 @@ class DataRegime(object):
             data_kwargs = dict(setting['data'])
             name = data_kwargs.get('name', '')
             collate = None
-            if setting['transform'].get('device_augment'):
+            if setting['transform'].get('device_resized_crop'):
+                spec = resized_crop_spec(**setting['transform'])
+                self._data = decoded_dataset(transform=spec, **data_kwargs)
+                collate = ResizedCropCollate(spec)
+            elif setting['transform'].get('device_augment'):
                 spec = device_augment_spec(**setting['transform'])
                 self._data = u8_dataset(input_size=setting['transform'].get('input_size'), **data_kwargs)
                 collate = AugmentCollate(spec)
@@ -234,7 +310,8 @@ class DataRegime(object):
             elif data_kwargs.get('transform') is None:
                 # real images: build the transform the regime asks for (reference data.py:101-102) -- never fall back
                 # to a bare ToTensor(), which would train on unnormalised, unaugmented, variable-size images
-                tf = {k: v for k, v in setting['transform'].items() if v is not None and k != 'device_augment'}
+                tf = {k: v for k, v in setting['transform'].items()
+                      if v is not None and k not in ('device_augment', 'device_resized_crop')}
                 data_kwargs['transform'] = real_dataset_transform(**tf)
             if collate is None:
                 self._data = get_dataset(**data_kwargs)

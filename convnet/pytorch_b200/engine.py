@@ -320,6 +320,16 @@ class Runtime(object):
         """-> (tensor, relayout function, (N, C, H, W)).  ``mix`` (ops.Mix): MixUp / CutMix applied by the relayout
         kernel itself (the reference mixes the fp32 batch before the forward pass, trainer.py:119-135).  ``aug``
         (ops.Aug): x holds the B un-augmented uint8 images and the relayout writes their B*D augmented copies."""
+        if isinstance(aug, ops.Rrc):
+            # x is the flat uint8 region buffer; the relayout resamples the B*D crops (mode 0 or the mode-2 stem)
+            if mix is not None:
+                raise B200Error('the resized crop on the device is not combined with MixUp / CutMix')
+            if x.dtype != torch.uint8 or x.dim() != 1:
+                raise B200Error('the resized crop on the device needs the flat uint8 region buffer; got %s %s'
+                                % (x.dtype, tuple(x.shape)))
+            OH, OW = aug.size
+            return x, (lambda t, cpad, **kw: ops.input_prep_u8_rrc(t, cpad, aug, **kw)), \
+                (aug.draws.shape[0], aug.lut.shape[0], OH, OW)
         if x.dtype == torch.uint8:
             if x.dim() != 4 or x.shape[-1] > 4:
                 raise B200Error('uint8 network inputs must be NHWC [N, H, W, C<=4]; got %s' % (tuple(x.shape),))
@@ -638,7 +648,8 @@ class Runtime(object):
         Returns (logits, stats): logits detached, stats = fp32[3] device tensor {mean loss, top-1 %, top-5 %}."""
         if x.device.type != 'cuda':
             raise B200Error('B200 runtime needs CUDA inputs (no CPU fallback); got %s' % x.device)
-        n_rows = x.shape[0] * (aug.duplicates if aug is not None else 1)
+        n_rows = aug.draws.shape[0] if isinstance(aug, ops.Rrc) else \
+            x.shape[0] * (aug.duplicates if aug is not None else 1)
         if target.dtype != torch.int64 or target.dim() != 1 or target.shape[0] != n_rows or not target.is_cuda:
             raise B200Error('train_step: target must be a CUDA int64 vector with one class index per sample')
         logits, tape = self.run_forward(x, True, True, mix=mix, aug=aug)

@@ -7,7 +7,8 @@
 
 Additions over the reference: ``--dtype bfloat16`` (compute type of the B200 kernels; parameters stay fp32
 masters in the arena), ``synthetic_*`` datasets, ``--b200 {auto,on,off}`` (auto: on for CUDA devices),
-``--device-augment`` (batch augmentation of the CIFAR transform done in the input relayout kernel), and
+``--device-augment`` (batch augmentation of the CIFAR transform done in the input relayout kernel),
+``--device-resized-crop`` (the ImageNet RandomResizedCrop + flip resampled in the input relayout kernel), and
 rank/world are read from the torchrun environment when ``--local_rank`` is not given.
 """
 import argparse
@@ -74,6 +75,9 @@ def build_parser():
     a('--device-augment', action='store_true', default=False,
       help='CIFAR training: ship uint8 images and per-copy draws, and crop / flip / cutout the --duplicates copies '
            'inside the input relayout on the GPU')
+    a('--device-resized-crop', action='store_true', default=False,
+      help='ImageNet training: the loader workers only decode and draw the crop boxes and flips; the input relayout '
+           'on the GPU resamples the crops (Pillow-exact bilinear), flips and normalises them')
     a('--autoaugment', action='store_true', default=False, help='autoaugment policies (ignored for synthetic data)')
     a('--grad-clip', default=-1, type=float, help='maximum grad norm value, -1 for none')
     a('--loss-scale', default=1, type=float, help='loss scale for mixed precision training')
@@ -239,7 +243,7 @@ def main_worker(args):
                       'num_workers': args.workers, 'pin_memory': True, 'drop_last': True,
                       'distributed': args.distributed, 'duplicates': args.duplicates,
                       'autoaugment': args.autoaugment, 'cutout': {'holes': 1, 'length': 16} if args.cutout else None,
-                      'device_augment': args.device_augment}
+                      'device_augment': args.device_augment, 'device_resized_crop': args.device_resized_crop}
     if hasattr(model, 'sampled_data_regime'):
         probs, configs = zip(*model.sampled_data_regime)
         train_data = SampledDataRegime([DataRegime(None, defaults={**train_defaults, **cfg}) for cfg in configs],

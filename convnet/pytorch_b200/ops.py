@@ -478,6 +478,86 @@ class Aug(object):
     def holes(self):
         return (self.params.shape[-1] - 3) // 4
 
+    @property
+    def key(self):
+        """what a captured step depends on besides the input's shape (the draws are refreshed in place)"""
+        return ('aug', tuple(self.params.shape), self.duplicates, self.pad, self.lut.data_ptr())
+
+    @property
+    def tables(self):
+        return (self.params,)
+
+    def with_tables(self, tables):
+        return Aug(tables[0], self.lut, self.duplicates, self.pad)
+
+
+class Rrc(object):
+    """Device-side tables of one resized-crop step (utils/augment.py ResizedCropBatch): ``index`` int64 [B, 3] {byte
+    offset, h, w} of each image's region in the uint8 region buffer, ``draws`` int32 [B*D, 5] {y, x, h, w, flip} of each
+    copy's crop box inside its region, ``lut`` fp32 [C, 256], ``size`` (OH, OW).  ``host`` holds CPU copies of index and
+    draws plus the number of region bytes in use: input_prep_u8_rrc validates them before any launch, without a device
+    read-back.  The kernel reads the tables at run time, so a captured graph follows new values in place."""
+    __slots__ = ('index', 'draws', 'lut', 'duplicates', 'size', 'host')
+
+    def __init__(self, index, draws, lut, duplicates, size, host):
+        self.index, self.draws, self.lut, self.duplicates = index, draws, lut, int(duplicates)
+        self.size, self.host = (int(size[0]), int(size[1])), host
+
+    @property
+    def key(self):
+        return ('rrc', tuple(self.index.shape), self.duplicates, self.size, self.lut.data_ptr())
+
+    @property
+    def tables(self):
+        return (self.index, self.draws)
+
+    def with_tables(self, tables):
+        return Rrc(tables[0], tables[1], self.lut, self.duplicates, self.size, self.host)
+
+
+def check_rrc_tables(index, draws, nbytes, C, D):
+    """Host-side validation of resized-crop tables (CPU int64 [B, 3] index, int32 [B*D, 5] draws): every region lies
+    inside the first ``nbytes`` bytes of the buffer and every crop box inside its region.  Raises B200Error."""
+    if index.dim() != 2 or index.shape[1] != 3 or draws.dim() != 2 or draws.shape[1] != 5 \
+            or draws.shape[0] != index.shape[0] * D:
+        raise _l.B200Error("input_prep_u8_rrc: index must be [B, 3] and draws [B*D, 5]; got %s, %s (D=%d)"
+                           % (tuple(index.shape), tuple(draws.shape), D))
+    off, h, w = (index[:, k].long() for k in range(3))
+    if bool(((off < 0) | (h < 1) | (w < 1) | (h > 65535) | (w > 65535) | (off + h * w * C > nbytes)).any()):
+        raise _l.B200Error("input_prep_u8_rrc: a region lies outside the %d-byte buffer" % nbytes)
+    d = draws.long()
+    rh, rw = h.repeat_interleave(D), w.repeat_interleave(D)
+    if bool(((d[:, 0] < 0) | (d[:, 1] < 0) | (d[:, 2] < 1) | (d[:, 3] < 1) | (d[:, 0] + d[:, 2] > rh)
+             | (d[:, 1] + d[:, 3] > rw) | (d[:, 4] < 0) | (d[:, 4] > 1)).any()):
+        raise _l.B200Error("input_prep_u8_rrc: a crop box lies outside its region")
+
+
+def input_prep_u8_rrc(regions, cpad, rrc, s2d=False, border=False, out=None):
+    """uint8 region buffer -> bf16 [B*D, OH, OW, cpad] (or the bordered space-to-depth layout): RandomResizedCrop with
+    Pillow's bilinear resample, flip and normalisation through rrc.lut; row b*D + d = copy d of image b."""
+    _chk(regions, torch.uint8, "regions"); _chk(rrc.index, torch.int64, "index"); _chk(rrc.draws, torch.int32, "draws")
+    _chk(rrc.lut, torch.float32, "lut")
+    if s2d and not border:
+        raise _l.B200Error("input_prep_u8_rrc: the space-to-depth layout needs the border (mode 2)")
+    if regions.dim() != 1 or rrc.lut.dim() != 2 or rrc.lut.shape[1] != 256:
+        raise _l.B200Error("input_prep_u8_rrc: regions must be a flat uint8 buffer and lut fp32 [C, 256]")
+    C, D = rrc.lut.shape[0], rrc.duplicates
+    (OH, OW), B = rrc.size, rrc.index.shape[0]
+    h_index, h_draws, nbytes = rrc.host
+    if nbytes > regions.numel() or tuple(h_index.shape) != tuple(rrc.index.shape) \
+            or tuple(h_draws.shape) != tuple(rrc.draws.shape):
+        raise _l.B200Error("input_prep_u8_rrc: host tables do not describe the device tables and buffer")
+    check_rrc_tables(h_index, h_draws, nbytes, C, D)
+    out = _prep_out(B * D, OH, OW, cpad, s2d, border, regions.device, out)
+    mode = 2 if s2d else 0
+    nbytes_read = int((h_index[:, 1].long() * h_index[:, 2].long()).sum()) * C
+    with _T('input_prep', 0, nbytes_read + 8 * rrc.index.numel() + 4 * rrc.draws.numel() + 2 * out.numel()):
+        _l.check(_l.load().b200_input_prep_u8_rrc(regions.data_ptr(), regions.numel(), rrc.index.data_ptr(),
+                                                  rrc.draws.data_ptr(), B, D, C, OH, OW, cpad, mode,
+                                                  rrc.lut.data_ptr(), out.data_ptr(), _stream()),
+                 "b200_input_prep_u8_rrc")
+    return out
+
 
 def input_prep_u8_aug(x_nhwc_u8, cpad, aug, out=None):
     """uint8 NHWC [N,H,W,C] -> bf16 NHWC [N*D, H, W, cpad]: the D augmented copies of every image (crop, flip, Cutout)

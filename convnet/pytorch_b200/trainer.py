@@ -18,9 +18,10 @@ SURVEY.md section 2.3 C1/C2), and the per-tensor unscale / clip loops of the ref
 MixUp / CutMix (``mixup`` / ``cutmix``, trainer.py:44-51,119-138): drawn on the host per training chunk by
 utils/mixup.py; on the fused B200 path the input relayout and loss kernels do the mixing (see ``_upload_mix``).
 
-Batch augmentation on the device (a loader yielding utils.augment.AugmentedBatch, data.py ``device_augment``): on the
-fused B200 path the stem relayout kernel writes the B*D augmented copies from the uint8 images and their draws; every
-other path trains on ``AugmentedBatch.apply()``, the same fp32 batch.  The meters count B*D samples.
+Augmentation on the device (a loader yielding a utils.augment.DeviceBatch: an AugmentedBatch of data.py
+``device_augment`` or a ResizedCropBatch of ``device_resized_crop``): on the fused B200 path the stem relayout kernel
+writes the B*D augmented copies from the uint8 data and its draws; every other path trains on the batch's ``apply()``,
+the same fp32 batch.  The meters count B*D samples.
 """
 import logging
 import random
@@ -34,7 +35,7 @@ from torch.nn.utils import clip_grad_norm_
 
 from .lib import B200Error, MIX_CUTMIX, MIX_MIXUP
 from .utils import regularization
-from .utils.augment import AugmentedBatch
+from .utils.augment import DeviceBatch, ResizedCropBatch
 from .utils.meters import AverageMeter, accuracy
 from .utils.mixup import CutMix, MixUp
 
@@ -79,41 +80,56 @@ def _cuda_prefetch(loader, device, dtype):
     """Yield device-resident batches one step ahead: batch i+1 is copied host->device on a side stream while
     step i computes (the reference issues a blocking copy at the top of every step, trainer.py:116-117).
     The copies land in a ring of three persistent device buffers per (shape, dtype): no caching-allocator traffic per
-    step (a fresh 154 MB tensor per batch that is handed across streams made the allocator stall now and then)."""
+    step (a fresh 154 MB tensor per batch that is handed across streams made the allocator stall now and then).
+    A DeviceBatch's tensors travel together, in the same slot.  The region buffer of a ResizedCropBatch changes size
+    every step: its slots are keyed on a capacity instead, which grows by at least half when a batch does not fit."""
     copy_stream = torch.cuda.Stream(device=device)
-    ring = {}          # (shape, dtype) of x and y -> [[x_buf, y_buf, consumed_event or None, draws_buf], ...]
+    ring = {}          # shapes and dtypes -> [[x_buf, y_buf, consumed_event or None, (other device tensors)], ...]
     turn = {}
+    capacity = {}      # ring key of ragged batches -> region-buffer bytes
 
     def stage(inputs, target):
-        # an AugmentedBatch: its uint8 images and its draw table travel together, in the same slot
-        spec = inputs.spec if isinstance(inputs, AugmentedBatch) else None
-        draws = inputs.params if spec is not None else None
-        x = inputs.images if spec is not None else inputs
+        batch = inputs if isinstance(inputs, DeviceBatch) else None
+        host = batch.tensors if batch is not None else (inputs,)
+        x, rest = host[0], host[1:]
         x_dtype = x.dtype if x.dtype == torch.uint8 else dtype     # uint8 image batches stay uint8
-        key = (tuple(x.shape), x_dtype, tuple(target.shape), target.dtype,
-               tuple(draws.shape) if draws is not None else None)
+        ragged = isinstance(batch, ResizedCropBatch)
+        key = (type(batch), None if ragged else tuple(x.shape), x_dtype, tuple(target.shape), target.dtype,
+               tuple((tuple(t.shape), t.dtype) for t in rest))
+        shape = tuple(x.shape)
+        if ragged:
+            cap = capacity.get(key, 0)
+            if x.numel() > cap:
+                cap = capacity[key] = -(-max(x.numel(), cap * 3 // 2) // (1 << 20)) * (1 << 20)
+            shape = (cap,)
         slots = ring.setdefault(key, [])
         k = turn.get(key, 0)
         turn[key] = (k + 1) % 3
-        if len(slots) <= k:
-            slots.append([torch.empty(x.shape, device=device, dtype=x_dtype),
-                          torch.empty(target.shape, device=device, dtype=target.dtype), None,
-                          torch.empty(draws.shape, device=device, dtype=draws.dtype) if draws is not None else None])
+        if len(slots) <= k or tuple(slots[k][0].shape) != shape:
+            if len(slots) > k and slots[k][2] is not None:
+                slots[k][2].synchronize()                 # a grown region buffer replaces one its step has finished with
+            new = [torch.empty(shape, device=device, dtype=x_dtype),
+                   torch.empty(target.shape, device=device, dtype=target.dtype), None,
+                   tuple(torch.empty(t.shape, device=device, dtype=t.dtype) for t in rest)]
+            if len(slots) <= k:
+                slots.append(new)
+            else:
+                slots[k] = new
         slot = slots[k]
         with torch.cuda.stream(copy_stream):
             if slot[2] is not None:
                 copy_stream.wait_event(slot[2])            # the step that read this slot has been enqueued AND has run
-            slot[0].copy_(x, non_blocking=True)
+            (slot[0][:x.numel()] if ragged else slot[0]).copy_(x, non_blocking=True)
             slot[1].copy_(target, non_blocking=True)
-            if draws is not None:
-                slot[3].copy_(draws, non_blocking=True)
+            for d, t in zip(slot[3], rest):
+                d.copy_(t, non_blocking=True)
             ready = torch.cuda.Event()
             ready.record(copy_stream)
-        return slot, ready, spec
+        return slot, ready, batch
 
-    def hand_over(slot, ready, spec):
+    def hand_over(slot, ready, batch):
         torch.cuda.current_stream(device).wait_event(ready)
-        return (slot[0] if spec is None else AugmentedBatch(slot[0], slot[3], spec)), slot[1]
+        return (slot[0] if batch is None else batch.replace((slot[0],) + slot[3])), slot[1]
 
     def release(slot):
         ev = torch.cuda.Event()
@@ -277,15 +293,15 @@ class Trainer(object):
         a new shape, unsupported configuration).  Gradients land in the arena exactly as in the eager path.
         ``mix`` (ops.Mix, from _upload_mix): the step mixes its input; the graph reads the permutation, lambda and box
         from their persistent device buffers, so every replay uses the values uploaded for that step.
-        ``aug`` (ops.Aug, from _device_aug): the step augments its uint8 images on the device; the graph reads the draws
-        from a static buffer refreshed like the input, so every replay uses that step's draws."""
+        ``aug`` (ops.Aug or ops.Rrc, from _device_aug): the step augments its uint8 data on the device; the graph reads
+        the draw tables from static buffers refreshed like the input, so every replay uses that step's draws."""
         if not self._graph_eligible() or not inputs.is_cuda:
             return None
         # loss / gradient scales are NOT part of the key: they reach the kernels through a device scalar; neither are
         # the mixing draws (device buffers) -- only the kind of mixing
         key = (tuple(inputs.shape), inputs.dtype, tuple(target.shape), target.dtype, self._model.training,
                mix.kind if mix is not None else 0,
-               (tuple(aug.params.shape), aug.duplicates, aug.pad, aug.lut.data_ptr()) if aug is not None else None)
+               aug.key if aug is not None else None)
         st = self._graphs.get(key)
         if st is None:
             st = self._graphs[key] = {'seen': 0, 'graph': None}
@@ -310,7 +326,8 @@ class Trainer(object):
         st['x'].copy_(inputs, non_blocking=True)
         st['y'].copy_(target, non_blocking=True)
         if aug is not None:
-            st['aug'].copy_(aug.params, non_blocking=True)
+            for dst, src in zip(st['aug'], aug.tables):
+                dst.copy_(src, non_blocking=True)
         self._upstream()                          # refresh the device scalar if a scale changed
         st['graph'].replay()
         self.graph_replays += 1
@@ -322,7 +339,7 @@ class Trainer(object):
         x_s, y_s = torch.empty_like(inputs), torch.empty_like(target)
         x_s.copy_(inputs)
         y_s.copy_(target)
-        aug_s = ops.Aug(aug.params.clone(), aug.lut, aug.duplicates, aug.pad) if aug is not None else None
+        aug_s = aug.with_tables(tuple(t.clone() for t in aug.tables)) if aug is not None else None
         if self._graph_pool is None:
             self._graph_pool = torch.cuda.graph_pool_handle()
         graph = torch.cuda.CUDAGraph()
@@ -347,7 +364,7 @@ class Trainer(object):
                 out = self.model(x_s)
                 loss = self.criterion(out, y_s)
                 torch.autograd.backward(loss, grad_tensors=[up])
-        st.update(graph=graph, x=x_s, y=y_s, aug=aug_s.params if aug_s is not None else None, out=out, loss=loss,
+        st.update(graph=graph, x=x_s, y=y_s, aug=aug_s.tables if aug_s is not None else None, out=out, loss=loss,
                   stats=stats, launches=lib.launch_count() - n0)
 
     def release_graphs(self):
@@ -416,12 +433,11 @@ class Trainer(object):
             self.optimizer.zero_grad()
             self.optimizer.update(self.epoch, self.training_steps)
         aug = None
-        if isinstance(inputs_batch, AugmentedBatch):
+        if isinstance(inputs_batch, DeviceBatch):
             if training and self.b200 is not None and chunk_batch == 1 and not average_output \
                     and 'cuda' in str(self.device) and self._hooks_static() and self._plain_ce_eps() is not None \
                     and target_batch.dtype == torch.long and target_batch.dim() == 1:
-                aug = self._device_aug(inputs_batch)
-                inputs_batch = inputs_batch.images
+                aug, inputs_batch = self._device_aug(inputs_batch)
             else:
                 inputs_batch = inputs_batch.apply()     # the same fp32 batch the fused relayout would compute
 
@@ -571,18 +587,25 @@ class Trainer(object):
 
     # ------------------------------------------------------------------ batch augmentation on the device
     def _device_aug(self, batch):
-        """-> ops.Aug over the batch's draws on the training device and a persistent device LUT of its normalisation
-        (one per statistics, channel count and device, so that a captured graph keeps reading a live tensor)."""
+        """-> (ops.Aug or ops.Rrc over the batch's draws on the training device and a persistent device LUT of its
+        normalisation -- one per statistics, channel count and device, so that a captured graph keeps reading a live
+        tensor --, the uint8 tensor the relayout reads).  Resized-crop tables are validated on the host here: a graph
+        replay runs the kernel without passing through ops.input_prep_u8_rrc."""
         from . import ops
         spec = batch.spec
         device = torch.device(self.device)
-        C = batch.images.shape[-1]
+        C = batch.channels if isinstance(batch, ResizedCropBatch) else batch.images.shape[-1]
         key = (tuple(spec.normalize['mean']), tuple(spec.normalize['std']), C, str(device))
         lut = self._aug_luts.get(key)
         if lut is None:
             lut = self._aug_luts[key] = spec.lut(C).to(device)
+        if isinstance(batch, ResizedCropBatch):
+            ops.check_rrc_tables(batch.host[0], batch.host[1], batch.nbytes, C, spec.duplicates)
+            rrc = ops.Rrc(batch.index.to(device, non_blocking=True), batch.draws.to(device, non_blocking=True), lut,
+                          spec.duplicates, spec.size, batch.host + (batch.nbytes,))
+            return rrc, batch.regions
         params = batch.params.to(device, non_blocking=True).reshape(-1, batch.params.shape[-1])
-        return ops.Aug(params, lut, spec.duplicates, spec.padding)
+        return ops.Aug(params, lut, spec.duplicates, spec.padding), batch.images
 
     def _check_device_augment(self, training, average_output):
         if average_output:
@@ -630,9 +653,9 @@ class Trainer(object):
                 meters['prec5'].update(float(v[2]), n)
 
         for i, (inputs, target) in enumerate(batches):
-            if isinstance(inputs, AugmentedBatch):
+            if isinstance(inputs, DeviceBatch):
                 self._check_device_augment(training, average_output)
-            duplicates = not isinstance(inputs, AugmentedBatch) and inputs.dim() > 4  # B x D x C x H x W
+            duplicates = not isinstance(inputs, DeviceBatch) and inputs.dim() > 4  # B x D x C x H x W
             if training and duplicates and self.adapt_grad_norm is not None and i % self.adapt_grad_norm == 0:
                 per_copy = sum(float(self._grad_norm(inputs.select(1, j), target)) for j in range(inputs.size(1)))
                 per_copy /= inputs.size(1)
@@ -646,7 +669,7 @@ class Trainer(object):
                                                      expand_target=not average_output)
             output, loss, grad = self._step(inputs, target, training=training, average_output=average_output,
                                             chunk_batch=chunk_batch)
-            n = inputs.rows if isinstance(inputs, AugmentedBatch) else inputs.size(0)
+            n = inputs.rows if isinstance(inputs, DeviceBatch) else inputs.size(0)
             if torch.is_tensor(loss):              # fused statistics: asynchronous read-back
                 if pinned is None:
                     pinned = torch.empty((ring, 3), dtype=torch.float32).pin_memory()

@@ -39,6 +39,17 @@ class Cutout(object):
         return img * torch.from_numpy(mask).expand_as(img)
 
 
+def normalize_lut(normalize, C):
+    """fp32 [C, 256]: entry [c][u] = Normalize(ToTensor(u)) in torchvision's fp32 arithmetic -- u.float().div(255),
+    then .sub(mean[c]).div(std[c])."""
+    if len(normalize['mean']) < C or len(normalize['std']) < C:
+        raise ValueError('normalisation statistics for fewer than %d channels' % C)
+    u = torch.arange(256, dtype=torch.uint8).to(torch.float32).div(255).expand(C, 256)
+    mean = torch.as_tensor(normalize['mean'][:C], dtype=torch.float32).view(C, 1)
+    std = torch.as_tensor(normalize['std'][:C], dtype=torch.float32).view(C, 1)
+    return u.sub(mean).div(std).contiguous()
+
+
 class BatchAugment(object):
     """``duplicates`` copies per image of RandomCrop(padding) + RandomHorizontalFlip (``flip``) + ToTensor + Normalize
     (``normalize``: {'mean', 'std'}) + Cutout (``cutout``: None or {'holes', 'length'})."""
@@ -83,12 +94,7 @@ class BatchAugment(object):
         then .sub(mean[c]).div(std[c])."""
         t = self._luts.get(C)
         if t is None:
-            if len(self.normalize['mean']) < C or len(self.normalize['std']) < C:
-                raise ValueError('BatchAugment: normalisation statistics for fewer than %d channels' % C)
-            u = torch.arange(256, dtype=torch.uint8).to(torch.float32).div(255).expand(C, 256)
-            mean = torch.as_tensor(self.normalize['mean'][:C], dtype=torch.float32).view(C, 1)
-            std = torch.as_tensor(self.normalize['std'][:C], dtype=torch.float32).view(C, 1)
-            t = self._luts[C] = u.sub(mean).div(std).contiguous()
+            t = self._luts[C] = normalize_lut(self.normalize, C)
         return t
 
     def apply(self, images, params):
@@ -121,9 +127,19 @@ class BatchAugment(object):
         return v
 
 
-class AugmentedBatch(object):
-    """What a device-augmenting loader yields in place of the [B, D, C, H, W] batch: the B uint8 NHWC ``images``, the
-    int16 ``params`` [B, D, P] of ``spec`` (a BatchAugment).  The batch stands for spec.duplicates * B rows."""
+class DeviceBatch(object):
+    """What a device-augmenting loader yields in place of the fp32 batch.  ``rows``: the number of training rows it
+    stands for; ``apply()``: that fp32 NCHW batch, computed on the host (every non-fused path and the tests' oracle);
+    ``pin_memory()``; ``tensors``: the host tensors the device needs, which ``replace`` swaps for their device copies."""
+    __slots__ = ()
+
+    def pin_memory(self):
+        return self.replace(tuple(t.pin_memory() for t in self.tensors))
+
+
+class AugmentedBatch(DeviceBatch):
+    """The B uint8 NHWC ``images`` and the int16 ``params`` [B, D, P] of ``spec`` (a BatchAugment).  The batch stands
+    for spec.duplicates * B rows."""
     __slots__ = ('images', 'params', 'spec')
 
     def __init__(self, images, params, spec):
@@ -137,8 +153,12 @@ class AugmentedBatch(object):
         """-> fp32 NCHW [B*D, C, H, W] on the images' device."""
         return self.spec.apply(self.images, self.params)
 
-    def pin_memory(self):
-        return AugmentedBatch(self.images.pin_memory(), self.params.pin_memory(), self.spec)
+    @property
+    def tensors(self):
+        return (self.images, self.params)
+
+    def replace(self, tensors):
+        return AugmentedBatch(tensors[0], tensors[1], self.spec)
 
 
 class AugmentCollate(object):
@@ -154,4 +174,122 @@ class AugmentCollate(object):
         target = torch.as_tensor([int(t) for _, t in batch], dtype=torch.long)
         B, H, W, _ = images.shape
         return AugmentedBatch(images, self.spec.sample(B, H, W), self.spec), \
+            target.repeat_interleave(self.spec.duplicates)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# RandomResizedCrop on the device (the ImageNet training transform, preprocess.py:71-77 of the reference).  The loader
+# workers decode and draw; each image ships only its region -- the bounding box of its D crop boxes -- in one flat
+# uint8 buffer, and the stem relayout kernel resamples, flips and normalises (ops.input_prep_u8_rrc).
+
+class ResizedCrop(object):
+    """``duplicates`` copies per image of RandomResizedCrop(size, scale, ratio) (bilinear) + RandomHorizontalFlip +
+    ToTensor + Normalize (``normalize``: {'mean', 'std'})."""
+
+    def __init__(self, size, duplicates=1, normalize=None, scale=(0.08, 1.0), ratio=(3. / 4., 4. / 3.)):
+        self.size = (int(size), int(size)) if isinstance(size, int) else (int(size[0]), int(size[1]))
+        self.duplicates = int(duplicates)
+        self.normalize = normalize or _IMAGE_STATS
+        self.scale, self.ratio = scale, ratio
+        if self.duplicates < 1 or min(self.size) < 1:
+            raise ValueError('ResizedCrop: duplicates and size must be >= 1')
+        self._luts = {}
+
+    def lut(self, C):
+        t = self._luts.get(C)
+        if t is None:
+            t = self._luts[C] = normalize_lut(self.normalize, C)
+        return t
+
+    def draw(self, img):
+        """int32 [D, 5] crop boxes {top, left, height, width, flip} in the coordinates of ``img`` (a PIL image): for
+        each copy RandomResizedCrop.get_params, then torch.rand(1) < 0.5 -- the reference transform's calls in its
+        order, so equal seeds give its per-image stream."""
+        import torchvision.transforms as T
+        out = torch.empty((self.duplicates, 5), dtype=torch.int32)
+        for d in range(self.duplicates):
+            i, j, h, w = T.RandomResizedCrop.get_params(img, self.scale, self.ratio)
+            out[d] = torch.tensor([i, j, h, w, int(torch.rand(1) < 0.5)], dtype=torch.int32)
+        return out
+
+    def __call__(self, img):
+        """PIL image -> (uint8 HWC region, int32 [D, 5] draws relative to the region): the loader's per-image work."""
+        draws = self.draw(img)
+        y0, x0 = int(draws[:, 0].min()), int(draws[:, 1].min())
+        y1, x1 = int((draws[:, 0] + draws[:, 2]).max()), int((draws[:, 1] + draws[:, 3]).max())
+        a = np.asarray(img)
+        region = torch.from_numpy(np.array(a[y0:y1, x0:x1].reshape(y1 - y0, x1 - x0, -1), copy=True))
+        draws[:, 0] -= y0
+        draws[:, 1] -= x0
+        return region, draws
+
+    def apply(self, regions, index, draws, C):
+        """-> fp32 NCHW [B*D, C, OH, OW]: torchvision's own resized_crop / hflip / to_tensor / normalize on PIL images
+        built from the C-channel regions (the reference's arithmetic by construction)."""
+        import torchvision.transforms.functional as F
+        from PIL import Image
+        from torchvision.transforms import InterpolationMode
+        D = draws.shape[0] // index.shape[0]
+        regions = regions.cpu()
+        out = []
+        for b in range(index.shape[0]):
+            off, h, w = (int(v) for v in index[b])
+            px = regions[off:off + h * w * C].reshape(h, w, C).numpy()
+            img = Image.fromarray(px[:, :, 0] if C == 1 else px, 'L' if C == 1 else 'RGB')
+            for d in range(D):
+                y, x, ch, cw, flip = (int(v) for v in draws[b * D + d])
+                t = F.resized_crop(img, y, x, ch, cw, list(self.size), InterpolationMode.BILINEAR)
+                if flip:
+                    t = F.hflip(t)
+                out.append(F.normalize(F.to_tensor(t), **self.normalize))
+        return torch.stack(out)
+
+
+class ResizedCropBatch(DeviceBatch):
+    """B images' regions in one flat uint8 buffer ``regions`` (HWC, ``channels`` per pixel, the first ``nbytes`` bytes
+    in use), ``index`` int64 [B, 3] {byte offset, h, w} and ``draws`` int32 [B*D, 5] {y, x, h, w, flip} of ``spec`` (a
+    ResizedCrop) relative to each region.  Stands for B*D rows, row b*D + d = copy d of image b.  ``host`` keeps the CPU
+    index and draws once the tensors have been staged on a device (their validation needs no device read-back)."""
+    __slots__ = ('regions', 'index', 'draws', 'spec', 'channels', 'nbytes', 'host')
+
+    def __init__(self, regions, index, draws, spec, channels, nbytes=None, host=None):
+        self.regions, self.index, self.draws, self.spec = regions, index, draws, spec
+        self.channels = int(channels)
+        self.nbytes = int(regions.numel() if nbytes is None else nbytes)
+        self.host = host if host is not None else (index, draws)
+
+    @property
+    def rows(self):
+        return self.draws.shape[0]
+
+    def apply(self):
+        """-> fp32 NCHW [B*D, C, OH, OW] on the host."""
+        return self.spec.apply(self.regions[:self.nbytes], self.host[0], self.host[1], self.channels)
+
+    @property
+    def tensors(self):
+        return (self.regions, self.index, self.draws)
+
+    def replace(self, tensors):
+        return ResizedCropBatch(tensors[0], tensors[1], tensors[2], self.spec, self.channels, self.nbytes, self.host)
+
+
+class ResizedCropCollate(object):
+    """DataLoader ``collate_fn`` of a resized-crop loader: packs the (region, draws) samples made by ResizedCrop in the
+    workers into one ResizedCropBatch.  -> (batch, target repeated to B*D, row b*D + d)."""
+
+    def __init__(self, spec):
+        self.spec = spec
+
+    def __call__(self, batch):
+        regions = [r for (r, _), _ in batch]
+        sizes = [r.numel() for r in regions]
+        offsets = [0]
+        for s in sizes[:-1]:
+            offsets.append(offsets[-1] + s)
+        index = torch.tensor([[o, r.shape[0], r.shape[1]] for o, r in zip(offsets, regions)], dtype=torch.int64)
+        draws = torch.cat([d for (_, d), _ in batch])
+        target = torch.as_tensor([int(t) for _, t in batch], dtype=torch.long)
+        flat = torch.cat([r.reshape(-1) for r in regions])
+        return ResizedCropBatch(flat, index, draws, self.spec, regions[0].shape[2]), \
             target.repeat_interleave(self.spec.duplicates)

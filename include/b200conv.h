@@ -5,7 +5,7 @@
  * The reference has no FFI of its own (it is pure Python on top of torch.nn); every entry point
  * below replaces one implicit torch/cuDNN/ATen operator the reference invokes, cited per function
  * as reference file:line (paths under the reference tree).  INTEGRATION.md shows the ctypes stubs.
- * 46 entry points.
+ * 47 entry points.
  *
  * Conventions
  *  - every function returns 0 on success or a negative B200_ERR_* code; b200_last_error() gives text.
@@ -192,6 +192,18 @@ int b200_input_prep_u8_mix(const uint8_t* x_nhwc, int N, int C, int H, int W, in
  * reads them at run time, so a captured CUDA graph follows each step's draws. */
 int b200_input_prep_u8_aug(const uint8_t* x_nhwc, int N, int D, int C, int H, int W, int Cpad, int pad, const float* lut,
                            const int16_t* params, int holes, void* out, b200_stream_t stream);
+/* RandomResizedCrop + RandomHorizontalFlip + ToTensor + Normalize of the ImageNet training transform (preprocess.py:71-77,
+ * with multi_transform's duplicates, :105-112) fused into the stem relayout.  regions: one DEVICE uint8 buffer of
+ * region_bytes bytes holding B uint8 HWC images' regions; index (DEVICE int64 [B][3]) = {byte offset, h, w} of each;
+ * draws (DEVICE int32 [B*D][5]) = {y, x, h, w, flip} of each copy's crop box inside its region.  Output row n is copy
+ * n % D of image n / D: the crop resampled to OH x OW exactly as Pillow's 8-bit BILINEAR resize does (the crop is the
+ * whole image: taps clamp at its edges), mirrored when flip != 0, then v = lut[c][u] (DEVICE fp32 [C][256]) rounded once
+ * to bf16.  mode 0: out [B*D][OH][OW][Cpad] (Cpad >= C); mode 2: the padded space-to-depth layout of b200_input_prep
+ * (even OH, OW; Cpad >= 4C).  C <= 4, OW <= 512, B*D <= 65535.  Any table values are memory-safe (every read is clamped
+ * to its region and to region_bytes); the grid depends on (B*D, OH, OW) only, so a captured graph follows new tables. */
+int b200_input_prep_u8_rrc(const uint8_t* regions, long long region_bytes, const long long* index, const int* draws,
+                           int B, int D, int C, int OH, int OW, int Cpad, int mode, const float* lut, void* out,
+                           b200_stream_t stream);
 /* bf16 [K][T][C] -> bf16 [C][T][K] (dgrad weight layout), multi-tensor: n tensors described by
  * device arrays. */
 int b200_weight_transpose(const void* src, void* dst, int K, int T, int C, b200_stream_t stream);
