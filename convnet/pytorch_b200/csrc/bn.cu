@@ -12,28 +12,10 @@
 // accumulators).  The backward reduction writes one partial row per block and a second tiny kernel sums them in a
 // fixed order (no atomics: same-address fp64 atomics at the end of ~600 blocks cost more than the extra launch).
 // The workspace must be zero before first use and must not be shared by concurrent streams.
-#include "common.cuh"
-#include "host.h"
+#include "bn_common.cuh"
 
 namespace b200 {
 
-constexpr int kBnThreads = 256;
-constexpr int kBnMaxC = 2048;
-constexpr int kBnMaxBlocks = 1184;  // 8 per SM on 148 SMs
-constexpr int kReplicas = 16;         // accumulator copies: spreads same-address fp64 atomics over 16 lines
-constexpr int kAccumFloats = kReplicas * 2 * kBnMaxC * 2 + 64;  // replicas x 2*C doubles + ticket counter
-constexpr int kMaxPartialBlocks = 6 * 148;                         // backward reduce: per-block partial rows
-constexpr int kWsFloats = kAccumFloats + kMaxPartialBlocks * 2 * kBnMaxC;
-
-struct RowMap {
-  int cv, rows_per_iter;
-};
-static inline RowMap make_rowmap(int C) {
-  RowMap m;
-  m.cv = C / 8;
-  m.rows_per_iter = kBnThreads / m.cv;
-  return m;
-}
 static inline int reduce_blocks(long long M, int C, const RowMap& rm, int resident_per_sm = 6) {
   long long iters = (M + rm.rows_per_iter - 1) / rm.rows_per_iter;
   long long want = (iters + 7) / 8;          // >= 8 row-iterations per block
@@ -45,63 +27,6 @@ static inline int reduce_blocks(long long M, int C, const RowMap& rm, int reside
   if (want < 1) want = 1;
   return (int)want;
 }
-// backward reduce (two-stage, no atomics): one resident wave of fat blocks, each at least 4 row-iterations
-static inline int partial_blocks(long long M, const RowMap& rm, int resident_per_sm) {
-  long long iters = (M + rm.rows_per_iter - 1) / rm.rows_per_iter;
-  long long want = (iters + 3) / 4;
-  long long cap = (long long)resident_per_sm * sm_count();
-  if (cap > kMaxPartialBlocks) cap = kMaxPartialBlocks;
-  if (want > cap) want = cap;
-  if (want < 1) want = 1;
-  return (int)want;
-}
-static inline int stream_blocks(long long M, const RowMap& rm) {
-  long long iters = (M + rm.rows_per_iter - 1) / rm.rows_per_iter;
-  long long blocks = (iters + 15) / 16;
-  if (blocks < 1) blocks = 1;
-  if (blocks > 4 * kBnMaxBlocks) blocks = 4 * kBnMaxBlocks;
-  return (int)blocks;
-}
-
-__device__ __forceinline__ void load8(const __nv_bfloat16* p, float (&f)[8]) {
-  const uint4 u = *reinterpret_cast<const uint4*>(p);
-  float2 a = unpack_bf16x2(u.x), b = unpack_bf16x2(u.y), c = unpack_bf16x2(u.z), d = unpack_bf16x2(u.w);
-  f[0] = a.x; f[1] = a.y; f[2] = b.x; f[3] = b.y; f[4] = c.x; f[5] = c.y; f[6] = d.x; f[7] = d.y;
-}
-// streaming 128-bit load: read-only path, no L1 allocation (every byte is touched once per kernel)
-__device__ __forceinline__ uint4 ld_stream(const __nv_bfloat16* p) {
-  uint4 u;
-  asm volatile("ld.global.nc.L1::no_allocate.v4.u32 {%0,%1,%2,%3}, [%4];"
-               : "=r"(u.x), "=r"(u.y), "=r"(u.z), "=r"(u.w) : "l"(p));
-  return u;
-}
-__device__ __forceinline__ void unpack8(const uint4& u, float (&f)[8]) {
-  float2 a = unpack_bf16x2(u.x), b = unpack_bf16x2(u.y), c = unpack_bf16x2(u.z), d = unpack_bf16x2(u.w);
-  f[0] = a.x; f[1] = a.y; f[2] = b.x; f[3] = b.y; f[4] = c.x; f[5] = c.y; f[6] = d.x; f[7] = d.y;
-}
-__device__ __forceinline__ void store8(__nv_bfloat16* p, const float (&f)[8]) {
-  uint4 u;
-  u.x = pack_bf16x2(f[0], f[1]); u.y = pack_bf16x2(f[2], f[3]);
-  u.z = pack_bf16x2(f[4], f[5]); u.w = pack_bf16x2(f[6], f[7]);
-  *reinterpret_cast<uint4*>(p) = u;
-}
-__device__ __forceinline__ void loadf8(const float* p, float (&f)[8]) {
-  const float4 a = __ldg(reinterpret_cast<const float4*>(p));
-  const float4 b = __ldg(reinterpret_cast<const float4*>(p) + 1);
-  f[0] = a.x; f[1] = a.y; f[2] = a.z; f[3] = a.w; f[4] = b.x; f[5] = b.y; f[6] = b.z; f[7] = b.w;
-}
-// 1 where the activation passes the gradient, evaluated on the PRE-activation value (same test as act_mask on y)
-__device__ __forceinline__ int act_mask_value(float pre, int act) {
-  if (act == B200_ACT_RELU) return pre > 0.f ? 1 : 0;
-  if (act == B200_ACT_RELU6) return (pre > 0.f && pre < 6.f) ? 1 : 0;
-  return 1;
-}
-__device__ __forceinline__ float act_mask(float v, int act) {
-  if (act == B200_ACT_RELU) return v > 0.f ? 1.f : 0.f;
-  if (act == B200_ACT_RELU6) return (v > 0.f && v < 6.f) ? 1.f : 0.f;
-  return 1.f;
-}
-
 // Block partials -> fp64 global accumulators; returns true in the LAST block of the grid (after a grid-wide
 // happens-before: every other block's atomics are visible).
 __device__ __forceinline__ bool accumulate_and_elect(float (&acc)[16], int cv, int rows_per_iter, int C,
@@ -266,25 +191,6 @@ __global__ void bn_eval_coeffs_kernel(int C, const float* gamma, const float* be
   shift[c] = (beta ? beta[c] : 0.f) - rm[c] * sc;
 }
 
-// Activation-mask layout ("row quads"): the bytes of rows 4q..4q+3 for one 8-channel vector form ONE 32-bit word,
-// word index q * (C/8) + v8.  A backward thread that owns ROWS consecutive rows fetches their masks with a single
-// 16/32-bit load -- with a plain [row][C/8] byte layout every row cost its own load instruction, and the kernels are
-// bound by requests in flight, not by bytes (that version was slower than re-reading the bf16 output).
-__device__ __forceinline__ long long mask_byte_index(long long row, int cv8, int v8) {
-  return (((row >> 2) * cv8 + v8) << 2) + (row & 3);
-}
-// mask bytes of rows [row0, row0 + ROWS) (row0 % ROWS == 0, ROWS in {2, 4, 8}) for vector v8: byte u = row row0 + u
-template <int ROWS>
-__device__ __forceinline__ unsigned long long mask_rows(const uint8_t* __restrict__ amask, long long row0, int cv8,
-                                                        int v8) {
-  const uint8_t* p = amask + mask_byte_index(row0, cv8, v8);
-  if (ROWS == 2) return __ldg(reinterpret_cast<const unsigned short*>(p));
-  if (ROWS == 4) return __ldg(reinterpret_cast<const unsigned int*>(p));
-  const unsigned long long lo = __ldg(reinterpret_cast<const unsigned int*>(p));
-  const unsigned long long hi = __ldg(reinterpret_cast<const unsigned int*>(p + 4LL * cv8));
-  return lo | (hi << 32);
-}
-
 // ---- forward apply ------------------------------------------------------------------------------
 template <int MODE>  // 0: none, 1: + residual, 2: + (z2*scale2+shift2)
 __global__ void __launch_bounds__(kBnThreads) bn_apply_kernel(
@@ -340,38 +246,6 @@ __global__ void __launch_bounds__(kBnThreads) bn_apply_kernel(
 // g = dy where act'(.) passes, else +0 (selected, not multiplied: dy * 0 would give -0 for negative dy, unlike the
 // mask-bit source and torch's threshold backward), where the activation argument is y when given, else recomputed as
 // z*scale+shift (bit-identical to the forward's fused multiply-add).
-template <int VEC> struct RawVec;
-template <> struct RawVec<4> { uint2 u; };
-template <> struct RawVec<8> { uint4 u; };
-__device__ __forceinline__ RawVec<4> ldv(const __nv_bfloat16* p, RawVec<4>*) {
-  RawVec<4> r;
-  asm volatile("ld.global.nc.L1::no_allocate.v2.u32 {%0,%1}, [%2];" : "=r"(r.u.x), "=r"(r.u.y) : "l"(p));
-  return r;
-}
-__device__ __forceinline__ RawVec<8> ldv(const __nv_bfloat16* p, RawVec<8>*) {
-  RawVec<8> r;
-  r.u = ld_stream(p);
-  return r;
-}
-__device__ __forceinline__ void unpackv(const RawVec<4>& r, float (&f)[4]) {
-  const float2 a = unpack_bf16x2(r.u.x), b = unpack_bf16x2(r.u.y);
-  f[0] = a.x; f[1] = a.y; f[2] = b.x; f[3] = b.y;
-}
-__device__ __forceinline__ void unpackv(const RawVec<8>& r, float (&f)[8]) { unpack8(r.u, f); }
-__device__ __forceinline__ void storev(__nv_bfloat16* p, const float (&f)[4]) {
-  uint2 u;
-  u.x = pack_bf16x2(f[0], f[1]); u.y = pack_bf16x2(f[2], f[3]);
-  *reinterpret_cast<uint2*>(p) = u;
-}
-__device__ __forceinline__ void storev(__nv_bfloat16* p, const float (&f)[8]) { store8(p, f); }
-template <int VEC>
-__device__ __forceinline__ void loadfv(const float* p, float (&f)[VEC]) {
-#pragma unroll
-  for (int i = 0; i < VEC; i += 4) {
-    const float4 a = __ldg(reinterpret_cast<const float4*>(p + i));
-    f[i] = a.x; f[i + 1] = a.y; f[i + 2] = a.z; f[i + 3] = a.w;
-  }
-}
 
 // ---- backward reduce: dbeta = sum g, dgamma = sum g * xhat ------------------------------------------
 // SRC: activation argument 0 recomputed from z, 1 = y, 2 = mask bits
@@ -573,19 +447,6 @@ __global__ void __launch_bounds__(kBnThreads, MINB) bn_bwd_dx_kernel(
   }
 }
 
-template <int VEC>
-static inline RowMap make_rowmap_v(int C) {
-  RowMap m;
-  m.cv = C / VEC;
-  m.rows_per_iter = kBnThreads / m.cv;
-  return m;
-}
-
-static int check_c(int C, const char* who) {
-  B200_REQUIRE(C > 0 && C % 8 == 0 && C <= kBnMaxC, B200_ERR_UNSUPPORTED,
-               "%s: C=%d must be a multiple of 8 and <= %d", who, C, kBnMaxC);
-  return B200_OK;
-}
 static inline double* ws_accum(float* ws) { return reinterpret_cast<double*>(ws); }
 static inline unsigned* ws_ticket(float* ws) { return reinterpret_cast<unsigned*>(ws + kReplicas * 2 * kBnMaxC * 2); }
 

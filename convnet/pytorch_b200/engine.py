@@ -191,10 +191,14 @@ class _Conv(object):
 
 
 class _BN(object):
+    """one BatchNorm layer: nn.BatchNorm2d, or L1BatchNorm2d (``l1``: mean-absolute-deviation scale, csrc/bn_l1.cu)"""
+
     def __init__(self, arena, mod):
+        from .models.modules.lp_norm import L1BatchNorm2d
         if not mod.affine or not mod.track_running_stats:
             raise B200Error('BatchNorm2d without affine/running stats is not supported')
         self.mod = mod
+        self.l1 = isinstance(mod, L1BatchNorm2d)
         self.C = mod.num_features
         sw, sb = arena.slot(mod.weight), arena.slot(mod.bias)
         self.gamma = arena.kernel_view(arena.p32, sw)
@@ -248,7 +252,8 @@ class _SE(object):
 
 class _Unit(object):
     """saved state of one conv+BN unit for backward."""
-    __slots__ = ('x', 'z', 'y', 'w', 'desc', 'mean', 'invstd', 'scale', 'shift', 'sums', 'conv', 'bn', 'act', 'mask')
+    __slots__ = ('x', 'z', 'y', 'w', 'desc', 'mean', 'invstd', 'scale', 'shift', 'sums', 'conv', 'bn', 'act', 'mask',
+                 'sign_sum')
 
 
 class Runtime(object):
@@ -261,7 +266,9 @@ class Runtime(object):
         for name, buf in model.named_buffers():
             buf.data = buf.data.to(device)
         self._anchor = self.arena.slots[0].param
-        self._max_c = max([m.num_features for m in model.modules() if isinstance(m, nn.BatchNorm2d)] + [8])
+        from .models.modules.lp_norm import L1BatchNorm2d
+        self._max_c = max([m.num_features for m in model.modules() if isinstance(m, (nn.BatchNorm2d, L1BatchNorm2d))]
+                          + [8])
         self._ws = torch.zeros(ops.bn_workspace_floats(self._max_c), device=device, dtype=torch.float32)
         self._wg_stream = torch.cuda.Stream(device=device)   # weight gradients on a second CUDA stream
         self._wg_keep = []
@@ -354,7 +361,8 @@ class Runtime(object):
         return x.float().contiguous(), (lambda t, cpad, **kw: ops.input_prep(t, cpad, mix=mix, **kw)), (N, C, H, W)
 
     # ---- inference: BatchNorm folded into the convolution (reference utils/absorb_bn.py:18-48) ----------------
-    # w' = w * gamma/sqrt(var+eps) per output channel, b' = beta - mean*gamma/sqrt(var+eps): one kernel computes
+    # w' = w * gamma/sqrt(var+eps) per output channel, b' = beta - mean*gamma/sqrt(var+eps) (L1 BN: running_var is
+    # the scale itself, w' = w * gamma*running_var, b' = beta - running_mean*gamma*running_var): one kernel computes
     # act(conv(x, w') + b' [+ residual]) -- no z tensor, no separate BN pass.  Folded weights are cached until the
     # parameters or the running statistics change (arena.version).
     def _folded(self, conv, bn):
@@ -365,7 +373,7 @@ class Runtime(object):
         m = bn.mod
         coef = self._coeffs(2 * bn.C)
         scale, shift = coef[:bn.C], coef[bn.C:]
-        ops.bn_eval_coeffs(bn.gamma, bn.beta, m.running_mean, m.running_var, m.eps, scale, shift)
+        self._eval_coeffs(bn, scale, shift)
         w32 = conv.w32 * scale.view(-1, 1, 1)                      # [K, T, C/g] fp32, once per version (not per step)
         if conv.groups == 1:
             wf = w32.to(torch.bfloat16).contiguous()
@@ -413,24 +421,39 @@ class Runtime(object):
 
     def _conv_and_coeffs(self, u, x, w16, training):
         """z = conv(x) and the BN coefficients; in training the statistics are accumulated by the conv epilogue
-        itself whenever the output width allows it (saves one full read of z)."""
-        if training and ops.can_fuse_bn_stats(u.desc.K):
+        itself whenever the output width allows it (saves one full read of z).  L1 BN needs the mean before it can
+        sum |z - mean|, so its statistics always come from bn_l1_stats."""
+        if training and not u.bn.l1 and ops.can_fuse_bn_stats(u.desc.K):
             u.z = ops.conv_fprop(x, w16, u.desc, bn_stats_ws=self._ws)
             self._bn_coeffs(u, training, fused=True)
         else:
             u.z = ops.conv_fprop(x, w16, u.desc)
             self._bn_coeffs(u, training)
 
+    def _eval_coeffs(self, bn, scale, shift):
+        m = bn.mod
+        if bn.l1:
+            ops.bn_l1_eval_coeffs(bn.gamma, bn.beta, m.running_mean, m.running_var, scale, shift)
+        else:
+            ops.bn_eval_coeffs(bn.gamma, bn.beta, m.running_mean, m.running_var, m.eps, scale, shift)
+
     def _bn_coeffs(self, u, training, fused=False):
         bn = u.bn
         C = bn.C
-        buf = self._coeffs(6 * C)
+        buf = self._coeffs((7 if bn.l1 else 6) * C)
         u.mean, u.invstd, u.scale, u.shift, u.sums = buf[0:C], buf[C:2 * C], buf[2 * C:3 * C], buf[3 * C:4 * C], \
             buf[4 * C:6 * C]
+        u.sign_sum = buf[6 * C:7 * C] if bn.l1 else None
         m = bn.mod
+        if training and self.sync_bn_world > 1 and bn.l1:
+            raise B200Error('SyncBatchNorm is not implemented for L1 BatchNorm')
         if training and self.sync_bn_world > 1 and not fused:
             raise B200Error('SyncBatchNorm on the B200 path needs the conv-epilogue statistics (output channels % 64 == 0)')
-        if training and fused:
+        if training and bn.l1:
+            # invstd holds the L1 scale s: bn_apply and the backward reduction use it like 1/std
+            ops.bn_l1_stats(u.z, bn.gamma, bn.beta, m.eps, m.momentum, m.running_mean, m.running_var, u.mean,
+                            u.invstd, u.sign_sum, u.scale, u.shift, self._ws)
+        elif training and fused:
             M = u.z.numel() // C
             if self.sync_bn_world > 1:
                 # the epilogue accumulators are fp64 [16 replicas][2][C] at the start of the BN workspace: ONE small
@@ -444,7 +467,7 @@ class Runtime(object):
             ops.bn_stats(u.z, bn.gamma, bn.beta, m.eps, m.momentum, m.running_mean, m.running_var,
                          m.num_batches_tracked, u.mean, u.invstd, u.scale, u.shift, self._ws)
         else:
-            ops.bn_eval_coeffs(bn.gamma, bn.beta, m.running_mean, m.running_var, m.eps, u.scale, u.shift)
+            self._eval_coeffs(bn, u.scale, u.shift)
         bias = getattr(u.conv, 'bias32', None) if u.conv is not None else None
         if bias is not None:            # conv bias in front of this BN (never on the ResNet / MobileNet-v2 paths)
             if training:                # the true pre-BN tensor is z + b: only the running mean sees it
@@ -486,7 +509,12 @@ class Runtime(object):
         if self.sync_bn_world > 1:
             self._sync_bn_sums(u.sums)
         g = torch.empty_like(dy) if want_g else None
-        dz = ops.bn_bwd_dx(dy, y_mask, u.z, act, u.mean, u.invstd, bn.gamma, bn.beta, u.sums, g_out=g, act_mask=mask)
+        if bn.l1:     # sums = {sum g*(z-mean)*s, sum g}: the reduction above ran with invstd = s
+            dz = ops.bn_l1_bwd_dx(dy, y_mask, u.z, act, u.mean, u.invstd, u.sign_sum, bn.gamma, bn.beta, u.sums,
+                                  g_out=g, act_mask=mask)
+        else:
+            dz = ops.bn_bwd_dx(dy, y_mask, u.z, act, u.mean, u.invstd, bn.gamma, bn.beta, u.sums, g_out=g,
+                               act_mask=mask)
         return dz, g
 
     # ---- weight gradients on a side stream ----------------------------------------------------------------
@@ -1078,6 +1106,9 @@ def enable_sync_batchnorm(model, process_group=None):
         raise B200Error('enable_sync_batchnorm needs a model converted by convert_b200')
     if not (dist.is_available() and dist.is_initialized()):
         raise B200Error('enable_sync_batchnorm needs an initialised process group')
+    from .models.modules.lp_norm import L1BatchNorm2d
+    if any(isinstance(m, L1BatchNorm2d) for m in model.modules()):
+        raise NotImplementedError('SyncBatchNorm is not implemented for L1 BatchNorm (bn_norm=\'L1\')')
     rt.sync_bn_group = process_group
     rt.sync_bn_world = dist.get_world_size(process_group)
     return model

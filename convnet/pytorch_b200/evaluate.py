@@ -70,12 +70,17 @@ parser = build_parser()
 
 def absorb_bn_torch(model):
     """utils/absorb_bn.py:52-66 for plain torch modules: fold every BatchNorm that directly follows a Conv2d / Linear
-    sibling into it and replace the BatchNorm by Identity."""
+    sibling into it and replace the BatchNorm by Identity.  An L1 BatchNorm folds with its running scale
+    (running_var holds s: y = (x - running_mean) * running_var * weight + bias)."""
+    from .models.modules.lp_norm import L1BatchNorm2d
     prev = None
     for name, m in list(model.named_children()):
-        if isinstance(m, (nn.BatchNorm2d, nn.BatchNorm1d)) and isinstance(prev, (nn.Conv2d, nn.Linear)):
+        if isinstance(m, (nn.BatchNorm2d, nn.BatchNorm1d, L1BatchNorm2d)) and isinstance(prev, (nn.Conv2d, nn.Linear)):
             with torch.no_grad():
-                inv = (m.running_var + m.eps).rsqrt() * (m.weight if m.affine else 1.0)
+                if isinstance(m, L1BatchNorm2d):
+                    inv = m.running_var * m.weight
+                else:
+                    inv = (m.running_var + m.eps).rsqrt() * (m.weight if m.affine else 1.0)
                 shape = (-1,) + (1,) * (prev.weight.dim() - 1)
                 prev.weight.mul_(inv.view(shape))
                 bias = prev.bias if prev.bias is not None else torch.zeros_like(m.running_mean)

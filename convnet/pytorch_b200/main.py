@@ -169,6 +169,10 @@ def main_worker(args):
     if args.model_config != '':
         model_config = dict(model_config, **literal_eval(args.model_config))
     model = models.__dict__[args.model](**model_config)
+    if args.sync_bn:
+        from .models.modules.lp_norm import L1BatchNorm2d
+        if any(isinstance(m, L1BatchNorm2d) for m in model.modules()):
+            raise NotImplementedError('--sync-bn is not implemented for L1 BatchNorm (bn_norm=\'L1\')')
     if args.sync_bn and not use_b200:
         model = nn.SyncBatchNorm.convert_sync_batchnorm(model)
     logging.info('created model with configuration: %s', model_config)

@@ -15,17 +15,24 @@ import math
 import torch
 import torch.nn as nn
 
+from .modules.lp_norm import L1BatchNorm2d
+
 __all__ = ['resnet', 'resnet_se']
+
+
+_BN_TYPES = (nn.BatchNorm2d, L1BatchNorm2d)
+_NORM_LAYERS = {None: nn.BatchNorm2d, 'L1': L1BatchNorm2d}    # model-config 'bn_norm'
 
 
 def init_model(model):
     """He-normal conv weights (fan-out), BN gamma=1/beta=0, zero-init of each block's last BN gamma,
-    fc ~ N(0, 0.01) with zero bias -- the reference's scheme (models/resnet.py:16-31), same RNG order."""
+    fc ~ N(0, 0.01) with zero bias -- the reference's scheme (models/resnet.py:16-31), same RNG order.  L1 BN layers
+    count as BN (the reference sees them through its rebinding of nn.BatchNorm2d)."""
     for m in model.modules():
         if isinstance(m, nn.Conv2d):
             fan_out = m.kernel_size[0] * m.kernel_size[1] * m.out_channels
             m.weight.data.normal_(0, math.sqrt(2. / fan_out))
-        elif isinstance(m, nn.BatchNorm2d):
+        elif isinstance(m, _BN_TYPES):
             m.weight.data.fill_(1)
             m.bias.data.zero_()
     for m in model.modules():
@@ -41,7 +48,7 @@ def weight_decay_config(value=1e-4, log=False):
     """WeightDecay regularizer on everything that is neither a bias nor inside a BatchNorm."""
     return {'name': 'WeightDecay', 'value': value, 'log': log,
             'filter': {'parameter_name': lambda n: not n.endswith('bias'),
-                       'module': lambda m: not isinstance(m, nn.BatchNorm2d)}}
+                       'module': lambda m: not isinstance(m, _BN_TYPES)}}
 
 
 def mixsize_config(sz, base_size, base_batch, base_duplicates, adapt_batch, adapt_duplicates):
@@ -70,13 +77,13 @@ class BasicBlock(nn.Module):
     """3x3 -> BN -> ReLU -> 3x3 -> BN, plus skip, ReLU."""
 
     def __init__(self, inplanes, planes, stride=1, expansion=1, downsample=None, groups=1,
-                 residual_block=None, dropout=0.):
+                 residual_block=None, dropout=0., norm_layer=nn.BatchNorm2d):
         super(BasicBlock, self).__init__()
         self.conv1 = conv3x3(inplanes, planes, stride, groups=groups)
-        self.bn1 = nn.BatchNorm2d(planes)
+        self.bn1 = norm_layer(planes)
         self.relu = nn.ReLU(inplace=True)
         self.conv2 = conv3x3(planes, expansion * planes, groups=groups)
-        self.bn2 = nn.BatchNorm2d(expansion * planes)
+        self.bn2 = norm_layer(expansion * planes)
         self.downsample = downsample
         self.residual_block = residual_block
         self.stride = stride
@@ -96,14 +103,14 @@ class Bottleneck(nn.Module):
     """1x1 -> 3x3 (carries the stride, 'v1.5') -> 1x1 with BN/ReLU in between, plus skip, ReLU."""
 
     def __init__(self, inplanes, planes, stride=1, expansion=4, downsample=None, groups=1,
-                 residual_block=None, dropout=0.):
+                 residual_block=None, dropout=0., norm_layer=nn.BatchNorm2d):
         super(Bottleneck, self).__init__()
         self.conv1 = nn.Conv2d(inplanes, planes, kernel_size=1, bias=False)
-        self.bn1 = nn.BatchNorm2d(planes)
+        self.bn1 = norm_layer(planes)
         self.conv2 = conv3x3(planes, planes, stride=stride, groups=groups)
-        self.bn2 = nn.BatchNorm2d(planes)
+        self.bn2 = norm_layer(planes)
         self.conv3 = nn.Conv2d(planes, planes * expansion, kernel_size=1, bias=False)
-        self.bn3 = nn.BatchNorm2d(planes * expansion)
+        self.bn3 = norm_layer(planes * expansion)
         self.relu = nn.ReLU(inplace=True)
         self.dropout = nn.Dropout(dropout or 0)
         self.downsample = downsample
@@ -123,6 +130,7 @@ class Bottleneck(nn.Module):
 
 class ResNet(nn.Module):
     _b200 = None  # set by engine.convert_b200
+    norm_layer = nn.BatchNorm2d   # class of every BN of the network (the constructors set it: L1BatchNorm2d for bn_norm='L1')
 
     def _make_layer(self, block, planes, blocks, expansion=1, stride=1, groups=1, residual_block=None,
                     dropout=None, mixup=False):
@@ -133,15 +141,15 @@ class ResNet(nn.Module):
         if stride != 1 or self.inplanes != out_planes:
             downsample = nn.Sequential(
                 nn.Conv2d(self.inplanes, out_planes, kernel_size=1, stride=stride, bias=False),
-                nn.BatchNorm2d(out_planes))
+                self.norm_layer(out_planes))
         if residual_block is not None:
             residual_block = residual_block(out_planes)
         stages = [block(self.inplanes, planes, stride, expansion=expansion, downsample=downsample, groups=groups,
-                        residual_block=residual_block, dropout=dropout)]
+                        residual_block=residual_block, dropout=dropout, norm_layer=self.norm_layer)]
         self.inplanes = out_planes
         for _ in range(1, blocks):
             stages.append(block(self.inplanes, planes, expansion=expansion, groups=groups,
-                                residual_block=residual_block, dropout=dropout))
+                                residual_block=residual_block, dropout=dropout, norm_layer=self.norm_layer))
         return nn.Sequential(*stages)
 
     def features(self, x):
@@ -162,13 +170,14 @@ class ResNet_imagenet(ResNet):
                  layers=[3, 4, 23, 3], width=[64, 128, 256, 512], expansion=4, groups=[1, 1, 1, 1],
                  regime='normal', scale_lr=1, ramp_up_lr=True, ramp_up_epochs=5, checkpoint_segments=0,
                  mixup=False, epochs=90, base_devices=4, base_device_batch=64, base_duplicates=1,
-                 base_image_size=224, mix_size_regime='D+'):
+                 base_image_size=224, mix_size_regime='D+', norm_layer=nn.BatchNorm2d):
         super(ResNet_imagenet, self).__init__()
         if checkpoint_segments:
             raise NotImplementedError('activation checkpointing is outside the B200 hot path (SURVEY 2, #23)')
+        self.norm_layer = norm_layer
         self.inplanes = inplanes
         self.conv1 = nn.Conv2d(3, inplanes, kernel_size=7, stride=2, padding=3, bias=False)
-        self.bn1 = nn.BatchNorm2d(inplanes)
+        self.bn1 = norm_layer(inplanes)
         self.relu = nn.ReLU(inplace=True)
         self.maxpool = nn.MaxPool2d(kernel_size=3, stride=2, padding=1)
         for i, (w, n, g) in enumerate(zip(width, layers, groups)):
@@ -233,12 +242,14 @@ class ResNet_imagenet(ResNet):
 
 class ResNet_cifar(ResNet):
     def __init__(self, num_classes=10, inplanes=16, block=BasicBlock, depth=18, width=[16, 32, 64],
-                 groups=[1, 1, 1], residual_block=None, regime='normal', dropout=None, mixup=False):
+                 groups=[1, 1, 1], residual_block=None, regime='normal', dropout=None, mixup=False,
+                 norm_layer=nn.BatchNorm2d):
         super(ResNet_cifar, self).__init__()
+        self.norm_layer = norm_layer
         self.inplanes = inplanes
         n = int((depth - 2) / 6)
         self.conv1 = nn.Conv2d(3, inplanes, kernel_size=3, stride=1, padding=1, bias=False)
-        self.bn1 = nn.BatchNorm2d(inplanes)
+        self.bn1 = norm_layer(inplanes)
         self.relu = nn.ReLU(inplace=True)
         self.maxpool = nn.Identity()
         self.layer1 = self._make_layer(block, width[0], n, groups=groups[0], residual_block=residual_block,
@@ -285,16 +296,23 @@ _IMAGENET_DEPTHS = {
 
 
 def _reject_out_of_scope(config):
-    for key in ('quantize', 'bn_norm'):
-        if config.pop(key, None):
-            raise NotImplementedError("model-config '%s' selects a research variant outside the B200 hot path "
-                                      "(SURVEY.md section 2, rows 24-25)" % key)
+    if config.pop('quantize', None):
+        raise NotImplementedError("model-config 'quantize' selects a research variant outside the B200 hot path "
+                                  "(SURVEY.md section 2, rows 24-25)")
+    bn_norm = config.pop('bn_norm', None) or None
+    if bn_norm not in _NORM_LAYERS:
+        raise NotImplementedError("model-config bn_norm=%r is outside the B200 hot path (supported: 'L1'; "
+                                  "SURVEY.md section 2, row 25)" % (bn_norm,))
+    if bn_norm is not None:
+        config['norm_layer'] = _NORM_LAYERS[bn_norm]
 
 
 def resnet(**config):
     """Factory with the reference's config grammar: dataset in {imagenet*, cifar10, cifar100}, depth, and
-    any constructor kwarg (regime, scale_lr, mix_size_regime, ...).  ``b200=True`` converts the model for
-    the B200 kernel path (equivalent to calling engine.convert_b200 on the result)."""
+    any constructor kwarg (regime, scale_lr, mix_size_regime, ...).  ``bn_norm='L1'`` builds every BatchNorm as
+    models.modules.lp_norm.L1BatchNorm2d (the reference rebinds torch.nn.BatchNorm2d for the whole process instead;
+    nothing global is touched here).  ``b200=True`` converts the model for the B200 kernel path (equivalent to
+    calling engine.convert_b200 on the result)."""
     dataset = config.pop('dataset', 'imagenet')
     use_b200 = config.pop('b200', False)
     _reject_out_of_scope(config)

@@ -274,6 +274,45 @@ def bn_bwd_dx(dy, y, z, act, mean, invstd, gamma, beta, sums, dz=None, g_out=Non
     return dz
 
 
+# ------------------------------------------------------------------------------------ L1 batch norm
+def bn_l1_stats(z, gamma, beta, eps, momentum, running_mean, running_var, mean, invstd, sign_sum, scale, shift,
+                workspace):
+    """L1 batch statistics of z [.., C]: mean, invstd = s = 1/(mean|z-mean|*sqrt(pi/2) + eps), sign_sum =
+    sum sign(z - mean), scale/shift for bn_apply; running buffers (optional) updated with the reference's momentum
+    convention.  Two reads of z."""
+    C = z.shape[-1]
+    M = z.numel() // C
+    _chk(z, bf16, "z")
+    with _T('bn_l1_stats', 0, 2 * 2 * z.numel()):
+        _l.check(_l.load().b200_bn_l1_stats(z.data_ptr(), M, C, _l.ptr(gamma), _l.ptr(beta), float(eps),
+                                            float(momentum), _l.ptr(running_mean), _l.ptr(running_var),
+                                            mean.data_ptr(), invstd.data_ptr(), sign_sum.data_ptr(), scale.data_ptr(),
+                                            shift.data_ptr(), workspace.data_ptr(), _stream()), "b200_bn_l1_stats")
+
+
+def bn_l1_eval_coeffs(gamma, beta, running_mean, running_var, scale, shift):
+    """eval-mode L1 BN: scale = gamma * running_var (the running scale s), shift = beta - running_mean * scale."""
+    C = running_mean.numel()
+    _l.check(_l.load().b200_bn_l1_eval_coeffs(C, _l.ptr(gamma), _l.ptr(beta), running_mean.data_ptr(),
+                                              running_var.data_ptr(), scale.data_ptr(), shift.data_ptr(), _stream()),
+             "b200_bn_l1_eval_coeffs")
+
+
+def bn_l1_bwd_dx(dy, y, z, act, mean, invstd, sign_sum, gamma, beta, sums, dz=None, g_out=None, act_mask=None):
+    """L1 BN input gradient; sums from bn_bwd_reduce called with invstd = s.  y / act_mask / g_out as bn_bwd_dx."""
+    C = z.shape[-1]
+    M = z.numel() // C
+    _chk(dy, bf16, "dy"); _chk(y, bf16, "y"); _chk(z, bf16, "z"); _chk(act_mask, torch.uint8, "act_mask")
+    if dz is None:
+        dz = torch.empty_like(z)
+    with _T('bn_l1_bwd_dx', 0, 2 * z.numel() * (3 + (y is not None and act_mask is None) + (g_out is not None))):
+        _l.check(_l.load().b200_bn_l1_bwd_dx(dy.data_ptr(), _l.ptr(y), _l.ptr(act_mask), z.data_ptr(), M, C, int(act),
+                                             mean.data_ptr(), invstd.data_ptr(), sign_sum.data_ptr(), _l.ptr(gamma),
+                                             _l.ptr(beta), sums.data_ptr(), dz.data_ptr(), _l.ptr(g_out), _stream()),
+                 "b200_bn_l1_bwd_dx")
+    return dz
+
+
 # ------------------------------------------------------------------------------------ pooling
 def _out(out, shape, dtype, device, name):
     """a caller-supplied output (checked: dtype, contiguity, shape) or a new tensor"""

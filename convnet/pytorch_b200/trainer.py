@@ -720,6 +720,9 @@ class Trainer(object):
 
     def calibrate_bn(self, data_loader, num_steps=None):
         """Re-estimate BN running statistics as a cumulative average over the loader (momentum=None)."""
+        from .models.modules.lp_norm import L1BatchNorm2d
+        if any(isinstance(m, L1BatchNorm2d) for m in self.model.modules()):
+            raise NotImplementedError('calibrate_bn is not implemented for L1 BatchNorm layers (bn_norm=\'L1\')')
         for m in self.model.modules():
             if isinstance(m, (nn.BatchNorm2d, nn.BatchNorm1d)):
                 m.momentum = None

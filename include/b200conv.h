@@ -5,7 +5,7 @@
  * The reference has no FFI of its own (it is pure Python on top of torch.nn); every entry point
  * below replaces one implicit torch/cuDNN/ATen operator the reference invokes, cited per function
  * as reference file:line (paths under the reference tree).  INTEGRATION.md shows the ctypes stubs.
- * 47 entry points.
+ * 50 entry points.
  *
  * Conventions
  *  - every function returns 0 on success or a negative B200_ERR_* code; b200_last_error() gives text.
@@ -132,6 +132,27 @@ int b200_bn_bwd_reduce(const void* dy, const void* y, const uint8_t* act_mask, c
 int b200_bn_bwd_dx(const void* dy, const void* y, const uint8_t* act_mask, const void* z, long long M, int C, int act,
                    const float* mean, const float* invstd, const float* gamma, const float* beta,
                    const float* sums, void* dz, void* g_out, b200_stream_t stream);
+
+/* ---- L1 batch norm (csrc/bn_l1.cu) --------------------------------------------------------------
+ * replaces L1BatchNorm2d train/eval forward + backward (models/modules/lp_norm.py:238-291, selected by
+ * models/resnet.py:393-399 with bn_norm='L1'): per channel mu = mean(z), L = mean|z - mu|,
+ * s = 1/(L*sqrt(pi/2) + eps), y = (z - mu)*s*gamma + beta.  b200_bn_apply applies it (scale/shift); the backward
+ * is b200_bn_bwd_reduce with invstd = s (dgamma/dbeta sums and arena accumulation) followed by b200_bn_l1_bwd_dx.
+ * batch statistics -> mean = mu, invstd = s, sign_sum = sum sign(z - mu) [C], scale/shift [C] for apply; running
+ * buffers (nullable) follow the reference: running_mean = running_mean*momentum + mu*(1 - momentum), running_var
+ * likewise with s.  Two reads of z, no atomics: the workspace (b200_bn_workspace_floats(C) floats, as for
+ * b200_bn_stats) holds per-block partial rows; its accumulators are neither read nor written. */
+int b200_bn_l1_stats(const void* z, long long M, int C, const float* gamma, const float* beta, float eps,
+                     float momentum, float* running_mean, float* running_var, float* mean, float* invstd,
+                     float* sign_sum, float* scale, float* shift, float* workspace, b200_stream_t stream);
+/* eval mode: scale = gamma*running_var, shift = beta - running_mean*scale */
+int b200_bn_l1_eval_coeffs(int C, const float* gamma, const float* beta, const float* running_mean,
+                           const float* running_var, float* scale, float* shift, b200_stream_t stream);
+/* dz = gamma*s*(g - sums[C+c]/M) - gamma*s*sqrt(pi/2)*sums[c]/M*(sign(z - mu) - sign_sum/M), sign(0) = 0, with
+ * g, y, act_mask, g_out as in b200_bn_bwd_dx and sums from b200_bn_bwd_reduce(..., invstd = s, ...) */
+int b200_bn_l1_bwd_dx(const void* dy, const void* y, const uint8_t* act_mask, const void* z, long long M, int C,
+                      int act, const float* mean, const float* invstd, const float* sign_sum, const float* gamma,
+                      const float* beta, const float* sums, void* dz, void* g_out, b200_stream_t stream);
 
 /* ---- pooling (csrc/pool.cu) -------------------------------------------------------------------
  * replaces nn.MaxPool2d(3,2,1) (models/resnet.py:230) and nn.AdaptiveAvgPool2d(1) (resnet.py:241) */
