@@ -9,7 +9,6 @@ namespace b200 {
 constexpr int kBnThreads = 256;
 constexpr int kBnMaxC = 2048;
 constexpr int kBnMaxBlocks = 1184;  // 8 per SM on 148 SMs
-constexpr int kReplicas = 16;         // accumulator copies: spreads same-address fp64 atomics over 16 lines
 constexpr int kAccumFloats = kReplicas * 2 * kBnMaxC * 2 + 64;  // replicas x 2*C doubles + ticket counter
 constexpr int kMaxPartialBlocks = 6 * 148;                         // backward reduce: per-block partial rows
 constexpr int kWsFloats = kAccumFloats + kMaxPartialBlocks * 2 * kBnMaxC;

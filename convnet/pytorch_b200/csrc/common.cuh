@@ -14,20 +14,16 @@
 
 namespace b200 {
 
+// The convolution kernels: two consumer warpgroups + a producer warpgroup (only warp 8 works: registers are allocated
+// per warpgroup in wgmma kernels, so 288 threads would cost as much as 384), 128 accumulator rows per tile.
+constexpr int kThreads = 384;
+constexpr int kTileM = 128;
+// BN workspace accumulators: [kReplicas][2][C] fp64 rows (sum, sum of squares).  A block adds into replica
+// blockIdx.x % kReplicas, which spreads same-address fp64 atomics over 16 lines.
+constexpr int kReplicas = 16;
+
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
-}
-
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred = 0;
-  asm volatile(
-      "{\n\t"
-      ".reg .pred P1;\n\t"
-      "elect.sync _|P1, 0xffffffff;\n\t"
-      "selp.b32 %0, 1, 0, P1;\n\t"
-      "}\n"
-      : "=r"(pred));
-  return pred != 0;
 }
 
 // ---------------------------------------------------------------- mbarrier
@@ -124,7 +120,6 @@ __device__ __forceinline__ void tma_store_4d(const void* tmap, const void* src, 
 }
 __device__ __forceinline__ void bulk_commit_group() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 __device__ __forceinline__ void bulk_wait_group_read0() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
-__device__ __forceinline__ void bulk_wait_group_read1() { asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory"); }
 __device__ __forceinline__ void bulk_wait_group0() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
@@ -192,6 +187,17 @@ __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
 __device__ __forceinline__ float2 unpack_bf16x2(uint32_t u) {
   __nv_bfloat162 v = *reinterpret_cast<__nv_bfloat162*>(&u);
   return __bfloat1622float2(v);
+}
+// Byte offset of element (row, c) in a convolution epilogue's bf16 staging tile: 64-channel boxes `pitch` bytes apart,
+// each [rows][128 B] in the 128B swizzle of the TMA store that writes it out.
+__device__ __forceinline__ uint32_t staged_offset(int row, int c, uint32_t pitch) {
+  return (c >> 6) * pitch + row * 128 + ((((c & 63) >> 3) ^ (row & 7)) << 4) + (c & 7) * 2;
+}
+// Adds one thread's (sum, sum of squares) of output channel n0 + col into this block's replica row of the BN workspace.
+__device__ __forceinline__ void flush_bn_stats(double* stats, int C, int n0, int col, float s1, float s2) {
+  double* dst = stats + (blockIdx.x % kReplicas) * 2 * C + n0 + col;
+  atomicAdd(dst, (double)s1);
+  atomicAdd(dst + C, (double)s2);
 }
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll

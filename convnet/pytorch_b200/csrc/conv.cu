@@ -22,12 +22,8 @@ namespace b200 {
 
 constexpr int kMaxStages = 8;
 constexpr int kMaxTaps = 32;
-constexpr int kThreads = 384;        // two consumer warpgroups + a producer warpgroup (only warp 8 works: registers are allocated
-                                     // per warpgroup in wgmma kernels, so 288 threads would cost as much as 384)
 constexpr int kConsumers = 256;
 constexpr int kProducerWarp = 8;
-constexpr int kTileM = 128;
-constexpr int kStatReplicas = 16;    // must match kReplicas of bn.cu (layout of the BN workspace accumulators)
 
 struct TapEntry {
   uint16_t off_w, off_h;  // im2col filter offsets (added to the base pixel)
@@ -60,7 +56,7 @@ struct IgemmParams {
   int window;            // > 0: block-diagonal convolution -- output channels [window*b, window*b + window) read source
                          // channels [window*b, window*b + window) only; the weight operand is [N_total][taps][window]
   uint32_t epi_bytes;    // one warpgroup's output staging tile
-  double* stats;         // fused BN statistics accumulators [kStatReplicas][2][N_total] (BN workspace) or nullptr
+  double* stats;         // fused BN statistics accumulators [kReplicas][2][N_total] (BN workspace) or nullptr
   void* out;
   const void* res;
   const float* bias;
@@ -238,12 +234,6 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   const int st_row0 = (wt / BN) * st_rows;
   int st_ntile = -1;
   float st_s1 = 0.f, st_s2 = 0.f;
-  auto flush_stats = [&]() {
-    double* dst = p.stats + (blockIdx.x % kStatReplicas) * 2 * p.N_total + st_ntile * BN + st_col;
-    atomicAdd(dst, (double)st_s1);
-    atomicAdd(dst + p.N_total, (double)st_s2);
-    st_s1 = 0.f; st_s2 = 0.f;
-  };
   const int IJ = p.I * p.J;
   if (p.b_stationary && walk_first < walk_end) mbar_wait(&bstat_bar, 0);
 
@@ -312,8 +302,7 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
               const int row = mh * 64 + r_lo + 8 * h;
-              uint32_t* dst = reinterpret_cast<uint32_t*>(epi_w + (c >> 6) * (kTileM * 128) + row * 128 +
-                                                          ((((c & 63) >> 3) ^ (row & 7)) << 4) + (c & 7) * 2);
+              uint32_t* dst = reinterpret_cast<uint32_t*>(epi_w + staged_offset(row, c, kTileM * 128));
               float v0 = acc[mh][j + 2 * h] + bias0, v1 = acc[mh][j + 2 * h + 1] + bias1;
               if (p.res != nullptr) {
                 const float2 t = unpack_bf16x2(*dst);
@@ -336,15 +325,16 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
             // back from the staged tile (rows beyond M_total are exact zeros).  Accumulated in registers across the
             // warpgroup's tiles while it stays on the same channel block, then one fp64 atomic each.
             if (st_ntile != n_tile) {
-              if (st_ntile >= 0) flush_stats();
+              if (st_ntile >= 0) {
+                flush_bn_stats(p.stats, p.N_total, st_ntile * BN, st_col, st_s1, st_s2);
+                st_s1 = 0.f; st_s2 = 0.f;
+              }
               st_ntile = n_tile;
             }
-            const uint8_t* col = epi_w + (st_col >> 6) * (kTileM * 128) + (st_col & 7) * 2;
-            const int j = (st_col & 63) >> 3;
             float s1 = 0.f, s2 = 0.f;
 #pragma unroll 8
             for (int r = st_row0; r < st_row0 + st_rows; ++r) {
-              const float vv = __bfloat162float(*reinterpret_cast<const __nv_bfloat16*>(col + r * 128 + ((j ^ (r & 7)) << 4)));
+              const float vv = __bfloat162float(*reinterpret_cast<const __nv_bfloat16*>(epi_w + staged_offset(r, st_col, kTileM * 128)));
               s1 += vv;
               s2 = fmaf(vv, vv, s2);
             }
@@ -372,7 +362,7 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       }
   }
   if constexpr (BN == 64 || BN == 128)
-    if (p.stats != nullptr && st_ntile >= 0) flush_stats();
+    if (p.stats != nullptr && st_ntile >= 0) flush_bn_stats(p.stats, p.N_total, st_ntile * BN, st_col, st_s1, st_s2);
   if (p.tma_store && leader) bulk_wait_group0();  // smem must outlive the last TMA store
 }
 
@@ -392,7 +382,6 @@ struct WgradParams {
   int c_chunks;         // ceil(C / ckB)
   int total_boxes;      // taps * c_chunks
   int boxes_per_cta;    // boxes_per_cta * ckB <= 256 accumulator columns, <= 8
-  int kt, k_groups;     // kt == 1: one k-tile (128 output channels) per CTA
   int k_tiles, col_groups, splits;
   int blocks_per_split, total_blocks;  // in units of bk pixels
   int num_stages;
@@ -437,12 +426,12 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_constan
   __syncthreads();
 
   // work decomposition
-  const int tiles = p.k_groups * p.col_groups;
+  const int tiles = p.k_tiles * p.col_groups;
   const int split = blockIdx.x / tiles;
   const int tile = blockIdx.x - split * tiles;
-  const int k_group = tile % p.k_groups;
-  const int cgroup = tile / p.k_groups;
-  const int k0 = k_group * kTileM;
+  const int k_tile = tile % p.k_tiles;
+  const int cgroup = tile / p.k_tiles;
+  const int k0 = k_tile * kTileM;
   const int box0 = cgroup * p.boxes_per_cta;
   const int nboxes = min(p.boxes_per_cta, p.total_boxes - box0);
   const int blk_begin = split * p.blocks_per_split;
@@ -545,7 +534,7 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_constan
     const int k = k0 + r_lo + 8 * h;
     if (k >= p.K_out) continue;
     if (p.partial != nullptr) {
-      // split-K: plain stores of this CTA's fp32 tile; conv_wgrad_reduce_kernel sums the splits into dw
+      // split-K: plain stores of this CTA's fp32 tile; launch_wgrad_reduce sums the splits into dw
       float* dst = p.partial + ((static_cast<long long>(tile) * p.splits + split) * kTileM + (r_lo + 8 * h)) * p.pitch;
 #pragma unroll
       for (int j = 0; j < NC / 2; j += 4)
@@ -568,12 +557,13 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_constan
   }
 }
 
-// dw[k][tap][c] += sum over splits of the partial tiles (fixed order => deterministic).  A block owns 32 consecutive
-// float4 outputs; its 8 warps each sum every 8th split (coalesced 512 B reads) and combine through shared memory --
-// with one thread per output the loop over up to 148 splits was a serial chain of L2 round trips.
+// dw[k][tap][c] += sum over splits of the partial tiles of both weight-gradient kernels (fixed order => deterministic;
+// layout in host.h, launch_wgrad_reduce).  A block owns 32 consecutive float4 outputs; its nw warps each sum every
+// nw-th split (coalesced 512 B reads) and combine through shared memory -- with one thread per output the loop over up
+// to 148 splits was a serial chain of L2 round trips.
 __global__ void __launch_bounds__(256) conv_wgrad_reduce_kernel(const float* __restrict__ partial, float* __restrict__ dw,
-                                                                int K_out, int taps, int C, int ckB, int c_chunks,
-                                                                int boxes_per_cta, int kt, int k_groups, int splits,
+                                                                int K_out, int taps, int C, int ck, int tap_stride,
+                                                                int cc_stride, int bpc, int k_tiles, int splits,
                                                                 int pitch) {
   __shared__ float4 red[8][32];
   const int c4n = C >> 2;
@@ -588,13 +578,11 @@ __global__ void __launch_bounds__(256) conv_wgrad_reduce_kernel(const float* __r
       tap = static_cast<int>((idx / c4n) % taps);
       k = static_cast<int>(idx / (static_cast<long long>(c4n) * taps));
       const int k_tile = k / kTileM, row = k - k_tile * kTileM;
-      const int k_group = k_tile / kt, j = k_tile - k_group * kt;
-      const int cc = c / ckB;
-      const int id = tap * c_chunks + cc;
-      const int cgroup = id / boxes_per_cta, x = id - cgroup * boxes_per_cta;
-      const int tile = cgroup * k_groups + k_group;
-      const float* src = partial + ((static_cast<long long>(tile) * splits) * kTileM + row) * pitch +
-                         (j * boxes_per_cta + x) * ckB + (c - cc * ckB);
+      const int cc = c / ck;
+      const int id = tap * tap_stride + cc * cc_stride;
+      const int cgroup = id / bpc, x = id - cgroup * bpc;
+      const int unit = cgroup * k_tiles + k_tile;
+      const float* src = partial + ((static_cast<long long>(unit) * splits) * kTileM + row) * pitch + x * ck + (c - cc * ck);
       for (int s2 = w; s2 < splits; s2 += nw) {
         const float4 v = __ldcg(reinterpret_cast<const float4*>(src + static_cast<long long>(s2) * kTileM * pitch));
         acc.x += v.x; acc.y += v.y; acc.z += v.z; acc.w += v.w;
@@ -655,42 +643,19 @@ static int encode_im2col(CUtensorMap* tm, const void* base, int Nimg, int H, int
   return B200_OK;
 }
 
-static int encode_tiled3(CUtensorMap* tm, const void* base, int d0, int d1, int d2, int b0, int b1, int b2) {
-  EncodeTiledFn fn = encode_tiled_fn();
-  B200_REQUIRE(fn != nullptr, B200_ERR_CUDA, "cuTensorMapEncodeTiled entry point unavailable");
-  cuuint64_t dims[3] = {(cuuint64_t)d0, (cuuint64_t)d1, (cuuint64_t)d2};
-  cuuint64_t strides[2] = {(cuuint64_t)d0 * 2, (cuuint64_t)d0 * d1 * 2};
-  cuuint32_t box[3] = {(cuuint32_t)b0, (cuuint32_t)b1, (cuuint32_t)b2};
-  cuuint32_t estr[3] = {1, 1, 1};
-  CUresult r = fn(tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void*>(base), dims, strides, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle_for_row_bytes(b0 * 2),
-                  CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  B200_REQUIRE(r == CUDA_SUCCESS, B200_ERR_CUDA, "cuTensorMapEncodeTiled(3d) failed (%d) dims=(%d,%d,%d) box=(%d,%d,%d)",
-               (int)r, d0, d1, d2, b0, b1, b2);
-  return B200_OK;
-}
-
-static int encode_tiled2(CUtensorMap* tm, const void* base, int d0, long long d1, int b0, int b1) {
-  EncodeTiledFn fn = encode_tiled_fn();
-  B200_REQUIRE(fn != nullptr, B200_ERR_CUDA, "cuTensorMapEncodeTiled entry point unavailable");
-  cuuint64_t dims[2] = {(cuuint64_t)d0, (cuuint64_t)d1};
-  cuuint64_t strides[1] = {(cuuint64_t)d0 * 2};
-  cuuint32_t box[2] = {(cuuint32_t)b0, (cuuint32_t)b1};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = fn(tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), dims, strides, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle_for_row_bytes(b0 * 2),
-                  CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  B200_REQUIRE(r == CUDA_SUCCESS, B200_ERR_CUDA, "cuTensorMapEncodeTiled(2d) failed (%d) dims=(%d,%lld) box=(%d,%d)",
-               (int)r, d0, d1, b0, b1);
-  return B200_OK;
-}
-
 static const int kSmemBudget = 200 * 1024;
 static const int kSmemBudgetMax = 224 * 1024;   // + 1 KB alignment slack + static barriers < the 227 KB per-CTA limit
 
-static int set_smem_attr(const void* fn, int bytes) {
-  cudaError_t e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
-  B200_REQUIRE(e == cudaSuccess, B200_ERR_CUDA, "cudaFuncSetAttribute(smem=%d): %s", bytes, cudaGetErrorString(e));
+int launch_wgrad_reduce(const float* partial, float* dw, int K_out, int taps, int C, int ck, int tap_stride,
+                        int cc_stride, int bpc, int k_tiles, int splits, int pitch, cudaStream_t stream) {
+  const long long total = static_cast<long long>(K_out) * taps * (C / 4);
+  long long blocks = (total + 31) / 32;
+  if (blocks > 16LL * sm_count()) blocks = 16LL * sm_count();
+  int warps = 8;
+  while (warps > 1 && warps > splits) warps >>= 1;   // no idle warps when there are only a few splits
+  b200::launch(conv_wgrad_reduce_kernel, static_cast<int>(blocks), 32 * warps, 0, stream, partial, dw, K_out, taps, C, ck,
+               tap_stride, cc_stride, bpc, k_tiles, splits, pitch);
+  B200_CHECK_LAUNCH("conv_wgrad_reduce_kernel");
   return B200_OK;
 }
 
@@ -815,22 +780,22 @@ static int launch_igemm(const IgemmLaunch& L, cudaStream_t stream) {
   p.plain_a = (L.ntaps == 1 && L.trav == 1 && L.lower_w == 0 && L.lower_h == 0 && L.taps[0].off_w == 0 &&
                L.taps[0].off_h == 0 && L.I == L.SH && L.J == L.SW && L.s_pix == 0) ? 1 : 0;
   if (p.plain_a)
-    rc = encode_tiled2(&tmA, L.src, L.SC, (long long)p.M_total, p.ck, kTileM);
+    rc = encode_tiled(&tmA, L.src, 2, {L.SC, p.M_total}, {p.ck, kTileM}, "igemm A");
   else
     rc = encode_im2col(&tmA, L.src, L.Nimg, L.SH, L.SW, L.SC, p.ck, kTileM, L.lower_w, L.lower_h, upper_w, upper_h,
                        L.trav, L.s_pix, L.s_row, L.s_img);
   if (rc) return rc;
-  rc = encode_tiled3(&tmB, L.wmat, L.window ? L.window : L.SC, L.wtaps, L.Nout, p.ck, 1, p.block_n);
+  rc = encode_tiled(&tmB, L.wmat, 3, {L.window ? L.window : L.SC, L.wtaps, L.Nout}, {p.ck, 1, p.block_n}, "igemm B");
   if (rc) return rc;
 
   CUtensorMap tmC, tmR;
   memset(&tmC, 0, sizeof(tmC));
   memset(&tmR, 0, sizeof(tmR));
   if (p.tma_store) {
-    rc = encode_tiled2(&tmC, L.out, L.ldo, (long long)p.M_total, 64, kTileM);
+    rc = encode_tiled(&tmC, L.out, 2, {L.ldo, p.M_total}, {64, kTileM}, "igemm output");
     if (rc) return rc;
     if (L.res != nullptr) {
-      rc = encode_tiled2(&tmR, L.res, L.ldo, (long long)p.M_total, 64, kTileM);
+      rc = encode_tiled(&tmR, L.res, 2, {L.ldo, p.M_total}, {64, kTileM}, "igemm residual");
       if (rc) return rc;
     }
   }
@@ -1004,13 +969,10 @@ extern "C" int b200_conv_wgrad(const b200_conv_desc* d, const void* x, const voi
                "conv_wgrad: C=%d and K=%d must be multiples of 8", d->C, d->K);
   if (d->stride == 1 && d->pad_h == d->pad_w && d->P == d->H + 2 * d->pad_h - d->R + 1 &&
       d->Q == d->W + 2 * d->pad_w - d->S + 1 && d->x_pixel_stride == 0 &&
-      (d->window == 0 || d->window == 128) && halo_wgrad_eligible(d->P, d->Q, d->C, d->K, d->R, d->S, d->pad_h)) {
-    // partial tiles of the halo kernel must fit the split-K workspace (units * splits <= SMs, or one split)
-    const int units = ((d->window ? d->window : d->C) / 16) * ((d->K + kTileM - 1) / kTileM);   // 16-channel x chunks
-    if (units <= sm_count() + 8)
-      return launch_halo_wgrad(x, dy, dw, workspace, workspace_bytes, d->N, d->P, d->Q, d->C, d->K, d->R, d->S, d->pad_h,
-                               stream, d->window);
-  }
+      (d->window == 0 || d->window == 128) &&
+      halo_wgrad_eligible(d->P, d->Q, d->C, d->K, d->R, d->S, d->pad_h, d->window))
+    return launch_halo_wgrad(x, dy, dw, workspace, workspace_bytes, d->N, d->P, d->Q, d->C, d->K, d->R, d->S, d->pad_h,
+                             stream, d->window);
   B200_REQUIRE(d->window == 0 || d->window == 128, B200_ERR_UNSUPPORTED, "conv_wgrad: window must be 0 or 128");
   // window mode (block-diagonal): k-tile t pairs with input channels [128t, 128t+128) only; dw is [K][taps][128]
   const int Cw = d->window ? d->window : d->C;
@@ -1031,20 +993,18 @@ extern "C" int b200_conv_wgrad(const b200_conv_desc* d, const void* x, const voi
   // Tile shape: one k-tile (128 output channels, the two consumer warpgroups) x bpc channel boxes of x per CTA, with
   // bpc * ckB <= 256 accumulator columns (128 fp32 registers per consumer thread).  The x tile is fetched once for
   // all 128 output channels.
-  p.kt = 1;
   p.boxes_per_cta = 256 / p.ckB;
   if (p.boxes_per_cta > 8) p.boxes_per_cta = 8;
   if (p.boxes_per_cta > p.total_boxes) p.boxes_per_cta = p.total_boxes;
-  p.k_groups = (p.k_tiles + p.kt - 1) / p.kt;
   p.col_groups = (p.total_boxes + p.boxes_per_cta - 1) / p.boxes_per_cta;
   p.total_blocks = (p.M_total + p.bk - 1) / p.bk;
-  const int tiles = p.k_groups * p.col_groups;
+  const int tiles = p.k_tiles * p.col_groups;
   int splits = sm_count() / tiles;  // one wave: a CTA takes most of an SM's shared memory, two cannot share one
   if (splits > p.total_blocks) splits = p.total_blocks;
   if (splits < 1) splits = 1;
   p.blocks_per_split = (p.total_blocks + splits - 1) / splits;
   p.splits = (p.total_blocks + p.blocks_per_split - 1) / p.blocks_per_split;
-  p.stage_bytes = p.kt * (kTileM / p.ckA) * p.boxA_bytes + p.boxes_per_cta * p.boxB_bytes;
+  p.stage_bytes = (kTileM / p.ckA) * p.boxA_bytes + p.boxes_per_cta * p.boxB_bytes;
   p.stage_bytes = (p.stage_bytes + 1023u) & ~1023u;
   // 200 KB, not the full 224: the weight gradients run on the side stream BESIDE the main stream's BatchNorm kernels,
   // whose reduce blocks need ~10 KB of shared memory on the same SM
@@ -1052,7 +1012,7 @@ extern "C" int b200_conv_wgrad(const b200_conv_desc* d, const void* x, const voi
   if (p.num_stages > kMaxStages) p.num_stages = kMaxStages;
   if (p.num_stages < 2) p.num_stages = 2;
   p.dw = dw;
-  p.pitch = p.kt * p.boxes_per_cta * p.ckB;
+  p.pitch = p.boxes_per_cta * p.ckB;
   p.partial = nullptr;
   if (p.splits > 1) {
     const size_t need = static_cast<size_t>(tiles) * p.splits * kTileM * p.pitch * sizeof(float);
@@ -1064,20 +1024,20 @@ extern "C" int b200_conv_wgrad(const b200_conv_desc* d, const void* x, const voi
   }
   p.S_filter = d->S;
   CUtensorMap tmDy, tmX;
-  rc = encode_tiled2(&tmDy, dy, d->K, (long long)p.M_total, p.ckA, p.bk);
+  rc = encode_tiled(&tmDy, dy, 2, {d->K, p.M_total}, {p.ckA, p.bk}, "wgrad dy");
   if (rc) return rc;
   const int upper_w = p.lower_w + (d->Q - 1) * d->stride + 1 - d->W;
   const int upper_h = p.lower_h + (d->P - 1) * d->stride + 1 - d->H;
   p.plain_x = (d->R == 1 && d->S == 1 && d->stride == 1 && d->pad_h == 0 && d->pad_w == 0 && d->P == d->H &&
                d->Q == d->W && d->x_pixel_stride == 0) ? 1 : 0;
-  if (getenv("B200_WGRAD_DEBUG"))
+  if (getenv("B200_WGRAD_DEBUG"))   // keys kt (always 1) and k_groups (== k_tiles) stay for the parsers of this line
     fprintf(stderr, "[wgrad] K=%d C=%d taps=%d stride=%d ckA=%d ckB=%d kt=%d bpc=%d k_groups=%d col_groups=%d splits=%d "
             "bps=%d stages=%d stage=%u nc=%d nboxes_last=%d plain_x=%d partial=%d\n", d->K, d->C, p.taps_total,
-            d->stride, p.ckA, p.ckB, p.kt, p.boxes_per_cta, p.k_groups, p.col_groups, p.splits, p.blocks_per_split,
+            d->stride, p.ckA, p.ckB, 1, p.boxes_per_cta, p.k_tiles, p.col_groups, p.splits, p.blocks_per_split,
             p.num_stages, p.stage_bytes, p.pitch, p.total_boxes - (p.col_groups - 1) * p.boxes_per_cta, p.plain_x,
             p.partial != nullptr);
   if (p.plain_x)
-    rc = encode_tiled2(&tmX, x, d->C, (long long)p.M_total, p.ckB, p.bk);
+    rc = encode_tiled(&tmX, x, 2, {d->C, p.M_total}, {p.ckB, p.bk}, "wgrad x");
   else
     rc = encode_im2col(&tmX, x, d->N, d->H, d->W, d->C, p.ckB, p.bk, p.lower_w, p.lower_h, upper_w, upper_h,
                        d->stride, d->x_pixel_stride, d->x_row_stride, d->x_image_stride);
@@ -1089,14 +1049,8 @@ extern "C" int b200_conv_wgrad(const b200_conv_desc* d, const void* x, const voi
   const int grid = tiles * p.splits;
   b200::launch(kfn, grid, kThreads, smem_bytes, stream, tmDy, tmX, p);
   B200_CHECK_LAUNCH("conv_wgrad_kernel");
-  if (p.partial != nullptr) {
-    const long long total = static_cast<long long>(d->K) * p.taps_total * (Cw / 4);
-    long long blocks = (total + 31) / 32;
-    if (blocks > 16LL * sm_count()) blocks = 16LL * sm_count();
-    b200::launch(conv_wgrad_reduce_kernel, static_cast<int>(blocks), 32 * wgrad_reduce_warps(p.splits), 0, stream, p.partial, dw, d->K, p.taps_total, Cw, p.ckB,
-                                                                          p.c_chunks, p.boxes_per_cta, p.kt, p.k_groups,
-                                                                          p.splits, p.pitch);
-    B200_CHECK_LAUNCH("conv_wgrad_reduce_kernel");
-  }
-  return B200_OK;
+  if (p.partial == nullptr) return B200_OK;
+  // channel boxes are numbered tap-major, as in the kernel: id = tap * c_chunks + (c / ckB)
+  return launch_wgrad_reduce(p.partial, dw, d->K, p.taps_total, Cw, p.ckB, p.c_chunks, 1, p.boxes_per_cta, p.k_tiles,
+                             p.splits, p.pitch, stream);
 }

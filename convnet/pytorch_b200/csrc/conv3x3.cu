@@ -13,19 +13,14 @@
 // Pixel rows are 128 B (64-channel chunks, 128B swizzle) or, for the 16-channel stem, 32 B (32B swizzle, one K=16
 // MMA per tap).  When all weight slices of a CTA fit in shared memory (64x64 3x3, the stem) they are loaded once
 // ("stationary") instead of streaming through the ring with every tile.
-//
-// Same warp roles / TMA-store epilogue / fused BN statistics as conv_igemm_kernel.
 #include "common.cuh"
 #include "host.h"
 #include <stdlib.h>
 
 namespace b200 {
 
-constexpr int kHThreads = 384;   // two consumer warpgroups + the producer warpgroup (warp 8 issues the TMA)
-constexpr int kHTileM = 128;
 constexpr int kHMaxA = 6, kHMaxB = 8;
 constexpr int kHMaxTaps = 16;
-constexpr int kHStatReplicas = 16;
 
 struct HaloParams {
   int N, H, W, C, Kout;    // H x W: OUTPUT map (the source is (H+R-1-2*pad) x (W+S-1-2*pad))
@@ -50,7 +45,7 @@ struct HaloParams {
 // Descriptors are built once per operand buffer and advanced by adding (byte offset >> 4) to the address field, with
 // the tap / k-step loops fully unrolled.  BN = block_n (64, 128 or 256) sizes the accumulators exactly.
 template <int NTAPS, int KSTEPS, int BN>
-__global__ void __launch_bounds__(kHThreads, 1)
+__global__ void __launch_bounds__(kThreads, 1)
 conv_halo_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmB,
                  const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmR,
                  const __grid_constant__ HaloParams p) {
@@ -140,7 +135,7 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant_
   }
   // fused BN statistics: this thread owns one output column and a row range of every tile
   const int st_col = threadIdx.x % BN;
-  const int st_rows = kHTileM / (256 / BN);
+  const int st_rows = kTileM / (256 / BN);
   const int st_row0 = (threadIdx.x / BN) * st_rows;
   int st_ntile = -1;
   float st_s1 = 0.f, st_s2 = 0.f;
@@ -211,18 +206,15 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant_
 #pragma unroll
       for (int j = 0; j < BN / 2; j += 4) {
         const int c = 2 * j + c_lo;
-        {
-          uint32_t* dst = reinterpret_cast<uint32_t*>(epi + (c >> 6) * box_pitch + row * 128 +
-                                                      ((((c & 63) >> 3) ^ (row & 7)) << 4) + (c & 7) * 2);
-          float v0 = acc[j + 2 * h], v1 = acc[j + 2 * h + 1];
-          if (p.bias != nullptr) { v0 += __ldg(p.bias + nbase + c); v1 += __ldg(p.bias + nbase + c + 1); }
-          if (p.has_res) {
-            const float2 t2 = unpack_bf16x2(*dst);
-            v0 += t2.x;
-            v1 += t2.y;
-          }
-          *dst = pack_bf16x2(apply_act(v0, p.act), apply_act(v1, p.act));
+        uint32_t* dst = reinterpret_cast<uint32_t*>(epi + staged_offset(row, c, box_pitch));
+        float v0 = acc[j + 2 * h], v1 = acc[j + 2 * h + 1];
+        if (p.bias != nullptr) { v0 += __ldg(p.bias + nbase + c); v1 += __ldg(p.bias + nbase + c + 1); }
+        if (p.has_res) {
+          const float2 t2 = unpack_bf16x2(*dst);
+          v0 += t2.x;
+          v1 += t2.y;
         }
+        *dst = pack_bf16x2(apply_act(v0, p.act), apply_act(v1, p.act));
       }
     }
     fence_proxy_async();
@@ -233,29 +225,19 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant_
     }
     if (p.stats != nullptr) {
       if (st_ntile != n_tile) {
-        if (st_ntile >= 0) {
-          double* dst = p.stats + (blockIdx.x % kHStatReplicas) * 2 * p.Kout + st_ntile * BN + st_col;
-          atomicAdd(dst, (double)st_s1);
-          atomicAdd(dst + p.Kout, (double)st_s2);
-        }
+        if (st_ntile >= 0) flush_bn_stats(p.stats, p.Kout, st_ntile * BN, st_col, st_s1, st_s2);
         st_ntile = n_tile; st_s1 = 0.f; st_s2 = 0.f;
       }
       const int vrows = min(p.RT, p.H - h0) * p.W;   // staged rows that belong to the image
-      const uint8_t* col = epi + (st_col >> 6) * box_pitch + (st_col & 7) * 2;
-      const int j = (st_col & 63) >> 3;
       const int r_end = min(st_row0 + st_rows, vrows);
       for (int r = st_row0; r < r_end; ++r) {
-        const float x = __bfloat162float(*reinterpret_cast<const __nv_bfloat16*>(col + r * 128 + ((j ^ (r & 7)) << 4)));
+        const float x = __bfloat162float(*reinterpret_cast<const __nv_bfloat16*>(epi + staged_offset(r, st_col, box_pitch)));
         st_s1 += x;
         st_s2 = fmaf(x, x, st_s2);
       }
     }
   }
-  if (p.stats != nullptr && st_ntile >= 0) {
-    double* dst = p.stats + (blockIdx.x % kHStatReplicas) * 2 * p.Kout + st_ntile * BN + st_col;
-    atomicAdd(dst, (double)st_s1);
-    atomicAdd(dst + p.Kout, (double)st_s2);
-  }
+  if (p.stats != nullptr && st_ntile >= 0) flush_bn_stats(p.stats, p.Kout, st_ntile * BN, st_col, st_s1, st_s2);
   if (leader) bulk_wait_group0();
 }
 
@@ -271,21 +253,6 @@ static HaloKernelFn halo_kernel_for(int ntaps, int block_n) {
     return block_n == 64 ? conv_halo_kernel<16, 1, 64> : block_n == 128 ? conv_halo_kernel<16, 1, 128>
          : block_n == 256 ? conv_halo_kernel<16, 1, 256> : nullptr;
   return nullptr;
-}
-
-static int enc4(CUtensorMap* tm, const void* base, int C, int W, int H, int N, int b0, int b1, int b2) {
-  EncodeTiledFn fn = encode_tiled_fn();
-  B200_REQUIRE(fn != nullptr, B200_ERR_CUDA, "cuTensorMapEncodeTiled entry point unavailable");
-  cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)N};
-  cuuint64_t strides[3] = {(cuuint64_t)C * 2, (cuuint64_t)W * C * 2, (cuuint64_t)H * W * C * 2};
-  cuuint32_t box[4] = {(cuuint32_t)b0, (cuuint32_t)b1, (cuuint32_t)b2, 1};
-  cuuint32_t es[4] = {1, 1, 1, 1};
-  CUresult r = fn(tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(base), dims, strides, box, es,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle_for_row_bytes(b0 * 2), CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  B200_REQUIRE(r == CUDA_SUCCESS, B200_ERR_CUDA, "cuTensorMapEncodeTiled(4d) failed (%d) dims=(%d,%d,%d,%d) box=(%d,%d,%d)",
-               (int)r, C, W, H, N, b0, b1, b2);
-  return B200_OK;
 }
 
 // Geometry shared by the fprop/dgrad and wgrad halo kernels: stride-1 RxS taps over an H x W OUTPUT map.
@@ -331,7 +298,7 @@ int launch_halo(const void* src, const void* wmat, void* out, const void* res, c
   p.block_n = Nout / p.n_tiles;
   p.c_chunks = p.diag ? 1 : Cs / cw;
   p.a_box_bytes = (uint32_t)(p.RT + R - 1) * p.Wp * p.row_bytes;
-  uint32_t a_need = (uint32_t)(kHTileM + (R - 1) * p.Wp + (S - 1)) * p.row_bytes;
+  uint32_t a_need = (uint32_t)(kTileM + (R - 1) * p.Wp + (S - 1)) * p.row_bytes;
   if (a_need < p.a_box_bytes) a_need = p.a_box_bytes;
   p.a_bytes = (a_need + 1023u) & ~1023u;
   p.b_bytes = (uint32_t)p.block_n * p.row_bytes;
@@ -372,31 +339,23 @@ int launch_halo(const void* src, const void* wmat, void* out, const void* res, c
                "conv halo: shared memory budget exceeded (W=%d, block_n=%d)", W, p.block_n);
   CUtensorMap tmX, tmB, tmC, tmR;
   memset(&tmR, 0, sizeof(tmR));
-  int rc = enc4(&tmX, src, Cs, W + S - 1 - 2 * pad, H + R - 1 - 2 * pad, N, cw, p.Wp, p.RT + R - 1);
+  int rc = encode_tiled(&tmX, src, 4, {Cs, W + S - 1 - 2 * pad, H + R - 1 - 2 * pad, N}, {cw, p.Wp, p.RT + R - 1, 1},
+                        "conv halo source");
   if (rc) return rc;
-  {
-    EncodeTiledFn fn = encode_tiled_fn();
-    const int wc = p.diag ? window : Cs;      // channel extent of the weight operand: [Nout][taps][wc]
-    cuuint64_t dims[3] = {(cuuint64_t)wc, (cuuint64_t)p.ntaps, (cuuint64_t)Nout};
-    cuuint64_t strides[2] = {(cuuint64_t)wc * 2, (cuuint64_t)wc * p.ntaps * 2};
-    cuuint32_t box[3] = {(cuuint32_t)cw, 1, (cuuint32_t)p.block_n};
-    cuuint32_t es[3] = {1, 1, 1};
-    CUresult r = fn(&tmB, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void*>(wmat), dims, strides, box, es,
-                    CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle_for_row_bytes(p.row_bytes),
-                    CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    B200_REQUIRE(r == CUDA_SUCCESS, B200_ERR_CUDA, "conv halo: weight tensor map failed (%d)", (int)r);
-  }
-  rc = enc4(&tmC, out, Nout, W, H, N, 64, W, p.RT);
+  // the weight operand is [Nout][taps][window or Cs]
+  rc = encode_tiled(&tmB, wmat, 3, {p.diag ? window : Cs, p.ntaps, Nout}, {cw, 1, p.block_n}, "conv halo weights");
+  if (rc) return rc;
+  rc = encode_tiled(&tmC, out, 4, {Nout, W, H, N}, {64, W, p.RT, 1}, "conv halo output");
   if (rc) return rc;
   if (res) {
-    rc = enc4(&tmR, res, Nout, W, H, N, 64, W, p.RT);
+    rc = encode_tiled(&tmR, res, 4, {Nout, W, H, N}, {64, W, p.RT, 1}, "conv halo residual");
     if (rc) return rc;
   }
   const int smem_bytes = p.sa * (int)p.a_bytes + b_region + (int)epi_bytes + 1024;
   HaloKernelFn kfn = halo_kernel_for(p.ntaps, p.block_n);
   B200_REQUIRE(kfn != nullptr, B200_ERR_UNSUPPORTED, "conv halo: %d taps with block_n %d unsupported", p.ntaps, p.block_n);
-  cudaError_t e = cudaFuncSetAttribute((const void*)kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes);
-  B200_REQUIRE(e == cudaSuccess, B200_ERR_CUDA, "conv halo: smem attribute (%d bytes): %s", smem_bytes, cudaGetErrorString(e));
+  rc = set_smem_attr((const void*)kfn, smem_bytes);
+  if (rc) return rc;
   const int total = p.m_tiles * p.n_tiles;
   int grid = total < sm_count() ? total : sm_count();
   if (p.diag) {                       // a multiple of n_tiles: every CTA owns one n-tile
@@ -410,7 +369,7 @@ int launch_halo(const void* src, const void* wmat, void* out, const void* res, c
             "sa=%d sb=%d bias=%d res=%d act=%d stats=%d grid=%d\n", dir, N, H, W, Cs, Nout, p.ntaps, p.block_n,
             p.n_tiles, p.m_tiles, p.b_stationary, p.diag, p.sa, p.sb, bias != nullptr, res != nullptr, act,
             stats != nullptr, grid);
-  b200::launch(kfn, grid, kHThreads, smem_bytes, stream, tmX, tmB, tmC, tmR, p);
+  b200::launch(kfn, grid, kThreads, smem_bytes, stream, tmX, tmB, tmC, tmR, p);
   B200_CHECK_LAUNCH("conv_halo_kernel");
   return B200_OK;
 }
@@ -426,8 +385,7 @@ int launch_halo(const void* src, const void* wmat, void* out, const void* res, c
 // accumulator columns (72 registers per consumer thread), the stem's 16 taps 256.  The im2col kernel re-fetched x
 // once per tap.
 // One CTA owns a (k-tile, channel-chunk) unit and a contiguous range of pixel tiles (split-K over pixels); partial
-// fp32 tiles go to the workspace and conv_halo_wgrad_reduce_kernel adds them into dw in a fixed order.
-constexpr int kWThreads = 384;   // two consumer warpgroups + the producer warpgroup (warp 8 issues the TMA)
+// fp32 tiles go to the workspace and launch_wgrad_reduce adds them into dw in a fixed order.
 constexpr int kWMaxStages = 4;
 
 struct HaloWgradParams {
@@ -449,7 +407,7 @@ struct HaloWgradParams {
 // dy operand is then read from shared memory once per filter row instead of once per tap.
 // Consumer warpgroup wg owns output channels [k0 + 64 wg, k0 + 64 wg + 64): R accumulator blocks of S * cw columns.
 template <int R, int S>
-__global__ void __launch_bounds__(kWThreads, 1)
+__global__ void __launch_bounds__(kThreads, 1)
 conv_halo_wgrad_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_constant__ CUtensorMap tmX,
                        const __grid_constant__ HaloWgradParams p) {
   constexpr int kCols = S * 16;   // accumulator columns of one filter row (cw = 16 channels per x chunk)
@@ -465,7 +423,7 @@ conv_halo_wgrad_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_co
   {
     uint4* z = reinterpret_cast<uint4*>(smem);
     const int n16 = static_cast<int>(p.stages * stage_bytes) >> 4;
-    for (int i = threadIdx.x; i < n16; i += kWThreads) z[i] = make_uint4(0u, 0u, 0u, 0u);
+    for (int i = threadIdx.x; i < n16; i += kThreads) z[i] = make_uint4(0u, 0u, 0u, 0u);
   }
   if (threadIdx.x == 0) {
     for (int s = 0; s < p.stages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 8); }
@@ -480,7 +438,7 @@ conv_halo_wgrad_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_co
   const int unit = blockIdx.x - split * p.units;
   const int k_tile = unit % p.k_tiles;
   const int cc = unit / p.k_tiles;
-  const int k0 = k_tile * kHTileM;
+  const int k0 = k_tile * kTileM;
   const int t_begin = split * p.tiles_per_split;
   const int t_end = min(p.m_tiles, t_begin + p.tiles_per_split);
   const int ntiles = t_end - t_begin;
@@ -551,7 +509,7 @@ conv_halo_wgrad_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_co
   const int c_lo = 2 * (lane & 3);
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
-    float* dst = p.partial + ((static_cast<long long>(unit) * p.splits + split) * kHTileM + row + 8 * h) * p.ncols;
+    float* dst = p.partial + ((static_cast<long long>(unit) * p.splits + split) * kTileM + row + 8 * h) * p.ncols;
 #pragma unroll
     for (int r = 0; r < R; ++r)
 #pragma unroll
@@ -560,51 +518,12 @@ conv_halo_wgrad_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_co
   }
 }
 
-// dw[k][tap][c] += sum over splits of partial[unit(k_tile, cc)][split][k % 128][tap * cw + c % cw]
-// (same block organisation as conv_wgrad_reduce_kernel: 32 float4 outputs per block, 8 warps over the splits)
-__global__ void __launch_bounds__(256) conv_halo_wgrad_reduce_kernel(const float* __restrict__ partial,
-                                                                     float* __restrict__ dw, int K_out, int ntaps, int C,
-                                                                     int cw, int k_tiles, int splits, int ncols) {
-  __shared__ float4 red[8][32];
-  const int c4n = C >> 2;
-  const long long total = static_cast<long long>(K_out) * ntaps * c4n;
-  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5, nw = blockDim.x >> 5;
-  for (long long base = static_cast<long long>(blockIdx.x) * 32; base < total; base += static_cast<long long>(gridDim.x) * 32) {
-    const long long idx = base + lane;
-    float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
-    int c = 0, tap = 0, k = 0;
-    if (idx < total) {
-      c = static_cast<int>(idx % c4n) * 4;
-      tap = static_cast<int>((idx / c4n) % ntaps);
-      k = static_cast<int>(idx / (static_cast<long long>(c4n) * ntaps));
-      const int k_tile = k >> 7, row = k & 127;
-      const int cc = c / cw;
-      const int unit = cc * k_tiles + k_tile;
-      const float* src = partial + ((static_cast<long long>(unit) * splits) * kHTileM + row) * ncols + tap * cw + (c - cc * cw);
-      for (int s2 = w; s2 < splits; s2 += nw) {
-        const float4 v = __ldcg(reinterpret_cast<const float4*>(src + static_cast<long long>(s2) * kHTileM * ncols));
-        acc.x += v.x; acc.y += v.y; acc.z += v.z; acc.w += v.w;
-      }
-    }
-    red[w][lane] = acc;
-    __syncthreads();
-    if (w == 0 && idx < total) {
-      for (int j = 1; j < nw; ++j) {
-        const float4 v = red[j][lane];
-        acc.x += v.x; acc.y += v.y; acc.z += v.z; acc.w += v.w;
-      }
-      float4* d = reinterpret_cast<float4*>(dw + (static_cast<long long>(k) * ntaps + tap) * C + c);
-      float4 o = *d;
-      o.x += acc.x; o.y += acc.y; o.z += acc.z; o.w += acc.w;
-      *d = o;
-    }
-    __syncthreads();
-  }
-}
-
-bool halo_wgrad_eligible(int H, int W, int C, int K_out, int R, int S, int pad) {
-  if (!halo_geometry_ok(H, W, C, R, S, pad)) return false;
-  return K_out % 64 == 0;
+// The partial tiles must also fit the split-K workspace (b200_conv_wgrad_workspace_bytes): units * splits <= SMs, or
+// one split.
+bool halo_wgrad_eligible(int H, int W, int C, int K_out, int R, int S, int pad, int window) {
+  if (!halo_geometry_ok(H, W, C, R, S, pad) || K_out % 64 != 0) return false;
+  const int units = ((window ? window : C) / 16) * ((K_out + kTileM - 1) / kTileM);   // as in launch_halo_wgrad
+  return units <= sm_count() + 8;
 }
 
 int launch_halo_wgrad(const void* x, const void* dy, float* dw, void* workspace, size_t workspace_bytes, int N, int H,
@@ -627,7 +546,7 @@ int launch_halo_wgrad(const void* x, const void* dy, float* dw, void* workspace,
   p.tiles_per_img = (H + p.RT - 1) / p.RT;
   p.m_tiles = N * p.tiles_per_img;
   p.c_chunks = (window ? window : C) / p.cw;       // channel chunks that pair with one k-tile
-  p.k_tiles = (K_out + kHTileM - 1) / kHTileM;
+  p.k_tiles = (K_out + kTileM - 1) / kTileM;
   p.units = p.c_chunks * p.k_tiles;
   int splits = sm_count() / p.units;
   if (splits < 1) splits = 1;
@@ -643,44 +562,35 @@ int launch_halo_wgrad(const void* x, const void* dy, float* dw, void* workspace,
       p.x_off[r * S + s] = (uint16_t)(r * p.Wp + s);
       if (r * p.Wp + s > max_off) max_off = r * p.Wp + s;
     }
-  uint32_t x_need = (uint32_t)(kHTileM + max_off) * p.x_row_bytes;
+  uint32_t x_need = (uint32_t)(kTileM + max_off) * p.x_row_bytes;
   if (x_need < p.x_box_bytes) x_need = p.x_box_bytes;
   p.x_bytes = (x_need + 1023u) & ~1023u;
   p.stages = (212 * 1024) / (int)(p.a_bytes + p.x_bytes);
   if (p.stages > kWMaxStages) p.stages = kWMaxStages;
   B200_REQUIRE(p.stages >= 2, B200_ERR_UNSUPPORTED, "conv halo wgrad: shared memory budget exceeded (W=%d)", W);
-  const size_t need = (size_t)p.units * p.splits * kHTileM * p.ncols * sizeof(float);
+  const size_t need = (size_t)p.units * p.splits * kTileM * p.ncols * sizeof(float);
   B200_REQUIRE(workspace != nullptr && workspace_bytes >= need, B200_ERR_INVALID,
                "conv halo wgrad: workspace of %zu bytes needed (%zu given)", need, workspace_bytes);
   p.partial = reinterpret_cast<float*>(workspace);
   CUtensorMap tmDy, tmX;
-  int rc = enc4(&tmDy, dy, K_out, W, H, N, 64, p.Wp, p.RT);
+  int rc = encode_tiled(&tmDy, dy, 4, {K_out, W, H, N}, {64, p.Wp, p.RT, 1}, "conv halo wgrad dy");
   if (rc) return rc;
-  rc = enc4(&tmX, x, C, W + S - 1 - 2 * pad, H + R - 1 - 2 * pad, N, p.cw, p.Wp, p.halo_rows);
+  rc = encode_tiled(&tmX, x, 4, {C, W + S - 1 - 2 * pad, H + R - 1 - 2 * pad, N}, {p.cw, p.Wp, p.halo_rows, 1},
+                    "conv halo wgrad x");
   if (rc) return rc;
   const int smem_bytes = p.stages * (int)(p.a_bytes + p.x_bytes) + 1024;
-  const void* kfn = (p.ntaps == 9) ? (const void*)conv_halo_wgrad_kernel<3, 3> : (const void*)conv_halo_wgrad_kernel<4, 4>;
-  cudaError_t e = cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes);
-  B200_REQUIRE(e == cudaSuccess, B200_ERR_CUDA, "conv halo wgrad: smem attribute (%d bytes): %s", smem_bytes,
-               cudaGetErrorString(e));
+  const auto kfn = p.ntaps == 9 ? conv_halo_wgrad_kernel<3, 3> : conv_halo_wgrad_kernel<4, 4>;
+  rc = set_smem_attr((const void*)kfn, smem_bytes);
+  if (rc) return rc;
   if (getenv("B200_HALO_DEBUG"))
     fprintf(stderr, "[halo_wgrad] N=%d H=%d W=%d C=%d K=%d taps=%d k_tiles=%d c_chunks=%d m_tiles=%d units=%d "
             "splits=%d tiles_per_split=%d stages=%d grid=%d\n", N, H, W, C, K_out, p.ntaps, p.k_tiles, p.c_chunks,
             p.m_tiles, p.units, p.splits, p.tiles_per_split, p.stages, p.units * p.splits);
-  if (p.ntaps == 9)
-    b200::launch(conv_halo_wgrad_kernel<3, 3>, p.units * p.splits, kWThreads, smem_bytes, stream, tmDy, tmX, p);
-  else
-    b200::launch(conv_halo_wgrad_kernel<4, 4>, p.units * p.splits, kWThreads, smem_bytes, stream, tmDy, tmX, p);
+  b200::launch(kfn, p.units * p.splits, kThreads, smem_bytes, stream, tmDy, tmX, p);
   B200_CHECK_LAUNCH("conv_halo_wgrad_kernel");
-  const int Cw = window ? window : C;                 // row length of dw: [K][taps][Cw]
-  const long long total = (long long)K_out * p.ntaps * (Cw / 4);
-  long long blocks64 = (total + 31) / 32;
-  if (blocks64 > 16LL * sm_count()) blocks64 = 16LL * sm_count();
-  const int blocks = (int)blocks64;
-  b200::launch(conv_halo_wgrad_reduce_kernel, blocks, 32 * wgrad_reduce_warps(p.splits), 0, stream, p.partial, dw, K_out, p.ntaps, Cw, p.cw, p.k_tiles, p.splits,
-                                                            p.ncols);
-  B200_CHECK_LAUNCH("conv_halo_wgrad_reduce_kernel");
-  return B200_OK;
+  // dw is [K][taps][window or C]; channel boxes are numbered chunk-major, as the units: id = (c / cw) * taps + tap
+  return launch_wgrad_reduce(p.partial, dw, K_out, p.ntaps, window ? window : C, p.cw, 1, p.ntaps, p.ntaps, p.k_tiles,
+                             p.splits, p.ncols, stream);
 }
 
 }  // namespace b200
