@@ -240,14 +240,8 @@ __global__ void __launch_bounds__(kBnThreads) bn_apply_kernel(
   }
 }
 
-// ---- backward kernels -----------------------------------------------------------------------------
-// Thread mapping: VEC channels per thread (VEC=4: 64-bit accesses, half the per-channel coefficient registers of
-// VEC=8, which is what keeps these 2-read(+1-write) streams at the occupancy of bn_apply; VEC=8 only for C > 1024).
-// g = dy where act'(.) passes, else +0 (selected, not multiplied: dy * 0 would give -0 for negative dy, unlike the
-// mask-bit source and torch's threshold backward), where the activation argument is y when given, else recomputed as
-// z*scale+shift (bit-identical to the forward's fused multiply-add).
-
-// ---- backward reduce: dbeta = sum g, dgamma = sum g * xhat ------------------------------------------
+// ---- backward kernels (bodies in bn_common.cuh) --------------------------------------------------
+// backward reduce: dbeta = sum g, dgamma = sum g * xhat
 // SRC: activation argument 0 recomputed from z, 1 = y, 2 = mask bits
 template <int VEC, int ROWS, int MINB, int SRC>
 __global__ void __launch_bounds__(kBnThreads, MINB) bn_bwd_reduce_kernel(
@@ -255,85 +249,8 @@ __global__ void __launch_bounds__(kBnThreads, MINB) bn_bwd_reduce_kernel(
     const __nv_bfloat16* __restrict__ z, long long M, int C, int cv, int rows_per_iter, int act,
     const float* __restrict__ mean, const float* __restrict__ invstd, const float* __restrict__ gamma,
     const float* __restrict__ beta, float* __restrict__ partial) {
-  const int t = threadIdx.x;
-  const bool active = t < rows_per_iter * cv;
-  const int r0 = t / cv, v = t - r0 * cv;
-  // SRC 2 (mask words): a thread owns ROWS CONSECUTIVE rows (one mask load); block ranges are multiples of 8 rows
-  const long long rows_per_block = SRC == 2 ? (((M + gridDim.x - 1) / gridDim.x + 7) & ~7LL) : (M + gridDim.x - 1) / gridDim.x;
-  const long long row_begin = blockIdx.x * rows_per_block;
-  const long long row_end = min(M, row_begin + rows_per_block);
-  constexpr long long kRowStep = SRC == 2 ? 1 : 0;       // distance between a thread's rows: 1 or rows_per_iter
-  float acc[2 * VEC];
-#pragma unroll
-  for (int i = 0; i < 2 * VEC; ++i) acc[i] = 0.f;
-  if (active) {
-    float mu[VEC], sc[VEC], sh[VEC];
-    loadfv<VEC>(mean + v * VEC, mu);
-    if (SRC == 0 && act != B200_ACT_NONE) {
-      float is[VEC];
-      loadfv<VEC>(invstd + v * VEC, is);
-      if (gamma) loadfv<VEC>(gamma + v * VEC, sc);
-      if (beta) loadfv<VEC>(beta + v * VEC, sh);
-#pragma unroll
-      for (int i = 0; i < VEC; ++i) {
-        sc[i] = (gamma ? sc[i] : 1.f) * is[i];
-        sh[i] = (beta ? sh[i] : 0.f) - mu[i] * sc[i];
-      }
-    }
-    const long long col = (long long)v * VEC;
-    const long long rstep = kRowStep ? 1 : rows_per_iter;
-    for (long long r = row_begin + (kRowStep ? (long long)r0 * ROWS : r0); r < row_end;
-         r += (long long)ROWS * rows_per_iter) {
-      RawVec<VEC> rd[ROWS], rz[ROWS], ry[ROWS];
-      unsigned long long rm = 0;
-      bool ok[ROWS];
-      if (SRC == 2) rm = mask_rows<ROWS>(amask, r, C >> 3, (int)(col >> 3)) >> (col & 7 & ~(VEC - 1));
-#pragma unroll
-      for (int u = 0; u < ROWS; ++u) {
-        const long long rr = r + (long long)u * rstep;
-        ok[u] = rr < row_end;
-        if (ok[u]) {
-          rd[u] = ldv(dy + rr * C + col, (RawVec<VEC>*)nullptr);
-          rz[u] = ldv(z + rr * C + col, (RawVec<VEC>*)nullptr);
-          if (SRC == 1) ry[u] = ldv(y + rr * C + col, (RawVec<VEC>*)nullptr);
-        }
-      }
-#pragma unroll
-      for (int u = 0; u < ROWS; ++u) {
-        if (!ok[u]) continue;
-        float da[VEC], za[VEC], ya[VEC];
-        unpackv(rd[u], da);
-        unpackv(rz[u], za);
-        if (SRC == 1) unpackv(ry[u], ya);
-#pragma unroll
-        for (int i = 0; i < VEC; ++i) {
-          float g = da[i];
-          if (SRC == 2) g = ((rm >> (8 * u + i)) & 1ull) ? g : 0.f;
-          else if (act != B200_ACT_NONE && act_mask(SRC == 1 ? ya[i] : fmaf(za[i], sc[i], sh[i]), act) == 0.f) g = 0.f;
-          acc[i] = fmaf(g, za[i] - mu[i], acc[i]);   // the 1/std factor is applied once per channel below
-          acc[VEC + i] += g;
-        }
-      }
-    }
-    float is[VEC];
-    loadfv<VEC>(invstd + v * VEC, is);
-#pragma unroll
-    for (int i = 0; i < VEC; ++i) acc[i] *= is[i];
-  }
-  // block partial: fold the rows_per_iter row groups in shared memory, one coalesced row of 2C floats per block
-  __shared__ float red[kBnThreads][2 * VEC + 1];
-#pragma unroll
-  for (int i = 0; i < 2 * VEC; ++i) red[t][i] = acc[i];
-  __syncthreads();
-  float* dst = partial + (size_t)blockIdx.x * 2 * C;
-  for (int o = t; o < 2 * C; o += kBnThreads) {
-    const int stat = o / C;
-    const int c = o - stat * C;
-    const int vv = c / VEC, e = c - vv * VEC;
-    float sacc = 0.f;
-    for (int r = 0; r < rows_per_iter; ++r) sacc += red[r * cv + vv][stat * VEC + e];
-    dst[o] = sacc;
-  }
+  bn_bwd_reduce_body<VEC, ROWS, SRC>(dy, y, amask, z, M, C, cv, rows_per_iter, act, mean, invstd, gamma, beta,
+                                     partial, 1.f);
 }
 
 // second stage: sums[o] = sum over blocks of partial[b][o]  (o in [0, 2C): dgamma then dbeta); a block of 256
@@ -370,6 +287,11 @@ __global__ void __launch_bounds__(kBnThreads) bn_bwd_reduce_final_kernel(const f
     else if (dbeta_acc) dbeta_acc[o - C] += f;
   }
 }
+void launch_bwd_reduce_final(const float* partial, int nblocks, int C, float* sums, float* dgamma_acc,
+                             float* dbeta_acc, cudaStream_t stream) {
+  b200::launch(bn_bwd_reduce_final_kernel, (2 * C + 3) / 4, kBnThreads, 0, stream, partial, nblocks, C, sums, dgamma_acc,
+                                                                           dbeta_acc);
+}
 
 // ---- backward dx --------------------------------------------------------------------------------
 template <int VEC, int ROWS, int MINB, int SRC>   // SRC as in bn_bwd_reduce_kernel
@@ -379,72 +301,8 @@ __global__ void __launch_bounds__(kBnThreads, MINB) bn_bwd_dx_kernel(
     const float* __restrict__ mean, const float* __restrict__ invstd, const float* __restrict__ gamma,
     const float* __restrict__ beta, const float* __restrict__ sums, __nv_bfloat16* __restrict__ dz,
     __nv_bfloat16* __restrict__ g_out) {
-  const int t = threadIdx.x;
-  if (t >= rows_per_iter * cv) return;
-  const int r0 = t / cv, v = t - r0 * cv;
-  const long long rows_per_block = SRC == 2 ? (((M + gridDim.x - 1) / gridDim.x + 7) & ~7LL) : (M + gridDim.x - 1) / gridDim.x;
-  const long long row_begin = blockIdx.x * rows_per_block;
-  const long long row_end = min(M, row_begin + rows_per_block);
-  constexpr long long kRowStep = SRC == 2 ? 1 : 0;       // as in bn_bwd_reduce_kernel
-  // dz = A*g + B*z + Cc  with A = gamma*istd, B = -gamma*istd^2*dgamma/M, Cc = -A*dbeta/M - B*mean;
-  // the activation argument recomputed from z is z*A + sh
-  float A[VEC], B[VEC], Cc[VEC], sh[VEC];
-  {
-    float mu[VEC], is[VEC], dg[VEC], dbt[VEC];
-    loadfv<VEC>(mean + v * VEC, mu);
-    loadfv<VEC>(invstd + v * VEC, is);
-    if (gamma) loadfv<VEC>(gamma + v * VEC, A);
-    if (beta) loadfv<VEC>(beta + v * VEC, sh);
-    loadfv<VEC>(sums + v * VEC, dg);
-    loadfv<VEC>(sums + C + v * VEC, dbt);
-    const float invM = 1.f / (float)M;
-#pragma unroll
-    for (int i = 0; i < VEC; ++i) {
-      const float gm = gamma ? A[i] : 1.f;
-      A[i] = gm * is[i];
-      B[i] = -gm * is[i] * is[i] * dg[i] * invM;
-      Cc[i] = -A[i] * dbt[i] * invM - B[i] * mu[i];
-      sh[i] = (beta ? sh[i] : 0.f) - mu[i] * A[i];
-    }
-  }
-  const long long col = (long long)v * VEC;
-  const long long rstep = kRowStep ? 1 : rows_per_iter;
-  for (long long r = row_begin + (kRowStep ? (long long)r0 * ROWS : r0); r < row_end;
-       r += (long long)ROWS * rows_per_iter) {
-    RawVec<VEC> rd[ROWS], rz[ROWS], ry[ROWS];
-    unsigned long long rm = 0;
-    bool ok[ROWS];
-    if (SRC == 2) rm = mask_rows<ROWS>(amask, r, C >> 3, (int)(col >> 3)) >> (col & 7 & ~(VEC - 1));
-#pragma unroll
-    for (int u = 0; u < ROWS; ++u) {
-      const long long rr = r + (long long)u * rstep;
-      ok[u] = rr < row_end;
-      if (ok[u]) {
-        rd[u] = ldv(dy + rr * C + col, (RawVec<VEC>*)nullptr);
-        rz[u] = ldv(z + rr * C + col, (RawVec<VEC>*)nullptr);
-        if (SRC == 1) ry[u] = ldv(y + rr * C + col, (RawVec<VEC>*)nullptr);
-      }
-    }
-#pragma unroll
-    for (int u = 0; u < ROWS; ++u) {
-      if (!ok[u]) continue;
-      const long long rr = r + (long long)u * rstep;
-      float da[VEC], za[VEC], ya[VEC];
-      unpackv(rd[u], da);
-      unpackv(rz[u], za);
-      if (SRC == 1) unpackv(ry[u], ya);
-#pragma unroll
-      for (int i = 0; i < VEC; ++i) {
-        float g = da[i];
-        if (SRC == 2) g = ((rm >> (8 * u + i)) & 1ull) ? g : 0.f;
-        else if (act != B200_ACT_NONE && act_mask(SRC == 1 ? ya[i] : fmaf(za[i], A[i], sh[i]), act) == 0.f) g = 0.f;
-        da[i] = g;
-        za[i] = A[i] * g + B[i] * za[i] + Cc[i];
-      }
-      storev(dz + rr * C + col, za);
-      if (g_out) storev(g_out + rr * C + col, da);
-    }
-  }
+  bn_bwd_dx_body<VEC, ROWS, SRC>(dy, y, amask, z, M, C, cv, rows_per_iter, act, mean, invstd, gamma, beta, sums, dz,
+                                 g_out, 1.f);
 }
 
 static inline double* ws_accum(float* ws) { return reinterpret_cast<double*>(ws); }
@@ -563,8 +421,7 @@ extern "C" int b200_bn_bwd_reduce(const void* dy, const void* y, const uint8_t* 
 #undef B200_LAUNCH_RED
 #undef B200_RED_ARGS
   B200_CHECK_LAUNCH("bn_bwd_reduce_kernel");
-  b200::launch(bn_bwd_reduce_final_kernel, (2 * C + 3) / 4, kBnThreads, 0, stream, partial, blocks, C, sums, dgamma_acc,
-                                                                           dbeta_acc);
+  launch_bwd_reduce_final(partial, blocks, C, sums, dgamma_acc, dbeta_acc, stream);
   B200_CHECK_LAUNCH("bn_bwd_reduce_final_kernel");
   return B200_OK;
 }

@@ -253,7 +253,7 @@ class _SE(object):
 class _Unit(object):
     """saved state of one conv+BN unit for backward."""
     __slots__ = ('x', 'z', 'y', 'w', 'desc', 'mean', 'invstd', 'scale', 'shift', 'sums', 'conv', 'bn', 'act', 'mask',
-                 'sign_sum')
+                 'sign_sum', 'drop')
 
 
 class Runtime(object):
@@ -394,9 +394,11 @@ class Runtime(object):
         u.y = ops.conv_fprop(x, wf, u.desc, bias=bf, residual=residual, act=act)
         return u
 
-    def _unit_fwd(self, x, conv, bn, act, training, tape, residual=None, other=None):
+    def _unit_fwd(self, x, conv, bn, act, training, tape, residual=None, other=None, drop=None):
         """z = conv(x); BN statistics (train) / running-stat coefficients (eval);
-        y = act(bn(z) + residual | + bn_other(z_other)).  Returns y and (if tape) the saved unit."""
+        y = act(bn(z) + residual | + bn_other(z_other)).  Returns y and (if tape) the saved unit.
+        drop = (layer, p): in training y = dropout(relu(bn(z))) with the mask of (self.dropout_key, layer); ignored in
+        eval mode."""
         if not training and FOLD_BN_EVAL and not self._want_tape:
             return self._unit_fwd_folded(x, conv, bn, act, residual=residual, other=other)
         N, H, W, _ = x.shape
@@ -405,6 +407,13 @@ class Runtime(object):
         u.desc = conv.desc(N, H, W)
         u.w = conv.kernel_weights()
         self._conv_and_coeffs(u, x, u.w, training)
+        u.drop = drop if training else None
+        if u.drop is not None:
+            # the kept-and-positive bits are the only record of the mask: the backward reads them, never the stream
+            u.mask = torch.empty(ops.bn_act_mask_bytes(u.z.numel() // u.z.shape[-1], u.z.shape[-1]), device=self.device,
+                                 dtype=torch.uint8)
+            u.y = ops.bn_apply_dropout(u.z, u.scale, u.shift, self.dropout_key, drop[0], drop[1], u.mask)
+            return u
         # a join (something is added before the activation) cannot recompute act'(.) from z alone: keep one bit per
         # element instead of re-reading the bf16 output in both backward kernels (row-quad words, one extra load per
         # thread and iteration; -0.74 ms/step on ResNet-50)
@@ -503,6 +512,12 @@ class Runtime(object):
         """BN (+activation) backward of unit u: returns dz (and g = dy*act'(.) when want_g).
         y_mask=None with an activation: the mask is recomputed from z inside the kernels (no read of y)."""
         bn = u.bn
+        drop = getattr(u, 'drop', None)
+        if drop is not None:        # dropout(relu(bn(z))): g = bit ? dy * c : 0 from the forward's mask bits
+            ops.bn_bwd_reduce_dropout(dy, u.z, u.mask, drop[1], u.mean, u.invstd, u.sums, bn.dgamma, bn.dbeta, self._ws)
+            if self.sync_bn_world > 1:
+                self._sync_bn_sums(u.sums)
+            return ops.bn_bwd_dx_dropout(dy, u.z, u.mask, drop[1], u.mean, u.invstd, bn.gamma, u.sums), None
         mask = getattr(u, 'mask', None) if y_mask is not None else None
         ops.bn_bwd_reduce(dy, y_mask, u.z, act, u.mean, u.invstd, bn.gamma, bn.beta, u.sums, bn.dgamma, bn.dbeta,
                           self._ws, act_mask=mask)
@@ -778,6 +793,7 @@ class ResNetRuntime(Runtime):
 
     def _build(self):
         from .models.resnet import BasicBlock, Bottleneck
+        from .models.modules.lp_norm import L1BatchNorm2d
         m, a = self.model, self.arena
         self.imagenet_stem = m.conv1.kernel_size == (7, 7)
         if self.imagenet_stem:
@@ -792,16 +808,28 @@ class ResNetRuntime(Runtime):
         self.stem_bn = _BN(a, m.bn1)
         self.has_maxpool = isinstance(m.maxpool, nn.MaxPool2d)
         self.blocks = []
+        n_drop = 0
         for lname in ('layer1', 'layer2', 'layer3', 'layer4'):
             layer = getattr(m, lname)
             if isinstance(layer, nn.Identity):
                 continue
             for blk in layer:
-                if isinstance(blk.dropout, nn.Dropout) and blk.dropout.p != 0:
+                p = float(blk.dropout.p) if isinstance(blk.dropout, nn.Dropout) else 0.0
+                if p != 0 and not isinstance(blk, BasicBlock):
                     raise B200Error('dropout inside residual blocks is not supported on the B200 path')
                 spec = {'kind': 'bottleneck' if isinstance(blk, Bottleneck) else 'basic'}
                 if not isinstance(blk, (BasicBlock, Bottleneck)):
                     raise B200Error('unknown block type %s' % type(blk).__name__)
+                # BasicBlock dropout after relu(bn1(conv1(x))): fused into that unit's apply and backward (dropout.cu),
+                # layer index = position among the network's dropout layers (part of the mask's Philox counter)
+                spec['drop'] = None
+                if p != 0:
+                    if not 0.0 < p < 1.0:
+                        raise B200Error('dropout rate %r inside residual blocks: the B200 path needs 0 < p < 1' % p)
+                    if isinstance(blk.bn1, L1BatchNorm2d):
+                        raise B200Error('dropout with L1 BatchNorm is not supported on the B200 path')
+                    spec['drop'] = (n_drop, p)
+                    n_drop += 1
                 names = ('conv1', 'conv2', 'conv3') if spec['kind'] == 'bottleneck' else ('conv1', 'conv2')
                 spec['convs'] = [_Conv(a, getattr(blk, n)) for n in names]
                 spec['bns'] = [_BN(a, getattr(blk, n.replace('conv', 'bn'))) for n in names]
@@ -812,6 +840,9 @@ class ResNetRuntime(Runtime):
                 spec['se'] = _SE(a, blk.residual_block) if blk.residual_block is not None else None
                 self.blocks.append(spec)
         self._head_build(m.fc)
+        # one 64-bit Philox key per training step, drawn on the device with torch's CUDA generator (a captured step
+        # draws a fresh one on every replay; torch.manual_seed makes runs reproducible)
+        self.dropout_key = torch.zeros(1, device=self.device, dtype=torch.int64) if n_drop else None
 
     # ---- stem ---------------------------------------------------------------------------------------
     def _stem_fwd(self, x, training, mix=None, aug=None):
@@ -874,7 +905,7 @@ class ResNetRuntime(Runtime):
         units = []
         h = x
         for i in range(len(convs) - 1):
-            u = self._unit_fwd(h, convs[i], bns[i], ACT_RELU, training, True)
+            u = self._unit_fwd(h, convs[i], bns[i], ACT_RELU, training, True, drop=spec['drop'] if i == 0 else None)
             units.append(u)
             h = u.y
         down, se_tape = None, None
@@ -920,6 +951,8 @@ class ResNetRuntime(Runtime):
         self._want_tape = want_tape
         if training:
             self.arena.version += 1          # running statistics change: folded inference weights become stale
+            if self.dropout_key is not None:
+                self.dropout_key.random_(-2 ** 63, None)         # the full 64-bit range
         h, stem = self._stem_fwd(x, training, mix, aug)
         saved = []
         for spec in self.blocks:

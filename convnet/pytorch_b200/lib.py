@@ -54,6 +54,9 @@ SIGNATURES = {
     "b200_bn_l1_stats": [_vp, _ll, _i, _vp, _vp, _f, _f, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp],
     "b200_bn_l1_eval_coeffs": [_i, _vp, _vp, _vp, _vp, _vp, _vp, _vp],
     "b200_bn_l1_bwd_dx": [_vp, _vp, _vp, _vp, _ll, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp],
+    "b200_bn_apply_dropout": [_vp, _ll, _i, _vp, _vp, _vp, _i, ctypes.c_uint, _f, _vp, _vp, _vp],
+    "b200_bn_bwd_reduce_dropout": [_vp, _vp, _vp, _ll, _i, _f, _vp, _vp, _vp, _vp, _vp, _vp, _vp],
+    "b200_bn_bwd_dx_dropout": [_vp, _vp, _vp, _ll, _i, _f, _vp, _vp, _vp, _vp, _vp, _vp],
     "b200_maxpool3x3s2_fwd": [_vp, _i, _i, _i, _i, _vp, _vp, _vp],
     "b200_maxpool3x3s2_bwd": [_vp, _vp, _i, _i, _i, _i, _vp, _vp],
     "b200_bn_apply_maxpool3x3s2": [_vp, _i, _i, _i, _i, _vp, _vp, _i, _vp, _vp, _vp],

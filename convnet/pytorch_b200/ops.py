@@ -313,6 +313,62 @@ def bn_l1_bwd_dx(dy, y, z, act, mean, invstd, sign_sum, gamma, beta, sums, dz=No
     return dz
 
 
+# ------------------------------------------------------------------------------------ dropout in residual blocks
+def dropout_threshold(p):
+    """(T, c) of dropout rate 0 <= p < 1: an element is kept iff its 16-bit Philox uniform is < T = round((1-p)*65536)
+    (computed in double; keep probability T/65536), and kept values are scaled by c = fp32(1/(1-p)) as in torch."""
+    p = float(p)
+    if not 0.0 <= p < 1.0:
+        raise _l.B200Error('dropout rate must be in [0, 1), got %r' % p)
+    return int(round((1.0 - p) * 65536.0)), float(ctypes.c_float(1.0 / (1.0 - p)).value)
+
+
+def bn_apply_dropout(z, scale, shift, key, layer, p, act_mask, out=None):
+    """y = dropout(relu(z*scale + shift)) with the Philox mask of (key, layer) (csrc/dropout.cu); act_mask receives
+    keep && pre > 0 for bn_bwd_*_dropout.  key: int64 device tensor of one element, read by the kernel."""
+    C = z.shape[-1]
+    M = z.numel() // C
+    _chk(z, bf16, "z"); _chk(key, torch.int64, "key"); _chk(act_mask, torch.uint8, "act_mask")
+    if act_mask is None or act_mask.numel() != bn_act_mask_bytes(M, C):
+        raise _l.B200Error("act_mask must hold bn_act_mask_bytes(M, C) bytes")
+    T, c = dropout_threshold(p)
+    if out is None:
+        out = torch.empty_like(z)
+    with _T('bn_apply_dropout', 0, 2 * 2 * z.numel() + act_mask.numel()):
+        _l.check(_l.load().b200_bn_apply_dropout(z.data_ptr(), M, C, scale.data_ptr(), shift.data_ptr(), key.data_ptr(),
+                                                 int(layer), T, c, out.data_ptr(), act_mask.data_ptr(), _stream()),
+                 "b200_bn_apply_dropout")
+    return out
+
+
+def bn_bwd_reduce_dropout(dy, z, act_mask, p, mean, invstd, sums, dgamma_acc, dbeta_acc, workspace):
+    """bn_bwd_reduce of a bn_apply_dropout unit: g = bit ? dy*c : 0"""
+    C = z.shape[-1]
+    M = z.numel() // C
+    _chk(dy, bf16, "dy"); _chk(z, bf16, "z"); _chk(act_mask, torch.uint8, "act_mask")
+    _, c = dropout_threshold(p)
+    with _T('bn_bwd_reduce_dropout', 0, 2 * 2 * z.numel() + act_mask.numel()):
+        _l.check(_l.load().b200_bn_bwd_reduce_dropout(dy.data_ptr(), act_mask.data_ptr(), z.data_ptr(), M, C, c,
+                                                      mean.data_ptr(), invstd.data_ptr(), sums.data_ptr(),
+                                                      _l.ptr(dgamma_acc), _l.ptr(dbeta_acc), workspace.data_ptr(),
+                                                      _stream()), "b200_bn_bwd_reduce_dropout")
+
+
+def bn_bwd_dx_dropout(dy, z, act_mask, p, mean, invstd, gamma, sums, dz=None):
+    """bn_bwd_dx of a bn_apply_dropout unit: g = bit ? dy*c : 0"""
+    C = z.shape[-1]
+    M = z.numel() // C
+    _chk(dy, bf16, "dy"); _chk(z, bf16, "z"); _chk(act_mask, torch.uint8, "act_mask")
+    _, c = dropout_threshold(p)
+    if dz is None:
+        dz = torch.empty_like(z)
+    with _T('bn_bwd_dx_dropout', 0, 2 * 3 * z.numel() + act_mask.numel()):
+        _l.check(_l.load().b200_bn_bwd_dx_dropout(dy.data_ptr(), act_mask.data_ptr(), z.data_ptr(), M, C, c,
+                                                  mean.data_ptr(), invstd.data_ptr(), _l.ptr(gamma), sums.data_ptr(),
+                                                  dz.data_ptr(), _stream()), "b200_bn_bwd_dx_dropout")
+    return dz
+
+
 # ------------------------------------------------------------------------------------ pooling
 def _out(out, shape, dtype, device, name):
     """a caller-supplied output (checked: dtype, contiguity, shape) or a new tensor"""

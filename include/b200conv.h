@@ -5,7 +5,7 @@
  * The reference has no FFI of its own (it is pure Python on top of torch.nn); every entry point
  * below replaces one implicit torch/cuDNN/ATen operator the reference invokes, cited per function
  * as reference file:line (paths under the reference tree).  INTEGRATION.md shows the ctypes stubs.
- * 50 entry points.
+ * 53 entry points.
  *
  * Conventions
  *  - every function returns 0 on success or a negative B200_ERR_* code; b200_last_error() gives text.
@@ -153,6 +153,24 @@ int b200_bn_l1_eval_coeffs(int C, const float* gamma, const float* beta, const f
 int b200_bn_l1_bwd_dx(const void* dy, const void* y, const uint8_t* act_mask, const void* z, long long M, int C,
                       int act, const float* mean, const float* invstd, const float* sign_sum, const float* gamma,
                       const float* beta, const float* sums, void* dz, void* g_out, b200_stream_t stream);
+
+/* ---- dropout inside residual blocks (csrc/dropout.cu) ---------------------------------------------
+ * replaces nn.Dropout(p) after relu(bn1(conv1(x))) of a CIFAR BasicBlock (models/resnet.py:81-118) in training mode.
+ * Mask stream: Philox4x32-10 with key {k0, k1} = low / high word of *key (64 bits, device memory: a captured graph reads
+ * the value of each replay); the 8-channel vector g = (row*C + c)/8 of dropout layer `layer` uses counter
+ * {g & 0xffffffff, g >> 32, layer, 0} and keeps its element j iff ((w[j/2] >> 16*(j%2)) & 0xffff) < T for the four
+ * output words w.  T = round((1 - p) * 65536) (T <= 65536), c = fp32(1/(1 - p)).
+ * y = keep && pre > 0 ? pre*c : +0 with pre = z*scale + shift; act_mask (required, b200_bn_act_mask_bytes(M, C) bytes,
+ * row-quad layout as b200_bn_apply) receives keep && pre > 0. */
+int b200_bn_apply_dropout(const void* z, long long M, int C, const float* scale, const float* shift, const uint64_t* key,
+                          int layer, unsigned T, float c, void* y, uint8_t* act_mask, b200_stream_t stream);
+/* b200_bn_bwd_reduce / b200_bn_bwd_dx of that unit with g = bit ? dy*c : +0 (bits from b200_bn_apply_dropout) */
+int b200_bn_bwd_reduce_dropout(const void* dy, const uint8_t* act_mask, const void* z, long long M, int C, float c,
+                               const float* mean, const float* invstd, float* sums, float* dgamma_acc, float* dbeta_acc,
+                               float* workspace, b200_stream_t stream);
+int b200_bn_bwd_dx_dropout(const void* dy, const uint8_t* act_mask, const void* z, long long M, int C, float c,
+                           const float* mean, const float* invstd, const float* gamma, const float* sums, void* dz,
+                           b200_stream_t stream);
 
 /* ---- pooling (csrc/pool.cu) -------------------------------------------------------------------
  * replaces nn.MaxPool2d(3,2,1) (models/resnet.py:230) and nn.AdaptiveAvgPool2d(1) (resnet.py:241) */
