@@ -12,6 +12,9 @@
 // coefficients sit in a per-thread shared-memory slab of kRrcTaps taps (rebuilt per row when a column has more taps, so
 // the scale is unbounded); vertical coefficients are computed per chunk of kRrcYChunk intermediate rows.  The grid
 // depends only on (B*D, OH) and there is no workspace: a captured CUDA graph replays with new tables and regions.
+//
+// The same arithmetic (the rrc_* helpers below) serves the small fixed-size resample of the CIFAR Mix&Match transform,
+// input_prep_aug_resize_kernel at the end of this file.
 #include "common.cuh"
 #include "host.h"
 
@@ -209,9 +212,145 @@ __global__ void __launch_bounds__(kRrcMaxOW) input_prep_rrc_kernel(
   }
 }
 
+// ---- the CIFAR Mix&Match transform (preprocess.py:44-54 with input_size != scale_size): RandomCrop(padding) ->
+// Resize -> RandomHorizontalFlip -> ToTensor -> Normalize [-> Cutout], D copies per image ---------------------------
+// Every copy resamples the same H x W window size to OH x OW, so the two coefficient tables depend on the launch only:
+// one block owns one copy, builds both tables once in shared memory, stages the zero-padded crop window as uint8, runs
+// the horizontal pass into a shared uint8 [H][OW][C] and lets each thread finish one output pixel (vertical pass, flip,
+// LUT, Cutout, store).  Nothing passes through global memory between the passes, there is no workspace and the grid
+// depends only on N*D: a captured CUDA graph replays with new images and draws.
+constexpr int kAugRsThreads = 256;
+constexpr int kAugRsMaxIn = 64;     // source side: the window and the intermediate stay in shared memory
+constexpr int kAugRsMaxOut = 128;
+
+// first tap, tap count and 22-bit coefficients of output index i of an in -> out resample; taps bounds the count
+__device__ __forceinline__ void rrc_table(const RrcAxis& a, int i, int taps, int* first, int* count, int* coef) {
+  double center;
+  int lo, cnt;
+  rrc_bounds(a, i, center, lo, cnt);
+  cnt = min(cnt, taps);
+  const double ww = rrc_sum(a, center, lo, cnt);
+  first[i] = lo;
+  count[i] = cnt;
+  for (int t = 0; t < cnt; ++t) coef[i * taps + t] = rrc_coef(rrc_tri(a, center, lo + t), ww);
+}
+
+__global__ void __launch_bounds__(kAugRsThreads) input_prep_aug_resize_kernel(
+    const uint8_t* __restrict__ x, int D, int C, int H, int W, int OH, int OW, int Cpad, int pad, int tx, int ty,
+    const float* __restrict__ lut, const int16_t* __restrict__ params, int holes, __nv_bfloat16* __restrict__ out) {
+  extern __shared__ __align__(16) unsigned char aug_rs_smem[];
+  int* xfirst = reinterpret_cast<int*>(aug_rs_smem);          // [OW]
+  int* xcount = xfirst + OW;                                  // [OW]
+  int* yfirst = xcount + OW;                                  // [OH]
+  int* ycount = yfirst + OH;                                  // [OH]
+  int* kx = ycount + OH;                                      // [OW][tx]
+  int* ky = kx + OW * tx;                                     // [OH][ty]
+  uint8_t* win = reinterpret_cast<uint8_t*>(ky + OH * ty);    // [H][W][C]   the padded crop window
+  uint8_t* mid = win + H * W * C;                             // [H][OW][C]  after the horizontal pass
+
+  const int n = blockIdx.x;                     // output row n: copy n % D of image n / D
+  const int16_t* pr = params + (long long)n * (3 + 4 * holes);
+  const int oy = __ldg(pr + 0) - pad, ox = __ldg(pr + 1) - pad;
+  const bool flip = __ldg(pr + 2) != 0;
+
+  const RrcAxis ax = rrc_axis(W, OW), ay = rrc_axis(H, OH);
+  for (int i = threadIdx.x; i < OW + OH; i += kAugRsThreads) {
+    if (i < OW) rrc_table(ax, i, tx, xfirst, xcount, kx);
+    else rrc_table(ay, i - OW, ty, yfirst, ycount, ky);
+  }
+  // any draw values are safe: a source pixel is read only when it lies inside the image, else RandomCrop's fill 0
+  const uint8_t* src = x + (long long)(n / D) * H * W * C;
+  for (int e = threadIdx.x; e < H * W; e += kAugRsThreads) {
+    const int sy = e / W + oy, sx = e % W + ox;
+    const bool ok = sy >= 0 && sy < H && sx >= 0 && sx < W;
+    for (int c = 0; c < C; ++c) win[e * C + c] = ok ? __ldg(src + (sy * W + sx) * C + c) : (uint8_t)0;
+  }
+  __syncthreads();
+
+  for (int e = threadIdx.x; e < H * OW; e += kAugRsThreads) {
+    const int r = e / OW, xx = e % OW;
+    const int* k = kx + xx * tx;
+    const uint8_t* p = win + (r * W + xfirst[xx]) * C;
+    int h[4] = {1 << 21, 1 << 21, 1 << 21, 1 << 21};
+    for (int t = 0; t < xcount[xx]; ++t)
+#pragma unroll
+      for (int c = 0; c < 4; ++c)
+        if (c < C) h[c] += (int)p[t * C + c] * k[t];
+#pragma unroll
+    for (int c = 0; c < 4; ++c)
+      if (c < C) mid[e * C + c] = (uint8_t)rrc_clip8(h[c]);
+  }
+  __syncthreads();
+
+  for (int e = threadIdx.x; e < OH * OW; e += kAugRsThreads) {
+    const int yy = e / OW, xx = e % OW;
+    const int* k = ky + yy * ty;
+    const uint8_t* p = mid + (yfirst[yy] * OW + xx) * C;
+    int v[4] = {1 << 21, 1 << 21, 1 << 21, 1 << 21};
+    for (int t = 0; t < ycount[yy]; ++t)
+#pragma unroll
+      for (int c = 0; c < 4; ++c)
+        if (c < C) v[c] += (int)p[t * OW * C + c] * k[t];
+    // the flip mirrors the resized picture; the Cutout boxes are in its (output) coordinates
+    const int j = flip ? OW - 1 - xx : xx;
+    bool cut = false;
+    for (int hh = 0; hh < holes; ++hh) {
+      const int16_t* b = pr + 3 + 4 * hh;
+      cut |= yy >= __ldg(b + 0) && yy < __ldg(b + 1) && j >= __ldg(b + 2) && j < __ldg(b + 3);
+    }
+    float f[4];
+#pragma unroll
+    for (int c = 0; c < 4; ++c) {
+      f[c] = 0.f;
+      if (c < C) {
+        f[c] = __ldg(lut + c * 256 + rrc_clip8(v[c]));
+        if (cut) f[c] = __fmul_rn(f[c], 0.f);
+      }
+    }
+    __nv_bfloat16* o = out + (((long long)n * OH + yy) * OW + j) * Cpad;
+    uint4 u = {pack_bf16x2(f[0], f[1]), pack_bf16x2(f[2], f[3]), 0u, 0u};
+    for (int c0 = 0; c0 < Cpad; c0 += 8) {
+      *reinterpret_cast<uint4*>(o + c0) = u;
+      u = make_uint4(0u, 0u, 0u, 0u);
+    }
+  }
+}
+
+// upper bound of the taps of one output index: hi - lo <= 2 * support + 1, and never more than the source
+static int aug_rs_taps(int in, int out) {
+  const int support = in > out ? (in + out - 1) / out : 1;
+  const int taps = 2 * support + 1;
+  return taps < in ? taps : in;
+}
+
 }  // namespace b200
 
 using namespace b200;
+
+extern "C" int b200_input_prep_u8_aug_resize(const uint8_t* x_nhwc, int N, int D, int C, int H, int W, int OH, int OW,
+                                             int Cpad, int pad, const float* lut, const int16_t* params, int holes,
+                                             void* out, b200_stream_t stream) {
+  B200_REQUIRE(x_nhwc && out && lut && params && N > 0 && D > 0 && C > 0 && C <= 4 && H > 0 && W > 0 && OH > 0 && OW > 0,
+               B200_ERR_INVALID, "input_prep_u8_aug_resize: bad argument (C must be 1..4)");
+  B200_REQUIRE(Cpad % 8 == 0 && Cpad >= C, B200_ERR_INVALID,
+               "input_prep_u8_aug_resize: Cpad must be a multiple of 8 and >= C");
+  B200_REQUIRE(pad >= 0 && holes >= 0 && holes <= 64, B200_ERR_INVALID,
+               "input_prep_u8_aug_resize: pad=%d holes=%d out of range", pad, holes);
+  B200_REQUIRE(H <= kAugRsMaxIn && W <= kAugRsMaxIn && OH <= kAugRsMaxOut && OW <= kAugRsMaxOut, B200_ERR_UNSUPPORTED,
+               "input_prep_u8_aug_resize: %dx%d -> %dx%d above %d px sources or %d px outputs", H, W, OH, OW,
+               kAugRsMaxIn, kAugRsMaxOut);
+  B200_REQUIRE((long long)N * D <= 0x7fffffffLL, B200_ERR_UNSUPPORTED, "input_prep_u8_aug_resize: N*D too large");
+  const int tx = aug_rs_taps(W, OW), ty = aug_rs_taps(H, OH);
+  const size_t smem = (size_t)(2 * OW + 2 * OH + OW * tx + OH * ty) * sizeof(int) + (size_t)H * W * C + (size_t)H * OW * C;
+  cudaError_t e = cudaFuncSetAttribute(input_prep_aug_resize_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       (int)smem);
+  B200_REQUIRE(e == cudaSuccess, B200_ERR_CUDA, "input_prep_u8_aug_resize: smem attribute (%d bytes): %s", (int)smem,
+               cudaGetErrorString(e));
+  b200::launch(input_prep_aug_resize_kernel, N * D, kAugRsThreads, smem, (cudaStream_t)stream, x_nhwc, D, C, H, W, OH,
+               OW, Cpad, pad, tx, ty, lut, params, holes, (__nv_bfloat16*)out);
+  B200_CHECK_LAUNCH("input_prep_aug_resize_kernel");
+  return B200_OK;
+}
 
 extern "C" int b200_input_prep_u8_rrc(const uint8_t* regions, long long region_bytes, const long long* index,
                                       const int* draws, int B, int D, int C, int OH, int OW, int Cpad, int mode,

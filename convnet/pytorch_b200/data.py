@@ -15,7 +15,9 @@ Lighting are out of scope (SURVEY.md section 2).
 Batch augmentation on the device (transform key ``device_augment``, CIFAR-style training only): the loader yields
 (utils.augment.AugmentedBatch of the B uint8 NHWC images and their per-copy draws, target repeated to B*D) and the
 stem relayout kernel writes the B*D augmented copies.  Real cifar10 / cifar100 read the dataset's uint8 ``.data``;
-synthetic_cifar* use a pool of uniform uint8 images.
+synthetic_cifar* use a pool of uniform uint8 images.  When ``input_size`` differs from ``scale_size`` (the Mix&Match
+``sampled*`` regimes on cifar10 / cifar100: crops of the 32-px images resized to 16 / 24 / 48 px) the same kernel path
+resizes each crop; a synthetic pool is generated at ``input_size`` and is never resized.
 
 RandomResizedCrop on the device (transform key ``device_resized_crop``, ImageNet-style training only): the workers
 decode and draw the reference's crop boxes and flips per image; the loader yields (utils.augment.ResizedCropBatch of
@@ -166,17 +168,25 @@ def device_augment_spec(transform_name='cifar10', input_size=None, scale_size=No
         raise ValueError('device_augment is a training transform (augment=True); evaluation loaders do not take it')
     if autoaugment or num_crops != 1:
         raise NotImplementedError('device_augment does not reproduce autoaugment / multi-crop')
-    if scale_size is not None and input_size is not None and scale_size != input_size:
-        raise NotImplementedError('device_augment does not resize: scale_size %s != input_size %s'
-                                  % (scale_size, input_size))
+    # the reference crops at scale_size (32 unless set) and resizes to input_size when the two differ (preprocess.py:
+    # 44-54,134-143): the Mix&Match size regimes.  A synthetic dataset has no scale_size: its "transform" is its
+    # geometry, the pool is generated at input_size, and a setting that asks for both sizes is refused as before.
+    if (transform_name or '').startswith('synthetic'):
+        if scale_size is not None and input_size is not None and scale_size != input_size:
+            raise NotImplementedError('device_augment does not resize a synthetic pool (it is generated at input_size): '
+                                      'scale_size %s != input_size %s' % (scale_size, input_size))
+    elif scale_size is None:
+        scale_size = 32
+    resize = input_size if scale_size is not None and input_size is not None and scale_size != input_size else None
     return BatchAugment(padding=padding or 4, flip=True, cutout=cutout, duplicates=duplicates or 1,
-                        normalize=normalize or _IMAGE_STATS)
+                        normalize=normalize or _IMAGE_STATS, resize=resize)
 
 
-def u8_dataset(name, input_size=None, split='train', download=True, datasets_path='~/Datasets', synthetic_length=None,
-               **_):
+def u8_dataset(name, input_size=None, scale_size=None, split='train', download=True, datasets_path='~/Datasets',
+               synthetic_length=None, **_):
     """uint8 NHWC samples for device augmentation: the dataset's own uint8 array (cifar10 / cifar100), or a pool of
-    256 uniform uint8 images for synthetic_cifar*."""
+    256 uniform uint8 images at ``input_size`` for synthetic_cifar*.  The real images have the size the transform crops
+    at (``scale_size``, 32); a resize to ``input_size`` happens on the device."""
     train = split == 'train'
     if name in ('synthetic_cifar10', 'synthetic_cifar100'):
         size, classes, n_train, n_val = _SYNTHETIC[name]
@@ -187,9 +197,9 @@ def u8_dataset(name, input_size=None, split='train', download=True, datasets_pat
         return U8Images(images, torch.randint(0, classes, (length,), generator=g))
     if name in ('cifar10', 'cifar100'):
         import torchvision.datasets as tvd
-        if input_size not in (None, 32):
-            raise NotImplementedError('device_augment does not resize: %s images are 32x32, input_size %s'
-                                      % (name, input_size))
+        if scale_size not in (None, 32):
+            raise NotImplementedError('device_augment crops at the image size: %s images are 32x32, scale_size %s'
+                                      % (name, scale_size))
         cls = tvd.CIFAR10 if name == 'cifar10' else tvd.CIFAR100
         ds = cls(root=os.path.join(os.path.expanduser(datasets_path), name), train=train, download=download)
         return U8Images(ds.data, ds.targets)
@@ -302,7 +312,8 @@ class DataRegime(object):
                 collate = ResizedCropCollate(spec)
             elif setting['transform'].get('device_augment'):
                 spec = device_augment_spec(**setting['transform'])
-                self._data = u8_dataset(input_size=setting['transform'].get('input_size'), **data_kwargs)
+                self._data = u8_dataset(input_size=setting['transform'].get('input_size'),
+                                        scale_size=setting['transform'].get('scale_size'), **data_kwargs)
                 collate = AugmentCollate(spec)
             elif name in _SYNTHETIC:  # the "transform" of a synthetic dataset is just its geometry
                 data_kwargs['input_size'] = setting['transform'].get('input_size')

@@ -350,7 +350,8 @@ class Runtime(object):
                         raise B200Error('batch augmentation on the device needs the CIFAR-style 3x3 stem '
                                         '(the space-to-depth stem layouts are not supported)')
                     return ops.input_prep_u8_aug(t, cpad, aug, **kw)
-                return x.contiguous(), prep_aug, (N * aug.duplicates, C, H, W)
+                OH, OW = aug.out_hw or (H, W)       # the stem sees the resized copies, not the uint8 images' size
+                return x.contiguous(), prep_aug, (N * aug.duplicates, C, OH, OW)
             mean = getattr(self.model, 'input_mean', self.input_mean)
             std = getattr(self.model, 'input_std', self.input_std)
             return x.contiguous(), (lambda t, cpad, **kw: ops.input_prep_u8(t, cpad, mean[:C], std[:C], mix=mix, **kw)), \

@@ -69,6 +69,7 @@ SIGNATURES = {
     "b200_input_prep_u8_mix": [_vp, _i, _i, _i, _i, _i, _i, ctypes.POINTER(ctypes.c_float),
                                ctypes.POINTER(ctypes.c_float), _vp, _vp, _i, _vp, _vp],
     "b200_input_prep_u8_aug": [_vp, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _i, _vp, _vp],
+    "b200_input_prep_u8_aug_resize": [_vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _i, _vp, _vp],
     "b200_input_prep_u8_rrc": [_vp, _ll, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp],
     "b200_weight_transpose": [_vp, _vp, _i, _i, _i, _vp],
     "b200_weight_transpose_batched": [_vp, _vp, _vp, _i, _i, _vp],

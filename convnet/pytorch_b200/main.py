@@ -7,7 +7,8 @@
 
 Additions over the reference: ``--dtype bfloat16`` (compute type of the B200 kernels; parameters stay fp32
 masters in the arena), ``synthetic_*`` datasets, ``--b200 {auto,on,off}`` (auto: on for CUDA devices),
-``--device-augment`` (batch augmentation of the CIFAR transform done in the input relayout kernel),
+``--device-augment`` (batch augmentation of the CIFAR transform done in the input relayout kernel, with the Resize of
+the Mix&Match ``sampled*`` regimes),
 ``--device-resized-crop`` (the ImageNet RandomResizedCrop + flip resampled in the input relayout kernel), and
 rank/world are read from the torchrun environment when ``--local_rank`` is not given.
 """
@@ -73,8 +74,8 @@ def build_parser():
     a('--cutout', action='store_true', default=False,
       help='cutout augmentations (ignored for synthetic data unless --device-augment)')
     a('--device-augment', action='store_true', default=False,
-      help='CIFAR training: ship uint8 images and per-copy draws, and crop / flip / cutout the --duplicates copies '
-           'inside the input relayout on the GPU')
+      help='CIFAR training: ship uint8 images and per-copy draws, and crop / resize (Mix&Match size regimes) / flip / '
+           'cutout the --duplicates copies inside the input relayout on the GPU')
     a('--device-resized-crop', action='store_true', default=False,
       help='ImageNet training: the loader workers only decode and draw the crop boxes and flips; the input relayout '
            'on the GPU resamples the crops (Pillow-exact bilinear), flips and normalises them')

@@ -563,11 +563,13 @@ def input_prep_u8(x_nhwc_u8, cpad, mean, std, s2d=False, border=False, mix=None,
 class Aug(object):
     """Device-side draws of one batch-augmentation step (utils/augment.py): ``params`` int16 [N*D, 3 + 4*holes] rows
     {oy, ox, flip, y1, y2, x1, x2, ...}, ``lut`` fp32 [C, 256] (ToTensor + Normalize of each uint8 value), ``duplicates``
-    D, ``pad`` the crop padding.  The kernel reads params at run time, so a captured graph follows new draws in place."""
-    __slots__ = ('params', 'lut', 'duplicates', 'pad')
+    D, ``pad`` the crop padding, ``out_hw`` (OH, OW) when the crop is resized (the Mix&Match CIFAR regimes; None: the
+    copies keep the images' size).  The kernel reads params at run time, so a captured graph follows new draws in place."""
+    __slots__ = ('params', 'lut', 'duplicates', 'pad', 'out_hw')
 
-    def __init__(self, params, lut, duplicates, pad):
+    def __init__(self, params, lut, duplicates, pad, out_hw=None):
         self.params, self.lut, self.duplicates, self.pad = params, lut, int(duplicates), int(pad)
+        self.out_hw = (int(out_hw[0]), int(out_hw[1])) if out_hw is not None else None
 
     @property
     def holes(self):
@@ -576,14 +578,14 @@ class Aug(object):
     @property
     def key(self):
         """what a captured step depends on besides the input's shape (the draws are refreshed in place)"""
-        return ('aug', tuple(self.params.shape), self.duplicates, self.pad, self.lut.data_ptr())
+        return ('aug', tuple(self.params.shape), self.duplicates, self.pad, self.lut.data_ptr(), self.out_hw)
 
     @property
     def tables(self):
         return (self.params,)
 
     def with_tables(self, tables):
-        return Aug(tables[0], self.lut, self.duplicates, self.pad)
+        return Aug(tables[0], self.lut, self.duplicates, self.pad, self.out_hw)
 
 
 class Rrc(object):
@@ -656,7 +658,8 @@ def input_prep_u8_rrc(regions, cpad, rrc, s2d=False, border=False, out=None):
 
 def input_prep_u8_aug(x_nhwc_u8, cpad, aug, out=None):
     """uint8 NHWC [N,H,W,C] -> bf16 NHWC [N*D, H, W, cpad]: the D augmented copies of every image (crop, flip, Cutout)
-    normalised through aug.lut, row n*D + d = copy d of image n."""
+    normalised through aug.lut, row n*D + d = copy d of image n.  With aug.out_hw = (OH, OW) every crop is resized
+    (Pillow's bilinear resample) before the flip: bf16 [N*D, OH, OW, cpad], Cutout boxes in output coordinates."""
     _chk(x_nhwc_u8, torch.uint8, "x"); _chk(aug.params, torch.int16, "aug params"); _chk(aug.lut, torch.float32, "lut")
     N, H, W, C = x_nhwc_u8.shape
     D = aug.duplicates
@@ -664,6 +667,15 @@ def input_prep_u8_aug(x_nhwc_u8, cpad, aug, out=None):
             or tuple(aug.lut.shape) != (C, 256):
         raise _l.B200Error("input_prep_u8_aug: params must be int16 [N*D, 3+4*holes] and lut fp32 [C, 256]; got %s, %s"
                            % (tuple(aug.params.shape), tuple(aug.lut.shape)))
+    if aug.out_hw is not None:
+        OH, OW = aug.out_hw
+        out = _prep_out(N * D, OH, OW, cpad, False, False, x_nhwc_u8.device, out)
+        with _T('input_prep', 0, D * x_nhwc_u8.numel() + 2 * aug.params.numel() + 2 * out.numel()):
+            _l.check(_l.load().b200_input_prep_u8_aug_resize(x_nhwc_u8.data_ptr(), N, D, C, H, W, OH, OW, cpad, aug.pad,
+                                                             aug.lut.data_ptr(), aug.params.data_ptr(), aug.holes,
+                                                             out.data_ptr(), _stream()),
+                     "b200_input_prep_u8_aug_resize")
+        return out
     out = _prep_out(N * D, H, W, cpad, False, False, x_nhwc_u8.device, out)
     with _T('input_prep', 0, x_nhwc_u8.numel() + 2 * aug.params.numel() + 2 * out.numel()):
         _l.check(_l.load().b200_input_prep_u8_aug(x_nhwc_u8.data_ptr(), N, D, C, H, W, cpad, aug.pad,

@@ -605,7 +605,9 @@ class Trainer(object):
                           spec.duplicates, spec.size, batch.host + (batch.nbytes,))
             return rrc, batch.regions
         params = batch.params.to(device, non_blocking=True).reshape(-1, batch.params.shape[-1])
-        return ops.Aug(params, lut, spec.duplicates, spec.padding), batch.images
+        # a resize to the images' own size is the identity: that case stays on the kernel without the resample
+        out_hw = spec.resize if spec.resize != tuple(batch.images.shape[1:3]) else None
+        return ops.Aug(params, lut, spec.duplicates, spec.padding, out_hw), batch.images
 
     def _check_device_augment(self, training, average_output):
         if average_output:

@@ -9,7 +9,7 @@ augmented, normalised copies (ops.input_prep_u8_aug).  ``BatchAugment.apply`` re
 gather: it is the CPU path, the path of every non-fused configuration and the tests' oracle.
 
 Draw row of one copy (int16): (oy, ox, flip, y1, y2, x1, x2, ...) -- crop offsets in the padded image U{0..2p}, flip
-in {0, 1}, then one [y1, y2) x [x1, x2) box per Cutout hole in output coordinates.  The distributions are the
+in {0, 1}, then one [y1, y2) x [x1, x2) box per Cutout hole in output coordinates.  With ``resize`` the crop is resized before the flip, and "output" is the resized copy.  The distributions are the
 reference's; the draws are made with one RNG call per quantity and batch, so they do not replay its per-image stream
 (which depends on the DataLoader worker seeding anyway).
 """
@@ -51,18 +51,25 @@ def normalize_lut(normalize, C):
 
 
 class BatchAugment(object):
-    """``duplicates`` copies per image of RandomCrop(padding) + RandomHorizontalFlip (``flip``) + ToTensor + Normalize
-    (``normalize``: {'mean', 'std'}) + Cutout (``cutout``: None or {'holes', 'length'})."""
+    """``duplicates`` copies per image of RandomCrop(padding) [+ Resize(``resize``), bilinear] + RandomHorizontalFlip
+    (``flip``) + ToTensor + Normalize (``normalize``: {'mean', 'std'}) + Cutout (``cutout``: None or {'holes',
+    'length'}).  ``resize``: None, S or (OH, OW) -- the Mix&Match CIFAR size regimes crop at the images' size and resize
+    the crop (preprocess.py:44-54 of the reference with input_size != scale_size)."""
 
-    def __init__(self, padding=4, flip=True, cutout=None, duplicates=1, normalize=None):
+    def __init__(self, padding=4, flip=True, cutout=None, duplicates=1, normalize=None, resize=None):
         self.padding = int(padding)
         self.flip = bool(flip)
         self.holes = int(cutout['holes']) if cutout else 0
         self.length = int(cutout['length']) if cutout else 0
         self.duplicates = int(duplicates)
         self.normalize = normalize or _IMAGE_STATS
+        if resize is not None:
+            resize = (int(resize), int(resize)) if isinstance(resize, int) else (int(resize[0]), int(resize[1]))
+        self.resize = resize
         if self.padding < 0 or self.duplicates < 1 or self.holes < 0 or self.length < 0:
             raise ValueError('BatchAugment: padding, holes and length must be >= 0 and duplicates >= 1')
+        if resize is not None and min(resize) < 1:
+            raise ValueError('BatchAugment: resize must be >= 1')
         self._luts = {}
 
     @property
@@ -71,7 +78,8 @@ class BatchAugment(object):
         return 3 + 4 * self.holes
 
     def sample(self, B, H, W):
-        """-> int16 [B, D, 3 + 4*holes] draws for B images of H x W pixels."""
+        """-> int16 [B, D, 3 + 4*holes] draws for B images of H x W pixels: the crop offsets against the images, the
+        Cutout boxes against the output (the resized copy when ``resize`` is set)."""
         D, p = self.duplicates, self.padding
         if max(H, W) + 2 * p > 32767:
             raise ValueError('BatchAugment: %dx%d images with padding %d do not fit the int16 draws' % (H, W, p))
@@ -81,6 +89,7 @@ class BatchAugment(object):
         if self.flip:
             out[..., 2] = (torch.rand(B, D) < 0.5).to(torch.int16)                 # RandomHorizontalFlip: rand < p
         if self.holes:
+            H, W = self.resize or (H, W)
             y = np.random.randint(H, size=(B, D, self.holes))
             x = np.random.randint(W, size=(B, D, self.holes))
             half = self.length // 2
@@ -107,6 +116,8 @@ class BatchAugment(object):
         if N % B or (p.shape[1] - 3) % 4:
             raise ValueError('BatchAugment.apply: draws %s do not match %d images' % (tuple(params.shape), B))
         D, holes = N // B, (p.shape[1] - 3) // 4
+        if self.resize is not None:
+            return self._apply_resized(images.cpu(), p.cpu(), D, holes).to(dev)
         r, c = torch.arange(H, device=dev), torch.arange(W, device=dev)
         sy = r + p[:, 0:1] - self.padding                                           # [N, H]
         sx = torch.where(p[:, 2:3] != 0, W - 1 - c, c) + p[:, 1:2] - self.padding   # [N, W]
@@ -125,6 +136,41 @@ class BatchAugment(object):
                 mask.masked_fill_(inside, 0.)
             v = v * mask[:, None]
         return v
+
+    def _apply_resized(self, images, p, D, holes):
+        """The resizing form of apply(), -> fp32 NCHW [B*D, C, OH, OW]: torchvision's own pad / crop / resize / hflip /
+        to_tensor / normalize on PIL images and the reference's Cutout mask (its arithmetic by construction).  Three
+        channels make one RGB image; any other count is resampled channel by channel (the filter does not mix them)."""
+        import torchvision.transforms.functional as F
+        from PIL import Image
+        from torchvision.transforms import InterpolationMode
+        B, H, W, C = images.shape
+        OH, OW = self.resize
+        mean, std = list(self.normalize['mean'][:C]), list(self.normalize['std'][:C])
+        if len(mean) < C or len(std) < C:
+            raise ValueError('normalisation statistics for fewer than %d channels' % C)
+        planes = [(slice(0, 3), 'RGB')] if C == 3 else [(c, 'L') for c in range(C)]
+        out = []
+        for b in range(B):
+            px = images[b].numpy()
+            padded = [F.pad(Image.fromarray(np.ascontiguousarray(px[:, :, sel]), mode), self.padding)
+                      for sel, mode in planes]
+            for d in range(D):
+                row = [int(v) for v in p[b * D + d]]
+                chans = []
+                for img in padded:
+                    t = F.resize(F.crop(img, row[0], row[1], H, W), [OH, OW], InterpolationMode.BILINEAR)
+                    chans.append(F.to_tensor(F.hflip(t) if row[2] else t))
+                t = F.normalize(torch.cat(chans), mean, std)
+                if holes:
+                    mask = np.ones((OH, OW), np.float32)
+                    for h in range(holes):
+                        y1, y2, x1, x2 = (min(max(v, 0), lim) for v, lim in zip(row[3 + 4 * h:7 + 4 * h],
+                                                                                 (OH, OH, OW, OW)))
+                        mask[y1:y2, x1:x2] = 0.
+                    t = t * torch.from_numpy(mask).expand_as(t)
+                out.append(t)
+        return torch.stack(out)
 
 
 class DeviceBatch(object):

@@ -231,7 +231,22 @@ int b200_input_prep_u8_mix(const uint8_t* x_nhwc, int N, int C, int H, int W, in
  * reads them at run time, so a captured CUDA graph follows each step's draws. */
 int b200_input_prep_u8_aug(const uint8_t* x_nhwc, int N, int D, int C, int H, int W, int Cpad, int pad, const float* lut,
                            const int16_t* params, int holes, void* out, b200_stream_t stream);
-/* RandomResizedCrop + RandomHorizontalFlip + ToTensor + Normalize of the ImageNet training transform (preprocess.py:71-77,
+/* The same transform with the Resize of the Mix&Match CIFAR size regimes (preprocess.py:44-54 with input_size !=
+ * scale_size: RandomCrop(padding) -> Resize -> RandomHorizontalFlip -> ToTensor -> Normalize [-> Cutout]): uint8 NHWC
+ * images x_nhwc [N][H][W][C] (C <= 4) -> out bf16 [N*D][OH][OW][Cpad].  Output row n' is copy n' % D of image n' / D
+ * with the DEVICE draw row params[n'] = int16 {oy, ox, flip, y1, y2, x1, x2, ...} as above, the boxes in OUTPUT
+ * coordinates (Cutout acts on the resized tensor):
+ *   w[r][c] = (0 <= r + oy - pad < H && 0 <= c + ox - pad < W) ? x[n'/D][r + oy - pad][c + ox - pad] : 0  (H x W),
+ *   p = w resampled to OH x OW exactly as Pillow's 8-bit BILINEAR resize does (the padded zeros are part of the
+ *       picture: the filter blends them into the border; horizontal pass into uint8, then the vertical pass),
+ *   u = p[r][flip ? OW-1-c : c],   v = lut[ch][u],   v = v * 0.f inside any box, then one rounding to bf16.
+ * OH == H && OW == W gives the bytes of b200_input_prep_u8_aug (the filter at scale 1 is the identity).  C <= 4,
+ * H, W <= 64, OH, OW <= 128.  Any draw values are memory-safe; the grid depends on N*D only and there is no
+ * workspace, so a captured CUDA graph follows each step's images and draws. */
+int b200_input_prep_u8_aug_resize(const uint8_t* x_nhwc, int N, int D, int C, int H, int W, int OH, int OW, int Cpad,
+                                  int pad, const float* lut, const int16_t* params, int holes, void* out,
+                                  b200_stream_t stream);
+/* RandomResizedCrop +RandomHorizontalFlip + ToTensor + Normalize of the ImageNet training transform (preprocess.py:71-77,
  * with multi_transform's duplicates, :105-112) fused into the stem relayout.  regions: one DEVICE uint8 buffer of
  * region_bytes bytes holding B uint8 HWC images' regions; index (DEVICE int64 [B][3]) = {byte offset, h, w} of each;
  * draws (DEVICE int32 [B*D][5]) = {y, x, h, w, flip} of each copy's crop box inside its region.  Output row n is copy
