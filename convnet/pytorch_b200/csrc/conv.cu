@@ -711,13 +711,13 @@ static int launch_igemm(const IgemmLaunch& L, cudaStream_t stream) {
   p.ck = pick_ck(L.SC);
   p.c_chunks = (L.SC + p.ck - 1) / p.ck;
   p.window = L.window;
-  if (L.window) {   // block-diagonal: one or two n-tiles per window, the K loop covers the window's channels only
-    B200_REQUIRE(L.window % 64 == 0 && L.window <= 256 && L.SC == L.Nout && L.Nout % L.window == 0, B200_ERR_UNSUPPORTED,
-                 "igemm: window %d needs C == K (C=%d K=%d), K %% window == 0", L.window, L.SC, L.Nout);
-    p.block_n = L.window <= 128 ? L.window : L.window / 2;
-    p.n_tiles = L.Nout / p.block_n;
+  if (L.window) {   // block-diagonal: one 64-wide n-tile per window, the K loop covers the window's channels only
+    B200_REQUIRE(L.window == 64 && L.SC == L.Nout && L.Nout % 64 == 0, B200_ERR_UNSUPPORTED,
+                 "igemm: window %d needs window 64, C == K (C=%d K=%d), K %% 64 == 0", L.window, L.SC, L.Nout);
+    p.block_n = 64;
+    p.n_tiles = L.Nout / 64;
     p.ck = 64;
-    p.c_chunks = L.window / 64;
+    p.c_chunks = 1;
   }
   p.ntaps = L.ntaps;
   p.a_bytes = kTileM * p.ck * 2;
@@ -813,10 +813,10 @@ static int launch_igemm(const IgemmLaunch& L, cudaStream_t stream) {
                                       : (total_tiles + grid - 1) / grid;
     fprintf(stderr, "[igemm] M=%d C=%d N=%d taps=%d os=%d block_n=%d n_tiles=%d m_tiles=%d ck=%d k_iters=%d stages=%d "
             "tma_store=%d plain_a=%d bstat=%d own=%d out_fp32=%d bias=%d res=%d act=%d stats=%d grid=%d max_tiles=%d "
-            "smem=%d\n",
+            "smem=%d window=%d xs=%d\n",
             p.M_total, L.SC, L.Nout, L.ntaps, L.os, p.block_n, p.n_tiles, p.m_tiles, p.ck, L.ntaps * p.c_chunks,
             p.num_stages, p.tma_store, p.plain_a, p.b_stationary, p.own_ntile, p.out_fp32, L.bias != nullptr,
-            L.res != nullptr, p.act, L.stats != nullptr, grid, max_tiles, smem_bytes);
+            L.res != nullptr, p.act, L.stats != nullptr, grid, max_tiles, smem_bytes, L.window, (int)L.s_pix);
   }
   b200::launch(kfn, grid, kThreads, smem_bytes, stream, tmA, tmB, tmC, tmR, p);
   B200_CHECK_LAUNCH("conv_igemm_kernel");
@@ -850,6 +850,7 @@ extern "C" int b200_conv_fprop(const b200_conv_desc* d, const void* x, const voi
   if (rc) return rc;
   B200_REQUIRE(x && w && y, B200_ERR_INVALID, "conv_fprop: null pointer");
   B200_REQUIRE(d->C % 8 == 0, B200_ERR_UNSUPPORTED, "conv_fprop: C=%d must be a multiple of 8 (pad the input)", d->C);
+  B200_REQUIRE(d->window == 0 || d->window == 64, B200_ERR_UNSUPPORTED, "conv_fprop: window must be 0 or 64");
   if (d->stride == 1 && d->pad_h == d->pad_w && d->P == d->H + 2 * d->pad_h - d->R + 1 &&
       d->Q == d->W + 2 * d->pad_w - d->S + 1 && d->x_pixel_stride == 0 && (!ep || !ep->out_fp32) &&
       !(ep && ep->bias && ep->bn_stats_workspace) && (d->window == 0 || d->window == 64) &&
@@ -888,6 +889,7 @@ extern "C" int b200_conv_dgrad(const b200_conv_desc* d, const void* dy, const vo
   cudaStream_t stream = (cudaStream_t)stream_;
   B200_REQUIRE(dy && wt && dx, B200_ERR_INVALID, "conv_dgrad: null pointer");
   B200_REQUIRE(d->K % 8 == 0, B200_ERR_UNSUPPORTED, "conv_dgrad: K=%d must be a multiple of 8", d->K);
+  B200_REQUIRE(d->window == 0 || d->window == 64, B200_ERR_UNSUPPORTED, "conv_dgrad: window must be 0 or 64");
   const int st = d->stride;
   B200_REQUIRE(st == 1 || st == 2, B200_ERR_UNSUPPORTED, "conv_dgrad: stride %d unsupported", st);
   if (d->R == 3 && d->S == 3 && st == 1 && d->pad_h == 1 && d->pad_w == 1 && d->P == d->H && d->Q == d->W &&
@@ -1032,10 +1034,10 @@ extern "C" int b200_conv_wgrad(const b200_conv_desc* d, const void* x, const voi
                d->Q == d->W && d->x_pixel_stride == 0) ? 1 : 0;
   if (getenv("B200_WGRAD_DEBUG"))   // keys kt (always 1) and k_groups (== k_tiles) stay for the parsers of this line
     fprintf(stderr, "[wgrad] K=%d C=%d taps=%d stride=%d ckA=%d ckB=%d kt=%d bpc=%d k_groups=%d col_groups=%d splits=%d "
-            "bps=%d stages=%d stage=%u nc=%d nboxes_last=%d plain_x=%d partial=%d\n", d->K, d->C, p.taps_total,
-            d->stride, p.ckA, p.ckB, 1, p.boxes_per_cta, p.k_tiles, p.col_groups, p.splits, p.blocks_per_split,
-            p.num_stages, p.stage_bytes, p.pitch, p.total_boxes - (p.col_groups - 1) * p.boxes_per_cta, p.plain_x,
-            p.partial != nullptr);
+            "bps=%d stages=%d stage=%u nc=%d nboxes_last=%d plain_x=%d partial=%d window=%d xs=%d\n", d->K, d->C,
+            p.taps_total, d->stride, p.ckA, p.ckB, 1, p.boxes_per_cta, p.k_tiles, p.col_groups, p.splits,
+            p.blocks_per_split, p.num_stages, p.stage_bytes, p.pitch, p.total_boxes - (p.col_groups - 1) * p.boxes_per_cta,
+            p.plain_x, p.partial != nullptr, d->window, d->x_pixel_stride);
   if (p.plain_x)
     rc = encode_tiled(&tmX, x, 2, {d->C, p.M_total}, {p.ckB, p.bk}, "wgrad x");
   else

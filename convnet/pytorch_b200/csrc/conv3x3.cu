@@ -584,8 +584,8 @@ int launch_halo_wgrad(const void* x, const void* dy, float* dw, void* workspace,
   if (rc) return rc;
   if (getenv("B200_HALO_DEBUG"))
     fprintf(stderr, "[halo_wgrad] N=%d H=%d W=%d C=%d K=%d taps=%d k_tiles=%d c_chunks=%d m_tiles=%d units=%d "
-            "splits=%d tiles_per_split=%d stages=%d grid=%d\n", N, H, W, C, K_out, p.ntaps, p.k_tiles, p.c_chunks,
-            p.m_tiles, p.units, p.splits, p.tiles_per_split, p.stages, p.units * p.splits);
+            "splits=%d tiles_per_split=%d stages=%d grid=%d window=%d\n", N, H, W, C, K_out, p.ntaps, p.k_tiles,
+            p.c_chunks, p.m_tiles, p.units, p.splits, p.tiles_per_split, p.stages, p.units * p.splits, window);
   b200::launch(kfn, p.units * p.splits, kThreads, smem_bytes, stream, tmDy, tmX, p);
   B200_CHECK_LAUNCH("conv_halo_wgrad_kernel");
   // dw is [K][taps][window or C]; channel boxes are numbered chunk-major, as the units: id = (c / cw) * taps + tap

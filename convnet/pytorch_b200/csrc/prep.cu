@@ -462,20 +462,23 @@ extern "C" int b200_cast_f32_to_bf16(const float* src, void* dst, long long n, b
 //               c = W*(k/W) + cl lies in the group of k, else 0                                   (fprop operand)
 //   transposed: bf16 [C][T][W],  out[c][t][kl] = the same weight seen from input channel c, k = W*(c/W) + kl (dgrad operand)
 //   unpack    : dw_g[k][t][cl] += dw_win[k][t][first(k) + cl - W*(k/W)]   from the windowed fp32 gradient [K][T][W]
-// W == C reproduces the dense block-diagonal expansion.
+// W == C is the dense block-diagonal expansion, for any C and K (ResNeXt's C != K stage entries): window origin 0,
+// operands [K][T][C] (fprop) and [C][T][K] (dgrad), unpack from a dense [K][T][C] gradient.
 namespace b200 {
 __global__ void __launch_bounds__(256) group_pack_kernel(const float* __restrict__ wg, int K, int T, int C, int groups,
                                                          int Wd, int transpose, __nv_bfloat16* __restrict__ out) {
   const int cg = C / groups, kg = K / groups;
+  const bool dense = Wd == C;
   const int rows = transpose ? C : K;
-  const long long total = (long long)rows * T * Wd;
+  const int width = (transpose && dense) ? K : Wd;   // row length of the operand
+  const long long total = (long long)rows * T * width;
   for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
        idx += (long long)gridDim.x * blockDim.x) {
-    const int l = (int)(idx % Wd);
-    const int t = (int)((idx / Wd) % T);
-    const int row = (int)(idx / ((long long)Wd * T));
+    const int l = (int)(idx % width);
+    const int t = (int)((idx / width) % T);
+    const int row = (int)(idx / ((long long)width * T));
     int k, c;
-    if (transpose) { c = row; k = (c / Wd) * Wd + l; } else { k = row; c = (k / Wd) * Wd + l; }
+    if (transpose) { c = row; k = dense ? l : (c / Wd) * Wd + l; } else { k = row; c = dense ? l : (k / Wd) * Wd + l; }
     float v = 0.f;
     if (k < K && c < C) {
       const int grp = k / kg;
@@ -494,7 +497,7 @@ __global__ void __launch_bounds__(256) group_unpack_kernel(const float* __restri
     const int t = (int)((idx / cg) % T);
     const int k = (int)(idx / ((long long)cg * T));
     const int c = (k / kg) * cg + cl;
-    dwg[idx] += dw_win[((long long)k * T + t) * Wd + (c - (k / Wd) * Wd)];
+    dwg[idx] += dw_win[((long long)k * T + t) * Wd + (Wd == C ? c : c - (k / Wd) * Wd)];
   }
 }
 }  // namespace b200
@@ -506,7 +509,7 @@ extern "C" int b200_group_weight_pack(const float* w_grouped, int K, int T, int 
   B200_REQUIRE(window > 0 && window % (C / groups) == 0 && window % (K / groups) == 0 && (window == C || (C == K && C % window == 0)),
                B200_ERR_UNSUPPORTED, "group_weight_pack: window %d must be a multiple of the group width and divide C == K",
                window);
-  const long long total = (long long)(transpose ? C : K) * T * window;
+  const long long total = (long long)(transpose ? C : K) * T * ((transpose && window == C) ? K : window);
   b200::launch(b200::group_pack_kernel, b200::grid_cap(total, 256), 256, 0, (cudaStream_t)stream,
       w_grouped, K, T, C, groups, window, transpose, (__nv_bfloat16*)out_bf16);
   B200_CHECK_LAUNCH("group_pack_kernel");
@@ -515,9 +518,11 @@ extern "C" int b200_group_weight_pack(const float* w_grouped, int K, int T, int 
 
 extern "C" int b200_group_wgrad_unpack(const float* dw_win, int K, int T, int C, int groups, int window, float* dw_grouped,
                                        b200_stream_t stream) {
-  B200_REQUIRE(dw_win && dw_grouped && K > 0 && T > 0 && C > 0 && groups > 0 && C % groups == 0 && K % groups == 0 &&
-                   window > 0 && window % (C / groups) == 0,
+  B200_REQUIRE(dw_win && dw_grouped && K > 0 && T > 0 && C > 0 && groups > 0 && C % groups == 0 && K % groups == 0,
                B200_ERR_INVALID, "group_wgrad_unpack: bad argument");
+  B200_REQUIRE(window > 0 && window % (C / groups) == 0 && window % (K / groups) == 0 && (window == C || (C == K && C % window == 0)),
+               B200_ERR_UNSUPPORTED, "group_wgrad_unpack: window %d must be a multiple of the group width and divide C == K",
+               window);
   const long long total = (long long)K * T * (C / groups);
   b200::launch(b200::group_unpack_kernel, b200::grid_cap(total, 256), 256, 0, (cudaStream_t)stream, dw_win, K, T, C, groups, window,
                                                                                        dw_grouped);

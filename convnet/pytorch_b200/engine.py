@@ -185,7 +185,8 @@ class _Conv(object):
                                      self.window or self.C)
 
     def dgrad_weights(self):
-        """grouped convolutions: [C, R*S, window] operand of dgrad, packed from the fp32 master."""
+        """grouped convolutions: [C, R*S, 64] operand of dgrad (dense [C, R*S, K] fallback), packed from the fp32
+        master."""
         return ops.group_weight_pack(self.w32, self.K, self.R * self.S, self.C, self.groups, self.window or self.C,
                                      transpose=True)
 

@@ -728,9 +728,13 @@ def stem_wgrad_from_s2d(dw_s2d, K, C, cpad, dw):
 
 def group_weight_pack(w32_grouped, K, T, C, groups, window, transpose=False, out=None):
     """fp32 [K,T,C/g] -> bf16 [K,T,window] (or [C,T,window] transposed): the block-diagonal operand of a grouped
-    convolution at window granularity (window == C: dense expansion)."""
+    convolution at window granularity.  window == C is the dense expansion for any C and K: [K,T,C] (or [C,T,K])."""
+    shape = (C, T, K if window == C else window) if transpose else (K, T, window)
     if out is None:
-        out = torch.empty((C if transpose else K, T, window), device=w32_grouped.device, dtype=bf16)
+        out = torch.empty(shape, device=w32_grouped.device, dtype=bf16)
+    _chk(out, bf16, "out")
+    if tuple(out.shape) != shape:
+        raise _l.B200Error("group_weight_pack: out must be %s, got %s" % (shape, tuple(out.shape)))
     with _T('weight_transpose', 0, 2 * out.numel()):
         _l.check(_l.load().b200_group_weight_pack(w32_grouped.data_ptr(), K, T, C, groups, int(window), int(bool(transpose)),
                                                   out.data_ptr(), _stream()), "b200_group_weight_pack")

@@ -48,9 +48,11 @@ typedef struct {
    * consecutive "pixels" overlap: the space-to-depth ImageNet stem reads 4 neighbouring 16-channel pixels as
    * one 64-channel pixel this way (only x is affected; y / dy are always dense). */
   int x_pixel_stride, x_row_stride, x_image_stride;
-  /* 0: dense.  W > 0 (C == K, C % W == 0; fprop/dgrad W = 64, wgrad W = 128): block-diagonal convolution -- output
-   * channels [W*b, W*b+W) read input channels of the same window only; the weight operand is [K][R*S][W] (fprop),
-   * [C][R*S][W] (dgrad), the weight gradient [K][R*S][W].  This is how grouped convolutions run (b200_group_weight_pack). */
+  /* 0: dense.  W > 0 (C == K, C % W == 0, dense x; fprop/dgrad accept W = 64 only, wgrad W = 128 only, any other W is
+   * B200_ERR_UNSUPPORTED): block-diagonal convolution -- output channels [W*b, W*b+W) read input channels of the same
+   * window only; the weight operand is [K][R*S][W] (fprop), [C][R*S][W] (dgrad), the weight gradient [K][R*S][W].  This
+   * is how grouped convolutions with C == K run (b200_group_weight_pack); C != K runs dense on the block-diagonal
+   * expansion. */
   int window;
 } b200_conv_desc;
 
@@ -269,11 +271,13 @@ int b200_weight_transpose_batched(const void* src_base, void* dst_base, const in
 int b200_stem_weight_to_s2d(const float* w, int K, int C, int Cpad, void* w_s2d, b200_stream_t stream);
 int b200_stem_wgrad_from_s2d(const float* dw_s2d, int K, int C, int Cpad, float* dw, b200_stream_t stream);
 int b200_cast_f32_to_bf16(const float* src, void* dst, long long n, b200_stream_t stream);
-/* grouped convolution (nn.Conv2d(groups=g), models/resnext.py:10-16; C == K): block diagonal at any window W that is a
- * multiple of the group width.  pack: fp32 master [K][T][C/g] -> bf16 [K][T][W] (transpose = 0, fprop operand of
- * b200_conv_fprop with desc.window = W) or [C][T][W] (transpose = 1, dgrad operand); unpack: dw_grouped += the entries of
- * the windowed fp32 gradient [K][T][W] (b200_conv_wgrad with desc.window) that belong to each output channel's group.
- * W == C is the dense block-diagonal expansion. */
+/* grouped convolution (nn.Conv2d(groups=g), models/resnext.py:10-16): with C == K block diagonal at any window W that is
+ * a multiple of the group width and divides C.  pack: fp32 master [K][T][C/g] -> bf16 [K][T][W] (transpose = 0, fprop
+ * operand of b200_conv_fprop with desc.window = W) or [C][T][W] (transpose = 1, dgrad operand); unpack: dw_grouped +=
+ * the entries of the windowed fp32 gradient [K][T][W] (b200_conv_wgrad with desc.window) that belong to each output
+ * channel's group.
+ * W == C is the dense block-diagonal expansion, also for C != K (run with desc.window = 0): the fprop operand is
+ * [K][T][C], the dgrad operand [C][T][K], and unpack reads a dense [K][T][C] gradient.  Any other W needs C == K. */
 int b200_group_weight_pack(const float* w_grouped, int K, int T, int C, int groups, int window, int transpose,
                            void* out_bf16, b200_stream_t stream);
 int b200_group_wgrad_unpack(const float* dw_win, int K, int T, int C, int groups, int window, float* dw_grouped,

@@ -3,7 +3,11 @@ and wgrad) against fp64 torch, element by element.
 
 The shapes are generated from the device's SM count, so that each intended schedule (one tile per CTA, warpgroup 1
 computing tiles, five or more tiles per CTA, the M tail in a warpgroup-1 tile, owned-n-tile walks, ...) holds on any
-H100 variant.  Every case runs in two tiers:
+H100 variant.  Besides dense convolutions the sweep runs grouped ones the way the engine does (block-diagonal
+"window" mode -- 64-channel windows for fprop / dgrad, 128 for wgrad -- or the dense block-diagonal expansion, with
+operands from b200_group_weight_pack and the gradient kept by b200_group_wgrad_unpack; references use groups=) and the
+ImageNet stem's descriptors, including the wide-pixel one whose x strides make pixels overlap (reference input: the
+torch.as_strided view of the same buffer).  Every case runs in two tiers:
 
 * tier 1 -- exact arithmetic: sparse integer operands in [-2, 2] (integer bias, residual and initial dw), so every
   product and partial sum is an integer far below 2^13 and representable in fp32, and |y| <= 256 is exact in bf16.  The
@@ -33,7 +37,9 @@ bf16 = torch.bfloat16
 # tier-2 accumulation-error coefficients (|y - ref| beyond the output rounding, in units of absref).  Calibrated on an
 # NVIDIA H100 80GB HBM3 (132 SMs, 400 W power limit): the worst ratios over the sweep were 8.5e-8 for bf16 outputs
 # (halo dgrad, K = 256) and 1.4e-7 for fp32 outputs (fprop of a 64 -> 1000 fully connected layer), 5.6x and 6.9x
-# below these bounds; test_tier2_calibration_report prints them again.
+# below these bounds; test_tier2_calibration_report prints them again.  With the grouped and stem cases added (NVIDIA
+# H100 80GB HBM3, 132 SMs, 700 W power limit) the bf16 worst is unchanged and the fp32 worst is 1.45e-7 (the window-128
+# weight gradient of the K = 512 grouped case), 6.6x below.
 C_BF16 = 2.0 ** -21
 C_FP32 = 2.0 ** -20
 GUARD = 256               # elements before and after every output view (keeps TMA's 16-byte alignment)
@@ -51,10 +57,14 @@ def _sm_count():
 
 # ------------------------------------------------------------------------------------------------ the sweep
 def _case(N, H, W, C, K, R=1, S=1, stride=1, pad=(0, 0), ops='fdw', bias=False, res=False, act=0, fp32=False,
-          stats=False):
+          stats=False, groups=1, window=0, x_strides=None):
+    """groups > 1: a grouped convolution, run with desc.window = window (64; wgrad 128) or, window = 0, on the dense
+    block-diagonal expansion.  x_strides: (pixel, row, image) strides of x in elements (None: dense NHWC)."""
     pad = (pad, pad) if isinstance(pad, int) else tuple(pad)
+    assert window in (0, 64) and (not window or (groups > 1 and C == K and C % 128 == 0 and 64 % (C // groups) == 0)), \
+        'window mode as the engine runs it: C == K, C % 128 == 0 (128-wide wgrad windows), groups of <= 64 channels'
     return dict(N=N, H=H, W=W, C=C, K=K, R=R, S=S, stride=stride, pad=pad, ops=ops, bias=bias, res=res, act=act,
-                fp32=fp32, stats=stats)
+                fp32=fp32, stats=stats, groups=groups, window=window, x_strides=x_strides)
 
 
 def sweep(sm):
@@ -67,6 +77,8 @@ def sweep(sm):
     m_rr = -(-t3 // n_rr)
     own_ctas = sm // 2
     m_own = 4 * own_ctas + own_ctas // 2
+    per_win = sm // 8           # CTAs per 64-channel window of the K = 512 halo window launch (8 windows)
+    m_win_rr = -(-t3 // (2 * n_rr))   # 2 n_rr windows of 64 channels do not divide twice the grid either
     return {
         # igemm widths 16..128 with warpgroup 1 computing tiles; A-side ck 16 / 32 / 64; schedules
         'w16_c8_deep': _case(2 * t5 - 1, 8, 8, 8, 16),                                  # >= 5 tiles per CTA
@@ -102,6 +114,33 @@ def sweep(sm):
         'halo3_one_split': _case(1, 10, 10, 64, 64, 3, 3, 1, 1),
         'halo4_w64': _case(4, 32, 32, 16, 64, 4, 4, 1, 0, ops='fw'),
         'halo4_w128_stats': _case(3, 32, 32, 16, 128, 4, 4, 1, 0, ops='fw', stats=True),
+        # grouped convolutions in window mode (ResNeXt, C == K, 64 % (C/g) == 0): halo kernels with diag = 1 and the
+        # halo wgrad with window 128
+        'grp128_g32_28_stats': _case(8, 28, 28, 128, 128, 3, 3, 1, 1, stats=True, groups=32, window=64),
+        # diag epilogues; every window's CTAs take 2 or 3 tiles
+        'grp512_g32_14_res': _case(per_win + per_win // 4, 14, 14, 512, 512, 3, 3, 1, 1, res=True, act=1, groups=32,
+                                   window=64),
+        'grp512_g32_14_bias': _case(per_win + per_win // 4, 14, 14, 512, 512, 3, 3, 1, 1, bias=True, groups=32,
+                                    window=64),
+        # implicit GEMM: stride 2 (four dgrad residue classes, im2col wgrad at stride 2), 7x7 maps (halo ineligible,
+        # M tail, split wgrad), a 64-pixel map (one wgrad split) and a round-robin walk whose warpgroups change window
+        'grp256_g32_3x3s2_stats': _case(8, 28, 28, 256, 256, 3, 3, 2, 1, stats=True, groups=32, window=64),
+        'grp1024_g32_7_tail': _case(43, 7, 7, 1024, 1024, 3, 3, 1, 1, groups=32, window=64),
+        'grp256_g32_8_one_split': _case(1, 8, 8, 256, 256, 3, 3, 1, 1, groups=32, window=64),
+        'grp_rr_3x3s2_stats': _case(2 * m_win_rr - 1, 16, 16, 128 * n_rr, 128 * n_rr, 3, 3, 2, 1, stats=True,
+                                    groups=16 * n_rr, window=64),
+        # dense block-diagonal expansion (window == C): CIFAR ResNeXt's layer1 conv2 and its C != K stage entries
+        'grp64_g4_32_dense': _case(8, 32, 32, 64, 64, 3, 3, 1, 1, groups=4),
+        'grp16_64_g4_32_stats': _case(8, 32, 32, 16, 64, 3, 3, 1, 1, stats=True, groups=4),
+        'grp64_128_g8_s2_stats': _case(8, 32, 32, 64, 128, 3, 3, 2, 1, stats=True, groups=8),
+        'grp128_256_g16_s2_stats': _case(8, 16, 16, 128, 256, 3, 3, 2, 1, stats=True, groups=16),
+        # the engine's ImageNet stem descriptors: 224 px on the 4x4 halo kernel (bordered 115 x 115 x 16 tensor), and
+        # 256 / 288 px as 4x1 convolutions over overlapping 64-channel "wide pixels" of the bordered tensor
+        'stem224_halo4_stats': _case(2, 115, 115, 16, 64, 4, 4, 1, 0, ops='fw', stats=True),
+        'stem256_wide_stats': _case(2, 131, 128, 64, 64, 4, 1, 1, 0, ops='fw', stats=True,
+                                    x_strides=(16, 131 * 16, 131 * 131 * 16)),
+        'stem288_wide_stats_odd': _case(3, 147, 144, 64, 64, 4, 1, 1, 0, ops='fw', stats=True,
+                                        x_strides=(16, 147 * 16, 147 * 147 * 16)),
     }
 
 
@@ -112,8 +151,30 @@ def _get(name):
     return sweep(_sm_count())[name]
 
 
-def _desc(cs):
-    return _ops().make_desc(cs['N'], cs['H'], cs['W'], cs['C'], cs['K'], cs['R'], cs['S'], cs['stride'], cs['pad'])
+def _wgrad_window(cs):
+    return 128 if cs['window'] else 0
+
+
+def _desc(cs, wgrad=False):
+    return _ops().make_desc(cs['N'], cs['H'], cs['W'], cs['C'], cs['K'], cs['R'], cs['S'], cs['stride'], cs['pad'],
+                            x_strides=cs['x_strides'] or (0, 0, 0),
+                            window=_wgrad_window(cs) if wgrad else cs['window'])
+
+
+def _cg(cs):
+    return cs['C'] // cs['groups']
+
+
+def _x_shape(cs):
+    """the tensor the kernels read x from: NHWC, or the flat buffer that strided-x descriptors address"""
+    if cs['x_strides'] is None:
+        return (cs['N'], cs['H'], cs['W'], cs['C'])
+    return (cs['N'] * cs['x_strides'][2],)
+
+
+def _wgrad_shape(cs):
+    """the weight gradient b200_conv_wgrad writes: [K, R*S, C], or [K, R*S, 128] in window mode"""
+    return (cs['K'], cs['R'] * cs['S'], _wgrad_window(cs) or cs['C'])
 
 
 def _gen(name, tier):
@@ -129,23 +190,86 @@ def _nhwc(t):
     return t.permute(0, 2, 3, 1)
 
 
+def _xview(x, cs):
+    """[N, H, W, C] view of what the kernels read as x: for strided-x descriptors neighbouring pixels overlap"""
+    if cs['x_strides'] is None:
+        return x
+    ps, rs, ims = cs['x_strides']
+    assert (cs['H'] - 1) * rs + (cs['W'] - 1) * ps + cs['C'] <= ims, 'x strides address past the image'
+    return torch.as_strided(x, (cs['N'], cs['H'], cs['W'], cs['C']), (ims, rs, ps, 1))
+
+
 def _w_kcrs(w, cs):
-    return w.double().view(cs['K'], cs['R'], cs['S'], cs['C']).permute(0, 3, 1, 2)
+    return w.double().view(cs['K'], cs['R'], cs['S'], _cg(cs)).permute(0, 3, 1, 2)
 
 
 def ref_fprop(x, w, cs):
-    return _nhwc(F.conv2d(_nchw(x), _w_kcrs(w, cs), stride=cs['stride'], padding=cs['pad']))
+    """w: the fp32 master [K, R*S, C/g]"""
+    return _nhwc(F.conv2d(_nchw(_xview(x, cs)), _w_kcrs(w, cs), stride=cs['stride'], padding=cs['pad'],
+                          groups=cs['groups']))
 
 
 def ref_dgrad(dy, w, cs):
     size = (cs['N'], cs['C'], cs['H'], cs['W'])
-    return _nhwc(conv2d_input(size, _w_kcrs(w, cs), _nchw(dy), stride=cs['stride'], padding=cs['pad']))
+    return _nhwc(conv2d_input(size, _w_kcrs(w, cs), _nchw(dy), stride=cs['stride'], padding=cs['pad'],
+                              groups=cs['groups']))
 
 
 def ref_wgrad(x, dy, cs):
-    g = conv2d_weight(_nchw(x), (cs['K'], cs['C'], cs['R'], cs['S']), _nchw(dy), stride=cs['stride'],
+    """the dense weight gradient [K, R*S, C] (grouped cases: including the entries between groups)"""
+    g = conv2d_weight(_nchw(_xview(x, cs)), (cs['K'], cs['C'], cs['R'], cs['S']), _nchw(dy), stride=cs['stride'],
                       padding=cs['pad'])
     return g.permute(0, 2, 3, 1).reshape(cs['K'], cs['R'] * cs['S'], cs['C'])
+
+
+def _group_cols(K, C, groups, width, device):
+    """[K, C/g]: where input channel i of output channel k's group sits in a row of `width` channels -- the row of the
+    window that holds k (window mode, C == K), or the whole row (width == C: the dense expansion)"""
+    assert width == C or (C == K and C % width == 0)
+    cg, kg = C // groups, K // groups
+    k = torch.arange(K, device=device).view(K, 1)
+    c = (k // kg) * cg + torch.arange(cg, device=device).view(1, cg)
+    return c if width == C else c - (k // width) * width
+
+
+def _take_cols(t, cols):
+    """t [rows, T, width], cols [rows, n] -> [rows, T, n] with out[r, t, i] = t[r, t, cols[r, i]]"""
+    return t.gather(2, cols.unsqueeze(1).expand(t.shape[0], t.shape[1], cols.shape[1]))
+
+
+def pack_ref(w32, K, T, C, groups, window, transpose):
+    """the b200_group_weight_pack contract, restated: the dense block-diagonal weight [K, T, C], cut into the rows of
+    each output channel's window ([K, T, window]); transposed, the same from each input channel's side ([C, T, window]).
+    window == C is the dense expansion for any C and K: [K, T, C], transposed [C, T, K]."""
+    assert window == C or (C == K and C % window == 0)
+    cg, kg = C // groups, K // groups
+    dense = torch.zeros(K, T, C, dtype=w32.dtype, device=w32.device)
+    for g in range(groups):
+        dense[g * kg:(g + 1) * kg, :, g * cg:(g + 1) * cg] = w32[g * kg:(g + 1) * kg]
+    if transpose:
+        dense = dense.permute(2, 1, 0)
+    if window == C:
+        return dense.contiguous()
+    rows = dense.shape[0]
+    cols = (torch.arange(rows, device=w32.device) // window * window).view(rows, 1) + \
+        torch.arange(window, device=w32.device).view(1, window)
+    return _take_cols(dense, cols)
+
+
+def ref_wgrad_kernel_layout(dense, cs):
+    """the dense gradient as b200_conv_wgrad writes it: unchanged, or in window mode each output channel's window"""
+    W = _wgrad_window(cs)
+    if not W:
+        return dense
+    K = cs['K']
+    assert K == cs['C'] and K % W == 0
+    cols = (torch.arange(K, device=dense.device) // W * W).view(K, 1) + torch.arange(W, device=dense.device).view(1, W)
+    return _take_cols(dense, cols)
+
+
+def ref_wgrad_grouped(dense, cs):
+    """[K, R*S, C/g]: the gradient of the grouped master weight"""
+    return _take_cols(dense, _group_cols(cs['K'], cs['C'], cs['groups'], cs['C'], dense.device))
 
 
 def _act(v, act):
@@ -190,9 +314,9 @@ def call_fprop(cs, x, w, bias, res):
     return y, sums
 
 
-def call_dgrad(cs, dy, w, res):
+def call_dgrad(cs, dy, wt, res):
+    """wt: the dgrad operand (_operands)"""
     ops = _ops()
-    wt = ops.weight_transpose(w)
     buf, dx = _guarded((cs['N'], cs['H'], cs['W'], cs['C']), bf16, float('nan'))
     ops.conv_dgrad(dy, wt, _desc(cs), out=dx, residual=res)
     torch.cuda.synchronize()
@@ -203,10 +327,49 @@ def call_dgrad(cs, dy, w, res):
 def call_wgrad(cs, x, dy, dw0):
     buf, dw = _guarded(tuple(dw0.shape), torch.float32, 0.0)
     dw.copy_(dw0)
-    _ops().conv_wgrad(x, dy, _desc(cs), dw)
+    _ops().conv_wgrad(x, dy, _desc(cs, wgrad=True), dw)
     torch.cuda.synchronize()
     _check_written(buf, dw, 'wgrad')
     return dw
+
+
+def call_pack(w32, K, T, C, groups, window, transpose):
+    """b200_group_weight_pack into a guarded NaN-filled buffer, checked bit for bit against pack_ref"""
+    want = pack_ref(w32, K, T, C, groups, window, transpose)
+    buf, out = _guarded(tuple(want.shape), bf16, float('nan'))
+    _ops().group_weight_pack(w32, K, T, C, groups, window, transpose=transpose, out=out)
+    torch.cuda.synchronize()
+    _check_written(buf, out, 'group_weight_pack')
+    bad = out.float() != want
+    assert not bool(bad.any()), 'group_weight_pack(C=%d K=%d groups=%d window=%d transpose=%d): %d of %d elements ' \
+        'differ, first at %s' % (C, K, groups, window, transpose, int(bad.sum()), bad.numel(),
+                                 tuple(bad.nonzero()[0].tolist()))
+    return out
+
+
+def call_unpack(dw_win, K, T, C, groups, window, dwg0):
+    """b200_group_wgrad_unpack (dw_g += ...) onto a guarded copy of dwg0, checked bit for bit"""
+    buf, dwg = _guarded(tuple(dwg0.shape), torch.float32, 0.0)
+    dwg.copy_(dwg0)
+    _ops().group_wgrad_unpack(dw_win, K, T, C, groups, window, dwg)
+    torch.cuda.synchronize()
+    _check_written(buf, dwg, 'group_wgrad_unpack')
+    want = dwg0 + _take_cols(dw_win, _group_cols(K, C, groups, window, dw_win.device))
+    bad = dwg != want
+    assert not bool(bad.any()), 'group_wgrad_unpack(C=%d K=%d groups=%d window=%d): %d of %d elements differ, first ' \
+        'at %s' % (C, K, groups, window, int(bad.sum()), bad.numel(), tuple(bad.nonzero()[0].tolist()))
+    return dwg
+
+
+def _operands(cs, w32):
+    """(fprop, dgrad) bf16 weight operands from the fp32 master w32 [K, R*S, C/g] (values exact in bf16): the cast and
+    its transpose, or for grouped cases the packings of b200_group_weight_pack (window 64, or C: the dense expansion)"""
+    if cs['groups'] == 1:
+        w = w32.to(bf16)
+        return w, _ops().weight_transpose(w)
+    K, T, C, g = cs['K'], cs['R'] * cs['S'], cs['C'], cs['groups']
+    win = cs['window'] or C
+    return call_pack(w32, K, T, C, g, win, False), call_pack(w32, K, T, C, g, win, True)
 
 
 def _res_fprop(cs):
@@ -242,14 +405,16 @@ def test_tier1_exact(name):
     cs = _get(name)
     g = _gen(name, 1)
     N, H, W, C, K, RS = cs['N'], cs['H'], cs['W'], cs['C'], cs['K'], cs['R'] * cs['S']
+    cg, kg = _cg(cs), K // cs['groups']
     P, Q = _outshape(cs)
     dev = 'cuda'
     if 'f' in cs['ops']:
-        d = _density(C * RS, 8 if cs['stats'] else 16)
-        x, w = _ints((N, H, W, C), d, g), _ints((K, RS, C), d, g)
+        d = _density(cg * RS, 8 if cs['stats'] else 16)
+        x, w = _ints(_x_shape(cs), d, g), _ints((K, RS, cg), d, g)
         bias = torch.randint(-4, 5, (K,), generator=g).float().to(dev) if cs['bias'] else None
         res = _ints((N, P, Q, K), 0.5, g).to(dev).to(bf16) if _res_fprop(cs) else None
-        x, w = x.to(dev).to(bf16), w.to(dev).to(bf16)
+        x, w = x.to(dev).to(bf16), w.to(dev)
+        wf, _ = _operands(cs, w)
         pre = ref_fprop(x, w, cs)
         absref = ref_fprop(x.abs(), w.abs(), cs)
         if bias is not None:
@@ -258,8 +423,8 @@ def test_tier1_exact(name):
             pre, absref = pre + res.double(), absref + res.double().abs()
         _exact_preconditions(absref, 'fprop', not cs['fp32'])
         ref = _act(pre, cs['act'])
-        y, sums = call_fprop(cs, x, w, bias, res)
-        y2, sums2 = call_fprop(cs, x, w, bias, res)
+        y, sums = call_fprop(cs, x, wf, bias, res)
+        y2, sums2 = call_fprop(cs, x, wf, bias, res)
         assert torch.equal(y, y2), 'fprop is not deterministic'
         want = ref.to(y.dtype)
         bad = (y != want)
@@ -272,31 +437,41 @@ def test_tier1_exact(name):
             assert torch.equal(sums[0], flat.sum(0)), 'fused statistics: per-channel sum differs'
             assert torch.equal(sums[1], (flat * flat).sum(0)), 'fused statistics: per-channel sum of squares differs'
     if 'd' in cs['ops']:
-        d = _density(K * RS, 16)
-        dy, w = _ints((N, P, Q, K), d, g).to(dev).to(bf16), _ints((K, RS, C), d, g).to(dev).to(bf16)
+        d = _density(kg * RS, 16)
+        dy, w = _ints((N, P, Q, K), d, g).to(dev).to(bf16), _ints((K, RS, cg), d, g).to(dev)
         res = _ints((N, H, W, C), 0.5, g).to(dev).to(bf16) if _res_dgrad(cs) else None
+        _, wt = _operands(cs, w)
         ref = ref_dgrad(dy, w, cs)
         absref = ref_dgrad(dy.abs(), w.abs(), cs)
         if res is not None:
             ref, absref = ref + res.double(), absref + res.double().abs()
         _exact_preconditions(absref, 'dgrad', True)
-        dx = call_dgrad(cs, dy, w, res)
-        assert torch.equal(dx, call_dgrad(cs, dy, w, res)), 'dgrad is not deterministic'
+        dx = call_dgrad(cs, dy, wt, res)
+        assert torch.equal(dx, call_dgrad(cs, dy, wt, res)), 'dgrad is not deterministic'
         bad = dx != ref.to(bf16)
         assert not bool(bad.any()), 'dgrad: %d of %d elements differ, first at %s' % (
             int(bad.sum()), bad.numel(), tuple(bad.nonzero()[0].tolist()))
     if 'w' in cs['ops']:
         d = _density(N * P * Q, 256)
-        x, dy = _ints((N, H, W, C), d, g).to(dev).to(bf16), _ints((N, P, Q, K), d, g).to(dev).to(bf16)
-        dw0 = torch.randint(-8, 9, (K, RS, C), generator=g).float().to(dev)
-        ref = ref_wgrad(x, dy, cs)
+        x, dy = _ints(_x_shape(cs), d, g).to(dev).to(bf16), _ints((N, P, Q, K), d, g).to(dev).to(bf16)
+        dw0 = torch.randint(-8, 9, _wgrad_shape(cs), generator=g).float().to(dev)
+        dense = ref_wgrad(x, dy, cs)
+        ref = ref_wgrad_kernel_layout(dense, cs)
         _exact_preconditions(ref_wgrad(x.abs(), dy.abs(), cs) + 8, 'wgrad', False)
         zero = torch.zeros_like(dw0)
-        assert torch.equal(call_wgrad(cs, x, dy, zero), call_wgrad(cs, x, dy, zero)), 'wgrad is not deterministic'
+        dwz = call_wgrad(cs, x, dy, zero)
+        assert torch.equal(dwz, call_wgrad(cs, x, dy, zero)), 'wgrad is not deterministic'
         dw = call_wgrad(cs, x, dy, dw0)
         bad = dw.double() != ref + dw0.double()
         assert not bool(bad.any()), 'wgrad (dw += ...): %d of %d elements differ, first at %s' % (
             int(bad.sum()), bad.numel(), tuple(bad.nonzero()[0].tolist()))
+        if cs['groups'] > 1:
+            # keep each output channel's group (unpack, dw_g += ...): the gradient of the grouped master weight
+            dwg0 = torch.randint(-8, 9, (K, RS, cg), generator=g).float().to(dev)
+            dwg = call_unpack(dwz, K, RS, C, cs['groups'], _wgrad_window(cs) or C, dwg0)
+            bad = dwg.double() != ref_wgrad_grouped(dense, cs) + dwg0.double()
+            assert not bool(bad.any()), 'grouped wgrad: %d of %d elements differ, first at %s' % (
+                int(bad.sum()), bad.numel(), tuple(bad.nonzero()[0].tolist()))
 
 
 # ------------------------------------------------------------------------------------------------ tier 2
@@ -328,11 +503,13 @@ def test_tier2_rounding(name):
     cs = _get(name)
     g = _gen(name, 2)
     N, H, W, C, K, RS = cs['N'], cs['H'], cs['W'], cs['C'], cs['K'], cs['R'] * cs['S']
+    cg = _cg(cs)
     P, Q = _outshape(cs)
     dev = 'cuda'
-    x = torch.randn(N, H, W, C, generator=g).to(dev).to(bf16)
-    w = (torch.randn(K, RS, C, generator=g) / math.sqrt(RS * C)).to(dev).to(bf16)
+    x = torch.randn(*_x_shape(cs), generator=g).to(dev).to(bf16)
+    w = (torch.randn(K, RS, cg, generator=g) / math.sqrt(RS * cg)).to(dev).to(bf16).float()
     dy = torch.randn(N, P, Q, K, generator=g).to(dev).to(bf16)
+    wf, wt = _operands(cs, w)
     if 'f' in cs['ops']:
         bias = torch.randn(K, generator=g).to(dev) if cs['bias'] else None
         res = torch.randn(N, P, Q, K, generator=g).to(dev).to(bf16) if _res_fprop(cs) else None
@@ -341,22 +518,23 @@ def test_tier2_rounding(name):
             pre, absref = pre + bias.double(), absref + bias.double().abs()
         if res is not None:
             pre, absref = pre + res.double(), absref + res.double().abs()
-        y, _ = call_fprop(cs, x, w, bias, res)
-        assert torch.equal(y, call_fprop(cs, x, w, bias, res)[0]), 'fprop is not deterministic'
+        y, _ = call_fprop(cs, x, wf, bias, res)
+        assert torch.equal(y, call_fprop(cs, x, wf, bias, res)[0]), 'fprop is not deterministic'
         _check_bound(y, _act(pre, cs['act']), absref, '%s fprop' % name)
     if 'd' in cs['ops']:
         res = torch.randn(N, H, W, C, generator=g).to(dev).to(bf16) if _res_dgrad(cs) else None
         ref, absref = ref_dgrad(dy, w, cs), ref_dgrad(dy.abs(), w.abs(), cs)
         if res is not None:
             ref, absref = ref + res.double(), absref + res.double().abs()
-        dx = call_dgrad(cs, dy, w, res)
-        assert torch.equal(dx, call_dgrad(cs, dy, w, res)), 'dgrad is not deterministic'
+        dx = call_dgrad(cs, dy, wt, res)
+        assert torch.equal(dx, call_dgrad(cs, dy, wt, res)), 'dgrad is not deterministic'
         _check_bound(dx, ref, absref, '%s dgrad' % name)
     if 'w' in cs['ops']:
-        zero = torch.zeros(K, RS, C, device=dev)
+        zero = torch.zeros(_wgrad_shape(cs), device=dev)
         dw = call_wgrad(cs, x, dy, zero)
         assert torch.equal(dw, call_wgrad(cs, x, dy, zero)), 'wgrad is not deterministic'
-        _check_bound(dw, ref_wgrad(x, dy, cs), ref_wgrad(x.abs(), dy.abs(), cs), '%s wgrad' % name)
+        _check_bound(dw, ref_wgrad_kernel_layout(ref_wgrad(x, dy, cs), cs),
+                     ref_wgrad_kernel_layout(ref_wgrad(x.abs(), dy.abs(), cs), cs), '%s wgrad' % name)
 
 
 def test_tier2_calibration_report():
@@ -381,7 +559,7 @@ def _parse(text, case, op, cs):
         m = _LINE.match(line.strip())
         if m:
             r = {k: int(v) for k, v in (kv.split('=') for kv in m.group(2).split())}
-            r.update(kind=m.group(1), case=case, op=op, filt=(cs['R'], cs['S']))
+            r.update(kind=m.group(1), case=case, op=op, filt=(cs['R'], cs['S']), conv_stride=cs['stride'])
             recs.append(r)
     return recs
 
@@ -472,6 +650,30 @@ def _requirements():
         'halo wgrad one split': lambda r: hw(r) and r['splits'] == 1,
         'halo wgrad many splits': lambda r: hw(r) and r['splits'] > 1,
     })
+    # grouped convolutions in window mode, and the ImageNet stem's descriptors
+    req.update({
+        'igemm window fprop stride 1': lambda r: igf(r) and r['window'] == 64 and r['conv_stride'] == 1,
+        'igemm window fprop stride 2': lambda r: igf(r) and r['window'] == 64 and r['conv_stride'] == 2,
+        'igemm window dgrad stride 1': lambda r: igd(r) and r['window'] == 64 and r['os'] == 1,
+        'igemm window dgrad stride 2': lambda r: igd(r) and r['window'] == 64 and r['os'] == 2,
+        'igemm window + statistics': lambda r: ig(r) and r['window'] == 64 and r['stats'],
+        'igemm window, M tail': lambda r: ig(r) and r['window'] == 64 and r['M'] % 128 != 0,
+        'igemm window, warpgroup changes window':
+            lambda r: ig(r) and r['window'] == 64 and not r['own'] and (2 * r['grid']) % r['n_tiles'] != 0
+            and r['max_tiles'] >= 3,
+        'halo diag fprop': lambda r: ha(r) and r['diag'] and r['dir'] == 0,
+        'halo diag dgrad': lambda r: ha(r) and r['diag'] and r['dir'] == 1,
+        'halo diag statistics': lambda r: ha(r) and r['diag'] and r['stats'],
+        'halo diag residual + ReLU': lambda r: ha(r) and r['diag'] and r['res'] and r['act'] == 1,
+        'halo diag bias': lambda r: ha(r) and r['diag'] and r['bias'],
+        'wgrad window 128, split': lambda r: wg(r) and r['window'] == 128 and r['partial'] == 1,
+        'wgrad window 128, one split': lambda r: wg(r) and r['window'] == 128 and r['partial'] == 0,
+        'wgrad window 128, stride 2': lambda r: wg(r) and r['window'] == 128 and r['stride'] == 2,
+        'halo wgrad window 128': lambda r: hw(r) and r['window'] == 128,
+        'igemm x pixel stride + statistics': lambda r: igf(r) and r['xs'] > 0 and r['stats'],
+        'wgrad x pixel stride': lambda r: wg(r) and r['xs'] > 0,
+        'halo 4x4 stem K = 64 + statistics': lambda r: ha(r) and r['taps'] == 16 and r['K'] == 64 and r['stats'],
+    })
     return req
 
 
@@ -485,18 +687,19 @@ def test_sweep_coverage(monkeypatch, capfd):
     for name, cs in sweep(_sm_count()).items():
         N, H, W, C, K, RS = cs['N'], cs['H'], cs['W'], cs['C'], cs['K'], cs['R'] * cs['S']
         P, Q = _outshape(cs)
-        x = torch.zeros(N, H, W, C, device='cuda', dtype=bf16)
-        w = torch.zeros(K, RS, C, device='cuda', dtype=bf16)
+        x = torch.zeros(_x_shape(cs), device='cuda', dtype=bf16)
+        wf, wt = _operands(cs, torch.zeros(K, RS, _cg(cs), device='cuda'))
         dy = torch.zeros(N, P, Q, K, device='cuda', dtype=bf16)
+        capfd.readouterr()
         if 'f' in cs['ops']:
-            call_fprop(cs, x, w, torch.zeros(K, device='cuda') if cs['bias'] else None,
+            call_fprop(cs, x, wf, torch.zeros(K, device='cuda') if cs['bias'] else None,
                        torch.zeros(N, P, Q, K, device='cuda', dtype=bf16) if _res_fprop(cs) else None)
             recs += _parse(capfd.readouterr().err, name, 'fprop', cs)
         if 'd' in cs['ops']:
-            call_dgrad(cs, dy, w, torch.zeros(N, H, W, C, device='cuda', dtype=bf16) if _res_dgrad(cs) else None)
+            call_dgrad(cs, dy, wt, torch.zeros(N, H, W, C, device='cuda', dtype=bf16) if _res_dgrad(cs) else None)
             recs += _parse(capfd.readouterr().err, name, 'dgrad', cs)
         if 'w' in cs['ops']:
-            call_wgrad(cs, x, dy, torch.zeros(K, RS, C, device='cuda'))
+            call_wgrad(cs, x, dy, torch.zeros(_wgrad_shape(cs), device='cuda'))
             recs += _parse(capfd.readouterr().err, name, 'wgrad', cs)
     missing = []
     lines = []
@@ -509,3 +712,147 @@ def test_sweep_coverage(monkeypatch, capfd):
     with capfd.disabled():
         print('\n' + '\n'.join(lines))
     assert not missing, 'configurations no longer reached by the sweep (SMs=%d): %s' % (_sm_count(), missing)
+
+
+# ------------------------------------------------------------------------------------------------ relayout kernels
+# (C, K, groups, window): C/g in {4, 8, 16, 32, 64}; windows 64, 128 and C; C == K, C < K (CIFAR ResNeXt's stage
+# entries) and C > K
+_PACK_CASES = [
+    (128, 128, 32, 64), (128, 128, 32, 128),
+    (256, 256, 32, 64), (256, 256, 32, 128), (256, 256, 32, 256),
+    (512, 512, 32, 64), (512, 512, 32, 128), (512, 512, 32, 512),
+    (1024, 1024, 32, 64), (1024, 1024, 32, 128), (1024, 1024, 32, 1024),
+    (256, 256, 4, 64), (256, 256, 4, 128), (256, 256, 4, 256),
+    (64, 64, 4, 64),
+    (16, 64, 4, 16), (64, 128, 8, 64), (128, 256, 16, 128), (64, 32, 2, 64), (128, 64, 2, 128),
+]
+
+
+@pytest.mark.parametrize('C,K,groups,window', _PACK_CASES)
+def test_group_weight_pack_and_unpack(C, K, groups, window):
+    """b200_group_weight_pack (both orientations) and b200_group_wgrad_unpack (dw_g += ...) bit for bit against the
+    index restatement of their contract, written into guarded buffers."""
+    g = torch.Generator().manual_seed(zlib.crc32(('pack/%d/%d/%d/%d' % (C, K, groups, window)).encode()))
+    T, cg = 9, C // groups
+    w32 = torch.randint(-256, 257, (K, T, cg), generator=g).float().cuda()      # exact in bf16
+    for transpose in (False, True):
+        call_pack(w32, K, T, C, groups, window, transpose)
+    dw_win = torch.randint(-1000, 1001, (K, T, window), generator=g).float().cuda()
+    dwg0 = torch.randint(-1000, 1001, (K, T, cg), generator=g).float().cuda()
+    call_unpack(dw_win, K, T, C, groups, window, dwg0)
+
+
+def test_group_pack_refuses_windows_outside_the_contract():
+    from convnet.pytorch_b200.lib import B200Error
+    ops = _ops()
+    for C, K, groups, window in ((16, 64, 4, 64), (256, 256, 64, 96), (256, 256, 32, 48)):
+        w32 = torch.zeros(K, 9, C // groups, device='cuda')
+        with pytest.raises(B200Error):
+            ops.group_weight_pack(w32, K, 9, C, groups, window, out=torch.zeros(K, 9, window, device='cuda',
+                                                                               dtype=bf16))
+        with pytest.raises(B200Error):
+            ops.group_wgrad_unpack(torch.zeros(K, 9, window, device='cuda'), K, 9, C, groups, window,
+                                   torch.zeros(K, 9, C // groups, device='cuda'))
+
+
+@pytest.mark.parametrize('window', [128, 256])
+def test_conv_window_other_than_64_refused(window):
+    """fprop / dgrad run block-diagonal windows of 64 channels only, wgrad of 128 only: other windows are refused
+    before anything is launched."""
+    from convnet.pytorch_b200.lib import B200Error
+    ops = _ops()
+    C = K = 512
+    x = torch.zeros(2, 8, 8, C, device='cuda', dtype=bf16)
+    w = torch.zeros(K, 9, window, device='cuda', dtype=bf16)
+    d = ops.make_desc(2, 8, 8, C, K, 3, 3, 1, 1, window=window)
+    with pytest.raises(B200Error):
+        ops.conv_fprop(x, w, d)
+    with pytest.raises(B200Error):
+        ops.conv_dgrad(x, w, d)
+    for ww in (64, 2 * window):
+        with pytest.raises(B200Error):
+            ops.conv_wgrad(x, x, ops.make_desc(2, 8, 8, C, K, 3, 3, 1, 1, window=ww),
+                           torch.zeros(K, 9, ww, device='cuda'))
+
+
+def _stem_taps(C):
+    """(s2d tap, channel block, r, s) of the 7x7/s2/p3 stem as a 4x4 convolution over the 2x2 space-to-depth input
+    with a 2-pixel low border: s2d tap (ah, aw), sub-pixel (bh, bw) at channels (2 bh + bw) C .. + C reads filter
+    tap r = 2 ah + bh - 1, s = 2 aw + bw - 1 when that lies inside the 7x7 filter"""
+    out = []
+    for ah in range(4):
+        for aw in range(4):
+            for bh in range(2):
+                for bw in range(2):
+                    r, s = 2 * ah + bh - 1, 2 * aw + bw - 1
+                    if 0 <= r < 7 and 0 <= s < 7:
+                        out.append((ah * 4 + aw, (bh * 2 + bw) * C, r, s))
+    return out
+
+
+@pytest.mark.parametrize('K,C,cpad', [(64, 3, 16), (24, 4, 16), (8, 1, 6)])
+def test_stem_weight_relayout(K, C, cpad):
+    """stem_weight_to_s2d (zeros in the slots no filter tap maps to and in the padding channels) and
+    stem_wgrad_from_s2d (dw += ... onto a non-zero dw) bit for bit against the index restatement"""
+    ops = _ops()
+    g = torch.Generator().manual_seed(K * 100 + C)
+    w = torch.randint(-256, 257, (K, 7, 7, C), generator=g).float().cuda()
+    want = torch.zeros(K, 16, cpad, device='cuda')
+    for tap, c0, r, s in _stem_taps(C):
+        want[:, tap, c0:c0 + C] = w[:, r, s]
+    buf, ws = _guarded((K, 16, cpad), bf16, float('nan'))
+    ops.stem_weight_to_s2d(w, K, C, cpad, ws)
+    torch.cuda.synchronize()
+    _check_written(buf, ws, 'stem_weight_to_s2d')
+    assert torch.equal(ws.float(), want)
+    dws = torch.randint(-1000, 1001, (K, 16, cpad), generator=g).float().cuda()
+    dw0 = torch.randint(-1000, 1001, (K, 7, 7, C), generator=g).float().cuda()
+    want = dw0.clone()
+    for tap, c0, r, s in _stem_taps(C):
+        want[:, r, s] += dws[:, tap, c0:c0 + C]
+    buf, dw = _guarded((K, 7, 7, C), torch.float32, 0.0)
+    dw.copy_(dw0)
+    ops.stem_wgrad_from_s2d(dws, K, C, cpad, dw)
+    torch.cuda.synchronize()
+    _check_written(buf, dw, 'stem_wgrad_from_s2d')
+    assert torch.equal(dw, want)
+
+
+@pytest.mark.parametrize('px,N', [(224, 2), (256, 1)])
+def test_stem_end_to_end_exact(px, N):
+    """The ImageNet stem as the engine runs it, in integers: input_prep (space-to-depth with the zero border), the
+    engine's descriptor for the width (4x4 halo convolution while Ws + 3 <= 128, else 4x1 over overlapping wide
+    pixels), stem_weight_to_s2d, and for the weight gradient conv_wgrad + stem_wgrad_from_s2d -- equal to the fp64
+    7x7 / stride 2 / pad 3 convolution and its weight gradient bit for bit."""
+    ops = _ops()
+    g = torch.Generator().manual_seed(px)
+    K, Cin, Hs = 64, 3, px // 2
+    d = _density(49 * Cin, 16)
+    x = _ints((N, Cin, px, px), d, g).cuda()
+    w = _ints((K, 7, 7, Cin), d, g).cuda()
+    xs = ops.input_prep(x, 16, s2d=True, border=True)
+    ws = torch.empty(K, 16, 16, device='cuda', dtype=bf16)
+    ops.stem_weight_to_s2d(w, K, Cin, 16, ws)
+    if Hs + 3 <= 128:
+        desc = ops.make_desc(N, Hs + 3, Hs + 3, 16, K, 4, 4, 1, 0, P=Hs, Q=Hs)
+    else:
+        desc = ops.make_desc(N, Hs + 3, Hs, 64, K, 4, 1, 1, 0, P=Hs, Q=Hs,
+                             x_strides=(16, (Hs + 3) * 16, (Hs + 3) * (Hs + 3) * 16))
+    y = ops.conv_fprop(xs, ws, desc)
+    ref = F.conv2d(x.double(), w.double().permute(0, 3, 1, 2), stride=2, padding=3)
+    _exact_preconditions(F.conv2d(x.double().abs(), w.double().abs().permute(0, 3, 1, 2), stride=2, padding=3),
+                         'stem fprop', True)
+    assert torch.equal(y.permute(0, 3, 1, 2).double(), ref), 'stem fprop differs'
+    dd = _density(N * Hs * Hs, 256)
+    x = _ints((N, Cin, px, px), dd, g).cuda()
+    dy = _ints((N, Hs, Hs, K), dd, g).cuda()
+    xs = ops.input_prep(x, 16, s2d=True, border=True)
+    dws = torch.zeros(K, 16, 16, device='cuda')
+    ops.conv_wgrad(xs, dy.to(bf16), desc, dws)
+    dw0 = torch.randint(-8, 9, (K, 7, 7, Cin), generator=g).float().cuda()
+    dw = ops.stem_wgrad_from_s2d(dws, K, Cin, 16, dw0.clone())
+    gref = conv2d_weight(x.double(), (K, Cin, 7, 7), dy.double().permute(0, 3, 1, 2), stride=2, padding=3)
+    _exact_preconditions(conv2d_weight(x.double().abs(), (K, Cin, 7, 7), dy.double().abs().permute(0, 3, 1, 2),
+                                       stride=2, padding=3) + 8, 'stem wgrad', False)
+    bad = dw.double() != gref.permute(0, 2, 3, 1) + dw0.double()
+    assert not bool(bad.any()), 'stem wgrad: %d of %d elements differ' % (int(bad.sum()), bad.numel())

@@ -409,6 +409,15 @@ def test_resnext50_grouped_against_bf16_oracle():
     _check_against_bf16_oracle(mine, ref, x, y)
 
 
+def test_resnext20_cifar_against_bf16_oracle():
+    """CIFAR ResNeXt (groups 4 / 8 / 16): the C != K stage entries (16 -> 64, 64 -> 128 and 128 -> 256) run on the dense
+    block-diagonal expansion of b200_group_weight_pack, the other grouped convolutions as well (C % 128 != 0 or
+    64 % (C/g) != 0), vs the bf16-emulating oracle."""
+    from convnet.pytorch_b200.models import resnext
+    ref, mine, x, y = _pair(resnext, dict(dataset='cifar10', depth=20), (3, 32, 32), 10, batch=32)
+    _check_against_bf16_oracle(mine, ref, x, y)
+
+
 def test_resnext101_32x4d_config_c3():
     """BASELINE config C3's model (ResNeXt-101 32x4d: depth 101, 32 groups, C/g = 4..32): T2 against the bf16 oracle
     at 64 px and T1 against stock torch fp32 (cuDNN grouped convolutions) at the full 224 px resolution."""
@@ -460,15 +469,19 @@ def test_trainer_cuda_graph_replay_matches_eager():
         assert _rel(s1[k], s0[k]) < 2e-3, '%s: %.3e' % (k, _rel(s1[k], s0[k]))
 
 
-@pytest.mark.parametrize("family", ["resnet50", "resnext50"])
+@pytest.mark.parametrize("family", ["resnet50", "resnext50", "resnext20_cifar"])
 def test_eval_with_folded_batchnorm(family):
     """Inference path: BN folded into the conv weights + epilogue bias (utils/absorb_bn.py:18-48 of the reference)
     must agree with the unfolded kernels and with stock torch eval; the folded-weight cache must follow parameter
-    and running-statistics updates."""
+    and running-statistics updates.  Grouped weights are folded through b200_group_weight_pack (CIFAR ResNeXt: also
+    its dense C != K expansion)."""
     from convnet.pytorch_b200 import engine
     from convnet.pytorch_b200.models import resnet, resnext
-    factory = resnet if family == "resnet50" else resnext
-    ref, mine, x, y = _pair(factory, dict(dataset='imagenet', depth=50), (3, 64, 64), 1000, steps=3, batch=8)
+    if family == "resnext20_cifar":
+        ref, mine, x, y = _pair(resnext, dict(dataset='cifar10', depth=20), (3, 32, 32), 10, steps=3, batch=8)
+    else:
+        factory = resnet if family == "resnet50" else resnext
+        ref, mine, x, y = _pair(factory, dict(dataset='imagenet', depth=50), (3, 64, 64), 1000, steps=3, batch=8)
     saved = engine.FOLD_BN_EVAL
     try:
         ref.eval(); mine.eval()
