@@ -57,14 +57,19 @@ def _sm_count():
 
 # ------------------------------------------------------------------------------------------------ the sweep
 def _case(N, H, W, C, K, R=1, S=1, stride=1, pad=(0, 0), ops='fdw', bias=False, res=False, act=0, fp32=False,
-          stats=False, groups=1, window=0, x_strides=None):
+          stats=False, groups=1, window=0, x_strides=None, res_f=None, res_d=None, P=None, Q=None):
     """groups > 1: a grouped convolution, run with desc.window = window (64; wgrad 128) or, window = 0, on the dense
-    block-diagonal expansion.  x_strides: (pixel, row, image) strides of x in elements (None: dense NHWC)."""
+    block-diagonal expansion.  x_strides: (pixel, row, image) strides of x in elements (None: dense NHWC).
+    res_f / res_d: a residual in the fprop / dgrad epilogue (default: res, and for dgrad only where R == 3 so that the
+    stride-2 residue classes are all non-empty).  P, Q: the output size (default: that of the padded convolution)."""
     pad = (pad, pad) if isinstance(pad, int) else tuple(pad)
     assert window in (0, 64) and (not window or (groups > 1 and C == K and C % 128 == 0 and 64 % (C // groups) == 0)), \
         'window mode as the engine runs it: C == K, C % 128 == 0 (128-wide wgrad windows), groups of <= 64 channels'
-    return dict(N=N, H=H, W=W, C=C, K=K, R=R, S=S, stride=stride, pad=pad, ops=ops, bias=bias, res=res, act=act,
-                fp32=fp32, stats=stats, groups=groups, window=window, x_strides=x_strides)
+    res_f = res if res_f is None else res_f
+    res_d = (res and R == 3) if res_d is None else res_d
+    return dict(N=N, H=H, W=W, C=C, K=K, R=R, S=S, stride=stride, pad=pad, ops=ops, bias=bias, res_f=res_f,
+                res_d=res_d, act=act, fp32=fp32, stats=stats, groups=groups, window=window, x_strides=x_strides, P=P,
+                Q=Q)
 
 
 def sweep(sm):
@@ -157,7 +162,7 @@ def _wgrad_window(cs):
 
 def _desc(cs, wgrad=False):
     return _ops().make_desc(cs['N'], cs['H'], cs['W'], cs['C'], cs['K'], cs['R'], cs['S'], cs['stride'], cs['pad'],
-                            x_strides=cs['x_strides'] or (0, 0, 0),
+                            P=cs['P'], Q=cs['Q'], x_strides=cs['x_strides'] or (0, 0, 0),
                             window=_wgrad_window(cs) if wgrad else cs['window'])
 
 
@@ -177,8 +182,9 @@ def _wgrad_shape(cs):
     return (cs['K'], cs['R'] * cs['S'], _wgrad_window(cs) or cs['C'])
 
 
-def _gen(name, tier):
-    return torch.Generator().manual_seed(zlib.crc32(('%s/%d' % (name, tier)).encode()))
+def _gen(name, tier, device='cpu'):
+    """the operand generator of a case; on 'cuda' the draws of large cases cost no host time (other values)"""
+    return torch.Generator(device=device).manual_seed(zlib.crc32(('%s/%d' % (name, tier)).encode()))
 
 
 # ------------------------------------------------------------------------------------------------ fp64 references
@@ -373,19 +379,18 @@ def _operands(cs, w32):
 
 
 def _res_fprop(cs):
-    return cs['res']
+    return cs['res_f']
 
 
 def _res_dgrad(cs):
-    # the residual epilogue of dgrad is exercised where the stride-2 residue classes are all non-empty
-    return cs['res'] and cs['R'] == 3
+    return cs['res_d']
 
 
 # ------------------------------------------------------------------------------------------------ tier 1
 def _ints(shape, density, g, lo=-2, hi=2):
-    v = torch.randint(lo, hi, shape, generator=g).float()
+    v = torch.randint(lo, hi, shape, generator=g, device=g.device).float()
     v = torch.where(v >= 0, v + 1, v)                       # {lo..hi} without 0
-    return torch.where(torch.rand(shape, generator=g) < density, v, torch.zeros(()))
+    return torch.where(torch.rand(shape, generator=g, device=g.device) < density, v, v.new_zeros(()))
 
 
 def _density(n, target):
@@ -400,18 +405,19 @@ def _exact_preconditions(absref, what, bf16_out):
         assert amax <= 256, '%s: |y| up to %g is not exact in bf16' % (what, amax)
 
 
-@pytest.mark.parametrize('name', _NAMES)
-def test_tier1_exact(name):
-    cs = _get(name)
-    g = _gen(name, 1)
+def check_exact(cs, tag, rng='cpu'):
+    """tier 1 of case cs (the directions in cs['ops']); tag seeds the operands (drawn on device rng) and names the
+    case"""
+    g = _gen(tag, 1, rng)
     N, H, W, C, K, RS = cs['N'], cs['H'], cs['W'], cs['C'], cs['K'], cs['R'] * cs['S']
     cg, kg = _cg(cs), K // cs['groups']
     P, Q = _outshape(cs)
     dev = 'cuda'
     if 'f' in cs['ops']:
-        d = _density(cg * RS, 8 if cs['stats'] else 16)
+        # fused statistics: the per-channel sum of y^2 over all M = N P Q output pixels must stay exact in fp32
+        d = _density(cg * RS, min(8, 2 ** 20 / (N * P * Q)) if cs['stats'] else 16)
         x, w = _ints(_x_shape(cs), d, g), _ints((K, RS, cg), d, g)
-        bias = torch.randint(-4, 5, (K,), generator=g).float().to(dev) if cs['bias'] else None
+        bias = torch.randint(-4, 5, (K,), generator=g, device=rng).float().to(dev) if cs['bias'] else None
         res = _ints((N, P, Q, K), 0.5, g).to(dev).to(bf16) if _res_fprop(cs) else None
         x, w = x.to(dev).to(bf16), w.to(dev)
         wf, _ = _operands(cs, w)
@@ -454,7 +460,7 @@ def test_tier1_exact(name):
     if 'w' in cs['ops']:
         d = _density(N * P * Q, 256)
         x, dy = _ints(_x_shape(cs), d, g).to(dev).to(bf16), _ints((N, P, Q, K), d, g).to(dev).to(bf16)
-        dw0 = torch.randint(-8, 9, _wgrad_shape(cs), generator=g).float().to(dev)
+        dw0 = torch.randint(-8, 9, _wgrad_shape(cs), generator=g, device=rng).float().to(dev)
         dense = ref_wgrad(x, dy, cs)
         ref = ref_wgrad_kernel_layout(dense, cs)
         _exact_preconditions(ref_wgrad(x.abs(), dy.abs(), cs) + 8, 'wgrad', False)
@@ -467,11 +473,16 @@ def test_tier1_exact(name):
             int(bad.sum()), bad.numel(), tuple(bad.nonzero()[0].tolist()))
         if cs['groups'] > 1:
             # keep each output channel's group (unpack, dw_g += ...): the gradient of the grouped master weight
-            dwg0 = torch.randint(-8, 9, (K, RS, cg), generator=g).float().to(dev)
+            dwg0 = torch.randint(-8, 9, (K, RS, cg), generator=g, device=rng).float().to(dev)
             dwg = call_unpack(dwz, K, RS, C, cs['groups'], _wgrad_window(cs) or C, dwg0)
             bad = dwg.double() != ref_wgrad_grouped(dense, cs) + dwg0.double()
             assert not bool(bad.any()), 'grouped wgrad: %d of %d elements differ, first at %s' % (
                 int(bad.sum()), bad.numel(), tuple(bad.nonzero()[0].tolist()))
+
+
+@pytest.mark.parametrize('name', _NAMES)
+def test_tier1_exact(name):
+    check_exact(_get(name), name)
 
 
 # ------------------------------------------------------------------------------------------------ tier 2
@@ -483,36 +494,38 @@ def _rel_l2(a, b):
     return float((a - b).norm() / (b.norm() + 1e-30))
 
 
-def _check_bound(y, ref, absref, what):
+def _check_bound(y, ref, absref, what, worst=WORST, coef=(C_BF16, C_FP32, 4e-3, 2e-5)):
+    """coef: (c for bf16 outputs, c for fp32 outputs, rel-L2 limit for bf16 outputs, rel-L2 limit for fp32 outputs)"""
     is_bf16 = y.dtype == bf16
-    rt, c = (2.0 ** -8, C_BF16) if is_bf16 else (0.0, C_FP32)
+    rt, c = (2.0 ** -8, coef[0]) if is_bf16 else (0.0, coef[1])
     err = (y.double() - ref).abs()
     excess = err - rt * ref.abs()
     ratio = float((excess / absref.clamp_min(1e-300)).max())
     key = 'bf16' if is_bf16 else 'fp32'
-    if ratio > WORST.get(key, (-math.inf, ''))[0]:
-        WORST[key] = (ratio, what)
+    if ratio > worst.get(key, (-math.inf, ''))[0]:
+        worst[key] = (ratio, what)
     bad = excess > c * absref
     assert not bool(bad.any()), '%s: %d elements outside |y-ref| <= %g |ref| + %g absref (worst ratio %.3g)' % (
         what, int(bad.sum()), rt, c, ratio)
-    assert _rel_l2(y, ref) < (4e-3 if is_bf16 else 2e-5), what
+    assert _rel_l2(y, ref) < (coef[2] if is_bf16 else coef[3]), what
 
 
-@pytest.mark.parametrize('name', _NAMES)
-def test_tier2_rounding(name):
-    cs = _get(name)
-    g = _gen(name, 2)
+def check_rounding(cs, tag, worst=WORST, rng='cpu', coef=(C_BF16, C_FP32, 4e-3, 2e-5)):
+    """tier 2 of case cs (operands drawn on device rng) with the bounds coef of _check_bound; the worst excess ratios
+    go into `worst`"""
+    name = tag
+    g = _gen(tag, 2, rng)
     N, H, W, C, K, RS = cs['N'], cs['H'], cs['W'], cs['C'], cs['K'], cs['R'] * cs['S']
     cg = _cg(cs)
     P, Q = _outshape(cs)
     dev = 'cuda'
-    x = torch.randn(*_x_shape(cs), generator=g).to(dev).to(bf16)
-    w = (torch.randn(K, RS, cg, generator=g) / math.sqrt(RS * cg)).to(dev).to(bf16).float()
-    dy = torch.randn(N, P, Q, K, generator=g).to(dev).to(bf16)
+    x = torch.randn(*_x_shape(cs), generator=g, device=rng).to(dev).to(bf16)
+    w = (torch.randn(K, RS, cg, generator=g, device=rng) / math.sqrt(RS * cg)).to(dev).to(bf16).float()
+    dy = torch.randn(N, P, Q, K, generator=g, device=rng).to(dev).to(bf16)
     wf, wt = _operands(cs, w)
     if 'f' in cs['ops']:
-        bias = torch.randn(K, generator=g).to(dev) if cs['bias'] else None
-        res = torch.randn(N, P, Q, K, generator=g).to(dev).to(bf16) if _res_fprop(cs) else None
+        bias = torch.randn(K, generator=g, device=rng).to(dev) if cs['bias'] else None
+        res = torch.randn(N, P, Q, K, generator=g, device=rng).to(dev).to(bf16) if _res_fprop(cs) else None
         pre, absref = ref_fprop(x, w, cs), ref_fprop(x.abs(), w.abs(), cs)
         if bias is not None:
             pre, absref = pre + bias.double(), absref + bias.double().abs()
@@ -520,21 +533,26 @@ def test_tier2_rounding(name):
             pre, absref = pre + res.double(), absref + res.double().abs()
         y, _ = call_fprop(cs, x, wf, bias, res)
         assert torch.equal(y, call_fprop(cs, x, wf, bias, res)[0]), 'fprop is not deterministic'
-        _check_bound(y, _act(pre, cs['act']), absref, '%s fprop' % name)
+        _check_bound(y, _act(pre, cs['act']), absref, '%s fprop' % name, worst, coef)
     if 'd' in cs['ops']:
-        res = torch.randn(N, H, W, C, generator=g).to(dev).to(bf16) if _res_dgrad(cs) else None
+        res = torch.randn(N, H, W, C, generator=g, device=rng).to(dev).to(bf16) if _res_dgrad(cs) else None
         ref, absref = ref_dgrad(dy, w, cs), ref_dgrad(dy.abs(), w.abs(), cs)
         if res is not None:
             ref, absref = ref + res.double(), absref + res.double().abs()
         dx = call_dgrad(cs, dy, wt, res)
         assert torch.equal(dx, call_dgrad(cs, dy, wt, res)), 'dgrad is not deterministic'
-        _check_bound(dx, ref, absref, '%s dgrad' % name)
+        _check_bound(dx, ref, absref, '%s dgrad' % name, worst, coef)
     if 'w' in cs['ops']:
         zero = torch.zeros(_wgrad_shape(cs), device=dev)
         dw = call_wgrad(cs, x, dy, zero)
         assert torch.equal(dw, call_wgrad(cs, x, dy, zero)), 'wgrad is not deterministic'
         _check_bound(dw, ref_wgrad_kernel_layout(ref_wgrad(x, dy, cs), cs),
-                     ref_wgrad_kernel_layout(ref_wgrad(x.abs(), dy.abs(), cs), cs), '%s wgrad' % name)
+                     ref_wgrad_kernel_layout(ref_wgrad(x.abs(), dy.abs(), cs), cs), '%s wgrad' % name, worst, coef)
+
+
+@pytest.mark.parametrize('name', _NAMES)
+def test_tier2_rounding(name):
+    check_rounding(_get(name), name)
 
 
 def test_tier2_calibration_report():
@@ -677,14 +695,12 @@ def _requirements():
     return req
 
 
-def test_sweep_coverage(monkeypatch, capfd):
-    """Every configuration of the table in _requirements() is reached by some launch of the sweep."""
-    for var in ('B200_IGEMM_DEBUG', 'B200_WGRAD_DEBUG', 'B200_HALO_DEBUG'):
-        monkeypatch.setenv(var, '1')
-    ops = _ops()
+def coverage_records(cases, capfd):
+    """launch every case of `cases` (name -> case) once on zeros and parse the per-launch debug lines (the caller
+    enables them) into records tagged with the case name and direction"""
     recs = []
     capfd.readouterr()
-    for name, cs in sweep(_sm_count()).items():
+    for name, cs in cases.items():
         N, H, W, C, K, RS = cs['N'], cs['H'], cs['W'], cs['C'], cs['K'], cs['R'] * cs['S']
         P, Q = _outshape(cs)
         x = torch.zeros(_x_shape(cs), device='cuda', dtype=bf16)
@@ -701,6 +717,18 @@ def test_sweep_coverage(monkeypatch, capfd):
         if 'w' in cs['ops']:
             call_wgrad(cs, x, dy, torch.zeros(_wgrad_shape(cs), device='cuda'))
             recs += _parse(capfd.readouterr().err, name, 'wgrad', cs)
+    return recs
+
+
+def enable_debug_lines(monkeypatch):
+    for var in ('B200_IGEMM_DEBUG', 'B200_WGRAD_DEBUG', 'B200_HALO_DEBUG'):
+        monkeypatch.setenv(var, '1')
+
+
+def test_sweep_coverage(monkeypatch, capfd):
+    """Every configuration of the table in _requirements() is reached by some launch of the sweep."""
+    enable_debug_lines(monkeypatch)
+    recs = coverage_records(sweep(_sm_count()), capfd)
     missing = []
     lines = []
     for label, pred in _requirements().items():

@@ -67,25 +67,26 @@ def _sm_count():
     return torch.cuda.get_device_properties(0).multi_processor_count
 
 
-def _gen(*key):
-    return torch.Generator().manual_seed(zlib.crc32('/'.join(str(k) for k in key).encode()))
+def _gen(*key, device='cpu'):
+    """the data generator of a case; on 'cuda' large draws cost no host time (other values)"""
+    return torch.Generator(device=device).manual_seed(zlib.crc32('/'.join(str(k) for k in key).encode()))
 
 
 # ------------------------------------------------------------------------------------------------ data
 def _ints(shape, lo, hi, g, dtype=bf16, density=1.0):
-    v = torch.randint(lo, hi + 1, shape, generator=g).to(f32)
+    v = torch.randint(lo, hi + 1, shape, generator=g, device=g.device).to(f32)
     if density < 1.0:
-        v = torch.where(torch.rand(shape, generator=g) < density, v, torch.zeros(()))
+        v = torch.where(torch.rand(shape, generator=g, device=g.device) < density, v, v.new_zeros(()))
     return v.to(DEV).to(dtype)
 
 
 def _pick(shape, choices, g):
     t = torch.tensor(choices, dtype=f32)
-    return t[torch.randint(0, len(choices), shape, generator=g)].to(DEV)
+    return t[torch.randint(0, len(choices), shape, generator=g, device=g.device).cpu()].to(DEV)
 
 
 def _randn(shape, g, scale=1.0, shift=0.0, dtype=bf16):
-    return (torch.randn(shape, generator=g) * scale + shift).to(DEV).to(dtype)
+    return (torch.randn(shape, generator=g, device=g.device) * scale + shift).to(DEV).to(dtype)
 
 
 # ------------------------------------------------------------------------------------------------ guarded outputs
@@ -305,9 +306,13 @@ def _stat_outputs(C):
 @pytest.mark.parametrize('tier', [1, 2])
 @pytest.mark.parametrize('name', _BN_NAMES)
 def test_bn_stats(name, tier):
+    check_bn_stats(*_bn_case(name), tier, name)
+
+
+def check_bn_stats(M, C, tier, name, rng='cpu'):
+    """bn_stats on an [M, C] z in the given tier; name seeds the data and names the case"""
     ops = _ops()
-    M, C = _bn_case(name)
-    g = _gen('bn_stats', name, tier)
+    g = _gen('bn_stats', name, tier, device=rng)
     eps = 1e-5
     if tier == 1:
         z = _ints((M, C), -4, 4, g)
@@ -497,8 +502,12 @@ def _bn_apply_call(z, sc, sh, act, mode, extra, with_mask, fill):
 @pytest.mark.parametrize('tier', [1, 2])
 @pytest.mark.parametrize('name', _BN_NAMES)
 def test_bn_apply(name, tier):
-    M, C = _bn_case(name)
-    g = _gen('bn_apply', name, tier)
+    check_bn_apply(*_bn_case(name), tier, name)
+
+
+def check_bn_apply(M, C, tier, name, rng='cpu'):
+    """bn_apply (three modes x three activations, with and without the mask) on [M, C] in the given tier"""
+    g = _gen('bn_apply', name, tier, device=rng)
     if tier == 1:
         z, res, z2 = _ints((M, C), -8, 8, g), _ints((M, C), -8, 8, g), _ints((M, C), -8, 8, g)
         sc, sc2 = _pick((C,), [-2, -1, -0.5, 0.5, 1, 2], g), _pick((C,), [-1, -0.5, 0.5, 1], g)
@@ -584,12 +593,14 @@ def _mask_with_padding(mask, M, C, pad):
 @pytest.mark.parametrize('tier', [1, 2])
 @pytest.mark.parametrize('name', _BN_NAMES)
 def test_bn_backward(name, tier):
-    """bn_bwd_reduce / bn_bwd_dx: every (VEC, ROWS, MINB) instantiation the shape selects x every activation x the
-    three activation sources (0: recomputed from z, 1: y, 2: mask bits)"""
+    check_bn_backward(*_bn_case(name), tier, name, affine=not name.endswith('_few'))   # '_few': NULL gamma / beta
+
+
+def check_bn_backward(M, C, tier, name, affine=True, rng='cpu'):
+    """bn_bwd_reduce / bn_bwd_dx on [M, C]: every (VEC, ROWS, MINB) instantiation the shape selects x every activation
+    x the three activation sources (0: recomputed from z, 1: y, 2: mask bits)"""
     ops = _ops()
-    M, C = _bn_case(name)
-    g = _gen('bn_bwd', name, tier)
-    affine = not name.endswith('_few')          # the '_few' cases run with NULL gamma / beta
+    g = _gen('bn_bwd', name, tier, device=rng)
     if tier == 1:
         z = _ints((M, C), -4, 4, g)
         dy = _ints((M, C), -3, 3, g, density=min(1.0, 2.0 ** 19 / (M * 6)))
