@@ -13,8 +13,9 @@
 // the scale is unbounded); vertical coefficients are computed per chunk of kRrcYChunk intermediate rows.  The grid
 // depends only on (B*D, OH) and there is no workspace: a captured CUDA graph replays with new tables and regions.
 //
-// The same arithmetic (the rrc_* helpers below) serves the small fixed-size resample of the CIFAR Mix&Match transform,
-// input_prep_aug_resize_kernel at the end of this file.
+// The same arithmetic (the rrc_* helpers below) serves the ImageNet evaluation transform (Resize + CenterCrop,
+// input_prep_scale_crop_kernel: the crop window of the whole image's resize, on the same block shape) and the small
+// fixed-size resample of the CIFAR Mix&Match transform, input_prep_aug_resize_kernel at the end of this file.
 #include "common.cuh"
 #include "host.h"
 
@@ -181,6 +182,158 @@ __global__ void __launch_bounds__(kRrcMaxOW) input_prep_rrc_kernel(
 
   // mode 0: [N][OH][OW][Cpad];  mode 2: [N][OH/2+3][OW/2+3][Cpad], data at (+2, +2), channel (dy*2+dx)*C + c.
   // The first band also writes the top border rows, the last band the bottom one.
+  const bool s2d = mode == 2;
+  const int PH = s2d ? OH / 2 + 3 : OH, PW = s2d ? OW / 2 + 3 : OW, brd = s2d ? 2 : 0;
+  const int r_lo = s2d ? (o0 == 0 ? 0 : o0 / 2 + brd) : o0;
+  const int r_hi = s2d ? (o0 + tb == OH ? PH : (o0 + tb) / 2 + brd) : o0 + tb;
+  const int total = (r_hi - r_lo) * PW;
+  for (int p = threadIdx.x; p < total; p += nt) {
+    const int pr = r_lo + p / PW, pc = p % PW;
+    const int i = pr - brd, jj = pc - brd;
+    const bool inside = !s2d || (i >= 0 && i < OH / 2 && jj >= 0 && jj < OW / 2);
+    __nv_bfloat16* o = out + (((long long)n * PH + pr) * PW + pc) * Cpad;
+    for (int c0 = 0; c0 < Cpad; c0 += 8) {
+      float f[8];
+#pragma unroll
+      for (int e = 0; e < 8; ++e) {
+        const int chn = c0 + e;
+        const int sub = s2d ? chn / C : (chn < C ? 0 : 4), c = s2d ? chn - sub * C : chn;
+        float v = 0.f;
+        if (sub < 4 && inside) {
+          const int ty = s2d ? 2 * i + (sub >> 1) : i, tx = s2d ? 2 * jj + (sub & 1) : jj;
+          v = __ldg(lut + c * 256 + tile[((size_t)(ty - o0) * OW + tx) * C + c]);
+        }
+        f[e] = v;
+      }
+      uint4 u;
+      u.x = pack_bf16x2(f[0], f[1]); u.y = pack_bf16x2(f[2], f[3]);
+      u.z = pack_bf16x2(f[4], f[5]); u.w = pack_bf16x2(f[6], f[7]);
+      *reinterpret_cast<uint4*>(o + c0) = u;
+    }
+  }
+}
+
+// ---- the ImageNet evaluation transform (the reference's scale_crop, preprocess.py:20-41, one crop): Resize(scale)
+// -> CenterCrop(size) -> ToTensor -> Normalize ------------------------------------------------------------------------
+// In Pillow's resample, output index xx of an in -> out resize depends on xx, in and out only.  So the centre crop of
+// the resized image is the full-image axis rrc_axis(W, RW) evaluated at output indices left .. left + OW - 1, and
+// likewise for rows: the resized image is never formed.  (Resizing the crop box instead, as the RRC kernel does, would
+// differ in the last bits.)  Each image ships only its support region, the source pixels the window's taps touch; pixel
+// (y, x) of the image is read at (y - y0, x - x0) of the region, clamped to the region and the buffer.  Output pixels
+// outside the resized image -- a crop larger than the image, which CenterCrop pads -- take uint8 0.  Block shape,
+// coefficient slab and vertical chunks are those of input_prep_rrc_kernel; one copy per image.
+__global__ void __launch_bounds__(kRrcMaxOW) input_prep_scale_crop_kernel(
+    const uint8_t* __restrict__ regions, long long region_bytes, const long long* __restrict__ index,
+    const int* __restrict__ geom, int C, int OH, int OW, int Cpad, int mode, const float* __restrict__ lut,
+    __nv_bfloat16* __restrict__ out) {
+  extern __shared__ __align__(16) unsigned char sc_smem[];
+  int* ktab = reinterpret_cast<int*>(sc_smem);                                   // [kRrcTaps][blockDim.x]
+  uint8_t* tile = sc_smem + (size_t)kRrcTaps * blockDim.x * sizeof(int);         // [kRrcRows][OW][C]
+  __shared__ RrcRow rows[kRrcRows];
+  __shared__ int vtab[kRrcRows * kRrcYChunk];
+
+  const int n = blockIdx.y;                     // image n
+  const int o0 = blockIdx.x * kRrcRows;
+  const int tb = min(kRrcRows, OH - o0);
+  const int xx = threadIdx.x;
+  const int nt = blockDim.x;
+
+  // geom = {y0, x0, H, W, RH, RW, top, left}; sizes clamped like the RRC region, so any table values are bounded work
+  const long long* ix = index + (long long)n * 3;
+  const int* gm = geom + (long long)n * 8;
+  const long long off = min(max(__ldg(ix + 0), 0LL), region_bytes - 1);
+  const long long rh = min(max(__ldg(ix + 1), 1LL), 65535LL), rw = min(max(__ldg(ix + 2), 1LL), 65535LL);
+  const long long ry0 = __ldg(gm + 0), rx0 = __ldg(gm + 1);
+  const int H = min(max(__ldg(gm + 2), 1), 65535), W = min(max(__ldg(gm + 3), 1), 65535);
+  const int RH = min(max(__ldg(gm + 4), 1), 65535), RW = min(max(__ldg(gm + 5), 1), 65535);
+  const long long top = __ldg(gm + 6), left = __ldg(gm + 7);
+
+  const RrcAxis ay = rrc_axis(H, RH), ax = rrc_axis(W, RW);
+  if (xx < tb) {
+    RrcRow r = {0.0, 0.0, 0, 0};                // a padded row: no taps
+    const long long yy = top + o0 + xx;
+    if (yy >= 0 && yy < RH) {
+      rrc_bounds(ay, (int)yy, r.center, r.ymin, r.cnt);
+      r.ww = rrc_sum(ay, r.center, r.ymin, r.cnt);
+    }
+    rows[xx] = r;
+  }
+  double xc = 0.0, xww = 0.0;
+  int xmin = 0, xcnt = 0;                       // a padded column: no taps
+  const long long xs = left + xx;
+  if (xx < OW && xs >= 0 && xs < RW) {
+    rrc_bounds(ax, (int)xs, xc, xmin, xcnt);
+    xww = rrc_sum(ax, xc, xmin, xcnt);
+  }
+  __syncthreads();
+  int ybeg = 0x7fffffff, yend = 0;
+  for (int r = 0; r < tb; ++r)
+    if (rows[r].cnt > 0) {
+      ybeg = min(ybeg, rows[r].ymin);
+      yend = max(yend, rows[r].ymin + rows[r].cnt);
+    }
+
+  int acc[kRrcRows][4];
+#pragma unroll
+  for (int r = 0; r < kRrcRows; ++r)
+#pragma unroll
+    for (int c = 0; c < 4; ++c) acc[r][c] = 1 << 21;
+  int built = -1;                               // first tap of the slab this thread holds
+
+  for (int yc = ybeg; yc < yend; yc += kRrcYChunk) {
+    __syncthreads();                            // the previous chunk's vertical coefficients are consumed
+    for (int e = threadIdx.x; e < kRrcRows * kRrcYChunk; e += nt) {
+      const int r = e / kRrcYChunk, t = yc + e % kRrcYChunk;
+      int k = 0;
+      if (r < tb && t >= rows[r].ymin && t < rows[r].ymin + rows[r].cnt)
+        k = rrc_coef(rrc_tri(ay, rows[r].center, t), rows[r].ww);
+      vtab[e] = k;
+    }
+    __syncthreads();
+    if (xx >= OW) continue;
+    const int y1 = min(yc + kRrcYChunk, yend);
+    for (int y = yc; y < y1; ++y) {
+      const long long row = off + min(max(y - ry0, 0LL), rh - 1) * rw * C;
+      int h[4] = {1 << 21, 1 << 21, 1 << 21, 1 << 21};
+      for (int t0 = 0; t0 < xcnt; t0 += kRrcTaps) {
+        const int te = min(kRrcTaps, xcnt - t0);
+        if (t0 != built) {
+          for (int t = 0; t < te; ++t) ktab[t * nt + xx] = rrc_coef(rrc_tri(ax, xc, xmin + t0 + t), xww);
+          built = t0;
+        }
+        for (int t = 0; t < te; ++t) {
+          const int k = ktab[t * nt + xx];
+          const long long p = row + min(max(xmin + t0 + t - rx0, 0LL), rw - 1) * C;
+#pragma unroll
+          for (int c = 0; c < 4; ++c)
+            if (c < C) h[c] += (int)__ldg(regions + min(p + c, region_bytes - 1)) * k;
+        }
+      }
+#pragma unroll
+      for (int c = 0; c < 4; ++c) h[c] = rrc_clip8(h[c]);
+#pragma unroll
+      for (int r = 0; r < kRrcRows; ++r) {
+        const int k = vtab[r * kRrcYChunk + (y - yc)];
+        if (k != 0) {
+#pragma unroll
+          for (int c = 0; c < 4; ++c) acc[r][c] += h[c] * k;
+        }
+      }
+    }
+  }
+
+  // a row or column without taps keeps acc = 2^21, which rrc_clip8 maps to 0: CenterCrop's fill
+  if (xx < OW) {
+#pragma unroll
+    for (int r = 0; r < kRrcRows; ++r)
+      if (r < tb)
+#pragma unroll
+        for (int c = 0; c < 4; ++c)
+          if (c < C) tile[((size_t)r * OW + xx) * C + c] = (uint8_t)rrc_clip8(acc[r][c]);
+  }
+  __syncthreads();
+
+  // the store of input_prep_rrc_kernel, restated so that kernel's code stays as it is
   const bool s2d = mode == 2;
   const int PH = s2d ? OH / 2 + 3 : OH, PW = s2d ? OW / 2 + 3 : OW, brd = s2d ? 2 : 0;
   const int r_lo = s2d ? (o0 == 0 ? 0 : o0 / 2 + brd) : o0;
@@ -379,5 +532,35 @@ extern "C" int b200_input_prep_u8_rrc(const uint8_t* regions, long long region_b
   b200::launch(input_prep_rrc_kernel, grid, threads, smem, (cudaStream_t)stream, regions, region_bytes, index, draws,
                D, C, OH, OW, Cpad, mode, lut, (__nv_bfloat16*)out);
   B200_CHECK_LAUNCH("input_prep_rrc_kernel");
+  return B200_OK;
+}
+
+extern "C" int b200_input_prep_u8_scale_crop(const uint8_t* regions, long long region_bytes, const long long* index,
+                                             const int* geom, int B, int C, int OH, int OW, int Cpad, int mode,
+                                             const float* lut, void* out, b200_stream_t stream) {
+  B200_REQUIRE(regions && index && geom && lut && out && region_bytes > 0 && B > 0 && C > 0 && C <= 4 && OH > 0 &&
+                   OW > 0,
+               B200_ERR_INVALID, "input_prep_u8_scale_crop: bad argument (C must be 1..4)");
+  B200_REQUIRE(OW <= kRrcMaxOW, B200_ERR_UNSUPPORTED, "input_prep_u8_scale_crop: OW=%d above %d", OW, kRrcMaxOW);
+  B200_REQUIRE(B <= 65535, B200_ERR_UNSUPPORTED, "input_prep_u8_scale_crop: B=%d above 65535", B);
+  B200_REQUIRE(Cpad % 8 == 0, B200_ERR_INVALID, "input_prep_u8_scale_crop: Cpad=%d must be a multiple of 8", Cpad);
+  if (mode == 0) {
+    B200_REQUIRE(Cpad >= C, B200_ERR_INVALID, "input_prep_u8_scale_crop: Cpad < C");
+  } else if (mode == 2) {
+    B200_REQUIRE(OH % 2 == 0 && OW % 2 == 0 && Cpad >= 4 * C, B200_ERR_UNSUPPORTED,
+                 "input_prep_u8_scale_crop: space-to-depth needs even OH, OW and Cpad >= 4C");
+  } else {
+    B200_REQUIRE(false, B200_ERR_UNSUPPORTED, "input_prep_u8_scale_crop: mode %d (0 or 2 only)", mode);
+  }
+  const int threads = (OW + 31) / 32 * 32;
+  const size_t smem = (size_t)kRrcTaps * threads * sizeof(int) + (size_t)kRrcRows * OW * C;
+  const dim3 grid((OH + kRrcRows - 1) / kRrcRows, B);
+  cudaError_t e = cudaFuncSetAttribute(input_prep_scale_crop_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       (int)smem);
+  B200_REQUIRE(e == cudaSuccess, B200_ERR_CUDA, "input_prep_u8_scale_crop: smem attribute (%d bytes): %s", (int)smem,
+               cudaGetErrorString(e));
+  b200::launch(input_prep_scale_crop_kernel, grid, threads, smem, (cudaStream_t)stream, regions, region_bytes, index,
+               geom, C, OH, OW, Cpad, mode, lut, (__nv_bfloat16*)out);
+  B200_CHECK_LAUNCH("input_prep_scale_crop_kernel");
   return B200_OK;
 }

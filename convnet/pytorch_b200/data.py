@@ -24,6 +24,11 @@ decode and draw the reference's crop boxes and flips per image; the loader yield
 the images' regions and draws, target repeated to B*D) and the stem relayout kernel resamples, flips and normalises.
 Real imagenet decodes with the reference's pil_loader (convert('RGB')); synthetic_imagenet uses a seeded pool of 64
 uniform uint8 images of 200-600 px.
+
+Resize + CenterCrop on the device (transform key ``device_scale_crop``, ImageNet-style evaluation only): the workers
+decode and compute each image's resized size, crop offsets and support region; the loader yields
+(utils.augment.ScaleCropBatch of the regions and geometry, target) and the stem relayout kernel resamples the crop
+window of each whole image's resize and normalises it.  Same datasets as ``device_resized_crop``.
 """
 import os
 from copy import deepcopy
@@ -33,7 +38,8 @@ import torch
 from torch.utils.data import Dataset, Subset
 from torch.utils.data.distributed import DistributedSampler
 
-from .utils.augment import AugmentCollate, BatchAugment, Cutout, ResizedCrop, ResizedCropCollate
+from .utils.augment import AugmentCollate, BatchAugment, Cutout, ResizedCrop, ResizedCropCollate, ScaleCrop, \
+    ScaleCropCollate
 from .utils.regime import Regime
 
 
@@ -157,7 +163,7 @@ def get_dataset(name, split='train', transform=None, target_transform=None, down
 
 def device_augment_spec(transform_name='cifar10', input_size=None, scale_size=None, normalize=None, augment=True,
                         cutout=None, autoaugment=False, padding=None, duplicates=1, num_crops=1, device_augment=True,
-                        device_resized_crop=False):
+                        device_resized_crop=False, device_scale_crop=False):
     """The BatchAugment of a ``device_augment`` transform setting: the CIFAR training transform of
     real_dataset_transform (pad-4 random crop + flip + ToTensor + Normalize [+ Cutout]) with its duplicates.  The
     settings it cannot reproduce raise."""
@@ -208,7 +214,8 @@ def u8_dataset(name, input_size=None, scale_size=None, split='train', download=T
 
 def resized_crop_spec(transform_name='imagenet', input_size=None, scale_size=None, normalize=None, augment=True,
                       cutout=None, autoaugment=False, padding=None, duplicates=1, num_crops=1, device_augment=False,
-                      device_resized_crop=True, interpolation='bilinear', color_jitter=None, lighting=None):
+                      device_resized_crop=True, interpolation='bilinear', color_jitter=None, lighting=None,
+                      device_scale_crop=False):
     """The ResizedCrop of a ``device_resized_crop`` transform setting: the imagenet training transform of
     real_dataset_transform (RandomResizedCrop(input_size) + flip + ToTensor + Normalize) with its duplicates.  The
     settings it cannot reproduce raise."""
@@ -229,6 +236,31 @@ def resized_crop_spec(transform_name='imagenet', input_size=None, scale_size=Non
     if str(interpolation).lower() != 'bilinear':
         raise NotImplementedError('device_resized_crop resamples bilinearly only; got %r' % (interpolation,))
     return ResizedCrop(input_size or 224, duplicates=duplicates or 1, normalize=normalize or _IMAGE_STATS)
+
+
+def scale_crop_spec(transform_name='imagenet', input_size=None, scale_size=None, normalize=None, augment=False,
+                    cutout=None, autoaugment=False, padding=None, duplicates=1, num_crops=1, device_augment=False,
+                    device_resized_crop=False, device_scale_crop=True, interpolation='bilinear'):
+    """The ScaleCrop of a ``device_scale_crop`` transform setting: the imagenet evaluation transform of
+    real_dataset_transform (Resize(scale_size) + CenterCrop(input_size) + ToTensor + Normalize, scale_size =
+    int(input_size * 8 / 7) unless set).  The settings it cannot reproduce raise."""
+    if 'imagenet' not in (transform_name or ''):
+        raise NotImplementedError('device_scale_crop reproduces the ImageNet evaluation transform only; got transform '
+                                  '%r' % transform_name)
+    if augment:
+        raise NotImplementedError('device_scale_crop is an evaluation transform (augment=False); training loaders do '
+                                  'not take it (ImageNet training: use device_resized_crop)')
+    if device_augment or device_resized_crop:
+        raise NotImplementedError('device_scale_crop and device_augment / device_resized_crop are different '
+                                  'transforms; set one per loader')
+    if num_crops != 1 or (duplicates or 1) != 1:
+        raise NotImplementedError('device_scale_crop makes one centre crop per image (no multi-crop / duplicates)')
+    if autoaugment or cutout:
+        raise NotImplementedError('device_scale_crop does not reproduce autoaugment / Cutout')
+    if str(interpolation).lower() != 'bilinear':
+        raise NotImplementedError('device_scale_crop resamples bilinearly only; got %r' % (interpolation,))
+    input_size = input_size or 224
+    return ScaleCrop(input_size, scale_size or int(input_size * 8 / 7), normalize=normalize or _IMAGE_STATS)
 
 
 class DecodedImages(Dataset):
@@ -255,8 +287,9 @@ def synthetic_imagenet_pool(n=64, lo=200, hi=600, seed=0):
 
 
 def decoded_dataset(name, transform, split='train', datasets_path='~/Datasets', synthetic_length=None, **_):
-    """Decode-only samples for device_resized_crop: ImageFolder with the reference's pil_loader (convert('RGB')) for
-    imagenet, the seeded synthetic_imagenet_pool for synthetic_imagenet; ``transform`` (a ResizedCrop) draws."""
+    """Decode-only samples for device_resized_crop and device_scale_crop: ImageFolder with the reference's pil_loader
+    (convert('RGB')) for imagenet, the seeded synthetic_imagenet_pool for synthetic_imagenet; ``transform`` (a
+    ResizedCrop or a ScaleCrop) does the per-image host work."""
     train = split == 'train'
     if name == 'synthetic_imagenet':
         _, classes, n_train, n_val = _SYNTHETIC[name]
@@ -268,14 +301,15 @@ def decoded_dataset(name, transform, split='train', datasets_path='~/Datasets', 
         import torchvision.datasets as tvd
         return tvd.ImageFolder(root=os.path.join(os.path.expanduser(datasets_path), name, 'train' if train else 'val'),
                                transform=transform)
-    raise NotImplementedError('device_resized_crop supports imagenet and synthetic_imagenet; got %r' % name)
+    raise NotImplementedError('device_resized_crop / device_scale_crop support imagenet and synthetic_imagenet; got %r'
+                              % name)
 
 
 _DATA_ARGS = {'name', 'split', 'transform', 'target_transform', 'download', 'datasets_path', 'synthetic_length'}
 _DATALOADER_ARGS = {'batch_size', 'shuffle', 'sampler', 'batch_sampler', 'num_workers', 'collate_fn', 'pin_memory',
                     'drop_last', 'timeout', 'worker_init_fn'}
 _TRANSFORM_ARGS = {'transform_name', 'input_size', 'scale_size', 'normalize', 'augment', 'cutout', 'duplicates',
-                   'num_crops', 'autoaugment', 'device_augment', 'device_resized_crop'}
+                   'num_crops', 'autoaugment', 'device_augment', 'device_resized_crop', 'device_scale_crop'}
 _OTHER_ARGS = {'distributed'}
 
 
@@ -306,7 +340,11 @@ class DataRegime(object):
             data_kwargs = dict(setting['data'])
             name = data_kwargs.get('name', '')
             collate = None
-            if setting['transform'].get('device_resized_crop'):
+            if setting['transform'].get('device_scale_crop'):
+                spec = scale_crop_spec(**setting['transform'])
+                self._data = decoded_dataset(transform=spec, **data_kwargs)
+                collate = ScaleCropCollate(spec)
+            elif setting['transform'].get('device_resized_crop'):
                 spec = resized_crop_spec(**setting['transform'])
                 self._data = decoded_dataset(transform=spec, **data_kwargs)
                 collate = ResizedCropCollate(spec)
@@ -322,7 +360,7 @@ class DataRegime(object):
                 # real images: build the transform the regime asks for (reference data.py:101-102) -- never fall back
                 # to a bare ToTensor(), which would train on unnormalised, unaugmented, variable-size images
                 tf = {k: v for k, v in setting['transform'].items()
-                      if v is not None and k not in ('device_augment', 'device_resized_crop')}
+                      if v is not None and k not in ('device_augment', 'device_resized_crop', 'device_scale_crop')}
                 data_kwargs['transform'] = real_dataset_transform(**tf)
             if collate is None:
                 self._data = get_dataset(**data_kwargs)

@@ -327,7 +327,8 @@ class Runtime(object):
     def _input(self, x, mix=None, aug=None):
         """-> (tensor, relayout function, (N, C, H, W)).  ``mix`` (ops.Mix): MixUp / CutMix applied by the relayout
         kernel itself (the reference mixes the fp32 batch before the forward pass, trainer.py:119-135).  ``aug``
-        (ops.Aug): x holds the B un-augmented uint8 images and the relayout writes their B*D augmented copies."""
+        (ops.Aug): x holds the B un-augmented uint8 images and the relayout writes their B*D augmented copies; with
+        ops.Rrc or ops.ScaleCropTables x is a flat uint8 region buffer and the relayout resamples it."""
         if isinstance(aug, ops.Rrc):
             # x is the flat uint8 region buffer; the relayout resamples the B*D crops (mode 0 or the mode-2 stem)
             if mix is not None:
@@ -338,6 +339,16 @@ class Runtime(object):
             OH, OW = aug.size
             return x, (lambda t, cpad, **kw: ops.input_prep_u8_rrc(t, cpad, aug, **kw)), \
                 (aug.draws.shape[0], aug.lut.shape[0], OH, OW)
+        if isinstance(aug, ops.ScaleCropTables):
+            # x is the flat uint8 region buffer; the relayout resamples each image's centre-crop window (evaluation)
+            if mix is not None:
+                raise B200Error('the scale crop on the device is not combined with MixUp / CutMix')
+            if x.dtype != torch.uint8 or x.dim() != 1:
+                raise B200Error('the scale crop on the device needs the flat uint8 region buffer; got %s %s'
+                                % (x.dtype, tuple(x.shape)))
+            OH, OW = aug.size
+            return x, (lambda t, cpad, **kw: ops.input_prep_u8_scale_crop(t, cpad, aug, **kw)), \
+                (aug.index.shape[0], aug.lut.shape[0], OH, OW)
         if x.dtype == torch.uint8:
             if x.dim() != 4 or x.shape[-1] > 4:
                 raise B200Error('uint8 network inputs must be NHWC [N, H, W, C<=4]; got %s' % (tuple(x.shape),))

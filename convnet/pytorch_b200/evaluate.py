@@ -1,7 +1,7 @@
 """Checkpoint evaluation CLI with the reference's evaluate.py flags (evaluate.py:28-193 of eladhoffer/convNet.pytorch).
 
     python -m convnet.pytorch_b200.evaluate results/run/checkpoint.pth.tar --dataset synthetic_imagenet \
-        [--calibrate-bn] [--absorb-bn] [--avg-out --duplicates 4] [-b 256] [--device cuda]
+        [--calibrate-bn] [--absorb-bn] [--avg-out --duplicates 4] [-b 256] [--device cuda] [--device-scale-crop]
 
 Flow (evaluate.py:101-193): load the checkpoint (its ``model`` / ``config`` entries override the command line) ->
 build the model from the registry -> ``load_state_dict`` -> optional ``--absorb-bn`` -> criterion -> Trainer ->
@@ -55,6 +55,9 @@ def build_parser():
     a('--mixup', default=None, type=float, help='mixup alpha coefficient - accepted for CLI parity, unused in evaluation')
     a('--duplicates', default=1, type=int, help='number of augmentations over single example')
     a('--augment', action='store_true', default=False, help='perform augmentations')
+    a('--device-scale-crop', action='store_true', default=False,
+      help='ImageNet: the loader workers only decode; the input relayout on the GPU resizes (Pillow-exact bilinear), '
+           'centre-crops and normalises the images')
     a('--calibrate-bn', action='store_true', default=False, help='calibrate bn stats')
     a('--calibrate-steps', default=200, type=int, help='forward passes of --calibrate-bn (reference: 200)')
     a('--avg-out', action='store_true', default=False, help='average outputs over the duplicates')
@@ -147,7 +150,7 @@ def main_worker(args):
     common = {'datasets_path': args.datasets_dir, 'name': args.dataset, 'input_size': args.input_size,
               'batch_size': args.batch_size, 'num_workers': args.workers, 'pin_memory': cuda, 'drop_last': False}
     val_data = DataRegime(None, defaults=dict(common, split='val', augment=args.augment, shuffle=False,
-                                              duplicates=args.duplicates))
+                                              duplicates=args.duplicates, device_scale_crop=args.device_scale_crop))
     if args.calibrate_bn:
         train_data = DataRegime(None, defaults=dict(common, split='train', augment=True, shuffle=True))
         trainer.calibrate_bn(train_data.get_loader(), num_steps=args.calibrate_steps)

@@ -71,6 +71,7 @@ SIGNATURES = {
     "b200_input_prep_u8_aug": [_vp, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _i, _vp, _vp],
     "b200_input_prep_u8_aug_resize": [_vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _i, _vp, _vp],
     "b200_input_prep_u8_rrc": [_vp, _ll, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp],
+    "b200_input_prep_u8_scale_crop": [_vp, _ll, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp],
     "b200_weight_transpose": [_vp, _vp, _i, _i, _i, _vp],
     "b200_weight_transpose_batched": [_vp, _vp, _vp, _i, _i, _vp],
     "b200_stem_weight_to_s2d": [_vp, _i, _i, _i, _vp, _vp],

@@ -9,7 +9,8 @@ Additions over the reference: ``--dtype bfloat16`` (compute type of the B200 ker
 masters in the arena), ``synthetic_*`` datasets, ``--b200 {auto,on,off}`` (auto: on for CUDA devices),
 ``--device-augment`` (batch augmentation of the CIFAR transform done in the input relayout kernel, with the Resize of
 the Mix&Match ``sampled*`` regimes),
-``--device-resized-crop`` (the ImageNet RandomResizedCrop + flip resampled in the input relayout kernel), and
+``--device-resized-crop`` (the ImageNet RandomResizedCrop + flip resampled in the input relayout kernel),
+``--device-scale-crop`` (the ImageNet evaluation Resize + CenterCrop resampled in the input relayout kernel), and
 rank/world are read from the torchrun environment when ``--local_rank`` is not given.
 """
 import argparse
@@ -79,6 +80,9 @@ def build_parser():
     a('--device-resized-crop', action='store_true', default=False,
       help='ImageNet training: the loader workers only decode and draw the crop boxes and flips; the input relayout '
            'on the GPU resamples the crops (Pillow-exact bilinear), flips and normalises them')
+    a('--device-scale-crop', action='store_true', default=False,
+      help='ImageNet validation: the loader workers only decode; the input relayout on the GPU resizes (Pillow-exact '
+           'bilinear), centre-crops and normalises the images')
     a('--autoaugment', action='store_true', default=False, help='autoaugment policies (ignored for synthetic data)')
     a('--grad-clip', default=-1, type=float, help='maximum grad norm value, -1 for none')
     a('--loss-scale', default=1, type=float, help='loss scale for mixed precision training')
@@ -237,7 +241,8 @@ def main_worker(args):
                           defaults={'datasets_path': args.datasets_dir, 'name': args.dataset, 'split': 'val',
                                     'augment': False, 'input_size': args.input_size,
                                     'batch_size': args.eval_batch_size, 'shuffle': False,
-                                    'num_workers': args.workers, 'pin_memory': True, 'drop_last': False})
+                                    'num_workers': args.workers, 'pin_memory': True, 'drop_last': False,
+                                    'device_scale_crop': args.device_scale_crop})
     if args.evaluate:
         res = trainer.validate(val_data.get_loader())
         logging.info(res)

@@ -656,6 +656,73 @@ def input_prep_u8_rrc(regions, cpad, rrc, s2d=False, border=False, out=None):
     return out
 
 
+class ScaleCropTables(object):
+    """Device-side tables of one scale-crop (evaluation) batch (utils/augment.py ScaleCropBatch): ``index`` int64 [B, 3]
+    {byte offset, h, w} of each image's support region in the uint8 region buffer, ``geom`` int32 [B, 8] {y0, x0, H, W,
+    RH, RW, top, left}, ``lut`` fp32 [C, 256], ``size`` (OH, OW).  ``host`` holds CPU copies of index and geom plus the
+    number of region bytes in use: input_prep_u8_scale_crop validates them before the launch, without a device
+    read-back."""
+    __slots__ = ('index', 'geom', 'lut', 'size', 'host')
+
+    def __init__(self, index, geom, lut, size, host):
+        self.index, self.geom, self.lut = index, geom, lut
+        self.size, self.host = (int(size[0]), int(size[1])), host
+
+
+def check_scale_crop_tables(index, geom, nbytes, C, size):
+    """Host-side validation of scale-crop tables (CPU int64 [B, 3] index, int32 [B, 8] geom) for an OH x OW ``size``:
+    every region lies inside the first ``nbytes`` bytes of the buffer and inside its image, and covers every source
+    pixel the crop window's taps read.  Raises B200Error."""
+    from .utils.augment import crop_support
+    if index.dim() != 2 or index.shape[1] != 3 or geom.dim() != 2 or geom.shape[1] != 8 \
+            or geom.shape[0] != index.shape[0]:
+        raise _l.B200Error("input_prep_u8_scale_crop: index must be [B, 3] and geom [B, 8]; got %s, %s"
+                           % (tuple(index.shape), tuple(geom.shape)))
+    off, h, w = (index[:, k].long() for k in range(3))
+    if bool(((off < 0) | (h < 1) | (w < 1) | (h > 65535) | (w > 65535) | (off + h * w * C > nbytes)).any()):
+        raise _l.B200Error("input_prep_u8_scale_crop: a region lies outside the %d-byte buffer" % nbytes)
+    OH, OW = size
+    for b, (y0, x0, H, W, RH, RW, top, left) in enumerate(geom.tolist()):
+        rh, rw = int(h[b]), int(w[b])
+        if not (1 <= H <= 65535 and 1 <= W <= 65535 and 1 <= RH <= 65535 and 1 <= RW <= 65535):
+            raise _l.B200Error("input_prep_u8_scale_crop: image %d has sizes %dx%d -> %dx%d outside 1..65535"
+                               % (b, H, W, RH, RW))
+        if y0 < 0 or x0 < 0 or y0 + rh > H or x0 + rw > W:
+            raise _l.B200Error("input_prep_u8_scale_crop: the region of image %d lies outside its %dx%d image"
+                               % (b, H, W))
+        for n, nr, start, n_out, lo, ext in ((H, RH, top, OH, y0, rh), (W, RW, left, OW, x0, rw)):
+            s = crop_support(n, nr, start, n_out)
+            if s is not None and (s[0] < lo or s[1] > lo + ext):
+                raise _l.B200Error("input_prep_u8_scale_crop: the region of image %d misses source pixels the crop "
+                                   "window reads" % b)
+
+
+def input_prep_u8_scale_crop(regions, cpad, sc, s2d=False, border=False, out=None):
+    """uint8 region buffer -> bf16 [B, OH, OW, cpad] (or the bordered space-to-depth layout): Resize + CenterCrop with
+    Pillow's bilinear resample of each whole image, and normalisation through sc.lut (a ScaleCropTables)."""
+    _chk(regions, torch.uint8, "regions"); _chk(sc.index, torch.int64, "index"); _chk(sc.geom, torch.int32, "geom")
+    _chk(sc.lut, torch.float32, "lut")
+    if s2d and not border:
+        raise _l.B200Error("input_prep_u8_scale_crop: the space-to-depth layout needs the border (mode 2)")
+    if regions.dim() != 1 or sc.lut.dim() != 2 or sc.lut.shape[1] != 256:
+        raise _l.B200Error("input_prep_u8_scale_crop: regions must be a flat uint8 buffer and lut fp32 [C, 256]")
+    C, (OH, OW), B = sc.lut.shape[0], sc.size, sc.index.shape[0]
+    h_index, h_geom, nbytes = sc.host
+    if nbytes > regions.numel() or tuple(h_index.shape) != tuple(sc.index.shape) \
+            or tuple(h_geom.shape) != tuple(sc.geom.shape):
+        raise _l.B200Error("input_prep_u8_scale_crop: host tables do not describe the device tables and buffer")
+    check_scale_crop_tables(h_index, h_geom, nbytes, C, sc.size)
+    out = _prep_out(B, OH, OW, cpad, s2d, border, regions.device, out)
+    mode = 2 if s2d else 0
+    nbytes_read = int((h_index[:, 1].long() * h_index[:, 2].long()).sum()) * C
+    with _T('input_prep', 0, nbytes_read + 8 * sc.index.numel() + 4 * sc.geom.numel() + 2 * out.numel()):
+        _l.check(_l.load().b200_input_prep_u8_scale_crop(regions.data_ptr(), regions.numel(), sc.index.data_ptr(),
+                                                         sc.geom.data_ptr(), B, C, OH, OW, cpad, mode,
+                                                         sc.lut.data_ptr(), out.data_ptr(), _stream()),
+                 "b200_input_prep_u8_scale_crop")
+    return out
+
+
 def input_prep_u8_aug(x_nhwc_u8, cpad, aug, out=None):
     """uint8 NHWC [N,H,W,C] -> bf16 NHWC [N*D, H, W, cpad]: the D augmented copies of every image (crop, flip, Cutout)
     normalised through aug.lut, row n*D + d = copy d of image n.  With aug.out_hw = (OH, OW) every crop is resized

@@ -21,7 +21,9 @@ utils/mixup.py; on the fused B200 path the input relayout and loss kernels do th
 Augmentation on the device (a loader yielding a utils.augment.DeviceBatch: an AugmentedBatch of data.py
 ``device_augment`` or a ResizedCropBatch of ``device_resized_crop``): on the fused B200 path the stem relayout kernel
 writes the B*D augmented copies from the uint8 data and its draws; every other path trains on the batch's ``apply()``,
-the same fp32 batch.  The meters count B*D samples.
+the same fp32 batch.  The meters count B*D samples.  Evaluation batches of ``device_scale_crop`` (a ScaleCropBatch:
+Resize + CenterCrop) take the same route: with a converted model in eval mode the relayout resamples each image's crop
+window and the eval forward runs on it; every other case evaluates the batch's ``apply()``.
 """
 import logging
 import random
@@ -35,7 +37,7 @@ from torch.nn.utils import clip_grad_norm_
 
 from .lib import B200Error, MIX_CUTMIX, MIX_MIXUP
 from .utils import regularization
-from .utils.augment import DeviceBatch, ResizedCropBatch
+from .utils.augment import DeviceBatch, ResizedCropBatch, ScaleCropBatch
 from .utils.meters import AverageMeter, accuracy
 from .utils.mixup import CutMix, MixUp
 
@@ -81,8 +83,9 @@ def _cuda_prefetch(loader, device, dtype):
     step i computes (the reference issues a blocking copy at the top of every step, trainer.py:116-117).
     The copies land in a ring of three persistent device buffers per (shape, dtype): no caching-allocator traffic per
     step (a fresh 154 MB tensor per batch that is handed across streams made the allocator stall now and then).
-    A DeviceBatch's tensors travel together, in the same slot.  The region buffer of a ResizedCropBatch changes size
-    every step: its slots are keyed on a capacity instead, which grows by at least half when a batch does not fit."""
+    A DeviceBatch's tensors travel together, in the same slot.  The region buffer of a ResizedCropBatch or ScaleCropBatch
+    changes size every step: its slots are keyed on a capacity instead, which grows by at least half when a batch does
+    not fit."""
     copy_stream = torch.cuda.Stream(device=device)
     ring = {}          # shapes and dtypes -> [[x_buf, y_buf, consumed_event or None, (other device tensors)], ...]
     turn = {}
@@ -93,7 +96,7 @@ def _cuda_prefetch(loader, device, dtype):
         host = batch.tensors if batch is not None else (inputs,)
         x, rest = host[0], host[1:]
         x_dtype = x.dtype if x.dtype == torch.uint8 else dtype     # uint8 image batches stay uint8
-        ragged = isinstance(batch, ResizedCropBatch)
+        ragged = isinstance(batch, (ResizedCropBatch, ScaleCropBatch))
         key = (type(batch), None if ragged else tuple(x.shape), x_dtype, tuple(target.shape), target.dtype,
                tuple((tuple(t.shape), t.dtype) for t in rest))
         shape = tuple(x.shape)
@@ -438,6 +441,10 @@ class Trainer(object):
                     and 'cuda' in str(self.device) and self._hooks_static() and self._plain_ce_eps() is not None \
                     and target_batch.dtype == torch.long and target_batch.dim() == 1:
                 aug, inputs_batch = self._device_aug(inputs_batch)
+            elif not training and isinstance(inputs_batch, ScaleCropBatch) and self.b200 is not None \
+                    and not self.model.training and chunk_batch == 1 and not average_output \
+                    and 'cuda' in str(self.device):
+                aug, inputs_batch = self._device_aug(inputs_batch)     # the eval forward reads the uint8 regions
             else:
                 inputs_batch = inputs_batch.apply()     # the same fp32 batch the fused relayout would compute
 
@@ -456,7 +463,7 @@ class Trainer(object):
                 and self._hooks_static() and self._plain_ce_eps() is not None \
                 and target.dtype == torch.long and target.dim() == 1
             mix = self._upload_mix(mixer, inputs) if (mixer is not None and fused) else None
-            if aug is not None and not fused:
+            if aug is not None and training and not fused:
                 raise B200Error('batch augmentation on the device: the fused training step is not available here')
             if training and chunk_batch == 1 and not average_output and (mixer is None or mix is not None):
                 replayed = self.graphed_forward_backward(inputs, target, mix, aug)
@@ -484,7 +491,10 @@ class Trainer(object):
                 inputs = mixer(inputs.clone() if isinstance(mixer, CutMix) else inputs)   # the caller's batch stays intact
             if training:
                 self.optimizer.pre_forward()
-            output = self.model(inputs)
+            if aug is not None:     # evaluation of a ScaleCropBatch: Runtime.forward's eval pass, fed by the relayout
+                output = self.b200.run_forward(inputs, False, False, aug=aug)[0]
+            else:
+                output = self.model(inputs)
             if average_output:
                 if isinstance(output, (list, tuple)):
                     output = [_average_duplicates(o, target) if o is not None else None for o in output]
@@ -587,18 +597,23 @@ class Trainer(object):
 
     # ------------------------------------------------------------------ batch augmentation on the device
     def _device_aug(self, batch):
-        """-> (ops.Aug or ops.Rrc over the batch's draws on the training device and a persistent device LUT of its
-        normalisation -- one per statistics, channel count and device, so that a captured graph keeps reading a live
-        tensor --, the uint8 tensor the relayout reads).  Resized-crop tables are validated on the host here: a graph
-        replay runs the kernel without passing through ops.input_prep_u8_rrc."""
+        """-> (ops.Aug, ops.Rrc or ops.ScaleCropTables over the batch's tables on the device and a persistent device LUT
+        of its normalisation -- one per statistics, channel count and device, so that a captured graph keeps reading a
+        live tensor --, the uint8 tensor the relayout reads).  Resized-crop tables are validated on the host here: a
+        graph replay runs the kernel without passing through ops.input_prep_u8_rrc.  Scale-crop (evaluation) steps are
+        not captured; ops.input_prep_u8_scale_crop validates their tables."""
         from . import ops
         spec = batch.spec
         device = torch.device(self.device)
-        C = batch.channels if isinstance(batch, ResizedCropBatch) else batch.images.shape[-1]
+        C = batch.channels if isinstance(batch, (ResizedCropBatch, ScaleCropBatch)) else batch.images.shape[-1]
         key = (tuple(spec.normalize['mean']), tuple(spec.normalize['std']), C, str(device))
         lut = self._aug_luts.get(key)
         if lut is None:
             lut = self._aug_luts[key] = spec.lut(C).to(device)
+        if isinstance(batch, ScaleCropBatch):
+            sc = ops.ScaleCropTables(batch.index.to(device, non_blocking=True), batch.geom.to(device, non_blocking=True),
+                                     lut, spec.size, batch.host + (batch.nbytes,))
+            return sc, batch.regions
         if isinstance(batch, ResizedCropBatch):
             ops.check_rrc_tables(batch.host[0], batch.host[1], batch.nbytes, C, spec.duplicates)
             rrc = ops.Rrc(batch.index.to(device, non_blocking=True), batch.draws.to(device, non_blocking=True), lut,

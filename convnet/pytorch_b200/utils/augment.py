@@ -339,3 +339,159 @@ class ResizedCropCollate(object):
         flat = torch.cat([r.reshape(-1) for r in regions])
         return ResizedCropBatch(flat, index, draws, self.spec, regions[0].shape[2]), \
             target.repeat_interleave(self.spec.duplicates)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Resize + CenterCrop on the device (the ImageNet evaluation transform, the reference's scale_crop, preprocess.py:20-41,
+# one crop).  The loader workers decode; each image ships only its support region -- the source pixels the crop
+# window's filter taps touch -- in one flat uint8 buffer, and the stem relayout kernel resamples the window of the
+# whole image's resize and normalises it (ops.input_prep_u8_scale_crop).
+
+def resample_taps(n_in, n_out, i):
+    """[first, end) source indices of output index ``i`` of Pillow's BILINEAR n_in -> n_out resample (ImagingResample's
+    bounds, in the double arithmetic the relayout kernel uses)."""
+    scale = n_in / n_out
+    support = scale if scale >= 1.0 else 1.0
+    center = (i + 0.5) * scale
+    return max(int(center - support + 0.5), 0), min(int(center + support + 0.5), n_in)
+
+
+def crop_support(n_in, n_resized, start, n_out):
+    """[first, end) source indices that output indices start .. start + n_out - 1 of an n_in -> n_resized resample read
+    (indices outside [0, n_resized) are padding and read nothing), or None when every index is padding."""
+    a, b = max(start, 0), min(start + n_out, n_resized)
+    if a >= b:
+        return None
+    return resample_taps(n_in, n_resized, a)[0], resample_taps(n_in, n_resized, b - 1)[1]
+
+
+class ScaleCrop(object):
+    """Resize(scale_size) (bilinear; skipped when scale_size == input_size) + CenterCrop(input_size) + ToTensor +
+    Normalize (``normalize``: {'mean', 'std'}): the reference's scale_crop."""
+
+    margin = 1      # source pixels shipped beyond the taps on each side (clamped to the image)
+
+    def __init__(self, input_size, scale_size=None, normalize=None):
+        self.input_size = int(input_size)
+        self.size = (self.input_size, self.input_size)
+        self.scale_size = int(scale_size) if scale_size is not None else int(self.input_size * 8 / 7)
+        self.normalize = normalize or _IMAGE_STATS
+        if min(self.size) < 1 or self.scale_size < 1:
+            raise ValueError('ScaleCrop: input_size and scale_size must be >= 1')
+        self._luts = {}
+
+    def lut(self, C):
+        t = self._luts.get(C)
+        if t is None:
+            t = self._luts[C] = normalize_lut(self.normalize, C)
+        return t
+
+    def resized_size(self, h, w):
+        """(RH, RW) of Resize(scale_size) on an h x w image: torchvision's _compute_resized_output_size (short side to
+        scale_size, long side int(scale_size * long / short)); (h, w) when scale_size == input_size (no Resize)."""
+        if self.scale_size == self.input_size:
+            return h, w
+        short, long = (w, h) if w <= h else (h, w)
+        new_short, new_long = self.scale_size, int(self.scale_size * long / short)
+        return (new_long, new_short) if w <= h else (new_short, new_long)
+
+    def geometry(self, h, w):
+        """int32 [8] {y0, x0, H, W, RH, RW, top, left} and the support region's (h, w) of an h x w image: the crop
+        origin in the resized image as CenterCrop computes it (int(round((RH - th) / 2.0)), or minus the top / left
+        padding when the crop is larger), the region the window's taps touch plus ``margin``."""
+        th, tw = self.size
+        rh, rw = self.resized_size(h, w)
+        top = -((th - rh) // 2) if th > rh else int(round((rh - th) / 2.0))
+        left = -((tw - rw) // 2) if tw > rw else int(round((rw - tw) / 2.0))
+        spans = []
+        for n, nr, start, n_out in ((h, rh, top, th), (w, rw, left, tw)):
+            s = crop_support(n, nr, start, n_out)
+            lo, hi = (0, 1) if s is None else (max(s[0] - self.margin, 0), min(s[1] + self.margin, n))
+            spans.append((lo, hi))
+        (y0, y1), (x0, x1) = spans
+        return torch.tensor([y0, x0, h, w, rh, rw, top, left], dtype=torch.int32), (y1 - y0, x1 - x0)
+
+    def __call__(self, img):
+        """PIL image -> (uint8 HWC support region, int32 [8] geometry): the loader's per-image work."""
+        w, h = img.size
+        geom, (rh, rw) = self.geometry(h, w)
+        y0, x0 = int(geom[0]), int(geom[1])
+        a = np.asarray(img)
+        region = torch.from_numpy(np.array(a[y0:y0 + rh, x0:x0 + rw].reshape(rh, rw, -1), copy=True))
+        return region, geom
+
+    def apply(self, regions, index, geom, C):
+        """-> fp32 NCHW [B, C, OH, OW]: each region pasted at (y0, x0) into a zero image of the original size, then
+        torchvision's own resize / center_crop / to_tensor / normalize on PIL images.  Pixels outside the support region
+        carry zero weight, so this is the reference's output (its arithmetic by construction).  Three channels make one
+        RGB image; any other count is resampled channel by channel (the filter does not mix them)."""
+        import torchvision.transforms.functional as F
+        from PIL import Image
+        from torchvision.transforms import InterpolationMode
+        regions = regions.cpu()
+        mean, std = list(self.normalize['mean'][:C]), list(self.normalize['std'][:C])
+        if len(mean) < C or len(std) < C:
+            raise ValueError('normalisation statistics for fewer than %d channels' % C)
+        out = []
+        for b in range(index.shape[0]):
+            off, h, w = (int(v) for v in index[b])
+            y0, x0, H, W = (int(v) for v in geom[b][:4])
+            full = np.zeros((H, W, C), np.uint8)
+            full[y0:y0 + h, x0:x0 + w] = regions[off:off + h * w * C].reshape(h, w, C).numpy()
+            planes = [Image.fromarray(full, 'RGB')] if C == 3 else \
+                [Image.fromarray(np.ascontiguousarray(full[:, :, c]), 'L') for c in range(C)]
+            chans = []
+            for img in planes:
+                if self.scale_size != self.input_size:
+                    img = F.resize(img, self.scale_size, InterpolationMode.BILINEAR)
+                chans.append(F.to_tensor(F.center_crop(img, list(self.size))))
+            out.append(F.normalize(torch.cat(chans), mean, std))
+        return torch.stack(out)
+
+
+class ScaleCropBatch(DeviceBatch):
+    """B images' support regions in one flat uint8 buffer ``regions`` (HWC, ``channels`` per pixel, the first ``nbytes``
+    bytes in use), ``index`` int64 [B, 3] {byte offset, h, w} and ``geom`` int32 [B, 8] {y0, x0, H, W, RH, RW, top,
+    left} of ``spec`` (a ScaleCrop).  Stands for B rows.  ``host`` keeps the CPU index and geometry once the tensors
+    have been staged on a device (their validation needs no device read-back)."""
+    __slots__ = ('regions', 'index', 'geom', 'spec', 'channels', 'nbytes', 'host')
+
+    def __init__(self, regions, index, geom, spec, channels, nbytes=None, host=None):
+        self.regions, self.index, self.geom, self.spec = regions, index, geom, spec
+        self.channels = int(channels)
+        self.nbytes = int(regions.numel() if nbytes is None else nbytes)
+        self.host = host if host is not None else (index, geom)
+
+    @property
+    def rows(self):
+        return self.index.shape[0]
+
+    def apply(self):
+        """-> fp32 NCHW [B, C, OH, OW] on the host."""
+        return self.spec.apply(self.regions[:self.nbytes], self.host[0], self.host[1], self.channels)
+
+    @property
+    def tensors(self):
+        return (self.regions, self.index, self.geom)
+
+    def replace(self, tensors):
+        return ScaleCropBatch(tensors[0], tensors[1], tensors[2], self.spec, self.channels, self.nbytes, self.host)
+
+
+class ScaleCropCollate(object):
+    """DataLoader ``collate_fn`` of a scale-crop loader: packs the (region, geometry) samples made by ScaleCrop in the
+    workers into one ScaleCropBatch.  -> (batch, target)."""
+
+    def __init__(self, spec):
+        self.spec = spec
+
+    def __call__(self, batch):
+        regions = [r for (r, _), _ in batch]
+        offsets = [0]
+        for r in regions[:-1]:
+            offsets.append(offsets[-1] + r.numel())
+        index = torch.tensor([[o, r.shape[0], r.shape[1]] for o, r in zip(offsets, regions)], dtype=torch.int64)
+        geom = torch.stack([g for (_, g), _ in batch])
+        target = torch.as_tensor([int(t) for _, t in batch], dtype=torch.long)
+        flat = torch.cat([r.reshape(-1) for r in regions])
+        return ScaleCropBatch(flat, index, geom, self.spec, regions[0].shape[2]), target

@@ -260,6 +260,20 @@ int b200_input_prep_u8_aug_resize(const uint8_t* x_nhwc, int N, int D, int C, in
 int b200_input_prep_u8_rrc(const uint8_t* regions, long long region_bytes, const long long* index, const int* draws,
                            int B, int D, int C, int OH, int OW, int Cpad, int mode, const float* lut, void* out,
                            b200_stream_t stream);
+/* Resize(scale) + CenterCrop(OH x OW) + ToTensor + Normalize of the ImageNet evaluation transform (preprocess.py:20-41,
+ * one crop) fused into the stem relayout.  regions: one DEVICE uint8 buffer of region_bytes bytes holding B images'
+ * support regions (HWC); index (DEVICE int64 [B][3]) = {byte offset, h, w} of each; geom (DEVICE int32 [B][8]) =
+ * {y0, x0, H, W, RH, RW, top, left}: the region's origin in the H x W image, the resized size RH x RW and the crop's
+ * origin in the resized image.  Output row n, pixel (o, x) is pixel (top + o, left + x) of image n resized to RH x RW
+ * exactly as Pillow's 8-bit BILINEAR resize of the WHOLE image does (image pixel (y, x) is read at (y - y0, x - x0) of
+ * the region), or uint8 0 outside the resized image (CenterCrop's padding); then v = lut[c][u] (DEVICE fp32 [C][256])
+ * rounded once to bf16.  RH == H, RW == W is the identity (no Resize).  mode 0: out [B][OH][OW][Cpad] (Cpad >= C);
+ * mode 2: the padded space-to-depth layout of b200_input_prep (even OH, OW; Cpad >= 4C).  C <= 4, OW <= 512,
+ * B <= 65535, any downscale factor.  Any table values are memory-safe (every read is clamped to its region and to
+ * region_bytes); the grid depends on (B, OH) only, so a captured graph follows new tables. */
+int b200_input_prep_u8_scale_crop(const uint8_t* regions, long long region_bytes, const long long* index,
+                                  const int* geom, int B, int C, int OH, int OW, int Cpad, int mode, const float* lut,
+                                  void* out, b200_stream_t stream);
 /* bf16 [K][T][C] -> bf16 [C][T][K] (dgrad weight layout), multi-tensor: n tensors described by
  * device arrays. */
 int b200_weight_transpose(const void* src, void* dst, int K, int T, int C, b200_stream_t stream);
