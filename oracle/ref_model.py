@@ -247,6 +247,92 @@ def forward(sd, x, training=True, buffers_out=None, quant=False, dropout_p=0.0):
     return F.linear(x, sd['fc.weight'], sd['fc.bias'])
 
 
+def _leaves(sd, keys, dtype, device):
+    """fp64 (``dtype``) copies of the state-dict entries ``keys`` on ``device``; the parameters among them require grad"""
+    local = {}
+    for k in keys:
+        v = sd[k].to(device)
+        if v.is_floating_point():
+            v = v.to(dtype)
+            if not (k.endswith('running_mean') or k.endswith('running_var')):
+                v = v.detach().clone().requires_grad_(True)
+        local[k] = v
+    return local
+
+
+def _vjp(y, dy, x, local):
+    params = [k for k, v in local.items() if torch.is_tensor(v) and v.requires_grad]
+    inputs = ([x] if x is not None else []) + [local[k] for k in params]
+    grads = torch.autograd.grad(y, inputs, dy.to(y.dtype))
+    dx = grads[0] if x is not None else None
+    return dx.detach() if dx is not None else None, dict(zip(params, (g.detach() for g in grads[len(inputs) - len(params):])))
+
+
+def resnet_block_vjp(sd, prefix, x, dy, stride, quant=True, block=None, training=True, dtype=torch.float64):
+    """Local reference of one residual block ``prefix`` (e.g. 'layer2.0') of a ResNet-family ``state_dict``: the block
+    run in ``dtype`` on the device of ``x`` (NCHW) with the storage roundings of ``quant``, and the vector-Jacobian
+    products of ``dy`` (the gradient arriving at its output; None: forward only).  ``block``: the block function (signature of ``_basic``;
+    default ``_basic`` / ``_bottleneck`` by the state dict) -- the L1 and dropout restatements plug in here.  A shared
+    squeeze-excitation gate appears under its canonical (first block's) names; the gradient of a stage's gate is the sum
+    of its blocks' VJPs.  Returns {'y', 'dx', 'grads': {name: grad}, 'bufs': {name: updated running buffer}}."""
+    if block is None:
+        block = _bottleneck if (prefix + '.conv3.weight') in sd else _basic
+    se = _se_canon(prefix + '.residual_block.transform.0.weight')[:-len('transform.0.weight')]
+    keys = [k for k in sd if k.startswith(prefix + '.') and not k.startswith(prefix + '.residual_block.')]
+    keys += [k for k in sd if k.startswith(se)] if se.endswith('residual_block.') else []
+    local = _leaves(sd, keys, dtype, x.device)
+    xx = x.to(dtype).requires_grad_(True)
+    bufs = {}
+    y = block(xx, local, prefix, stride, training, bufs, quant)
+    dx, grads = _vjp(y, dy, xx, local) if dy is not None else (None, {})
+    return {'y': y.detach(), 'dx': dx, 'grads': grads, 'bufs': {k: v.detach() for k, v in bufs.items()}}
+
+
+def resnet_stem_vjp(sd, x, dy, quant=True, bn=None, dtype=torch.float64):
+    """Local reference of the ResNet stem on its relayouted input ``x`` (NCHW, the bf16 values the convolution reads):
+    conv1 -> BN -> ReLU (-> 3x3/s2 max-pool for the 7x7 stem), with the VJPs of ``dy`` (None: forward only).  ``bn``: the BatchNorm function
+    (signature of ``_bn`` without ``quant``; default ``_bn``).  Returns {'y', 'grads', 'bufs'}."""
+    if bn is None:
+        bn = lambda t, sd_, p, training, bufs: _bn(t, sd_, p, training, bufs, quant)  # noqa: E731
+    local = _leaves(sd, [k for k in sd if k.startswith('conv1.') or k.startswith('bn1.')], dtype, x.device)
+    bufs = {}
+    imagenet = local['conv1.weight'].shape[-1] == 7
+    z = _conv(x.to(dtype), local, 'conv1', 2 if imagenet else 1, 3 if imagenet else 1, quant)
+    y = _q(F.relu(bn(z, local, 'bn1', True, bufs)), quant)
+    if imagenet:
+        y = F.max_pool2d(y, 3, 2, 1)
+    _, grads = _vjp(y, dy, None, local) if dy is not None else (None, {})
+    return {'y': y.detach(), 'grads': grads, 'bufs': {k: v.detach() for k, v in bufs.items()}}
+
+
+def resnet_head_vjp(sd, h, target, smooth_eps=0.0, soft=None, upstream=1.0, quant=True, dtype=torch.float64):
+    """Local reference of the classifier head on the last block's output ``h`` (NCHW): global average pool -> fc ->
+    mean cross-entropy (label smoothing ``smooth_eps``, or the soft MixUp / CutMix target of ``soft`` = (t2, lam):
+    lam * onehot(target) + (1 - lam) * onehot(t2)), differentiated with the upstream gradient ``upstream``.  The
+    gradient of the logits is stored in bf16 before the classifier's backward reads it.  Returns {'logits', 'loss',
+    'top1', 'top5' (percent of rows whose target is among the 1 / 5 largest logits), 'dlogits', 'grads', 'dh'}."""
+    w, b = sd['fc.weight'].to(h.device, dtype), sd['fc.bias'].to(h.device, dtype)
+    feat = _q(h.to(dtype).mean((2, 3)), quant)
+    logits = (feat @ w.t() + b).detach().requires_grad_(True)
+    n_cls = logits.shape[1]
+    if soft is None:
+        loss = cross_entropy(logits, target, smooth_eps)
+    else:
+        lam = float(soft[1])
+        q = lam * F.one_hot(target, n_cls).to(dtype) + (1.0 - lam) * F.one_hot(soft[0], n_cls).to(dtype)
+        loss = (-(q * F.log_softmax(logits, dim=-1)).sum(-1)).mean()
+    (dl,) = torch.autograd.grad(loss, [logits])
+    dl = _q(dl * upstream, quant)
+    dfeat = _q(dl @ w, quant)
+    HW = h.shape[2] * h.shape[3]
+    dh = (dfeat / HW)[:, :, None, None].expand(h.shape)
+    picked = logits.gather(1, target.view(-1, 1))
+    above = (logits > picked).sum(1)        # a row counts when fewer than k logits lie strictly above its target's
+    return {'logits': logits.detach(), 'loss': loss.detach(), 'top1': float((above < 1).double().mean()) * 100,
+            'top5': float((above < 5).double().mean()) * 100, 'dlogits': dl,
+            'grads': {'fc.weight': dl.t() @ feat, 'fc.bias': dl.sum(0)}, 'dh': _q(dh, quant)}
+
+
 def cross_entropy(logits, target, smooth_eps=0.0):
     """mean over the batch of -((1-eps-eps/C) lsm[t] + (eps/C) sum_c lsm[c])  (utils/cross_entropy.py:48-52);
     with eps = 0 this is F.cross_entropy (:20-24)."""
