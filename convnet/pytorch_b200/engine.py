@@ -287,6 +287,10 @@ class Runtime(object):
         self.sync_bn_world = 1
         self._fused_dl = None        # bf16 dlogits handed from _FusedCE.backward to run_backward (side channel)
         self._ce_dummy = torch.zeros((), device=device, dtype=torch.float32)
+        # activation checkpointing: while a checkpointed segment runs forward, _conv_and_coeffs records each unit's
+        # coefficient vectors here; while it is recomputed in the backward pass, it hands them back in the same order
+        self._coeffs_record = None
+        self._coeffs_replay = None
         self._build()
         self._setup_transposes()
 
@@ -451,6 +455,13 @@ class Runtime(object):
         else:
             u.z = ops.conv_fprop(x, w16, u.desc)
             self._bn_coeffs(u, training)
+        if self._coeffs_record is not None:
+            self._coeffs_record.append((u.mean, u.invstd, u.scale, u.shift, u.sums, u.sign_sum))
+        elif self._coeffs_replay is not None:
+            # recompute of a checkpointed segment: the statistics just computed went to scratch (their running-
+            # statistics update is the reference's second one); z is bitwise the forward's, and y is applied with the
+            # forward's coefficients so that it and every gradient are too
+            u.mean, u.invstd, u.scale, u.shift, u.sums, u.sign_sum = self._coeffs_replay.pop(0)
 
     def _eval_coeffs(self, bn, scale, shift):
         m = bn.mod
@@ -807,6 +818,7 @@ class ResNetRuntime(Runtime):
     def _build(self):
         from .models.resnet import BasicBlock, Bottleneck
         from .models.modules.lp_norm import L1BatchNorm2d
+        from .models.modules.checkpoint import CheckpointModule
         m, a = self.model, self.arena
         self.imagenet_stem = m.conv1.kernel_size == (7, 7)
         if self.imagenet_stem:
@@ -821,11 +833,18 @@ class ResNetRuntime(Runtime):
         self.stem_bn = _BN(a, m.bn1)
         self.has_maxpool = isinstance(m.maxpool, nn.MaxPool2d)
         self.blocks = []
+        # checkpoint_segments: [start, end) ranges of self.blocks whose activations the forward pass does not keep;
+        # the backward pass recomputes each range just before it needs it
+        self.segments = []
         n_drop = 0
         for lname in ('layer1', 'layer2', 'layer3', 'layer4'):
             layer = getattr(m, lname)
             if isinstance(layer, nn.Identity):
                 continue
+            if isinstance(layer, CheckpointModule):
+                base = len(self.blocks)
+                self.segments += [(base + a, base + b) for a, b in layer.segments()]
+                layer = layer.module
             for blk in layer:
                 p = float(blk.dropout.p) if isinstance(blk.dropout, nn.Dropout) else 0.0
                 if p != 0 and not isinstance(blk, BasicBlock):
@@ -968,21 +987,63 @@ class ResNetRuntime(Runtime):
                 self.dropout_key.random_(-2 ** 63, None)         # the full 64-bit range
         h, stem = self._stem_fwd(x, training, mix, aug)
         saved = []
-        for spec in self.blocks:
-            h, s = self._block_fwd(spec, h, training)
+        # eval and tapeless training forwards (calibrate_bn) keep nothing to recompute: only a backward pass needs it
+        ckpt = {a: b for a, b in self.segments} if (training and want_tape) else {}
+        i = 0
+        while i < len(self.blocks):
+            if i in ckpt:
+                # checkpointed segment: keep its input and each unit's coefficients; z, y and the masks are dropped
+                seg_in, coeffs = h, []
+                try:
+                    for spec in self.blocks[i:ckpt[i]]:
+                        self._coeffs_record = []
+                        h, _ = self._block_fwd(spec, h, training)
+                        coeffs.append(self._coeffs_record)
+                finally:
+                    self._coeffs_record = None
+                saved.append({'segment': (i, ckpt[i]), 'x': seg_in, 'coeffs': coeffs})
+                saved += [None] * (ckpt[i] - i - 1)
+                i = ckpt[i]
+                continue
+            h, s = self._block_fwd(self.blocks[i], h, training)
             saved.append(s if want_tape else None)
+            i += 1
         out, head = self._head_fwd(h, training, want_tape)
         tape = {'stem': stem, 'blocks': saved, 'head': head} if want_tape else None
         return out, tape
+
+    def _recompute(self, seg):
+        """the block tapes of a checkpointed segment, rebuilt from its input by the forward's own launches"""
+        h, tapes = seg['x'], []
+        a, b = seg['segment']
+        try:
+            for spec, coeffs in zip(self.blocks[a:b], seg['coeffs']):
+                self._coeffs_replay = list(coeffs)
+                h, s = self._block_fwd(spec, h, True)
+                tapes.append(s)
+        finally:
+            self._coeffs_replay = None
+        return tapes
 
     def run_backward(self, tape, dlogits, dl_bf16=None):
         self._transpose_weights()
         self._buckets_begin()
         d = self._head_bwd(tape['head'], dlogits, dl_bf16)
-        for spec, saved in zip(reversed(self.blocks), reversed(tape['blocks'])):
-            d = self._block_bwd(spec, saved, d)
+        blocks = list(tape['blocks'])
+        seg_start = {s['segment'][1] - 1: i for i, s in enumerate(blocks) if s is not None and 'segment' in s}
+        for i in range(len(self.blocks) - 1, -1, -1):
+            spec = self.blocks[i]
+            if i in seg_start:
+                a = seg_start[i]
+                blocks[a:i + 1] = self._recompute(blocks[a])
+            d = self._block_bwd(spec, blocks[i], d)
+            blocks[i] = None
             convs = spec['convs'] + ([spec['down'][0]] if spec['down'] is not None else [])
             self._bucket_point(self._spec_lo(convs))
+            if i in seg_start.values():
+                # end of a recomputed segment's backward: the side-stream wgrads still read its tensors; joining here
+                # lets the allocator hand them to the next segment instead of keeping every segment to the end
+                self._wgrad_join()
         self._stem_bwd(tape['stem'], d)
         self._wgrad_join()
         self._buckets_end()
@@ -1155,6 +1216,9 @@ def enable_sync_batchnorm(model, process_group=None):
     from .models.modules.lp_norm import L1BatchNorm2d
     if any(isinstance(m, L1BatchNorm2d) for m in model.modules()):
         raise NotImplementedError('SyncBatchNorm is not implemented for L1 BatchNorm (bn_norm=\'L1\')')
+    if getattr(rt, 'segments', None):
+        raise NotImplementedError('SyncBatchNorm is not implemented with checkpoint_segments: the recompute would '
+                                  'all-reduce every checkpointed layer\'s statistics a second time')
     rt.sync_bn_group = process_group
     rt.sync_bn_world = dist.get_world_size(process_group)
     return model

@@ -178,6 +178,9 @@ def main_worker(args):
         from .models.modules.lp_norm import L1BatchNorm2d
         if any(isinstance(m, L1BatchNorm2d) for m in model.modules()):
             raise NotImplementedError('--sync-bn is not implemented for L1 BatchNorm (bn_norm=\'L1\')')
+        from .models.modules.checkpoint import CheckpointModule
+        if any(isinstance(m, CheckpointModule) for m in model.modules()):
+            raise NotImplementedError('--sync-bn is not implemented with checkpoint_segments')
     if args.sync_bn and not use_b200:
         model = nn.SyncBatchNorm.convert_sync_batchnorm(model)
     logging.info('created model with configuration: %s', model_config)

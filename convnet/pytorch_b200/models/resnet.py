@@ -15,6 +15,7 @@ import math
 import torch
 import torch.nn as nn
 
+from .modules.checkpoint import CheckpointModule
 from .modules.lp_norm import L1BatchNorm2d
 
 __all__ = ['resnet', 'resnet_se']
@@ -172,8 +173,6 @@ class ResNet_imagenet(ResNet):
                  mixup=False, epochs=90, base_devices=4, base_device_batch=64, base_duplicates=1,
                  base_image_size=224, mix_size_regime='D+', norm_layer=nn.BatchNorm2d):
         super(ResNet_imagenet, self).__init__()
-        if checkpoint_segments:
-            raise NotImplementedError('activation checkpointing is outside the B200 hot path (SURVEY 2, #23)')
         self.norm_layer = norm_layer
         self.inplanes = inplanes
         self.conv1 = nn.Conv2d(3, inplanes, kernel_size=7, stride=2, padding=3, bias=False)
@@ -181,9 +180,11 @@ class ResNet_imagenet(ResNet):
         self.relu = nn.ReLU(inplace=True)
         self.maxpool = nn.MaxPool2d(kernel_size=3, stride=2, padding=1)
         for i, (w, n, g) in enumerate(zip(width, layers, groups)):
-            setattr(self, 'layer%d' % (i + 1),
-                    self._make_layer(block=block, planes=w, blocks=n, expansion=expansion,
-                                     stride=1 if i == 0 else 2, residual_block=residual_block, groups=g, mixup=mixup))
+            layer = self._make_layer(block=block, planes=w, blocks=n, expansion=expansion,
+                                     stride=1 if i == 0 else 2, residual_block=residual_block, groups=g, mixup=mixup)
+            if checkpoint_segments > 0:     # recompute in the backward pass (models/resnet.py:236-239)
+                layer = CheckpointModule(layer, min(checkpoint_segments, n))
+            setattr(self, 'layer%d' % (i + 1), layer)
         self.avgpool = nn.AdaptiveAvgPool2d(1)
         self.fc = nn.Linear(width[-1] * expansion, num_classes)
         init_model(self)
