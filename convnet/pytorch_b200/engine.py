@@ -342,7 +342,7 @@ class Runtime(object):
                                 % (x.dtype, tuple(x.shape)))
             OH, OW = aug.size
             return x, (lambda t, cpad, **kw: ops.input_prep_u8_rrc(t, cpad, aug, **kw)), \
-                (aug.draws.shape[0], aug.lut.shape[0], OH, OW)
+                (aug.rows, aug.lut.shape[0], OH, OW)
         if isinstance(aug, ops.ScaleCropTables):
             # x is the flat uint8 region buffer; the relayout resamples each image's centre-crop window (evaluation)
             if mix is not None:
@@ -367,7 +367,7 @@ class Runtime(object):
                                         '(the space-to-depth stem layouts are not supported)')
                     return ops.input_prep_u8_aug(t, cpad, aug, **kw)
                 OH, OW = aug.out_hw or (H, W)       # the stem sees the resized copies, not the uint8 images' size
-                return x.contiguous(), prep_aug, (N * aug.duplicates, C, OH, OW)
+                return x.contiguous(), prep_aug, (aug.rows, C, OH, OW)
             mean = getattr(self.model, 'input_mean', self.input_mean)
             std = getattr(self.model, 'input_std', self.input_std)
             return x.contiguous(), (lambda t, cpad, **kw: ops.input_prep_u8(t, cpad, mean[:C], std[:C], mix=mix, **kw)), \
@@ -700,7 +700,7 @@ class Runtime(object):
     def run_backward(self, tape, dlogits, dl_bf16=None):
         raise NotImplementedError
 
-    def train_step(self, x, target, smooth_eps=0.0, upstream=None, mix=None, aug=None):
+    def train_step(self, x, target, smooth_eps=0.0, upstream=None, mix=None, aug=None, reduce=True):
         """forward + mean softmax cross-entropy (label smoothing ``smooth_eps``) + backward of one batch as a straight
         sequence of library calls -- no autograd graph, no autograd worker thread, no ATen kernels: what Trainer runs
         (and captures into a CUDA graph) when the criterion is the plain CrossEntropyLoss of the reference
@@ -711,12 +711,13 @@ class Runtime(object):
         (1-lam)*onehot(target[perm]); ``smooth_eps`` is then ignored, as the reference's cross_entropy ignores it for
         soft targets (utils/cross_entropy.py:38-54).  Top-1 / top-5 still count against ``target``.
         ``aug`` (ops.Aug): x is the uint8 NHWC batch of B images and the step trains on its B*D augmented copies
-        (row b*D + d); ``target`` then has B*D entries.
+        (row b*D + d); ``target`` then has B*D entries, or aug.window's n.
+        ``reduce``: False keeps the data-parallel gradient buckets (grad_bucket_hook) out of this backward pass -- a
+        chunk of an accumulated batch whose summed gradients are all-reduced once, after its last chunk.
         Returns (logits, stats): logits detached, stats = fp32[3] device tensor {mean loss, top-1 %, top-5 %}."""
         if x.device.type != 'cuda':
             raise B200Error('B200 runtime needs CUDA inputs (no CPU fallback); got %s' % x.device)
-        n_rows = aug.draws.shape[0] if isinstance(aug, ops.Rrc) else \
-            x.shape[0] * (aug.duplicates if aug is not None else 1)
+        n_rows = aug.rows if aug is not None else x.shape[0]
         if target.dtype != torch.int64 or target.dim() != 1 or target.shape[0] != n_rows or not target.is_cuda:
             raise B200Error('train_step: target must be a CUDA int64 vector with one class index per sample')
         logits, tape = self.run_forward(x, True, True, mix=mix, aug=aug)
@@ -736,7 +737,13 @@ class Runtime(object):
                            grad_scale_dev=up)
         self.arena.rebind_grads()
         self.arena.grads_zero = False
-        self.run_backward(tape, logits, dl_bf16=dl)
+        hook = self.grad_bucket_hook
+        if not reduce:
+            self.grad_bucket_hook = None
+        try:
+            self.run_backward(tape, logits, dl_bf16=dl)
+        finally:
+            self.grad_bucket_hook = hook
         return logits, stats
 
 

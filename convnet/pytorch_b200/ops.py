@@ -564,28 +564,43 @@ class Aug(object):
     """Device-side draws of one batch-augmentation step (utils/augment.py): ``params`` int16 [N*D, 3 + 4*holes] rows
     {oy, ox, flip, y1, y2, x1, x2, ...}, ``lut`` fp32 [C, 256] (ToTensor + Normalize of each uint8 value), ``duplicates``
     D, ``pad`` the crop padding, ``out_hw`` (OH, OW) when the crop is resized (the Mix&Match CIFAR regimes; None: the
-    copies keep the images' size).  The kernel reads params at run time, so a captured graph follows new draws in place."""
-    __slots__ = ('params', 'lut', 'duplicates', 'pad', 'out_hw')
+    copies keep the images' size).  The kernel reads params at run time, so a captured graph follows new draws in place.
+    ``window`` (p, n): the step trains on rows [p, p + n) of these images' copies (a chunk of a larger batch, see
+    row_range); None: on all of them."""
+    __slots__ = ('params', 'lut', 'duplicates', 'pad', 'out_hw', 'window')
 
-    def __init__(self, params, lut, duplicates, pad, out_hw=None):
+    def __init__(self, params, lut, duplicates, pad, out_hw=None, window=None):
         self.params, self.lut, self.duplicates, self.pad = params, lut, int(duplicates), int(pad)
         self.out_hw = (int(out_hw[0]), int(out_hw[1])) if out_hw is not None else None
+        self.window = window
 
     @property
     def holes(self):
         return (self.params.shape[-1] - 3) // 4
 
     @property
+    def rows(self):
+        return self.window[1] if self.window is not None else self.params.shape[0]
+
+    @property
     def key(self):
         """what a captured step depends on besides the input's shape (the draws are refreshed in place)"""
-        return ('aug', tuple(self.params.shape), self.duplicates, self.pad, self.lut.data_ptr(), self.out_hw)
+        return ('aug', tuple(self.params.shape), self.duplicates, self.pad, self.lut.data_ptr(), self.out_hw,
+                self.window)
 
     @property
     def tables(self):
         return (self.params,)
 
     def with_tables(self, tables):
-        return Aug(tables[0], self.lut, self.duplicates, self.pad, self.out_hw)
+        return Aug(tables[0], self.lut, self.duplicates, self.pad, self.out_hw, self.window)
+
+    def row_range(self, r0, r1):
+        """-> (Aug, b0, b1): rows [r0, r1) of the B*D copies as a step over images [b0, b1) (x_nhwc[b0:b1]), whose
+        relayout computes the copies of those whole images and hands on the window of the chunk's rows."""
+        b0, b1, p = _image_range(r0, r1, self.duplicates)
+        D = self.duplicates
+        return Aug(self.params[b0 * D:b1 * D], self.lut, D, self.pad, self.out_hw, (p, r1 - r0)), b0, b1
 
 
 class Rrc(object):
@@ -593,23 +608,57 @@ class Rrc(object):
     offset, h, w} of each image's region in the uint8 region buffer, ``draws`` int32 [B*D, 5] {y, x, h, w, flip} of each
     copy's crop box inside its region, ``lut`` fp32 [C, 256], ``size`` (OH, OW).  ``host`` holds CPU copies of index and
     draws plus the number of region bytes in use: input_prep_u8_rrc validates them before any launch, without a device
-    read-back.  The kernel reads the tables at run time, so a captured graph follows new values in place."""
-    __slots__ = ('index', 'draws', 'lut', 'duplicates', 'size', 'host')
+    read-back.  The kernel reads the tables at run time, so a captured graph follows new values in place.
+    ``window`` (p, n): as for Aug."""
+    __slots__ = ('index', 'draws', 'lut', 'duplicates', 'size', 'host', 'window')
 
-    def __init__(self, index, draws, lut, duplicates, size, host):
+    def __init__(self, index, draws, lut, duplicates, size, host, window=None):
         self.index, self.draws, self.lut, self.duplicates = index, draws, lut, int(duplicates)
         self.size, self.host = (int(size[0]), int(size[1])), host
+        self.window = window
+
+    @property
+    def rows(self):
+        return self.window[1] if self.window is not None else self.draws.shape[0]
 
     @property
     def key(self):
-        return ('rrc', tuple(self.index.shape), self.duplicates, self.size, self.lut.data_ptr())
+        return ('rrc', tuple(self.index.shape), self.duplicates, self.size, self.lut.data_ptr(), self.window)
 
     @property
     def tables(self):
         return (self.index, self.draws)
 
     def with_tables(self, tables):
-        return Rrc(tables[0], tables[1], self.lut, self.duplicates, self.size, self.host)
+        return Rrc(tables[0], tables[1], self.lut, self.duplicates, self.size, self.host, self.window)
+
+    def row_range(self, r0, r1):
+        """-> (Rrc, b0, b1): rows [r0, r1) of the B*D crops as a step over the regions of images [b0, b1) (the region
+        buffer is shared: the index holds absolute offsets); see Aug.row_range."""
+        b0, b1, p = _image_range(r0, r1, self.duplicates)
+        D = self.duplicates
+        h_index, h_draws, nbytes = self.host
+        return Rrc(self.index[b0:b1], self.draws[b0 * D:b1 * D], self.lut, D, self.size,
+                   (h_index[b0:b1], h_draws[b0 * D:b1 * D], nbytes), (p, r1 - r0)), b0, b1
+
+
+def chunk_rows(rows, chunks):
+    """[(r0, r1), ...]: the row ranges of torch.chunk(chunks) over ``rows`` rows -- ceil(rows / chunks) rows each, the
+    last one fewer, and fewer than ``chunks`` ranges when the rows run out first."""
+    if rows < 1 or chunks < 1:
+        raise ValueError('chunk_rows: rows and chunks must be >= 1; got %d, %d' % (rows, chunks))
+    step = -(-rows // chunks)
+    return [(r, min(r + step, rows)) for r in range(0, rows, step)]
+
+
+def _image_range(r0, r1, D):
+    """rows [r0, r1) of a batch whose image b owns rows [b*D, (b+1)*D) -> (b0, b1, p): the images [b0, b1) that cover
+    them and the offset p of row r0 in their rows.  A chunk boundary may split one image's copies: both chunks then
+    compute that image's D copies and each keeps its own (at most 2 (D - 1) extra rows per chunk)."""
+    if not 0 <= r0 < r1:
+        raise _l.B200Error('row range [%d, %d) is empty' % (r0, r1))
+    b0, b1 = r0 // D, -(-r1 // D)
+    return b0, b1, r0 - b0 * D
 
 
 def check_rrc_tables(index, draws, nbytes, C, D):
@@ -631,7 +680,8 @@ def check_rrc_tables(index, draws, nbytes, C, D):
 
 def input_prep_u8_rrc(regions, cpad, rrc, s2d=False, border=False, out=None):
     """uint8 region buffer -> bf16 [B*D, OH, OW, cpad] (or the bordered space-to-depth layout): RandomResizedCrop with
-    Pillow's bilinear resample, flip and normalisation through rrc.lut; row b*D + d = copy d of image b."""
+    Pillow's bilinear resample, flip and normalisation through rrc.lut; row b*D + d = copy d of image b.  With
+    rrc.window = (p, n): rows [p, p + n) of that output."""
     _chk(regions, torch.uint8, "regions"); _chk(rrc.index, torch.int64, "index"); _chk(rrc.draws, torch.int32, "draws")
     _chk(rrc.lut, torch.float32, "lut")
     if s2d and not border:
@@ -653,7 +703,17 @@ def input_prep_u8_rrc(regions, cpad, rrc, s2d=False, border=False, out=None):
                                                   rrc.draws.data_ptr(), B, D, C, OH, OW, cpad, mode,
                                                   rrc.lut.data_ptr(), out.data_ptr(), _stream()),
                  "b200_input_prep_u8_rrc")
-    return out
+    return _window(out, rrc.window)
+
+
+def _window(out, window):
+    """rows [p, p + n) of a relayout output (a contiguous view: rows are its outermost dimension)"""
+    if window is None:
+        return out
+    p, n = window
+    if p < 0 or n < 1 or p + n > out.shape[0]:
+        raise _l.B200Error('relayout window (%d, %d) outside its %d rows' % (p, n, out.shape[0]))
+    return out[p:p + n]
 
 
 class ScaleCropTables(object):
@@ -726,7 +786,8 @@ def input_prep_u8_scale_crop(regions, cpad, sc, s2d=False, border=False, out=Non
 def input_prep_u8_aug(x_nhwc_u8, cpad, aug, out=None):
     """uint8 NHWC [N,H,W,C] -> bf16 NHWC [N*D, H, W, cpad]: the D augmented copies of every image (crop, flip, Cutout)
     normalised through aug.lut, row n*D + d = copy d of image n.  With aug.out_hw = (OH, OW) every crop is resized
-    (Pillow's bilinear resample) before the flip: bf16 [N*D, OH, OW, cpad], Cutout boxes in output coordinates."""
+    (Pillow's bilinear resample) before the flip: bf16 [N*D, OH, OW, cpad], Cutout boxes in output coordinates.  With
+    aug.window = (p, n): rows [p, p + n) of that output."""
     _chk(x_nhwc_u8, torch.uint8, "x"); _chk(aug.params, torch.int16, "aug params"); _chk(aug.lut, torch.float32, "lut")
     N, H, W, C = x_nhwc_u8.shape
     D = aug.duplicates
@@ -742,13 +803,13 @@ def input_prep_u8_aug(x_nhwc_u8, cpad, aug, out=None):
                                                              aug.lut.data_ptr(), aug.params.data_ptr(), aug.holes,
                                                              out.data_ptr(), _stream()),
                      "b200_input_prep_u8_aug_resize")
-        return out
+        return _window(out, aug.window)
     out = _prep_out(N * D, H, W, cpad, False, False, x_nhwc_u8.device, out)
     with _T('input_prep', 0, x_nhwc_u8.numel() + 2 * aug.params.numel() + 2 * out.numel()):
         _l.check(_l.load().b200_input_prep_u8_aug(x_nhwc_u8.data_ptr(), N, D, C, H, W, cpad, aug.pad,
                                                   aug.lut.data_ptr(), aug.params.data_ptr(), aug.holes,
                                                   out.data_ptr(), _stream()), "b200_input_prep_u8_aug")
-    return out
+    return _window(out, aug.window)
 
 
 def weight_transpose(w, out=None):

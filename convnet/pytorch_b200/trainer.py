@@ -18,6 +18,10 @@ SURVEY.md section 2.3 C1/C2), and the per-tensor unscale / clip loops of the ref
 MixUp / CutMix (``mixup`` / ``cutmix``, trainer.py:44-51,119-138): drawn on the host per training chunk by
 utils/mixup.py; on the fused B200 path the input relayout and loss kernels do the mixing (see ``_upload_mix``).
 
+Gradient accumulation (``chunk_batch`` N > 1, trainer.py:106-160): on the fused B200 path each torch.chunk of the batch
+runs as its own fused (captured) step with the loss gradient scaled by 1/N; gradients accumulate in the arena and the
+optimizer steps once.  Device-augmented batches are split over their B*D rows (ops.Aug.row_range).
+
 Augmentation on the device (a loader yielding a utils.augment.DeviceBatch: an AugmentedBatch of data.py
 ``device_augment`` or a ResizedCropBatch of ``device_resized_crop``): on the fused B200 path the stem relayout kernel
 writes the B*D augmented copies from the uint8 data and its draws; every other path trains on the batch's ``apply()``,
@@ -183,6 +187,7 @@ class Trainer(object):
         self.graph_replayed_launches = 0
         self.world_size = dist.get_world_size() if (distributed and dist.is_initialized()) else 1
         self._upstream_t, self._upstream_v = None, None
+        self._chunk_w = {}                     # (rows, chunk_batch, device) -> fp32 [k, 3] weights of the chunk meters
 
         if self.b200 is not None:
             self.model = model
@@ -211,13 +216,14 @@ class Trainer(object):
             dist.broadcast(buf, src=0)
         arena.sync_shadow()
 
-    def _allreduce_gradients(self):
+    def _allreduce_gradients(self, accumulated=False):
         """Sum of the gradient arena over the ranks (the 1/world factor is folded into the SGD kernel).  Normally the
         reduction already ran inside the backward pass -- NCCL all-reduces of arena ranges on a communication stream,
         launched as soon as a range is final and overlapped with the remaining backward kernels (inside the captured
         graph they are graph nodes) -- and nothing is left to do here; the flat all-reduce below serves runs whose
-        capture with in-graph all-reduces failed."""
-        if self.b200 is None or self.world_size <= 1 or self.b200.grad_bucket_hook is not None:
+        capture with in-graph all-reduces failed, and fused chunked steps (``accumulated``), whose backward passes keep
+        the buckets out: only the sum over the chunks is reduced."""
+        if self.b200 is None or self.world_size <= 1 or (self.b200.grad_bucket_hook is not None and not accumulated):
             return
         from . import ops
         g32 = self.b200.arena.g32
@@ -289,7 +295,7 @@ class Trainer(object):
             self._graph_static_ok = ok
         return self._graph_static_ok
 
-    def graphed_forward_backward(self, inputs, target, mix=None, aug=None):
+    def graphed_forward_backward(self, inputs, target, mix=None, aug=None, chunks=1):
         """Forward + criterion + backward of one device-resident batch through a captured CUDA graph.
         Returns (logits, loss, stats) -- detached device tensors; stats = fp32[3] {loss, top-1 %, top-5 %} when the fused
         loss kernel computed them, else None -- or None when this call has to run eagerly (warm-up steps of
@@ -297,14 +303,16 @@ class Trainer(object):
         ``mix`` (ops.Mix, from _upload_mix): the step mixes its input; the graph reads the permutation, lambda and box
         from their persistent device buffers, so every replay uses the values uploaded for that step.
         ``aug`` (ops.Aug or ops.Rrc, from _device_aug): the step augments its uint8 data on the device; the graph reads
-        the draw tables from static buffers refreshed like the input, so every replay uses that step's draws."""
+        the draw tables from static buffers refreshed like the input, so every replay uses that step's draws.
+        ``chunks`` > 1: one chunk of a batch split into that many (fused path only): the loss gradient is scaled by
+        1 / chunks, gradients accumulate, and the data-parallel buckets stay out of the graph."""
         if not self._graph_eligible() or not inputs.is_cuda:
             return None
         # loss / gradient scales are NOT part of the key: they reach the kernels through a device scalar; neither are
         # the mixing draws (device buffers) -- only the kind of mixing
         key = (tuple(inputs.shape), inputs.dtype, tuple(target.shape), target.dtype, self._model.training,
                mix.kind if mix is not None else 0,
-               aug.key if aug is not None else None)
+               aug.key if aug is not None else None, chunks > 1)
         st = self._graphs.get(key)
         if st is None:
             st = self._graphs[key] = {'seen': 0, 'graph': None}
@@ -313,7 +321,7 @@ class Trainer(object):
             if st['seen'] <= 2:
                 return None                       # eager warm-up (library handles, allocator, autotuned state)
             try:
-                self._capture(st, inputs, target, mix, aug)
+                self._capture(st, inputs, target, mix, aug, chunks)
             except Exception as e:  # noqa: BLE001  -- keep training eagerly if capture is impossible here
                 if self.b200.grad_bucket_hook is not None:
                     # NCCL inside the capture is the likely culprit: fall back to ONE flat all-reduce after the graph
@@ -331,13 +339,13 @@ class Trainer(object):
         if aug is not None:
             for dst, src in zip(st['aug'], aug.tables):
                 dst.copy_(src, non_blocking=True)
-        self._upstream()                          # refresh the device scalar if a scale changed
+        self._upstream(chunks)                    # refresh the device scalar if a scale changed
         st['graph'].replay()
         self.graph_replays += 1
         self.graph_replayed_launches += st['launches']
         return st['out'].detach(), st['loss'].detach(), st['stats']
 
-    def _capture(self, st, inputs, target, mix=None, aug=None):
+    def _capture(self, st, inputs, target, mix=None, aug=None, chunks=1):
         from . import lib, ops
         x_s, y_s = torch.empty_like(inputs), torch.empty_like(target)
         x_s.copy_(inputs)
@@ -348,7 +356,7 @@ class Trainer(object):
         graph = torch.cuda.CUDAGraph()
         torch.cuda.synchronize()
         n0 = lib.launch_count()
-        up = self._upstream()
+        up = self._upstream(chunks)
         eps = self._plain_ce_eps()
         # with NCCL all-reduces inside the capture, ProcessGroupNCCL's watchdog thread polls CUDA events concurrently: the
         # default "global" capture mode would treat that as a capture violation
@@ -361,7 +369,7 @@ class Trainer(object):
         with torch.cuda.graph(graph, pool=self._graph_pool, stream=self._capture_stream, capture_error_mode=mode):
             stats = None
             if eps is not None:            # the whole step is library calls: nothing of autograd inside the graph
-                out, stats = self.b200.train_step(x_s, y_s, eps, up, mix=mix, aug=aug_s)
+                out, stats = self.b200.train_step(x_s, y_s, eps, up, mix=mix, aug=aug_s, reduce=chunks == 1)
                 loss = stats[0]
             else:
                 out = self.model(x_s)
@@ -391,15 +399,18 @@ class Trainer(object):
             return float(c.smooth_eps or 0.0)
         return None
 
-    def _upstream(self):
+    def _upstream(self, chunks=1):
         """d(scaled loss)/d(loss) = grad_scale * loss_scale (trainer.py:158-161 of the reference multiplies the loss)
         as a persistent 0-dim device tensor handed to autograd.backward: no per-step scalar kernels, and a captured
-        graph reads the current value instead of a baked-in constant."""
+        graph reads the current value instead of a baked-in constant.  ``chunks`` > 1: that value divided by chunks in
+        fp32, what autograd hands the chunk's loss for the reference's ``loss / chunk_batch`` (trainer.py:146-147)."""
         v = 1.0
         if self.grad_scale is not None:
             v *= float(self.grad_scale)
         if self.loss_scale is not None:
             v *= float(self.loss_scale)
+        if chunks > 1:
+            v = float(np.float32(v) / np.float32(chunks))
         if self._upstream_t is None:
             self._upstream_t = torch.empty((), device=self.b200.device, dtype=torch.float32)
         if v != self._upstream_v:
@@ -435,11 +446,11 @@ class Trainer(object):
         if training:
             self.optimizer.zero_grad()
             self.optimizer.update(self.epoch, self.training_steps)
+        fused_batch = training and self._fused_training(average_output) \
+            and target_batch.dtype == torch.long and target_batch.dim() == 1
         aug = None
         if isinstance(inputs_batch, DeviceBatch):
-            if training and self.b200 is not None and chunk_batch == 1 and not average_output \
-                    and 'cuda' in str(self.device) and self._hooks_static() and self._plain_ce_eps() is not None \
-                    and target_batch.dtype == torch.long and target_batch.dim() == 1:
+            if fused_batch:
                 aug, inputs_batch = self._device_aug(inputs_batch)
             elif not training and isinstance(inputs_batch, ScaleCropBatch) and self.b200 is not None \
                     and not self.model.training and chunk_batch == 1 and not average_output \
@@ -448,8 +459,15 @@ class Trainer(object):
             else:
                 inputs_batch = inputs_batch.apply()     # the same fp32 batch the fused relayout would compute
 
-        chunks = zip(inputs_batch.chunk(chunk_batch, dim=0), target_batch.chunk(chunk_batch, dim=0))
-        for i, (inputs, target) in enumerate(chunks):
+        # fused chunked steps (gradient accumulation, trainer.py:114-147 of the reference): each chunk's logits and
+        # fp32[3] statistics are gathered on the device -- a graph replay overwrites its static outputs
+        accumulate = chunk_batch > 1 and fused_batch
+        if accumulate:
+            from . import ops
+            ranges = ops.chunk_rows(target_batch.size(0), chunk_batch)
+            chunk_stats = torch.empty((len(ranges), 3), device=self.device, dtype=torch.float32)
+            chunk_logits = None
+        for i, (inputs, target, aug_i) in enumerate(self._chunks(inputs_batch, target_batch, chunk_batch, aug)):
             is_u8 = inputs.dtype == torch.uint8
             target = target.to(self.device, non_blocking=True)
             if self.b200 is not None and inputs.dtype == torch.uint8:
@@ -459,12 +477,27 @@ class Trainer(object):
             mixer = None
             if training and (self.mixup is not None or self.cutmix is not None):
                 mixer = self._draw_mix(inputs.size(0), average_output)
-            fused = training and self.b200 is not None and chunk_batch == 1 and not average_output and inputs.is_cuda \
-                and self._hooks_static() and self._plain_ce_eps() is not None \
-                and target.dtype == torch.long and target.dim() == 1
+            fused = fused_batch and inputs.is_cuda
             mix = self._upload_mix(mixer, inputs) if (mixer is not None and fused) else None
             if aug is not None and training and not fused:
                 raise B200Error('batch augmentation on the device: the fused training step is not available here')
+            if accumulate:
+                r0, r1 = ranges[i]
+                self.optimizer.pre_forward()
+                replayed = self.graphed_forward_backward(inputs, target, mix, aug_i, chunks=chunk_batch)
+                if replayed is not None:
+                    output, chunk = replayed[0], replayed[2]
+                else:
+                    output, chunk = self.b200.train_step(inputs, target, self._plain_ce_eps(),
+                                                         self._upstream(chunk_batch), mix=mix, aug=aug_i, reduce=False)
+                if i == 0:
+                    self.optimizer.pre_backward()
+                if chunk_logits is None:
+                    chunk_logits = torch.empty((ranges[-1][1], output.shape[1]), device=output.device,
+                                               dtype=output.dtype)
+                chunk_logits[r0:r1].copy_(output)
+                chunk_stats[i].copy_(chunk)
+                continue
             if training and chunk_batch == 1 and not average_output and (mixer is None or mix is not None):
                 replayed = self.graphed_forward_backward(inputs, target, mix, aug)
                 if replayed is not None:
@@ -483,11 +516,11 @@ class Trainer(object):
                 self.optimizer.pre_backward()
                 continue
             if mixer is not None:
-                # generic path (chunked batches, other criteria): the reference's fp32 mixing of the batch on its device
-                # and the soft target through the criterion
+                # generic path (other criteria): the reference's fp32 mixing of the batch on its device and the soft
+                # target through the criterion
                 if is_u8:
-                    raise B200Error('mixup / cutmix of a uint8 batch needs the fused path (chunk_batch=1, plain '
-                                    'CrossEntropyLoss, a converted model); normalise the batch to fp32 otherwise')
+                    raise B200Error('mixup / cutmix of a uint8 batch needs the fused path (plain CrossEntropyLoss, a '
+                                    'converted model); normalise the batch to fp32 otherwise')
                 inputs = mixer(inputs.clone() if isinstance(mixer, CutMix) else inputs)   # the caller's batch stays intact
             if training:
                 self.optimizer.pre_forward()
@@ -522,9 +555,12 @@ class Trainer(object):
                         loss = loss * self.loss_scale
                     loss.backward()
 
+        if accumulate:
+            outputs = [chunk_logits]
+            stats = (chunk_stats * self._chunk_weights(ranges, chunk_batch)).sum(0)
         if training:
             if self.b200 is not None:
-                self._allreduce_gradients()
+                self._allreduce_gradients(accumulated=accumulate)
                 self.optimizer.set_grad_unscale(self.loss_scale if self.loss_scale is not None else 1.0,
                                                 self.world_size)
                 if self.grad_clip > 0:
@@ -543,6 +579,41 @@ class Trainer(object):
             self.training_steps += 1
 
         return (outputs[0] if len(outputs) == 1 else torch.cat(outputs, dim=0)), (stats if stats is not None else total_loss), grad
+
+    def _fused_training(self, average_output):
+        """True when a training step runs as the runtime's fused train_step (plain CrossEntropyLoss, static hooks, a
+        converted model on CUDA, no averaged outputs); the targets must also be class indices."""
+        return self.b200 is not None and not average_output and 'cuda' in str(self.device) and self._hooks_static() \
+            and self._plain_ce_eps() is not None
+
+    @staticmethod
+    def _chunks(inputs_batch, target_batch, chunk_batch, aug):
+        """-> (inputs, target, aug) per chunk: torch.chunk of the batch and its targets over the rows, the reference's
+        split (trainer.py:114-115).  With device augmentation the B*D rows are split the same way; each chunk's relayout
+        reads the images (or regions) that cover its rows and keeps just those rows (ops.Aug.row_range)."""
+        if chunk_batch == 1:
+            return [(inputs_batch, target_batch, aug)]
+        if aug is None:
+            return [(x, y, None) for x, y in zip(inputs_batch.chunk(chunk_batch, dim=0),
+                                                 target_batch.chunk(chunk_batch, dim=0))]
+        from . import ops
+        out = []
+        for r0, r1 in ops.chunk_rows(target_batch.size(0), chunk_batch):
+            a, b0, b1 = aug.row_range(r0, r1)
+            out.append((inputs_batch if isinstance(aug, ops.Rrc) else inputs_batch[b0:b1], target_batch[r0:r1], a))
+        return out
+
+    def _chunk_weights(self, ranges, chunk_batch):
+        """fp32 [k, 3] device weights that combine the chunks' {loss, top-1 %, top-5 %} into the step's meters as the
+        reference computes them: the loss is the sum of each chunk's loss / chunk_batch (trainer.py:146-151), the
+        accuracies are those of the concatenated outputs, so each chunk counts by its rows."""
+        rows = ranges[-1][1]
+        key = (rows, chunk_batch, str(self.device))
+        w = self._chunk_w.get(key)
+        if w is None:
+            w = self._chunk_w[key] = torch.tensor([[1.0 / chunk_batch, (r1 - r0) / rows, (r1 - r0) / rows]
+                                                   for r0, r1 in ranges], dtype=torch.float32).to(self.device)
+        return w
 
     # ------------------------------------------------------------------ input mixing (MixUp / CutMix)
     def _draw_mix(self, batch_size, average_output=False):
@@ -653,7 +724,8 @@ class Trainer(object):
             n_batches = -1
         tick = time.time()
         batches = _cuda_prefetch(data_loader, self.device, self._input_dtype()) \
-            if (self.b200 is not None and chunk_batch == 1) else data_loader
+            if (self.b200 is not None and (chunk_batch == 1 or (training and self._fused_training(average_output)))) \
+            else data_loader
         # lazy meters (B200 fused path): the step's {loss, prec1, prec5} come from the loss kernel as one device
         # tensor; it is copied to pinned host memory asynchronously every step and only awaited when a log line is
         # due, the ring is full or the loop ends -- no host synchronisation inside a step
