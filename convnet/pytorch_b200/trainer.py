@@ -18,9 +18,9 @@ SURVEY.md section 2.3 C1/C2), and the per-tensor unscale / clip loops of the ref
 MixUp / CutMix (``mixup`` / ``cutmix``, trainer.py:44-51,119-138): drawn on the host per training chunk by
 utils/mixup.py; on the fused B200 path the input relayout and loss kernels do the mixing (see ``_upload_mix``).
 
-Gradient accumulation (``chunk_batch`` N > 1, trainer.py:106-160): on the fused B200 path each torch.chunk of the batch
-runs as its own fused (captured) step with the loss gradient scaled by 1/N; gradients accumulate in the arena and the
-optimizer steps once.  Device-augmented batches are split over their B*D rows (ops.Aug.row_range).
+Fused training steps loop over the torch.chunks of the batch (``chunk_batch`` N, trainer.py:106-160), the whole batch
+being the one-chunk case: each chunk is a fused (captured) step with the loss gradient scaled by 1/N, gradients
+accumulate in the arena, the optimizer steps once.  Device-augmented batches split over B*D rows (ops.Aug.row_range).
 
 Augmentation on the device (a loader yielding a utils.augment.DeviceBatch: an AugmentedBatch of data.py
 ``device_augment`` or a ResizedCropBatch of ``device_resized_crop``): on the fused B200 path the stem relayout kernel
@@ -357,7 +357,7 @@ class Trainer(object):
         torch.cuda.synchronize()
         n0 = lib.launch_count()
         up = self._upstream(chunks)
-        eps = self._plain_ce_eps()
+        eps = self._plain_ce_eps() if self._fused_batch(False, target) else None   # graphed steps never average outputs
         # with NCCL all-reduces inside the capture, ProcessGroupNCCL's watchdog thread polls CUDA events concurrently: the
         # default "global" capture mode would treat that as a capture violation
         mode = 'thread_local' if self.b200.grad_bucket_hook is not None else 'global'
@@ -442,125 +442,77 @@ class Trainer(object):
         """-> (outputs, loss, grad norm or None).  ``loss`` is a float, or -- on the fused B200 path -- the fp32[3] device
         tensor {loss, top-1 %, top-5 %} of the loss kernel, which Trainer.forward reads back asynchronously
         (the reference synchronises three times per step here: trainer.py:153,226-227)."""
-        outputs, total_loss, grad, stats = [], 0, None, None
+        grad = None
         if training:
             self.optimizer.zero_grad()
             self.optimizer.update(self.epoch, self.training_steps)
-        fused_batch = training and self._fused_training(average_output) \
-            and target_batch.dtype == torch.long and target_batch.dim() == 1
-        aug = None
-        if isinstance(inputs_batch, DeviceBatch):
-            if fused_batch:
-                aug, inputs_batch = self._device_aug(inputs_batch)
-            elif not training and isinstance(inputs_batch, ScaleCropBatch) and self.b200 is not None \
-                    and not self.model.training and chunk_batch == 1 and not average_output \
-                    and 'cuda' in str(self.device):
-                aug, inputs_batch = self._device_aug(inputs_batch)     # the eval forward reads the uint8 regions
-            else:
+        fused = training and self._fused_batch(average_output, target_batch)
+        if fused:
+            output, loss = self._fused_step(inputs_batch, target_batch, chunk_batch)
+        elif not training and isinstance(inputs_batch, ScaleCropBatch) and self.b200 is not None \
+                and not self.model.training and chunk_batch == 1 and not average_output and 'cuda' in str(self.device):
+            # Runtime.forward's eval pass, fed by the relayout of the batch's uint8 regions
+            aug, regions = self._device_aug(inputs_batch)
+            regions, target = self._to_device(regions, target_batch)
+            output = self.b200.run_forward(regions, False, False, aug=aug)[0]
+            loss = float(self.criterion(output, target).detach())
+            output = output.detach()
+        else:
+            if isinstance(inputs_batch, DeviceBatch):
                 inputs_batch = inputs_batch.apply()     # the same fp32 batch the fused relayout would compute
-
-        # fused chunked steps (gradient accumulation, trainer.py:114-147 of the reference): each chunk's logits and
-        # fp32[3] statistics are gathered on the device -- a graph replay overwrites its static outputs
-        accumulate = chunk_batch > 1 and fused_batch
-        if accumulate:
-            from . import ops
-            ranges = ops.chunk_rows(target_batch.size(0), chunk_batch)
-            chunk_stats = torch.empty((len(ranges), 3), device=self.device, dtype=torch.float32)
-            chunk_logits = None
-        for i, (inputs, target, aug_i) in enumerate(self._chunks(inputs_batch, target_batch, chunk_batch, aug)):
-            is_u8 = inputs.dtype == torch.uint8
-            target = target.to(self.device, non_blocking=True)
-            if self.b200 is not None and inputs.dtype == torch.uint8:
-                inputs = inputs.to(self.device, non_blocking=True)
-            else:
-                inputs = inputs.to(self.device, dtype=self._input_dtype(), non_blocking=True)
-            mixer = None
-            if training and (self.mixup is not None or self.cutmix is not None):
-                mixer = self._draw_mix(inputs.size(0), average_output)
-            fused = fused_batch and inputs.is_cuda
-            mix = self._upload_mix(mixer, inputs) if (mixer is not None and fused) else None
-            if aug is not None and training and not fused:
-                raise B200Error('batch augmentation on the device: the fused training step is not available here')
-            if accumulate:
-                r0, r1 = ranges[i]
-                self.optimizer.pre_forward()
-                replayed = self.graphed_forward_backward(inputs, target, mix, aug_i, chunks=chunk_batch)
-                if replayed is not None:
-                    output, chunk = replayed[0], replayed[2]
-                else:
-                    output, chunk = self.b200.train_step(inputs, target, self._plain_ce_eps(),
-                                                         self._upstream(chunk_batch), mix=mix, aug=aug_i, reduce=False)
-                if i == 0:
-                    self.optimizer.pre_backward()
-                if chunk_logits is None:
-                    chunk_logits = torch.empty((ranges[-1][1], output.shape[1]), device=output.device,
-                                               dtype=output.dtype)
-                chunk_logits[r0:r1].copy_(output)
-                chunk_stats[i].copy_(chunk)
-                continue
-            if training and chunk_batch == 1 and not average_output and (mixer is None or mix is not None):
-                replayed = self.graphed_forward_backward(inputs, target, mix, aug)
-                if replayed is not None:
-                    outputs.append(replayed[0])
-                    if replayed[2] is not None:
-                        stats = replayed[2]
-                    else:
+            outputs, total_loss = [], 0
+            for i, (inputs, target, _) in enumerate(self._chunks(inputs_batch, target_batch, chunk_batch, None)):
+                is_u8 = inputs.dtype == torch.uint8
+                inputs, target = self._to_device(inputs, target)
+                mixer = None
+                if training and (self.mixup is not None or self.cutmix is not None):
+                    mixer = self._draw_mix(inputs.size(0), average_output)
+                if training and chunk_batch == 1 and not average_output and mixer is None:
+                    replayed = self.graphed_forward_backward(inputs, target)
+                    if replayed is not None:
+                        outputs.append(replayed[0])
                         total_loss += float(replayed[1])
-                    continue
-            if fused:
-                # eager form of the captured step (warm-up iterations of a new shape, use_graphs off)
-                self.optimizer.pre_forward()
-                output, stats = self.b200.train_step(inputs, target, self._plain_ce_eps(), self._upstream(), mix=mix,
-                                                     aug=aug)
-                outputs.append(output)
-                self.optimizer.pre_backward()
-                continue
-            if mixer is not None:
-                # generic path (other criteria): the reference's fp32 mixing of the batch on its device and the soft
-                # target through the criterion
-                if is_u8:
-                    raise B200Error('mixup / cutmix of a uint8 batch needs the fused path (plain CrossEntropyLoss, a '
-                                    'converted model); normalise the batch to fp32 otherwise')
-                inputs = mixer(inputs.clone() if isinstance(mixer, CutMix) else inputs)   # the caller's batch stays intact
-            if training:
-                self.optimizer.pre_forward()
-            if aug is not None:     # evaluation of a ScaleCropBatch: Runtime.forward's eval pass, fed by the relayout
-                output = self.b200.run_forward(inputs, False, False, aug=aug)[0]
-            else:
+                        continue
+                if mixer is not None:
+                    # the reference's fp32 mixing of the batch on its device and the soft target through the criterion
+                    if is_u8:
+                        raise B200Error('mixup / cutmix of a uint8 batch needs the fused path (plain CrossEntropyLoss, '
+                                        'a converted model); normalise the batch to fp32 otherwise')
+                    inputs = mixer(inputs.clone() if isinstance(mixer, CutMix) else inputs)   # the caller's batch stays intact
+                if training:
+                    self.optimizer.pre_forward()
                 output = self.model(inputs)
-            if average_output:
+                if average_output:
+                    if isinstance(output, (list, tuple)):
+                        output = [_average_duplicates(o, target) if o is not None else None for o in output]
+                    else:
+                        output = _average_duplicates(output, target)
+                if mixer is not None:
+                    target = mixer.mix_target(target, (output[0] if isinstance(output, (list, tuple)) else output).size(-1))
+                loss = self.criterion(output, target)
+                if chunk_batch > 1:
+                    loss = loss / chunk_batch
                 if isinstance(output, (list, tuple)):
-                    output = [_average_duplicates(o, target) if o is not None else None for o in output]
-                else:
-                    output = _average_duplicates(output, target)
-            if mixer is not None:
-                target = mixer.mix_target(target, (output[0] if isinstance(output, (list, tuple)) else output).size(-1))
-            loss = self.criterion(output, target)
-            if chunk_batch > 1:
-                loss = loss / chunk_batch
-            if isinstance(output, (list, tuple)):
-                output = output[0]
-            outputs.append(output.detach())
-            total_loss += float(loss.detach())
+                    output = output[0]
+                outputs.append(output.detach())
+                total_loss += float(loss.detach())
 
-            if training:
-                if i == 0:
-                    self.optimizer.pre_backward()
-                if self.b200 is not None and loss.dim() == 0 and loss.dtype == torch.float32:
-                    torch.autograd.backward(loss, grad_tensors=[self._upstream()])
-                else:
-                    if self.grad_scale is not None:
-                        loss = loss * self.grad_scale
-                    if self.loss_scale is not None:
-                        loss = loss * self.loss_scale
-                    loss.backward()
+                if training:
+                    if i == 0:
+                        self.optimizer.pre_backward()
+                    if self.b200 is not None and loss.dim() == 0 and loss.dtype == torch.float32:
+                        torch.autograd.backward(loss, grad_tensors=[self._upstream()])
+                    else:
+                        if self.grad_scale is not None:
+                            loss = loss * self.grad_scale
+                        if self.loss_scale is not None:
+                            loss = loss * self.loss_scale
+                        loss.backward()
+            output, loss = (outputs[0] if len(outputs) == 1 else torch.cat(outputs, dim=0)), total_loss
 
-        if accumulate:
-            outputs = [chunk_logits]
-            stats = (chunk_stats * self._chunk_weights(ranges, chunk_batch)).sum(0)
         if training:
             if self.b200 is not None:
-                self._allreduce_gradients(accumulated=accumulate)
+                self._allreduce_gradients(accumulated=fused and chunk_batch > 1)
                 self.optimizer.set_grad_unscale(self.loss_scale if self.loss_scale is not None else 1.0,
                                                 self.world_size)
                 if self.grad_clip > 0:
@@ -578,13 +530,58 @@ class Trainer(object):
                 self.optimizer.step()
             self.training_steps += 1
 
-        return (outputs[0] if len(outputs) == 1 else torch.cat(outputs, dim=0)), (stats if stats is not None else total_loss), grad
+        return output, loss, grad
+
+    def _fused_step(self, inputs_batch, target_batch, chunk_batch):
+        """-> (logits, fp32[3] statistics) of one training batch on the runtime's fused train_step.  Each torch.chunk of
+        the batch -- the whole batch when chunk_batch == 1 -- runs as one fused (captured) step with the loss gradient
+        scaled by 1 / chunk_batch; gradients accumulate in the arena (trainer.py:114-147 of the reference).  Several
+        chunks' logits and statistics are gathered on the device -- a graph replay overwrites its static outputs."""
+        aug = None
+        if isinstance(inputs_batch, DeviceBatch):
+            aug, inputs_batch = self._device_aug(inputs_batch)
+        if chunk_batch > 1:
+            from . import ops
+            ranges = ops.chunk_rows(target_batch.size(0), chunk_batch)
+            chunk_stats = torch.empty((len(ranges), 3), device=self.device, dtype=torch.float32)
+        for i, (inputs, target, aug_i) in enumerate(self._chunks(inputs_batch, target_batch, chunk_batch, aug)):
+            inputs, target = self._to_device(inputs, target)
+            mix = None
+            if self.mixup is not None or self.cutmix is not None:
+                mix = self._upload_mix(self._draw_mix(inputs.size(0)), inputs)
+            self.optimizer.pre_forward()       # static hooks (_hooks_static): this and pre_backward reach no-ops
+            replayed = self.graphed_forward_backward(inputs, target, mix, aug_i, chunks=chunk_batch)
+            if replayed is not None:
+                output, stats = replayed[0], replayed[2]
+            else:
+                output, stats = self.b200.train_step(inputs, target, self._plain_ce_eps(), self._upstream(chunk_batch),
+                                                     mix=mix, aug=aug_i, reduce=chunk_batch == 1)
+            if i == 0:
+                self.optimizer.pre_backward()
+            if chunk_batch == 1:
+                return output, stats
+            if i == 0:
+                chunk_logits = torch.empty((ranges[-1][1], output.shape[1]), device=output.device, dtype=output.dtype)
+            chunk_logits[ranges[i][0]:ranges[i][1]].copy_(output)
+            chunk_stats[i].copy_(stats)
+        return chunk_logits, (chunk_stats * self._chunk_weights(ranges, chunk_batch)).sum(0)
+
+    def _to_device(self, inputs, target):
+        """-> (inputs, target) on the device; a converted model's uint8 batches stay uint8 (its relayout normalises)."""
+        target = target.to(self.device, non_blocking=True)
+        if self.b200 is not None and inputs.dtype == torch.uint8:
+            return inputs.to(self.device, non_blocking=True), target
+        return inputs.to(self.device, dtype=self._input_dtype(), non_blocking=True), target
 
     def _fused_training(self, average_output):
         """True when a training step runs as the runtime's fused train_step (plain CrossEntropyLoss, static hooks, a
-        converted model on CUDA, no averaged outputs); the targets must also be class indices."""
+        converted model on CUDA, no averaged outputs); the targets must also be class indices (_fused_batch)."""
         return self.b200 is not None and not average_output and 'cuda' in str(self.device) and self._hooks_static() \
             and self._plain_ce_eps() is not None
+
+    def _fused_batch(self, average_output, target):
+        """True when a training batch with these targets runs as the runtime's fused train_step."""
+        return self._fused_training(average_output) and target.dtype == torch.long and target.dim() == 1
 
     @staticmethod
     def _chunks(inputs_batch, target_batch, chunk_batch, aug):
