@@ -208,53 +208,72 @@ class _BN(object):
         self.dbeta = arena.kernel_view(arena.g32, sb)
 
 
+class _Linear(object):
+    """nn.Linear as a 1x1 convolution on a 1x1 map: the bf16 weight [K,1,C] (K = out_features padded to 8, see Arena),
+    the fp32 bias and their gradient views in the arena."""
+
+    def __init__(self, arena, mod):
+        sw, sb = arena.slot(mod.weight), arena.slot(mod.bias)
+        self.C, self.K = mod.in_features, _round_up(mod.out_features, 8)
+        self.w16, self.gw = arena.kernel_view(arena.p16, sw), arena.kernel_view(arena.g32, sw)
+        self.b32, self.gb = arena.kernel_view(arena.p32, sb), arena.kernel_view(arena.g32, sb)
+
+    def desc(self, N, algo_macs=None):
+        return ops.make_desc(N, 1, 1, self.C, self.K, 1, 1, 1, 0, algo_macs=algo_macs)
+
+    def fwd(self, x, desc, act=ACT_NONE, out_fp32=False):
+        """x [N,1,1,C] bf16 -> act(x W^T + b) [N,1,1,K]."""
+        return ops.conv_fprop(x, self.w16, desc, bias=self.b32, act=act, out_fp32=out_fp32)
+
+    def bwd(self, rt, x, dy, desc):
+        """dy [N,1,1,K] bf16 -> dx; the weight and bias gradients accumulate into the arena (wgrad on the side
+        stream)."""
+        ops.colsum_bf16(dy.view(dy.shape[0], self.K), self.gb)
+        rt._wgrad_async(lambda: ops.conv_wgrad(x, dy, desc, self.gw), x, dy)
+        return ops.conv_dgrad(dy, ops.weight_transpose(self.w16), desc)
+
+
 class _SE(object):
     """squeeze-and-excitation gate (models/modules/se.py:6-25 of the reference): two tiny linear layers whose
-    parameters live in the arena like the classifier's (bf16 [K,1,C] kernel views, fp32 biases)."""
+    parameters live in the arena like the classifier's."""
 
     def __init__(self, arena, mod):
         from .models.modules.se import SEBlock
         if not isinstance(mod, SEBlock):
             raise B200Error('residual_block of type %s is outside the B200 hot path' % type(mod).__name__)
         l1, l2 = mod.transform[0], mod.transform[2]
-        self.C, self.hidden = l1.in_features, l1.out_features
-        if self.C % 8 or self.hidden % 8 or l2.out_features != self.C:
-            raise B200Error('SE gate: channel counts must be multiples of 8 (got %d -> %d)' % (self.C, self.hidden))
-        sw1, sb1, sw2, sb2 = (arena.slot(p) for p in (l1.weight, l1.bias, l2.weight, l2.bias))
-        self.w1, self.gw1 = arena.kernel_view(arena.p16, sw1), arena.kernel_view(arena.g32, sw1)
-        self.b1, self.gb1 = arena.kernel_view(arena.p32, sb1), arena.kernel_view(arena.g32, sb1)
-        self.w2, self.gw2 = arena.kernel_view(arena.p16, sw2), arena.kernel_view(arena.g32, sw2)
-        self.b2, self.gb2 = arena.kernel_view(arena.p32, sb2), arena.kernel_view(arena.g32, sb2)
+        if l1.in_features % 8 or l1.out_features % 8 or l2.out_features != l1.in_features:
+            raise B200Error('SE gate: channel counts must be multiples of 8 (got %d -> %d)'
+                            % (l1.in_features, l1.out_features))
+        self.l1, self.l2 = _Linear(arena, l1), _Linear(arena, l2)
 
     def fwd(self, r):
         """r' = r * sigmoid(W2 relu(W1 mean(r) + b1) + b2); returns (r', tape)."""
         N = r.shape[0]
         mean = ops.se_pool(r)                                                        # [N,1,1,C] bf16
-        d1 = ops.make_desc(N, 1, 1, self.C, self.hidden, 1, 1, 1, 0)
-        d2 = ops.make_desc(N, 1, 1, self.hidden, self.C, 1, 1, 1, 0)
-        h = ops.conv_fprop(mean, self.w1, d1, bias=self.b1, act=ACT_RELU)            # [N,1,1,C/ratio] bf16
-        logit = ops.conv_fprop(h, self.w2, d2, bias=self.b2, out_fp32=True).view(N, self.C)
+        d1, d2 = self.l1.desc(N), self.l2.desc(N)
+        h = self.l1.fwd(mean, d1, act=ACT_RELU)                                      # [N,1,1,C/ratio] bf16
+        logit = self.l2.fwd(h, d2, out_fp32=True).view(N, self.l2.K)
         return ops.se_scale_fwd(r, logit), (r, mean, h, logit, d1, d2)
 
     def bwd(self, rt, tape, g):
         """g = dL/dr' -> dL/dr; the gate's parameter gradients accumulate into the arena."""
         r, mean, h, logit, d1, d2 = tape
-        N = r.shape[0]
         dlogit = ops.se_bwd_reduce(g, r, logit)                                      # [N,1,1,C] bf16
-        ops.colsum_bf16(dlogit.view(N, self.C), self.gb2)
-        rt._wgrad_async(lambda: ops.conv_wgrad(h, dlogit, d2, self.gw2), h, dlogit)
-        dh = ops.conv_dgrad(dlogit, ops.weight_transpose(self.w2), d2)
-        dh = ops.act_bwd(dh, h, ACT_RELU)
-        ops.colsum_bf16(dh.view(N, self.hidden), self.gb1)
-        rt._wgrad_async(lambda: ops.conv_wgrad(mean, dh, d1, self.gw1), mean, dh)
-        dmean = ops.conv_dgrad(dh, ops.weight_transpose(self.w1), d1)
+        dh = ops.act_bwd(self.l2.bwd(rt, h, dlogit, d2), h, ACT_RELU)
+        dmean = self.l1.bwd(rt, mean, dh, d1)
         return ops.se_bwd_dx(g, logit, dmean)
 
 
 class _Unit(object):
-    """saved state of one conv+BN unit for backward."""
+    """saved state of one conv+BN unit for backward (conv is None for the stem, which is not a _Conv)."""
     __slots__ = ('x', 'z', 'y', 'w', 'desc', 'mean', 'invstd', 'scale', 'shift', 'sums', 'conv', 'bn', 'act', 'mask',
                  'sign_sum', 'drop')
+
+    def __init__(self, conv, bn, act, x):
+        for k in self.__slots__:
+            setattr(self, k, None)
+        self.conv, self.bn, self.act, self.x = conv, bn, act, x
 
 
 class Runtime(object):
@@ -291,6 +310,13 @@ class Runtime(object):
         # coefficient vectors here; while it is recomputed in the backward pass, it hands them back in the same order
         self._coeffs_record = None
         self._coeffs_replay = None
+        # checkpoint_segments: [start, end) ranges of self.blocks whose activations the forward pass does not keep;
+        # the backward pass recomputes each range just before it needs it
+        self.segments = []
+        # one 64-bit Philox key per training step for in-block dropout (set by _build when the model has any), drawn
+        # on the device with torch's CUDA generator (a captured step draws a fresh one on every replay;
+        # torch.manual_seed makes runs reproducible)
+        self.dropout_key = None
         self._build()
         self._setup_transposes()
 
@@ -315,7 +341,18 @@ class Runtime(object):
             ops.weight_transpose_batched(self.arena.p16, self._p16t, self._wt_jobs, self._wt_tiles)
 
     # ---- program construction (overridden per model family) -------------------------------------
+    # _build sets up the stem (_stem_build), self.blocks (one spec dict per block, run by the family's _block_fwd /
+    # _block_bwd; spec['dense'] lists the dense convolutions whose gradients are final after the block's backward)
+    # and the head (_head_build)
     def _build(self):
+        raise NotImplementedError
+
+    def _block_fwd(self, spec, x, training):
+        """-> (y, the block's tape)"""
+        raise NotImplementedError
+
+    def _block_bwd(self, spec, saved, dy):
+        """-> dx"""
         raise NotImplementedError
 
     # ---- small helpers ----------------------------------------------------------------------------
@@ -399,33 +436,30 @@ class Runtime(object):
         self._fold_cache[key] = (self.arena.version, wf, shift)
         return wf, shift
 
-    def _unit_fwd_folded(self, x, conv, bn, act, residual=None, other=None):
-        N, H, W, _ = x.shape
-        u = _Unit()
-        u.conv, u.bn, u.act, u.x = conv, bn, act, x
-        u.desc = conv.desc(N, H, W)
-        wf, bf = self._folded(conv, bn)
-        if other is not None:                # downsample branch: r = conv_ds'(x_block) + b_ds', added below
-            residual = other.y
-        u.z, u.mask = None, None
-        u.y = ops.conv_fprop(x, wf, u.desc, bias=bf, residual=residual, act=act)
-        return u
+    # Whether eval forwards fold BN into the convolutions (with FOLD_BN_EVAL on).  The MobileNet runtimes never have.
+    fold_bn_eval = True
 
-    def _unit_fwd(self, x, conv, bn, act, training, tape, residual=None, other=None, drop=None):
-        """z = conv(x); BN statistics (train) / running-stat coefficients (eval);
-        y = act(bn(z) + residual | + bn_other(z_other)).  Returns y and (if tape) the saved unit.
+    def _unit_fwd(self, x, conv, bn, act, training, residual=None, other=None, drop=None, apply=True):
+        """z = conv(x) (dense, grouped or depthwise); BN statistics (train) / running-stat coefficients (eval);
+        y = act(bn(z) + residual | + bn_other(z_other)).  Returns the saved unit.
         drop = (layer, p): in training y = dropout(relu(bn(z))) with the mask of (self.dropout_key, layer); ignored in
-        eval mode."""
-        if not training and FOLD_BN_EVAL and not self._want_tape:
-            return self._unit_fwd_folded(x, conv, bn, act, residual=residual, other=other)
+        eval mode.  apply=False stops after the coefficients (the downsample branch, whose apply is fused into the
+        block's last one as ``other``); folded, it is y = bn_ds(conv_ds(x)) in one kernel."""
         N, H, W, _ = x.shape
-        u = _Unit()
-        u.conv, u.bn, u.act, u.x = conv, bn, act, x
+        u = _Unit(conv, bn, act, x)
         u.desc = conv.desc(N, H, W)
+        if not training and FOLD_BN_EVAL and self.fold_bn_eval and not self._want_tape:
+            wf, bf = self._folded(conv, bn)
+            if other is not None:                # downsample branch: r = conv_ds'(x_block) + b_ds', added here
+                residual = other.y
+            u.y = ops.conv_fprop(x, wf, u.desc, bias=bf, residual=residual, act=act)
+            return u
         u.w = conv.kernel_weights()
-        self._conv_and_coeffs(u, x, u.w, training)
-        u.drop = drop if training else None
-        if u.drop is not None:
+        self._conv_and_coeffs(u, u.w, training)
+        if not apply:
+            return u
+        if training and drop is not None:
+            u.drop = drop
             # the kept-and-positive bits are the only record of the mask: the backward reads them, never the stream
             u.mask = torch.empty(ops.bn_act_mask_bytes(u.z.numel() // u.z.shape[-1], u.z.shape[-1]), device=self.device,
                                  dtype=torch.uint8)
@@ -434,8 +468,7 @@ class Runtime(object):
         # a join (something is added before the activation) cannot recompute act'(.) from z alone: keep one bit per
         # element instead of re-reading the bf16 output in both backward kernels (row-quad words, one extra load per
         # thread and iteration; -0.74 ms/step on ResNet-50)
-        u.mask = None
-        if tape and training and act != ACT_NONE and (other is not None or residual is not None):
+        if training and act != ACT_NONE and (other is not None or residual is not None):
             u.mask = torch.empty(ops.bn_act_mask_bytes(u.z.numel() // u.z.shape[-1], u.z.shape[-1]), device=self.device,
                                  dtype=torch.uint8)
         if other is not None:
@@ -445,15 +478,19 @@ class Runtime(object):
             u.y = ops.bn_apply(u.z, u.scale, u.shift, act, residual=residual, act_mask=u.mask)
         return u
 
-    def _conv_and_coeffs(self, u, x, w16, training):
+    def _conv_and_coeffs(self, u, w, training, fuse_stats=True):
         """z = conv(x) and the BN coefficients; in training the statistics are accumulated by the conv epilogue
-        itself whenever the output width allows it (saves one full read of z).  L1 BN needs the mean before it can
-        sum |z - mean|, so its statistics always come from bn_l1_stats."""
-        if training and not u.bn.l1 and ops.can_fuse_bn_stats(u.desc.K):
-            u.z = ops.conv_fprop(x, w16, u.desc, bn_stats_ws=self._ws)
+        itself whenever the output width allows it (saves one full read of z) and fuse_stats is set.  L1 BN needs the
+        mean before it can sum |z - mean|, so its statistics always come from bn_l1_stats; depthwise convolutions
+        have no such epilogue."""
+        if u.conv is not None and u.conv.kind == 'dw':
+            u.z = ops.dwconv_fprop(u.x, w, u.desc)
+            self._bn_coeffs(u, training)
+        elif fuse_stats and training and not u.bn.l1 and ops.can_fuse_bn_stats(u.desc.K):
+            u.z = ops.conv_fprop(u.x, w, u.desc, bn_stats_ws=self._ws)
             self._bn_coeffs(u, training, fused=True)
         else:
-            u.z = ops.conv_fprop(x, w16, u.desc)
+            u.z = ops.conv_fprop(u.x, w, u.desc)
             self._bn_coeffs(u, training)
         if self._coeffs_record is not None:
             self._coeffs_record.append((u.mean, u.invstd, u.scale, u.shift, u.sums, u.sign_sum))
@@ -501,7 +538,7 @@ class Runtime(object):
                          m.num_batches_tracked, u.mean, u.invstd, u.scale, u.shift, self._ws)
         else:
             self._eval_coeffs(bn, u.scale, u.shift)
-        bias = getattr(u.conv, 'bias32', None) if u.conv is not None else None
+        bias = u.conv.bias32 if u.conv is not None else None
         if bias is not None:            # conv bias in front of this BN (never on the ResNet / MobileNet-v2 paths)
             if training:                # the true pre-BN tensor is z + b: only the running mean sees it
                 if m.momentum is None:
@@ -510,19 +547,6 @@ class Runtime(object):
                     m.running_mean.add_(bias, alpha=float(m.momentum))
             else:
                 u.shift.add_(u.scale * bias)
-
-    def _stats_only(self, x, conv, bn, training):
-        """conv + BN coefficients without the apply (used for the downsample branch, fused into the main apply)."""
-        if not training and FOLD_BN_EVAL and not self._want_tape:
-            return self._unit_fwd_folded(x, conv, bn, ACT_NONE)       # y = bn_ds(conv_ds(x)) in one kernel
-        N, H, W, _ = x.shape
-        u = _Unit()
-        u.conv, u.bn, u.act, u.x = conv, bn, ACT_NONE, x
-        u.desc = conv.desc(N, H, W)
-        u.w = conv.kernel_weights()
-        self._conv_and_coeffs(u, x, u.w, training)
-        u.y = None
-        return u
 
     def _sync_bn_sums(self, sums):
         """SyncBatchNorm backward: the input gradient needs the GLOBAL d gamma / d beta sums divided by the global pixel
@@ -536,13 +560,13 @@ class Runtime(object):
         """BN (+activation) backward of unit u: returns dz (and g = dy*act'(.) when want_g).
         y_mask=None with an activation: the mask is recomputed from z inside the kernels (no read of y)."""
         bn = u.bn
-        drop = getattr(u, 'drop', None)
+        drop = u.drop
         if drop is not None:        # dropout(relu(bn(z))): g = bit ? dy * c : 0 from the forward's mask bits
             ops.bn_bwd_reduce_dropout(dy, u.z, u.mask, drop[1], u.mean, u.invstd, u.sums, bn.dgamma, bn.dbeta, self._ws)
             if self.sync_bn_world > 1:
                 self._sync_bn_sums(u.sums)
             return ops.bn_bwd_dx_dropout(dy, u.z, u.mask, drop[1], u.mean, u.invstd, bn.gamma, u.sums), None
-        mask = getattr(u, 'mask', None) if y_mask is not None else None
+        mask = u.mask if y_mask is not None else None
         ops.bn_bwd_reduce(dy, y_mask, u.z, act, u.mean, u.invstd, bn.gamma, bn.beta, u.sums, bn.dgamma, bn.dbeta,
                           self._ws, act_mask=mask)
         if self.sync_bn_world > 1:
@@ -604,13 +628,14 @@ class Runtime(object):
         self.grad_bucket_hook.finish()
         self._bucket_hi = None
 
-    @staticmethod
-    def _spec_lo(convs):
-        return min(c.slot.offset for c in convs)
-
     def _conv_bwd(self, u, dz, need_dx=True, residual=None):
         """wgrad into the gradient arena and (optionally) dgrad."""
         conv = u.conv
+        if conv.kind == 'dw':
+            # like the dense weight gradients: on the side stream (all depthwise wgrads share _dw_ws, the stream orders
+            # them), off the BN-backward -> dgrad chain
+            self._wgrad_async(lambda: ops.dwconv_wgrad(u.x, dz, u.desc, conv.g32, self._dw_ws), u.x, dz)
+            return ops.dwconv_dgrad(dz, conv.w16, u.desc) if need_dx else None
         if conv.groups == 1:
             self._wgrad_async(lambda: ops.conv_wgrad(u.x, dz, u.desc, conv.g32), u.x, dz)
         else:  # windowed (block-diagonal) wgrad into a scratch [K, T, window], then keep each channel's group
@@ -632,15 +657,8 @@ class Runtime(object):
 
     # ---- classifier head: global average pool -> (dropout) -> linear as a 1x1 conv on a 1x1 map ----------
     def _head_build(self, fc, dropout_p=0.0):
-        a = self.arena
-        sw, sb = a.slot(fc.weight), a.slot(fc.bias)
+        self.fc = _Linear(self.arena, fc)
         self.classes = fc.out_features
-        self.classes_pad = _round_up(self.classes, 8)
-        self.fc_in = fc.in_features
-        self.fc_w16 = a.kernel_view(a.p16, sw)       # [Kpad,1,C]
-        self.fc_gw = a.kernel_view(a.g32, sw)
-        self.fc_b = a.kernel_view(a.p32, sb)         # [Kpad]
-        self.fc_gb = a.kernel_view(a.g32, sb)
         self.dropout_p = float(dropout_p)
 
     def _head_fwd(self, h, training, want_tape):
@@ -652,33 +670,171 @@ class Runtime(object):
             keep = 1.0 - self.dropout_p
             mask = (torch.rand(feat.shape, device=self.device) < keep).to(torch.bfloat16) / keep
             feat = feat * mask
-        desc = ops.make_desc(N, 1, 1, self.fc_in, self.classes_pad, 1, 1, 1, 0, algo_macs=self.fc_in * self.classes)
-        logits = ops.conv_fprop(feat, self.fc_w16, desc, bias=self.fc_b, out_fp32=True).view(N, self.classes_pad)
-        out = logits if self.classes_pad == self.classes else logits[:, :self.classes]
+        fc = self.fc
+        desc = fc.desc(N, algo_macs=fc.C * self.classes)                 # the true MACs: fc.K is padded to 8
+        logits = fc.fwd(feat, desc, out_fp32=True).view(N, fc.K)
+        out = logits if fc.K == self.classes else logits[:, :self.classes]
         tape = {'feat': feat, 'mask': mask, 'last_shape': tuple(h.shape), 'fc_desc': desc,
                 'logits_pad': logits} if want_tape else None
         return out, tape
 
     def _head_bwd(self, tape, dlogits, dl_bf16=None):
-        N = dlogits.shape[0]
+        N, K = dlogits.shape[0], self.fc.K
         if dl_bf16 is not None:              # written by the fused softmax-CE kernel: bf16, padded, pad columns zero
             dl = dl_bf16
-        elif self.classes_pad == self.classes:
-            dl = torch.empty((N, self.classes_pad), device=self.device, dtype=torch.bfloat16)
+        elif K == self.classes:
+            dl = torch.empty((N, K), device=self.device, dtype=torch.bfloat16)
             ops.cast_bf16(dlogits.contiguous().float(), dl)
         else:
-            dl = torch.zeros((N, self.classes_pad), device=self.device, dtype=torch.bfloat16)
+            dl = torch.zeros((N, K), device=self.device, dtype=torch.bfloat16)
             dl[:, :self.classes].copy_(dlogits)
-        desc = tape['fc_desc']
-        dl4 = dl.view(N, 1, 1, self.classes_pad)
-        ops.colsum_bf16(dl, self.fc_gb)
-        feat = tape['feat']
-        self._wgrad_async(lambda: ops.conv_wgrad(feat, dl4, desc, self.fc_gw), feat, dl4)
-        wt = ops.weight_transpose(self.fc_w16)
-        dfeat = ops.conv_dgrad(dl4, wt, desc)
+        dfeat = self.fc.bwd(self, tape['feat'], dl.view(N, 1, 1, K), tape['fc_desc'])
         if tape['mask'] is not None:
             dfeat = dfeat * tape['mask']
         return ops.avgpool_bwd(dfeat, tape['last_shape'])
+
+    # ---- stem: conv -> BN -> activation (-> 3x3/s2 max-pool) on the relayout of the network input ----------
+    def _stem_build(self, conv, bn, act, maxpool=False, fused_stats=True):
+        """conv: a 7x7/s2 (3 input channels; run as space-to-depth) or 3x3 nn.Conv2d.  fused_stats=False takes the
+        separate bn_stats pass even where the conv epilogue could accumulate the statistics (the MobileNet stems
+        always have)."""
+        self.imagenet_stem = conv.kernel_size == (7, 7)
+        if conv.groups != 1 or conv.bias is not None or conv.dilation != (1, 1):
+            raise B200Error('unsupported stem: grouped, biased or dilated convolution')
+        if self.imagenet_stem:
+            if conv.stride != (2, 2) or conv.padding != (3, 3) or conv.in_channels != 3:
+                raise B200Error('unsupported 7x7 stem geometry')
+        elif conv.kernel_size != (3, 3) or conv.in_channels > 16 or conv.stride[0] != conv.stride[1] or \
+                conv.padding[0] != conv.padding[1]:
+            raise B200Error('unsupported stem geometry')
+        self.stem_conv, self.stem_bn, self.stem_act = conv, _BN(self.arena, bn), act
+        self.has_maxpool, self.stem_fused_stats = maxpool, fused_stats
+        s = self.arena.slot(conv.weight)
+        self.stem_w32 = self.arena.p32[s.offset:s.offset + s.numel]      # [K][R][S][C] fp32
+        self.stem_g32 = self.arena.g32[s.offset:s.offset + s.numel]
+
+    def _stem_fwd(self, x, training, mix=None, aug=None):
+        x, prep, (N, Cin, H, W) = self._input(x, mix, aug)
+        K = self.stem_conv.out_channels
+        if self.imagenet_stem:
+            ws = torch.empty((K, 16, 16), device=self.device, dtype=torch.bfloat16)
+            ops.stem_weight_to_s2d(self.stem_w32, K, Cin, 16, ws)
+            Hs, Ws = H // 2, W // 2
+            # 7x7/s2 -> space-to-depth 4x4/s1 on 16 channels -> 4x1 on "wide pixels": 4 neighbouring 32-byte
+            # pixels of the zero-bordered tensor are read as ONE 64-channel (128 B) pixel, so every tap row is a
+            # full 128B-swizzle TMA tile (4 loads per tile instead of 16 quarter-width ones).
+            xs = prep(x, 16, s2d=True, border=True)                # [N, Hs+3, Ws+3, 16], data at (+2,+2)
+            desc = ops.make_desc(N, Hs + 3, Ws, 64, K, 4, 1, 1, 0, P=Hs, Q=Ws,
+                                 x_strides=(16, (Ws + 3) * 16, (Hs + 3) * (Ws + 3) * 16), algo_macs=K * 49 * Cin)
+            if Ws + 3 <= 128:
+                # same bordered tensor described as the dense 4x4 / pad-0 convolution it is: the library runs it
+                # on the halo kernel (one 32-byte-row tile load per output row, weights stationary in smem)
+                desc = ops.make_desc(N, Hs + 3, Ws + 3, 16, K, 4, 4, 1, 0, P=Hs, Q=Ws, algo_macs=K * 49 * Cin)
+        else:
+            xs = prep(x, 16, s2d=False)
+            ws = torch.zeros((K, 9, 16), device=self.device, dtype=torch.bfloat16)
+            ws[:, :, :Cin].copy_(self.stem_w32.view(K, 9, Cin))       # 432-element pad+cast of the 3-channel stem
+            desc = ops.make_desc(N, H, W, 16, K, 3, 3, self.stem_conv.stride[0], self.stem_conv.padding[0],
+                                 algo_macs=K * 9 * Cin)
+        u = _Unit(None, self.stem_bn, self.stem_act, xs)
+        u.desc = desc
+        self._conv_and_coeffs(u, ws, training, fuse_stats=self.stem_fused_stats)
+        st = {'unit': u, 'cin': Cin}
+        if self.has_maxpool:
+            # bn1 -> relu -> maxpool in one pass: the [N, 112, 112, 64] activation is never written
+            out, st['argmax'] = ops.bn_apply_maxpool(u.z, u.scale, u.shift, u.act)
+        else:
+            u.y = ops.bn_apply(u.z, u.scale, u.shift, u.act)
+            out = u.y
+        return out, st
+
+    def _stem_bwd(self, st, dy):
+        u = st['unit']
+        if self.has_maxpool:
+            dy = ops.maxpool_bwd(dy, st['argmax'], tuple(u.z.shape))
+        dz, _ = self._bn_bwd(u, dy, None, u.act)   # mask recomputed from z: the activation is not needed
+        K, Cin = self.stem_conv.out_channels, st['cin']
+
+        def stem_wgrad():   # every wgrad shares the split-K workspace: all of them go through _wgrad_async
+            if self.imagenet_stem:
+                dws = torch.zeros((K, 16, 16), device=self.device, dtype=torch.float32)
+                ops.conv_wgrad(u.x, dz, u.desc, dws)
+                ops.stem_wgrad_from_s2d(dws, K, Cin, 16, self.stem_g32)
+            else:
+                dws = torch.zeros((K, 9, 16), device=self.device, dtype=torch.float32)
+                ops.conv_wgrad(u.x, dz, u.desc, dws)
+                self.stem_g32.view(K, 9, Cin).add_(dws[:, :, :Cin])
+        self._wgrad_async(stem_wgrad, u.x, dz)
+
+    # ---- whole network: stem, blocks, head; backward in reverse with the gradient buckets ---------------------
+    def run_forward(self, x, training, want_tape, mix=None, aug=None):
+        self._want_tape = want_tape
+        if training:
+            self.arena.version += 1          # running statistics change: folded inference weights become stale
+            if self.dropout_key is not None:
+                self.dropout_key.random_(-2 ** 63, None)         # the full 64-bit range
+        h, stem = self._stem_fwd(x, training, mix, aug)
+        saved = []
+        # eval and tapeless training forwards (calibrate_bn) keep nothing to recompute: only a backward pass needs it
+        ckpt = {a: b for a, b in self.segments} if (training and want_tape) else {}
+        i = 0
+        while i < len(self.blocks):
+            if i in ckpt:
+                # checkpointed segment: keep its input and each unit's coefficients; z, y and the masks are dropped
+                seg_in, coeffs = h, []
+                try:
+                    for spec in self.blocks[i:ckpt[i]]:
+                        self._coeffs_record = []
+                        h, _ = self._block_fwd(spec, h, training)
+                        coeffs.append(self._coeffs_record)
+                finally:
+                    self._coeffs_record = None
+                saved.append({'segment': (i, ckpt[i]), 'x': seg_in, 'coeffs': coeffs})
+                saved += [None] * (ckpt[i] - i - 1)
+                i = ckpt[i]
+                continue
+            h, s = self._block_fwd(self.blocks[i], h, training)
+            saved.append(s if want_tape else None)
+            i += 1
+        out, head = self._head_fwd(h, training, want_tape)
+        tape = {'stem': stem, 'blocks': saved, 'head': head} if want_tape else None
+        return out, tape
+
+    def _recompute(self, seg):
+        """the block tapes of a checkpointed segment, rebuilt from its input by the forward's own launches"""
+        h, tapes = seg['x'], []
+        a, b = seg['segment']
+        try:
+            for spec, coeffs in zip(self.blocks[a:b], seg['coeffs']):
+                self._coeffs_replay = list(coeffs)
+                h, s = self._block_fwd(spec, h, True)
+                tapes.append(s)
+        finally:
+            self._coeffs_replay = None
+        return tapes
+
+    def run_backward(self, tape, dlogits, dl_bf16=None):
+        self._transpose_weights()
+        self._buckets_begin()
+        d = self._head_bwd(tape['head'], dlogits, dl_bf16)
+        blocks = list(tape['blocks'])
+        seg_start = {s['segment'][1] - 1: i for i, s in enumerate(blocks) if s is not None and 'segment' in s}
+        for i in range(len(self.blocks) - 1, -1, -1):
+            spec = self.blocks[i]
+            if i in seg_start:
+                a = seg_start[i]
+                blocks[a:i + 1] = self._recompute(blocks[a])
+            d = self._block_bwd(spec, blocks[i], d)
+            blocks[i] = None
+            if spec['dense']:                # blocks of depthwise convolutions only have no bucket point
+                self._bucket_point(min(c.slot.offset for c in spec['dense']))
+            if i in seg_start.values():
+                # end of a recomputed segment's backward: the side-stream wgrads still read its tensors; joining here
+                # lets the allocator hand them to the next segment instead of keeping every segment to the end
+                self._wgrad_join()
+        self._stem_bwd(tape['stem'], d)
+        self._wgrad_join()
+        self._buckets_end()
 
     # ---- autograd glue ----------------------------------------------------------------------------
     def forward(self, x):
@@ -693,12 +849,6 @@ class Runtime(object):
         # autograd history, so a backward() through them fails loudly instead of using batch-statistics formulas
         logits, _ = self.run_forward(x, training, False)
         return logits
-
-    def run_forward(self, x, training, want_tape, mix=None, aug=None):
-        raise NotImplementedError
-
-    def run_backward(self, tape, dlogits, dl_bf16=None):
-        raise NotImplementedError
 
     def train_step(self, x, target, smooth_eps=0.0, upstream=None, mix=None, aug=None, reduce=True):
         """forward + mean softmax cross-entropy (label smoothing ``smooth_eps``) + backward of one batch as a straight
@@ -827,22 +977,8 @@ class ResNetRuntime(Runtime):
         from .models.modules.lp_norm import L1BatchNorm2d
         from .models.modules.checkpoint import CheckpointModule
         m, a = self.model, self.arena
-        self.imagenet_stem = m.conv1.kernel_size == (7, 7)
-        if self.imagenet_stem:
-            if m.conv1.stride != (2, 2) or m.conv1.padding != (3, 3) or m.conv1.in_channels != 3:
-                raise B200Error('unsupported 7x7 stem geometry')
-        elif m.conv1.kernel_size != (3, 3) or m.conv1.stride != (1, 1) or m.conv1.in_channels > 16:
-            raise B200Error('unsupported stem geometry')
-        self.stem_conv = m.conv1
-        s = a.slot(m.conv1.weight)
-        self.stem_w32 = a.p32[s.offset:s.offset + s.numel]      # [K][R][S][C] fp32
-        self.stem_g32 = a.g32[s.offset:s.offset + s.numel]
-        self.stem_bn = _BN(a, m.bn1)
-        self.has_maxpool = isinstance(m.maxpool, nn.MaxPool2d)
+        self._stem_build(m.conv1, m.bn1, ACT_RELU, maxpool=isinstance(m.maxpool, nn.MaxPool2d))
         self.blocks = []
-        # checkpoint_segments: [start, end) ranges of self.blocks whose activations the forward pass does not keep;
-        # the backward pass recomputes each range just before it needs it
-        self.segments = []
         n_drop = 0
         for lname in ('layer1', 'layer2', 'layer3', 'layer4'):
             layer = getattr(m, lname)
@@ -875,68 +1011,13 @@ class ResNetRuntime(Runtime):
                 spec['down'] = None
                 if blk.downsample is not None:
                     spec['down'] = (_Conv(a, blk.downsample[0]), _BN(a, blk.downsample[1]))
+                spec['dense'] = spec['convs'] + ([spec['down'][0]] if spec['down'] is not None else [])
                 # squeeze-excitation on the residual branch (resnet_se / resnext_se): one gate per stage, shared
                 spec['se'] = _SE(a, blk.residual_block) if blk.residual_block is not None else None
                 self.blocks.append(spec)
         self._head_build(m.fc)
-        # one 64-bit Philox key per training step, drawn on the device with torch's CUDA generator (a captured step
-        # draws a fresh one on every replay; torch.manual_seed makes runs reproducible)
-        self.dropout_key = torch.zeros(1, device=self.device, dtype=torch.int64) if n_drop else None
-
-    # ---- stem ---------------------------------------------------------------------------------------
-    def _stem_fwd(self, x, training, mix=None, aug=None):
-        x, prep, (N, Cin, H, W) = self._input(x, mix, aug)
-        K = self.stem_conv.out_channels
-        st = {}
-        if self.imagenet_stem:
-            ws = torch.empty((K, 16, 16), device=self.device, dtype=torch.bfloat16)
-            ops.stem_weight_to_s2d(self.stem_w32, K, Cin, 16, ws)
-            Hs, Ws = H // 2, W // 2
-            # 7x7/s2 -> space-to-depth 4x4/s1 on 16 channels -> 4x1 on "wide pixels": 4 neighbouring 32-byte
-            # pixels of the zero-bordered tensor are read as ONE 64-channel (128 B) pixel, so every tap row is a
-            # full 128B-swizzle TMA tile (4 loads per tile instead of 16 quarter-width ones).
-            xs = prep(x, 16, s2d=True, border=True)                # [N, Hs+3, Ws+3, 16], data at (+2,+2)
-            desc = ops.make_desc(N, Hs + 3, Ws, 64, K, 4, 1, 1, 0, P=Hs, Q=Ws,
-                                 x_strides=(16, (Ws + 3) * 16, (Hs + 3) * (Ws + 3) * 16), algo_macs=K * 49 * Cin)
-            if Ws + 3 <= 128:
-                # same bordered tensor described as the dense 4x4 / pad-0 convolution it is: the library runs it
-                # on the halo kernel (one 32-byte-row tile load per output row, weights stationary in smem)
-                desc = ops.make_desc(N, Hs + 3, Ws + 3, 16, K, 4, 4, 1, 0, P=Hs, Q=Ws, algo_macs=K * 49 * Cin)
-        else:
-            xs = prep(x, 16, s2d=False)
-            ws = torch.zeros((K, 9, 16), device=self.device, dtype=torch.bfloat16)
-            ws[:, :, :Cin].copy_(self.stem_w32.view(K, 9, Cin))       # 432-element pad+cast of the 3-channel stem
-            desc = ops.make_desc(N, H, W, 16, K, 3, 3, 1, 1, algo_macs=K * 9 * Cin)
-        u = _Unit()
-        u.conv, u.bn, u.act, u.x, u.desc = None, self.stem_bn, ACT_RELU, xs, desc
-        self._conv_and_coeffs(u, xs, ws, training)
-        st['unit'] = u
-        if self.has_maxpool:
-            # bn1 -> relu -> maxpool in one pass: the [N, 112, 112, 64] activation is never written
-            u.y = None
-            out, st['argmax'] = ops.bn_apply_maxpool(u.z, u.scale, u.shift, ACT_RELU)
-        else:
-            u.y = ops.bn_apply(u.z, u.scale, u.shift, ACT_RELU)
-            out = u.y
-        st['cin'] = Cin
-        return out, st
-
-    def _stem_bwd(self, st, dy):
-        u = st['unit']
-        if self.has_maxpool:
-            dy = ops.maxpool_bwd(dy, st['argmax'], tuple(u.z.shape))
-        dz, _ = self._bn_bwd(u, dy, None, ACT_RELU)   # mask recomputed from z: the activation is not needed
-        K, Cin = self.stem_conv.out_channels, st['cin']
-        def stem_wgrad():   # every wgrad shares the split-K workspace: all of them go through _wgrad_async
-            if self.imagenet_stem:
-                dws = torch.zeros((K, 16, 16), device=self.device, dtype=torch.float32)
-                ops.conv_wgrad(u.x, dz, u.desc, dws)
-                ops.stem_wgrad_from_s2d(dws, K, Cin, 16, self.stem_g32)
-            else:
-                dws = torch.zeros((K, 9, 16), device=self.device, dtype=torch.float32)
-                ops.conv_wgrad(u.x, dz, u.desc, dws)
-                self.stem_g32.view(K, 9, Cin).add_(dws[:, :, :Cin])
-        self._wgrad_async(stem_wgrad, u.x, dz)
+        if n_drop:
+            self.dropout_key = torch.zeros(1, device=self.device, dtype=torch.int64)
 
     # ---- residual blocks ----------------------------------------------------------------------------
     def _block_fwd(self, spec, x, training):
@@ -944,24 +1025,24 @@ class ResNetRuntime(Runtime):
         units = []
         h = x
         for i in range(len(convs) - 1):
-            u = self._unit_fwd(h, convs[i], bns[i], ACT_RELU, training, True, drop=spec['drop'] if i == 0 else None)
+            u = self._unit_fwd(h, convs[i], bns[i], ACT_RELU, training, drop=spec['drop'] if i == 0 else None)
             units.append(u)
             h = u.y
         down, se_tape = None, None
-        if spec.get('se') is not None:
+        if spec['se'] is not None:
             # residual = SE(downsample(x) | x): the gate needs the materialised residual, so the downsample branch
             # gets its own BN-apply pass here instead of being folded into the join
             r = x
             if spec['down'] is not None:
-                down = self._unit_fwd(x, spec['down'][0], spec['down'][1], ACT_NONE, training, True)
+                down = self._unit_fwd(x, spec['down'][0], spec['down'][1], ACT_NONE, training)
                 r = down.y
             r, se_tape = spec['se'].fwd(r)
-            last = self._unit_fwd(h, convs[-1], bns[-1], ACT_RELU, training, True, residual=r)
+            last = self._unit_fwd(h, convs[-1], bns[-1], ACT_RELU, training, residual=r)
         elif spec['down'] is not None:
-            down = self._stats_only(x, spec['down'][0], spec['down'][1], training)
-            last = self._unit_fwd(h, convs[-1], bns[-1], ACT_RELU, training, True, other=down)
+            down = self._unit_fwd(x, spec['down'][0], spec['down'][1], ACT_NONE, training, apply=False)
+            last = self._unit_fwd(h, convs[-1], bns[-1], ACT_RELU, training, other=down)
         else:
-            last = self._unit_fwd(h, convs[-1], bns[-1], ACT_RELU, training, True, residual=x)
+            last = self._unit_fwd(h, convs[-1], bns[-1], ACT_RELU, training, residual=x)
         units.append(last)
         return last.y, {'units': units, 'down': down, 'se': se_tape}
 
@@ -970,7 +1051,7 @@ class ResNetRuntime(Runtime):
         last = units[-1]
         # out = relu(bn_last(z) + skip): g = dy * (out > 0) feeds both branches
         dz, g = self._bn_bwd(last, dy, last.y, ACT_RELU, want_g=True)
-        if saved.get('se') is not None:
+        if saved['se'] is not None:
             g = spec['se'].bwd(self, saved['se'], g)          # through the gate: dL/d(residual before SE)
         if down is not None:
             dzd, _ = self._bn_bwd(down, g, None, ACT_NONE)
@@ -985,106 +1066,37 @@ class ResNetRuntime(Runtime):
         dz, _ = self._bn_bwd(u, d, None, ACT_RELU)
         return self._conv_bwd(u, dz, residual=skip)
 
-    # ---- whole network ------------------------------------------------------------------------------
-    def run_forward(self, x, training, want_tape, mix=None, aug=None):
-        self._want_tape = want_tape
-        if training:
-            self.arena.version += 1          # running statistics change: folded inference weights become stale
-            if self.dropout_key is not None:
-                self.dropout_key.random_(-2 ** 63, None)         # the full 64-bit range
-        h, stem = self._stem_fwd(x, training, mix, aug)
-        saved = []
-        # eval and tapeless training forwards (calibrate_bn) keep nothing to recompute: only a backward pass needs it
-        ckpt = {a: b for a, b in self.segments} if (training and want_tape) else {}
-        i = 0
-        while i < len(self.blocks):
-            if i in ckpt:
-                # checkpointed segment: keep its input and each unit's coefficients; z, y and the masks are dropped
-                seg_in, coeffs = h, []
-                try:
-                    for spec in self.blocks[i:ckpt[i]]:
-                        self._coeffs_record = []
-                        h, _ = self._block_fwd(spec, h, training)
-                        coeffs.append(self._coeffs_record)
-                finally:
-                    self._coeffs_record = None
-                saved.append({'segment': (i, ckpt[i]), 'x': seg_in, 'coeffs': coeffs})
-                saved += [None] * (ckpt[i] - i - 1)
-                i = ckpt[i]
-                continue
-            h, s = self._block_fwd(self.blocks[i], h, training)
-            saved.append(s if want_tape else None)
-            i += 1
-        out, head = self._head_fwd(h, training, want_tape)
-        tape = {'stem': stem, 'blocks': saved, 'head': head} if want_tape else None
-        return out, tape
-
-    def _recompute(self, seg):
-        """the block tapes of a checkpointed segment, rebuilt from its input by the forward's own launches"""
-        h, tapes = seg['x'], []
-        a, b = seg['segment']
-        try:
-            for spec, coeffs in zip(self.blocks[a:b], seg['coeffs']):
-                self._coeffs_replay = list(coeffs)
-                h, s = self._block_fwd(spec, h, True)
-                tapes.append(s)
-        finally:
-            self._coeffs_replay = None
-        return tapes
-
-    def run_backward(self, tape, dlogits, dl_bf16=None):
-        self._transpose_weights()
-        self._buckets_begin()
-        d = self._head_bwd(tape['head'], dlogits, dl_bf16)
-        blocks = list(tape['blocks'])
-        seg_start = {s['segment'][1] - 1: i for i, s in enumerate(blocks) if s is not None and 'segment' in s}
-        for i in range(len(self.blocks) - 1, -1, -1):
-            spec = self.blocks[i]
-            if i in seg_start:
-                a = seg_start[i]
-                blocks[a:i + 1] = self._recompute(blocks[a])
-            d = self._block_bwd(spec, blocks[i], d)
-            blocks[i] = None
-            convs = spec['convs'] + ([spec['down'][0]] if spec['down'] is not None else [])
-            self._bucket_point(self._spec_lo(convs))
-            if i in seg_start.values():
-                # end of a recomputed segment's backward: the side-stream wgrads still read its tensors; joining here
-                # lets the allocator hand them to the next segment instead of keeping every segment to the end
-                self._wgrad_join()
-        self._stem_bwd(tape['stem'], d)
-        self._wgrad_join()
-        self._buckets_end()
-
 
 class MobileNetRuntime(Runtime):
     """Pipeline for models.mobilenet_v2.MobileNet_v2: 1x1 expand / depthwise 3x3 / 1x1 project units with
     BN + ReLU6, identity skips, dropout + linear head (reference: models/mobilenet_v2.py:39-156)."""
 
+    # BN is not folded into the convolutions of an eval forward, and the stem takes the separate bn_stats pass (at
+    # width 2 its 64 channels would allow the fused epilogue statistics): both as these runtimes have always run
+    fold_bn_eval = False
+
     def _build(self):
-        m, a = self.model, self.arena
+        m = self.model
         f = m.features
-        conv0 = f.conv0[0]
-        if conv0.kernel_size != (3, 3) or conv0.in_channels > 16 or conv0.groups != 1:
-            raise B200Error('unsupported MobileNet stem')
-        self.stem_conv = conv0
-        s = a.slot(conv0.weight)
-        self.stem_w32 = a.p32[s.offset:s.offset + s.numel]
-        self.stem_g32 = a.g32[s.offset:s.offset + s.numel]
-        self.stem_bn = _BN(a, f.conv0[1])
+        self._stem_build(f.conv0[0], f.conv0[1], ACT_RELU6, fused_stats=False)
         self.blocks = []
         for name, mod in f.named_children():
             if not name.startswith('bottleneck'):
                 continue
             if mod.residual_block is not None:
                 raise B200Error('residual_block is outside the B200 hot path')
-            self.blocks.append({'add_res': mod.add_res, 'units': self._parse_units(list(mod.block))})
-        self.blocks.append({'add_res': False, 'units': self._parse_units(list(f.conv1))})
+            self.blocks.append(self._block_spec(list(mod.block), mod.add_res))
+        self.blocks.append(self._block_spec(list(f.conv1), False))
         drop, fc = m.classifier[0], m.classifier[1]
         self._head_build(fc, dropout_p=drop.p if isinstance(drop, nn.Dropout) else 0.0)
-        max_c = max(u[1].C for b in self.blocks for u in b['units'] if u[0] == 'dw')
+        self._dw_build()
+
+    def _dw_build(self):
+        max_c = max(c.C for b in self.blocks for c, _, _ in b['units'] if c.kind == 'dw')
         self._dw_ws = torch.empty(592 * 9 * max_c, device=self.device, dtype=torch.float32)
 
-    def _parse_units(self, layers):
+    def _block_spec(self, layers, add_res):
+        """[conv, BN, (ReLU6 | ReLU)] ... -> {'add_res', 'units': [(_Conv, _BN, act)], 'dense'}"""
         units, i = [], 0
         while i < len(layers):
             conv, bn = layers[i], layers[i + 1]
@@ -1092,96 +1104,26 @@ class MobileNetRuntime(Runtime):
             act = ACT_NONE
             if has_act:
                 act = ACT_RELU6 if isinstance(layers[i + 2], nn.ReLU6) else ACT_RELU
-            kind = 'dw' if conv.groups > 1 else 'dense'
-            units.append((kind, _Conv(self.arena, conv), _BN(self.arena, bn), act))
+            units.append((_Conv(self.arena, conv), _BN(self.arena, bn), act))
             i += 3 if has_act else 2
-        return units
+        return {'add_res': add_res, 'units': units, 'dense': [c for c, _, _ in units if c.kind != 'dw']}
 
-    def _mb_unit_fwd(self, x, kind, conv, bn, act, training, residual=None):
-        N, H, W, _ = x.shape
-        u = _Unit()
-        u.conv, u.bn, u.act, u.x = conv, bn, act, x
-        u.desc = conv.desc(N, H, W)
-        if kind == 'dw':
-            u.w = None
-            u.z = ops.dwconv_fprop(x, conv.w16, u.desc)
-            self._bn_coeffs(u, training)
-        else:
-            u.w = conv.kernel_weights()
-            self._conv_and_coeffs(u, x, u.w, training)
-        u.y = ops.bn_apply(u.z, u.scale, u.shift, act, residual=residual)
-        return u
+    def _block_fwd(self, spec, x, training):
+        h, units = x, []
+        for j, (conv, bn, act) in enumerate(spec['units']):
+            last = j == len(spec['units']) - 1
+            u = self._unit_fwd(h, conv, bn, act, training, residual=x if (last and spec['add_res']) else None)
+            units.append(u)
+            h = u.y
+        return h, units
 
-    def _mb_conv_bwd(self, kind, u, dz, need_dx=True, residual=None):
-        if kind == 'dw':
-            # like the dense weight gradients: on the side stream (all depthwise wgrads share _dw_ws, the stream orders
-            # them), off the BN-backward -> dgrad chain
-            self._wgrad_async(lambda: ops.dwconv_wgrad(u.x, dz, u.desc, u.conv.g32, self._dw_ws), u.x, dz)
-            return ops.dwconv_dgrad(dz, u.conv.w16, u.desc) if need_dx else None
-        return self._conv_bwd(u, dz, need_dx=need_dx, residual=residual)
-
-    def _stem_fwd(self, x, training, mix=None, aug=None):
-        x, prep, (N, Cin, H, W) = self._input(x, mix, aug)
-        K = self.stem_conv.out_channels
-        xs = prep(x, 16, s2d=False)
-        ws = torch.zeros((K, 9, 16), device=self.device, dtype=torch.bfloat16)
-        ws[:, :, :Cin].copy_(self.stem_w32.view(K, 9, Cin))
-        st, pad = self.stem_conv.stride[0], self.stem_conv.padding[0]
-        act = getattr(self, 'stem_act', ACT_RELU6)
-        u = _Unit()
-        u.conv, u.bn, u.act, u.x = None, self.stem_bn, act, xs
-        u.desc = ops.make_desc(N, H, W, 16, K, 3, 3, st, pad, algo_macs=K * 9 * Cin)
-        u.z = ops.conv_fprop(xs, ws, u.desc)
-        self._bn_coeffs(u, training)
-        u.y = ops.bn_apply(u.z, u.scale, u.shift, act)
-        return u.y, {'unit': u, 'cin': Cin}
-
-    def _stem_bwd(self, st, dy):
-        u = st['unit']
-        dz, _ = self._bn_bwd(u, dy, None, u.act)
-        K, Cin = self.stem_conv.out_channels, st['cin']
-        def stem_wgrad():
-            dws = torch.zeros((K, 9, 16), device=self.device, dtype=torch.float32)
-            ops.conv_wgrad(u.x, dz, u.desc, dws)
-            self.stem_g32.view(K, 9, Cin).add_(dws[:, :, :Cin])
-        self._wgrad_async(stem_wgrad, u.x, dz)
-
-    def run_forward(self, x, training, want_tape, mix=None, aug=None):
-        self._want_tape = want_tape
-        if training:
-            self.arena.version += 1
-        h, stem = self._stem_fwd(x, training, mix, aug)
-        saved = []
-        for spec in self.blocks:
-            xin, units = h, []
-            for j, (kind, conv, bn, act) in enumerate(spec['units']):
-                last = j == len(spec['units']) - 1
-                u = self._mb_unit_fwd(h, kind, conv, bn, act, training,
-                                      residual=xin if (last and spec['add_res']) else None)
-                units.append(u)
-                h = u.y
-            saved.append(units if want_tape else None)
-        out, head = self._head_fwd(h, training, want_tape)
-        tape = {'stem': stem, 'blocks': saved, 'head': head} if want_tape else None
-        return out, tape
-
-    def run_backward(self, tape, dlogits, dl_bf16=None):
-        self._transpose_weights()
-        self._buckets_begin()
-        d = self._head_bwd(tape['head'], dlogits, dl_bf16)
-        for spec, units in zip(reversed(self.blocks), reversed(tape['blocks'])):
-            skip = d if spec['add_res'] else None   # out = bn(z) + x (no activation): the skip gradient is dy itself
-            for j in range(len(units) - 1, -1, -1):
-                kind, _, _, act = spec['units'][j]
-                u = units[j]
-                dz, _ = self._bn_bwd(u, d, None, act)
-                d = self._mb_conv_bwd(kind, u, dz, residual=skip if j == 0 else None)
-            dense = [c for k, c, _, _ in spec['units'] if k != 'dw']
-            if dense:
-                self._bucket_point(self._spec_lo(dense))
-        self._stem_bwd(tape['stem'], d)
-        self._wgrad_join()
-        self._buckets_end()
+    def _block_bwd(self, spec, units, d):
+        skip = d if spec['add_res'] else None   # out = bn(z) + x (no activation): the skip gradient is dy itself
+        for j in range(len(units) - 1, -1, -1):
+            u = units[j]
+            dz, _ = self._bn_bwd(u, d, None, u.act)
+            d = self._conv_bwd(u, dz, residual=skip if j == 0 else None)
+        return d
 
 
 class MobileNetV1Runtime(MobileNetRuntime):
@@ -1190,23 +1132,12 @@ class MobileNetV1Runtime(MobileNetRuntime):
     MobileNetRuntime with ReLU instead of ReLU6 and no skips."""
 
     def _build(self):
-        m, a = self.model, self.arena
-        layers = list(m.features)
-        conv0, bn0 = layers[0], layers[1]
-        if conv0.kernel_size != (3, 3) or conv0.in_channels > 16 or conv0.groups != 1 or conv0.bias is not None:
-            raise B200Error('unsupported MobileNet stem')
-        self.stem_conv = conv0
-        s = a.slot(conv0.weight)
-        self.stem_w32 = a.p32[s.offset:s.offset + s.numel]
-        self.stem_g32 = a.g32[s.offset:s.offset + s.numel]
-        self.stem_bn = _BN(a, bn0)
-        self.stem_act = ACT_RELU6 if isinstance(layers[2], nn.ReLU6) else ACT_RELU
-        self.blocks = []
-        for mod in layers[3:]:
-            self.blocks.append({'add_res': False, 'units': self._parse_units(list(mod.components))})
-        self._head_build(m.fc, dropout_p=0.0)
-        max_c = max(u[1].C for b in self.blocks for u in b['units'] if u[0] == 'dw')
-        self._dw_ws = torch.empty(592 * 9 * max_c, device=self.device, dtype=torch.float32)
+        layers = list(self.model.features)
+        self._stem_build(layers[0], layers[1], ACT_RELU6 if isinstance(layers[2], nn.ReLU6) else ACT_RELU,
+                         fused_stats=False)
+        self.blocks = [self._block_spec(list(mod.components), False) for mod in layers[3:]]
+        self._head_build(self.model.fc, dropout_p=0.0)
+        self._dw_build()
 
 
 def enable_sync_batchnorm(model, process_group=None):
@@ -1223,7 +1154,7 @@ def enable_sync_batchnorm(model, process_group=None):
     from .models.modules.lp_norm import L1BatchNorm2d
     if any(isinstance(m, L1BatchNorm2d) for m in model.modules()):
         raise NotImplementedError('SyncBatchNorm is not implemented for L1 BatchNorm (bn_norm=\'L1\')')
-    if getattr(rt, 'segments', None):
+    if rt.segments:
         raise NotImplementedError('SyncBatchNorm is not implemented with checkpoint_segments: the recompute would '
                                   'all-reduce every checkpointed layer\'s statistics a second time')
     rt.sync_bn_group = process_group

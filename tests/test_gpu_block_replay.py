@@ -632,8 +632,9 @@ def _mutant_momentum(monkeypatch, rt, mine):
 def _mutant_se_scratch(monkeypatch, rt, mine):
     """layer3.1 writes its gate gradients to scratch instead of accumulating them into the stage's shared gate"""
     se = _spec(rt, mine, 'layer3.1')['se']
-    for a in ('gw1', 'gb1', 'gw2', 'gb2'):
-        monkeypatch.setattr(se, a, torch.zeros_like(getattr(se, a)))
+    for lin in (se.l1, se.l2):
+        for a in ('gw', 'gb'):
+            monkeypatch.setattr(lin, a, torch.zeros_like(getattr(lin, a)))
     return 'layer3', lambda q: 'residual_block' in q
 
 
@@ -663,7 +664,7 @@ def _mutant_upstream_bias(monkeypatch, rt, mine):
     orig = ops.colsum_bf16
 
     def colsum(m, out):
-        if out.data_ptr() == rt.fc_gb.data_ptr():
+        if out.data_ptr() == rt.fc.gb.data_ptr():
             m = (m.float() / 8.0).to(torch.bfloat16)
         return orig(m, out)
     monkeypatch.setattr(ops, 'colsum_bf16', colsum)

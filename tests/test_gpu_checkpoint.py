@@ -136,7 +136,7 @@ def test_recomputed_activations_bitwise(name, s):
                 units.append((ref['down'], rec['down']))
             for u, v in units:
                 for f in ('z', 'y', 'mask'):
-                    p, q = getattr(u, f, None), getattr(v, f, None)     # _stats_only units have no mask
+                    p, q = getattr(u, f), getattr(v, f)     # downsample units without the apply have no mask
                     assert (p is None) == (q is None) and (p is None or torch.equal(p, q)), (j, f)
                 for f in ('mean', 'invstd', 'scale', 'shift'):
                     assert torch.equal(getattr(u, f), getattr(v, f)), (j, f)
@@ -278,7 +278,7 @@ def _tape_bytes(blocks):
     for saved in blocks:
         units = list(saved['units']) + ([saved['down']] if saved['down'] is not None else [])
         for u in units:
-            for t in (u.z, u.y, getattr(u, 'mask', None)):
+            for t in (u.z, u.y, u.mask):
                 n += t.numel() * t.element_size() if t is not None else 0
     return n
 

@@ -307,8 +307,8 @@ def _mobilenet_parity(factory, stem_name, size=128, batch=32):
     mine.train()
     flat = [(None, None, rt.stem_bn, None, stem_name)]
     for spec in rt.blocks:
-        for kind, conv, bn, act in spec['units']:
-            flat.append((kind, conv, bn, act, conv.slot.name[:-len('.weight')]))
+        for conv, bn, act in spec['units']:
+            flat.append((conv.kind, conv, bn, act, conv.slot.name[:-len('.weight')]))
     assert len(flat) == len(units) and all(f[4] == u['conv'] for f, u in zip(flat, units))
     params = dict(mine.named_parameters())
     rt._transpose_weights()
@@ -324,10 +324,10 @@ def _mobilenet_parity(factory, stem_name, size=128, batch=32):
             dx = None
         else:
             skip = _nhwc(u['skip']) if u['skip'] is not None else None
-            uu = rt._mb_unit_fwd(_nhwc(u['x']), kind, conv, bn, act, True, residual=skip)
+            uu = rt._unit_fwd(_nhwc(u['x']), conv, bn, act, True, residual=skip)
             out = uu.y
             dz, _ = rt._bn_bwd(uu, dy, None, act)
-            dx = rt._mb_conv_bwd(kind, uu, dz)
+            dx = rt._conv_bwd(uu, dz)
         rt._wgrad_join()
         torch.cuda.synchronize()
         # d gamma and d beta are measured on ONE scale, the norm of the larger of the two: where a depthwise conv + BN
