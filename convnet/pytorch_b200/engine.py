@@ -667,9 +667,11 @@ class Runtime(object):
         mask = None
         if training and self.dropout_p > 0:
             # the Bernoulli draw uses torch's CUDA generator (RNG glue on a [N, C] tensor; mobilenet_v2.py:126)
+            # mask = keep / (1 - p) in fp32 and ONE rounding of the product to bf16, as F.dropout scales: a bf16 mask
+            # would carry a rounded scale (p = 0.1: 1.109375 instead of 1.1111) into every kept feature and gradient
             keep = 1.0 - self.dropout_p
-            mask = (torch.rand(feat.shape, device=self.device) < keep).to(torch.bfloat16) / keep
-            feat = feat * mask
+            mask = (torch.rand(feat.shape, device=self.device) < keep).float() * (1.0 / keep)
+            feat = (feat.float() * mask).to(torch.bfloat16)
         fc = self.fc
         desc = fc.desc(N, algo_macs=fc.C * self.classes)                 # the true MACs: fc.K is padded to 8
         logits = fc.fwd(feat, desc, out_fp32=True).view(N, fc.K)
@@ -690,7 +692,7 @@ class Runtime(object):
             dl[:, :self.classes].copy_(dlogits)
         dfeat = self.fc.bwd(self, tape['feat'], dl.view(N, 1, 1, K), tape['fc_desc'])
         if tape['mask'] is not None:
-            dfeat = dfeat * tape['mask']
+            dfeat = (dfeat.float() * tape['mask']).to(torch.bfloat16)
         return ops.avgpool_bwd(dfeat, tape['last_shape'])
 
     # ---- stem: conv -> BN -> activation (-> 3x3/s2 max-pool) on the relayout of the network input ----------

@@ -141,18 +141,66 @@ def _mb_conv_bn(x, sd, conv, bn, stride, pad, act, training, bufs, quant, skip=N
 _MBV1_STRIDES = (1, 2, 1, 2, 1, 2, 1, 1, 1, 1, 1, 2, 1)
 
 
-def forward_mobilenet_v1(sd, x, training=True, buffers_out=None, quant=False, trace=None):
-    """logits of a reference-layout MobileNet (v1) ``state_dict`` (models/mobilenet.py:39-156): stem conv/BN/ReLU, then
-    ``features.{i}.components`` = depthwise 3x3 (with bias) / BN / ReLU / 1x1 / BN / ReLU, average pool, ``fc``."""
-    x = _q(x, quant)
-    x = _mb_conv_bn(x, sd, 'features.0', 'features.1', 2, 1, 'relu', training, buffers_out, quant, trace=trace)
+def mobilenet_stem(sd):
+    """(conv, bn, stride, pad, act) of the 3x3/s2 stem of a MobileNet-v2 / v1 ``state_dict``"""
+    if 'features.conv0.0.weight' in sd:
+        return 'features.conv0.0', 'features.conv0.1', 2, 1, True
+    return 'features.0', 'features.1', 2, 1, 'relu'
+
+
+def mobilenet_blocks(sd):
+    """[(prefix, [(conv, bn, stride, pad, act)], add_res)] of the blocks after the stem of a MobileNet-v2 / v1
+    ``state_dict``: v2 -- ``features.bottleneck{i}.block`` ([1x1 expand / BN / ReLU6], depthwise 3x3 / BN / ReLU6,
+    1x1 project / BN, identity skip when stride == 1 and C_in == C_out), then ``features.conv1`` (1x1 / BN / ReLU6);
+    v1 -- ``features.{i}.components`` (depthwise 3x3 with bias / BN / ReLU, 1x1 / BN / ReLU).  ``act``: 'relu',
+    True (ReLU6) or False (none), as ``_mb_conv_bn`` takes it."""
+    out = []
+    if 'features.conv0.0.weight' in sd:
+        i = 0
+        while 'features.bottleneck%d.block.0.weight' % i in sd:
+            p = 'features.bottleneck%d.block' % i
+            stride, units, j = _MBV2_STRIDES[i], [], 0
+            w0 = sd[p + '.0.weight']
+            c_in = w0.shape[1] if w0.shape[1] != 1 else w0.shape[0]
+            if w0.shape[1] != 1:                    # expansion != 1: the block starts with the 1x1 expand conv
+                units.append((p + '.0', p + '.1', 1, 0, True))
+                j = 3
+            units.append(('%s.%d' % (p, j), '%s.%d' % (p, j + 1), stride, 1, True))
+            units.append(('%s.%d' % (p, j + 3), '%s.%d' % (p, j + 4), 1, 0, False))
+            out.append((p, units, stride == 1 and c_in == sd['%s.%d.weight' % (p, j + 3)].shape[0]))
+            i += 1
+        out.append(('features.conv1', [('features.conv1.0', 'features.conv1.1', 1, 0, True)], False))
+        return out
     idx = sorted({int(m.group(1)) for k in sd for m in [re.match(r'features\.(\d+)\.components\.', k)] if m})
     strides = _MBV1_STRIDES if len(idx) == 13 else tuple(s for j, s in enumerate(_MBV1_STRIDES) if not 6 <= j <= 10)
     for j, i in enumerate(idx):
         p = 'features.%d.components' % i
-        x = _mb_conv_bn(x, sd, p + '.0', p + '.1', strides[j], 1, 'relu', training, buffers_out, quant, trace=trace)
-        x = _mb_conv_bn(x, sd, p + '.3', p + '.4', 1, 0, 'relu', training, buffers_out, quant, trace=trace)
-    x = _q(x.mean((2, 3)), quant)
+        out.append((p, [(p + '.0', p + '.1', strides[j], 1, 'relu'), (p + '.3', p + '.4', 1, 0, 'relu')], False))
+    return out
+
+
+def _mb_block(x, sd, units, add_res, training, bufs, quant, trace=None):
+    """one MobileNet block: its conv/BN(/activation) units in order, the block input added to the last unit's output
+    when ``add_res``"""
+    inp = x
+    for j, (conv, bn, stride, pad, act) in enumerate(units):
+        skip = inp if (add_res and j == len(units) - 1) else None
+        x = _mb_conv_bn(x, sd, conv, bn, stride, pad, act, training, bufs, quant, skip=skip, trace=trace)
+    return x
+
+
+def _mb_features(sd, x, training, buffers_out, quant, trace):
+    x = _q(x, quant)
+    x = _mb_conv_bn(x, sd, *mobilenet_stem(sd), training, buffers_out, quant, trace=trace)
+    for _, units, add_res in mobilenet_blocks(sd):
+        x = _mb_block(x, sd, units, add_res, training, buffers_out, quant, trace=trace)
+    return _q(x.mean((2, 3)), quant)
+
+
+def forward_mobilenet_v1(sd, x, training=True, buffers_out=None, quant=False, trace=None):
+    """logits of a reference-layout MobileNet (v1) ``state_dict`` (models/mobilenet.py:39-156): stem conv/BN/ReLU, then
+    ``features.{i}.components`` = depthwise 3x3 (with bias) / BN / ReLU / 1x1 / BN / ReLU, average pool, ``fc``."""
+    x = _mb_features(sd, x, training, buffers_out, quant, trace)
     return F.linear(x, sd['fc.weight'], sd['fc.bias'])
 
 
@@ -196,27 +244,7 @@ def mobilenet_v2_unit_vjp(sd, unit, quant=True, dtype=torch.float64):
 
 def forward_mobilenet_v2(sd, x, training=True, buffers_out=None, quant=False, dropout_p=0.0, trace=None):
     """logits of a reference-layout MobileNet-v2 ``state_dict`` (models/mobilenet_v2.py:85-156)."""
-    x = _q(x, quant)
-    x = _mb_conv_bn(x, sd, 'features.conv0.0', 'features.conv0.1', 2, 1, True, training, buffers_out, quant, trace=trace)
-    i = 0
-    while 'features.bottleneck%d.block.0.weight' % i in sd:
-        p = 'features.bottleneck%d.block' % i
-        stride = _MBV2_STRIDES[i]
-        inp = x
-        j = 0
-        if sd[p + '.0.weight'].shape[1] != 1:        # expansion != 1: the block starts with the 1x1 expand conv
-            x = _mb_conv_bn(x, sd, p + '.0', p + '.1', 1, 0, True, training, buffers_out, quant, trace=trace)
-            j = 3
-        x = _mb_conv_bn(x, sd, '%s.%d' % (p, j), '%s.%d' % (p, j + 1), stride, 1, True, training, buffers_out, quant,
-                        trace=trace)
-        w_out = sd['%s.%d.weight' % (p, j + 3)]
-        add_res = stride == 1 and inp.size(1) == w_out.shape[0]
-        x = _mb_conv_bn(x, sd, '%s.%d' % (p, j + 3), '%s.%d' % (p, j + 4), 1, 0, False, training, buffers_out, quant,
-                        skip=inp if add_res else None, trace=trace)
-        i += 1
-    x = _mb_conv_bn(x, sd, 'features.conv1.0', 'features.conv1.1', 1, 0, True, training, buffers_out, quant,
-                    trace=trace)
-    x = _q(x.mean((2, 3)), quant)
+    x = _mb_features(sd, x, training, buffers_out, quant, trace)
     if training and dropout_p > 0:
         x = F.dropout(x, dropout_p, True)              # same torch generator stream as nn.Dropout in the reference
     return F.linear(x, sd['classifier.1.weight'], sd['classifier.1.bias'])
@@ -288,31 +316,60 @@ def resnet_block_vjp(sd, prefix, x, dy, stride, quant=True, block=None, training
     return {'y': y.detach(), 'dx': dx, 'grads': grads, 'bufs': {k: v.detach() for k, v in bufs.items()}}
 
 
-def resnet_stem_vjp(sd, x, dy, quant=True, bn=None, dtype=torch.float64):
-    """Local reference of the ResNet stem on its relayouted input ``x`` (NCHW, the bf16 values the convolution reads):
-    conv1 -> BN -> ReLU (-> 3x3/s2 max-pool for the 7x7 stem), with the VJPs of ``dy`` (None: forward only).  ``bn``: the BatchNorm function
-    (signature of ``_bn`` without ``quant``; default ``_bn``).  Returns {'y', 'grads', 'bufs'}."""
+def mobilenet_block_vjp(sd, prefix, x, dy, quant=True, training=True, dtype=torch.float64):
+    """Local reference of one MobileNet-v2 / v1 block ``prefix`` (a prefix of ``mobilenet_blocks``, e.g.
+    'features.bottleneck2.block', 'features.conv1' or 'features.3.components'), like ``resnet_block_vjp``: the block run
+    in ``dtype`` on the device of ``x`` (NCHW) with the storage roundings of ``quant`` and the vector-Jacobian products
+    of ``dy`` (None: forward only).  MobileNet-v1's depthwise biases get their (training mode: rounding-noise) gradient
+    like any parameter.  Returns {'y', 'dx', 'grads': {name: grad}, 'bufs': {name: updated running buffer}}."""
+    (units, add_res), = [(u, a) for p, u, a in mobilenet_blocks(sd) if p == prefix]
+    local = _leaves(sd, [k for k in sd if k.startswith(prefix + '.')], dtype, x.device)
+    xx = x.to(dtype).requires_grad_(True)
+    bufs = {}
+    y = _mb_block(xx, local, units, add_res, training, bufs, quant)
+    dx, grads = _vjp(y, dy, xx, local) if dy is not None else (None, {})
+    return {'y': y.detach(), 'dx': dx, 'grads': grads, 'bufs': {k: v.detach() for k, v in bufs.items()}}
+
+
+def resnet_stem_vjp(sd, x, dy, quant=True, bn=None, dtype=torch.float64, conv='conv1', norm='bn1', stride=None,
+                    padding=None, act='relu'):
+    """Local reference of the stem on its relayouted input ``x`` (NCHW, the bf16 values the convolution reads): conv
+    ``conv`` -> BN ``norm`` -> activation (-> 3x3/s2 max-pool for the 7x7 stem), with the VJPs of ``dy`` (None:
+    forward only).  Defaults: the ResNet stem (7x7/s2/pad 3 + max-pool or 3x3/s1/pad 1, ReLU); the MobileNet stems
+    pass their names, stride 2, padding 1 and ``act`` 'relu6' (v2) or 'relu' (v1), see ``mobilenet_stem``.  ``bn``:
+    the BatchNorm function (signature of ``_bn`` without ``quant``; default ``_bn``).  Returns {'y', 'grads',
+    'bufs'}."""
     if bn is None:
         bn = lambda t, sd_, p, training, bufs: _bn(t, sd_, p, training, bufs, quant)  # noqa: E731
-    local = _leaves(sd, [k for k in sd if k.startswith('conv1.') or k.startswith('bn1.')], dtype, x.device)
+    local = _leaves(sd, [k for k in sd if k.startswith(conv + '.') or k.startswith(norm + '.')], dtype, x.device)
     bufs = {}
-    imagenet = local['conv1.weight'].shape[-1] == 7
-    z = _conv(x.to(dtype), local, 'conv1', 2 if imagenet else 1, 3 if imagenet else 1, quant)
-    y = _q(F.relu(bn(z, local, 'bn1', True, bufs)), quant)
+    imagenet = local[conv + '.weight'].shape[-1] == 7
+    if stride is None:
+        stride, padding = (2, 3) if imagenet else (1, 1)
+    z = _conv(x.to(dtype), local, conv, stride, padding, quant)
+    y = bn(z, local, norm, True, bufs)
+    y = _q(F.relu6(y) if act == 'relu6' else F.relu(y), quant)
     if imagenet:
         y = F.max_pool2d(y, 3, 2, 1)
     _, grads = _vjp(y, dy, None, local) if dy is not None else (None, {})
     return {'y': y.detach(), 'grads': grads, 'bufs': {k: v.detach() for k, v in bufs.items()}}
 
 
-def resnet_head_vjp(sd, h, target, smooth_eps=0.0, soft=None, upstream=1.0, quant=True, dtype=torch.float64):
-    """Local reference of the classifier head on the last block's output ``h`` (NCHW): global average pool -> fc ->
-    mean cross-entropy (label smoothing ``smooth_eps``, or the soft MixUp / CutMix target of ``soft`` = (t2, lam):
-    lam * onehot(target) + (1 - lam) * onehot(t2)), differentiated with the upstream gradient ``upstream``.  The
-    gradient of the logits is stored in bf16 before the classifier's backward reads it.  Returns {'logits', 'loss',
+def resnet_head_vjp(sd, h, target, smooth_eps=0.0, soft=None, upstream=1.0, quant=True, dtype=torch.float64, fc='fc',
+                    drop=None):
+    """Local reference of the classifier head on the last block's output ``h`` (NCHW): global average pool ->
+    (dropout) -> linear ``fc`` ('fc', or MobileNet-v2's 'classifier.1') -> mean cross-entropy (label smoothing
+    ``smooth_eps``, or the soft MixUp / CutMix target of ``soft`` = (t2, lam): lam * onehot(target) + (1 - lam) *
+    onehot(t2)), differentiated with the upstream gradient ``upstream``.  ``drop`` = (keep, p): the 0/1 keep mask
+    [N, C] of a dropout with rate p, applied as F.dropout applies it, keep * x / (1 - p), with one storage rounding.
+    The gradient of the logits is stored in bf16 before the classifier's backward reads it.  Returns {'logits', 'loss',
     'top1', 'top5' (percent of rows whose target is among the 1 / 5 largest logits), 'dlogits', 'grads', 'dh'}."""
-    w, b = sd['fc.weight'].to(h.device, dtype), sd['fc.bias'].to(h.device, dtype)
+    w, b = sd[fc + '.weight'].to(h.device, dtype), sd[fc + '.bias'].to(h.device, dtype)
     feat = _q(h.to(dtype).mean((2, 3)), quant)
+    scale = None
+    if drop is not None:
+        scale = drop[0].to(h.device, dtype) / (1.0 - drop[1])
+        feat = _q(feat * scale, quant)
     logits = (feat @ w.t() + b).detach().requires_grad_(True)
     n_cls = logits.shape[1]
     if soft is None:
@@ -324,13 +381,15 @@ def resnet_head_vjp(sd, h, target, smooth_eps=0.0, soft=None, upstream=1.0, quan
     (dl,) = torch.autograd.grad(loss, [logits])
     dl = _q(dl * upstream, quant)
     dfeat = _q(dl @ w, quant)
+    if scale is not None:
+        dfeat = _q(dfeat * scale, quant)
     HW = h.shape[2] * h.shape[3]
     dh = (dfeat / HW)[:, :, None, None].expand(h.shape)
     picked = logits.gather(1, target.view(-1, 1))
     above = (logits > picked).sum(1)        # a row counts when fewer than k logits lie strictly above its target's
     return {'logits': logits.detach(), 'loss': loss.detach(), 'top1': float((above < 1).double().mean()) * 100,
-            'top5': float((above < 5).double().mean()) * 100, 'dlogits': dl,
-            'grads': {'fc.weight': dl.t() @ feat, 'fc.bias': dl.sum(0)}, 'dh': _q(dh, quant)}
+            'top5': float((above < 5).double().mean()) * 100, 'dlogits': dl, 'feat': feat,
+            'grads': {fc + '.weight': dl.t() @ feat, fc + '.bias': dl.sum(0)}, 'dh': _q(dh, quant)}
 
 
 def cross_entropy(logits, target, smooth_eps=0.0):

@@ -1,24 +1,28 @@
-"""Block-by-block replay of real ResNet-family training steps against fp64, teacher-forced from the engine's own tensors.
+"""Block-by-block replay of real ResNet-family and MobileNet training steps against fp64, teacher-forced from the
+engine's own tensors.
 
 The network-level checks (test_gpu_engine._check_against_bf16_oracle and its L1 / dropout copies) accept per-tensor
 errors of several percent, because a whole bf16-storage network is that sensitive to which way single roundings fall.
 A wiring error that moves one block's d gamma, one downsample gradient or one running variance by 1-3 % passes them.
 Here the inputs of every block are the engine's own, so only that block's rounding separates the two sides:
 
-  1. record one eager ``ResNetRuntime.train_step``: the stem / block / head methods of the runtime instance are wrapped
+  1. record one eager ``Runtime.train_step``: the stem / block / head methods of the runtime instance are wrapped
      so that each clones its input and output (x, y) and the gradient it receives and returns (dy, dx); the stem's
-     input is the relayout output (decoded from the bordered space-to-depth layout of the 7x7 stem), so MixUp / CutMix
-     steps replay like any other.  The arena gradients and the running buffers are read before and after the step;
+     input is the relayout output (decoded from the bordered space-to-depth layout of the 7x7 stem, or the padded
+     NHWC input of a 3x3 stem), so MixUp / CutMix steps replay like any other; the head's dropout mask is taken from
+     its tape.  The arena gradients and the running buffers are read before and after the step;
   2. run each block in fp64 on the GPU (``oracle.ref_model.resnet_block_vjp`` with the storage roundings of the kernel
      path; the L1 and dropout restatements of tests/l1_oracle.py and tests/dropout_oracle.py, the keep masks regenerated
-     from ``rt.dropout_key``), the stem (conv, BN, ReLU, max-pool) and the head (average pool, fc, cross-entropy with
-     label smoothing or the soft MixUp / CutMix target, the upstream gradient);
+     from ``rt.dropout_key``; ``oracle.ref_model.mobilenet_block_vjp`` for the MobileNet blocks), the stem (conv, BN,
+     ReLU / ReLU6, max-pool) and the head (average pool, dropout, fc, cross-entropy with label smoothing or the soft
+     MixUp / CutMix target, the upstream gradient);
   3. compare each block's y, dx, every parameter gradient and its running buffers after the step (the shared SE gate of
      a stage against the sum of its blocks' VJPs), and require the recorded tensors to chain bit for bit: block i's
      output is block i+1's input, block i+1's dx is block i's dy, and likewise at the stem and the head;
   4. inside the blocks, teacher-force every unit (_replay_units): each BatchNorm backward (dz, g, d gamma / d beta) on
-     the engine's own z and dy, the running statistics on the engine's own z, each convolution's dgrad and wgrad on the
-     engine's own x and dz.  A whole bottleneck block is ill-conditioned (see LOOSE), a single unit is not: these bounds
+     the engine's own z and dy (the ReLU6 gate 0 < pre < 6 as the kernels decide it), the running statistics on the
+     engine's own z (plus MobileNet-v1's depthwise bias), each convolution's dgrad and wgrad (depthwise: groups = C) on
+     the engine's own x and dz.  A whole bottleneck block is ill-conditioned (see LOOSE), a single unit is not: these bounds
      are tight on every configuration.
 
 Every bound and the worst value measured per quantity are printed (``-s``) with configuration and block.  Mutants
@@ -59,6 +63,23 @@ CONFIGS = {
                            mix=('mixup', 0.37)),
     'resnet20_cutmix': dict(family='resnet', cfg=dict(dataset='cifar10', depth=20), px=32, classes=10,
                             mix=('cutmix', (5, 21, 8, 30))),
+    # MobileNet-v2 (bench.py's config C4; 'drop': the rate of its head Dropout, set before conversion, default 0.2)
+    # and MobileNet-v1.  At 112 px the last stride-2 depthwise convolution reads an odd 7 x 7 map (-> 4 x 4)
+    'mobilenet_v2': dict(family='mobilenet_v2', cfg=dict(dataset='imagenet'), px=224, classes=1000),
+    'mobilenet_v2_112': dict(family='mobilenet_v2', cfg=dict(dataset='imagenet'), px=112, classes=1000),
+    # 'clip': BatchNorms whose gamma / beta are raised before the step so that their ReLU6 clips (see _raise_bns)
+    'mobilenet_v2_relu6': dict(family='mobilenet_v2', cfg=dict(dataset='imagenet'), px=112, classes=1000, drop=0.0,
+                               clip=('features.conv0.1', 'features.bottleneck2.block.1', 'features.bottleneck2.block.4',
+                                     'features.bottleneck5.block.4', 'features.bottleneck14.block.1',
+                                     'features.conv1.1')),
+    'mobilenet_v2_drop01': dict(family='mobilenet_v2', cfg=dict(dataset='imagenet'), px=112, classes=1000, drop=0.1),
+    'mobilenet_v2_smooth_upstream8': dict(family='mobilenet_v2', cfg=dict(dataset='imagenet'), px=112, classes=1000,
+                                          smooth=0.1, upstream=8.0),
+    'mobilenet_v2_cutmix': dict(family='mobilenet_v2', cfg=dict(dataset='imagenet'), px=112, classes=1000,
+                                mix=('cutmix', (17, 70, 9, 88))),
+    'mobilenet_v1': dict(family='mobilenet', cfg=dict(dataset='imagenet'), px=112, classes=1000),
+    'mobilenet_v1_shallow_w05': dict(family='mobilenet', cfg=dict(dataset='imagenet', shallow=True, width=0.5), px=112,
+                                     classes=1000),
 }
 
 # rel-L2 bounds per quantity class.  'affine': d gamma and d beta of one BN on ONE scale, the norm of the larger of the
@@ -74,6 +95,9 @@ BOUNDS = {
     # unit level (_replay_units): one bf16 rounding of dz / of the dgrad output, fp32 sums for the rest
     'unit dz': 3e-3, 'unit g': 1e-3, 'unit affine': 1e-4, 'unit running_mean': 2e-6, 'unit running_var': 2e-6,
     'unit dgrad': 3e-3, 'unit wgrad': 1e-4, 'unit coeffs': 1e-5,
+    # MobileNet-v1's depthwise bias: the engine's gradient is exactly zero (asserted); the reference's, sum(dz) over a
+    # training-mode BatchNorm, is fp64 rounding noise, measured against the norm of the same convolution's dW
+    'bias noise': 1e-10,
 }
 # The floors above hold for the CIFAR configurations (measured on an NVIDIA H100 80GB HBM3 at a 700 W power limit, worst
 # over five runs: dx 1.7e-3, dW 1.3e-3, affine 1.3e-3, running statistics 9.4e-6).  The whole blocks of the ImageNet
@@ -89,9 +113,18 @@ BOUNDS = {
 # d gamma / d beta 5.8e-7, wgrad 3.1e-5, BN coefficients 1.9e-7, running statistics 1.3e-7; logits 4.4e-6, loss 6.9e-6.
 LOOSE = dict(dx=4e-2, dW=5e-2, affine=6e-2, running_mean=1e-4, running_var=1e-4)
 LOOSE['SE grad'] = 3e-2
+# The MobileNet blocks (1x1 expand, depthwise 3x3 and 1x1 project units, each re-rounded to bf16 after its BatchNorm)
+# sit between the two.  Measured on an NVIDIA H100 80GB HBM3 at a 700 W power limit, worst over three runs of the
+# eight MobileNet configurations: dx 3.8e-3, dW 4.6e-3, affine 1.1e-2 (the BNs of the later units of a block, whose
+# inputs lie one or two units past the teacher-forced block input).  The same fp64 block reference evaluated in fp32
+# (same storage roundings, TF32 off) differs from itself by up to dx 1.3e-3, dW 1.4e-3, affine 2.2e-3 on the same
+# blocks (MobileNet-v2 at 224 px, v1 at 112 px).  The block outputs agree to 6.4e-4, and every unit-level bound holds
+# unchanged: dz 1.7e-3, dgrad 1.7e-3, wgrad 2.0e-5 (the depthwise weight gradients, up to 32 x 112 x 112 products
+# per element, included), d gamma / d beta 6.7e-7, running statistics 1.4e-7.
+MB_LOOSE = dict(dx=1e-2, dW=1e-2, affine=2e-2)
 for _c in CONFIGS.values():
     if _c['cfg']['dataset'] == 'imagenet':
-        _c['loose'] = LOOSE
+        _c['loose'] = MB_LOOSE if _c['family'].startswith('mobilenet') else LOOSE
 WORST = {}          # quantity class -> (value, bound, config, where)
 
 
@@ -118,7 +151,7 @@ def _report(title):
     for cls in BOUNDS:
         if cls in WORST:
             v, bound, config, where = WORST[cls]
-            lines.append('  %-14s %.3e  (bound %.0e; CIFAR %.0e)  %s %s' % (cls, v, bound, BOUNDS[cls], config, where))
+            lines.append('  %-14s %.3e  (bound %.1e; CIFAR %.1e)  %s %s' % (cls, v, bound, BOUNDS[cls], config, where))
     print('\n'.join(lines))
 
 
@@ -126,8 +159,33 @@ def _report(title):
 def _build(name):
     from convnet.pytorch_b200 import models
     c = CONFIGS[name]
-    ref, mine, x, y = _pair(getattr(models, c['family']), c['cfg'], (3, c['px'], c['px']), c['classes'], batch=BATCH)
+    factory = getattr(models, c['family'])
+    if 'drop' in c:
+        def factory(**cfg):
+            m = models.mobilenet_v2(**cfg)
+            m.classifier[0].p = c['drop']
+            return m
+    ref, mine, x, y = _pair(factory, c['cfg'], (3, c['px'], c['px']), c['classes'], batch=BATCH)
+    if 'clip' in c:
+        _raise_bns(mine, c['clip'])
     return ref, mine, x, y
+
+
+def _raise_bns(mine, names):
+    """gamma x 4 and beta + 3 on the named BatchNorms: bn(z) = 4 z^ + 3 with z^ ~ N(0, 1) takes its ReLU6 above 6 for
+    z^ > 0.75 and below 0 for z^ < -0.75, so both edges of the gate carry gradient (a few fp32 SGD steps leave almost
+    no pre-activation above 6)"""
+    params = dict(mine.named_parameters())
+    with torch.no_grad():
+        for n in names:
+            params[n + '.weight'].mul_(4.0)
+            params[n + '.bias'].add_(3.0)
+    mine._b200.arena.sync_shadow()
+
+
+def _is_mobilenet(mine):
+    from convnet.pytorch_b200.engine import MobileNetRuntime
+    return isinstance(mine._b200, MobileNetRuntime)
 
 
 def _step_args(name, x):
@@ -158,6 +216,10 @@ def _step_args(name, x):
 
 
 def _prefixes(model):
+    """[(block prefix, stride)] in the order of the runtime's blocks; MobileNet: the prefix of each block's first
+    convolution (stride None: oracle.ref_model.mobilenet_blocks knows it)"""
+    if _is_mobilenet(model):
+        return [(spec['units'][0][0].slot.name.rsplit('.', 2)[0], None) for spec in model._b200.blocks]
     out = []
     for li, lname in enumerate(('layer1', 'layer2', 'layer3', 'layer4')):
         layer = getattr(model, lname, None)
@@ -210,6 +272,8 @@ class _Tap(object):
         def head_fwd(h, training, want_tape):
             out, tape = orig['_head_fwd'](h, training, want_tape)
             self.head.update(h=h.clone(), logits=out.clone())
+            if tape is not None:            # the dropout mask (None without dropout) and the masked features
+                self.head.update(mask=None if tape['mask'] is None else tape['mask'].clone(), feat=tape['feat'].clone())
             return out, tape
 
         def head_bwd(tape, dlogits, dl_bf16=None):
@@ -308,7 +372,7 @@ def _errors(where, ref, grads, bufs, l1, prefix_cls=''):
     stem; BN affine pairs on one scale"""
     out = {}
     for k, g in ref['grads'].items():
-        if 'residual_block' in k:
+        if 'residual_block' in k or _conv_bias(k, ref['grads']):
             continue
         q = k[len(where) + 1:] if k.startswith(where + '.') else k
         if k.endswith('.weight') and g.dim() == 4:
@@ -328,8 +392,19 @@ def _errors(where, ref, grads, bufs, l1, prefix_cls=''):
     return out
 
 
+def _conv_bias(k, grads):
+    """a convolution bias (MobileNet-v1's depthwise layers, in front of a training-mode BatchNorm)"""
+    return k.endswith('.bias') and grads[k[:-len('bias')] + 'weight'].dim() == 4
+
+
 def _check_block(name, where, r, tap, failures, l1, prefix_cls=''):
     for k, g in r['grads'].items():
+        if _conv_bias(k, r['grads']):
+            # its true gradient is sum(dz) = 0 exactly: the engine writes zeros, the reference sums rounding noise
+            assert float(tap.grads[k].abs().max()) == 0.0, '%s %s: the gradient of %s is not zero' % (name, where, k)
+            _note('bias noise', float(g.norm()) / float(r['grads'][k[:-len('bias')] + 'weight'].norm()), name, where,
+                  failures, k[len(where) + 1:])
+            continue
         assert float(g.norm()) > 0, '%s %s: the reference gradient of %s is zero (vacuous state)' % (name, where, k)
         assert float(tap.grads[k].norm()) > 0, '%s %s: the gradient of %s is zero' % (name, where, k)
     for k, v in r['bufs'].items():
@@ -343,12 +418,18 @@ def _replay(name, mine, x, y, tap, soft=None, smooth=0.0, upstream=1.0):
     """-> failures [(where, quantity, value, bound)]; the exact chaining checks assert directly"""
     from oracle import ref_model
     rt = mine._b200
-    sd, failures, l1 = tap.sd, [], _is_l1(mine)
+    sd, failures, l1, mobile = tap.sd, [], _is_l1(mine), _is_mobilenet(mine)
     blocks = tap.blocks
     prefixes = _prefixes(mine)
     assert len(prefixes) == len(rt.blocks) == len(blocks)
-    for (p, _), spec in zip(prefixes, rt.blocks):
-        assert spec['convs'][0].slot.name == p + '.conv1.weight'
+    if mobile:
+        assert [p for p, _ in prefixes] == [p for p, _, _ in ref_model.mobilenet_blocks(sd)]
+        for (_, units, add_res), spec in zip(ref_model.mobilenet_blocks(sd), rt.blocks):
+            assert [c for c, _, _, _, _ in units] == [c.slot.name[:-len('.weight')] for c, _, _ in spec['units']]
+            assert add_res == spec['add_res']
+    else:
+        for (p, _), spec in zip(prefixes, rt.blocks):
+            assert spec['convs'][0].slot.name == p + '.conv1.weight'
     # ---- exact chaining of the recorded tensors
     chain = [('stem', tap.stem['y'], tap.stem['dy'])] + [(p, b['y'], b['dy']) for (p, _), b in zip(prefixes, blocks)]
     for (p, yo, dyo), b in zip(chain, blocks + [dict(x=tap.head['h'], dx=tap.head['dh'])]):
@@ -357,7 +438,10 @@ def _replay(name, mine, x, y, tap, soft=None, smooth=0.0, upstream=1.0):
     # ---- head
     target = y
     t2 = (target[soft[0].cuda()], soft[1]) if soft is not None else None
-    h = ref_model.resnet_head_vjp(sd, _nchw(tap.head['h']), target, smooth_eps=smooth, soft=t2, upstream=upstream)
+    fc = 'classifier.1' if 'classifier.1.weight' in sd else 'fc'
+    drop = _head_mask(name, rt, tap) if tap.head['mask'] is not None else None
+    h = ref_model.resnet_head_vjp(sd, _nchw(tap.head['h']), target, smooth_eps=smooth, soft=t2, upstream=upstream,
+                                  fc=fc, drop=drop)
     C = rt.classes
     _note('logits', _rel(tap.head['logits'], h['logits']), name, 'head', failures)
     _note('loss', abs(float(tap.stats[0]) - float(h['loss'])) / abs(float(h['loss'])), name, 'head', failures)
@@ -365,7 +449,7 @@ def _replay(name, mine, x, y, tap, soft=None, smooth=0.0, upstream=1.0):
         '%s head: top-1 / top-5 %s vs %.4f / %.4f' % (name, tap.stats.tolist(), h['top1'], h['top5'])
     assert float(tap.head['dl'][:, C:].abs().max() if tap.head['dl'].shape[1] > C else 0.0) == 0.0
     _note('dlogits', _rel(tap.head['dl'][:, :C], h['dlogits']), name, 'head', failures)
-    for k in ('fc.weight', 'fc.bias'):
+    for k in (fc + '.weight', fc + '.bias'):
         assert float(tap.grads[k].norm()) > 0
         _note('fc grad', _rel(tap.grads[k], h['grads'][k]), name, 'head', failures, k)
     _note('dh', _rel(_nchw(tap.head['dh']), h['dh']), name, 'head', failures)
@@ -373,9 +457,11 @@ def _replay(name, mine, x, y, tap, soft=None, smooth=0.0, upstream=1.0):
     masks = _dropout_masks(mine, tap.key, x) if tap.key is not None else None
     se_ref = {}
     for (p, stride), b in zip(prefixes, blocks):
-        fn = _block_fn(mine, p, masks)
         xb, dyb = _nchw(b['x']), _nchw(b['dy'])
-        r = ref_model.resnet_block_vjp(sd, p, xb, dyb, stride, block=fn)
+        if mobile:
+            r = ref_model.mobilenet_block_vjp(sd, p, xb, dyb)
+        else:
+            r = ref_model.resnet_block_vjp(sd, p, xb, dyb, stride, block=_block_fn(mine, p, masks))
         _note('y', _rel(_nchw(b['y']), r['y']), name, p, failures)
         _note('dx', _rel(_nchw(b['dx']), r['dx']), name, p, failures)
         _check_block(name, p, r, tap, failures, l1)
@@ -388,20 +474,53 @@ def _replay(name, mine, x, y, tap, soft=None, smooth=0.0, upstream=1.0):
     # ---- stem, past the input relayout
     stem_bn = (lambda t, sd_, pfx, tr, bufs: l1_oracle.bn_l1(t, sd_, pfx, tr, bufs)) if l1 else None
     xs = _decode_stem(tap.stem['xs'], 3, rt.imagenet_stem)
-    s = ref_model.resnet_stem_vjp(sd, xs, _nchw(tap.stem['dy']), bn=stem_bn)
+    stem = {}
+    if mobile:                  # 3x3/s2 conv, BN, ReLU6 (v2) / ReLU (v1), no max-pool
+        conv, norm, stride, pad, act = ref_model.mobilenet_stem(sd)
+        stem = dict(conv=conv, norm=norm, stride=stride, padding=pad, act='relu' if act == 'relu' else 'relu6')
+    s = ref_model.resnet_stem_vjp(sd, xs, _nchw(tap.stem['dy']), bn=stem_bn, **stem)
     _note('stem y', _rel(_nchw(tap.stem['y']), s['y']), name, 'stem', failures)
     _check_block(name, 'stem', s, tap, failures, l1, prefix_cls='stem ')
     return failures
 
 
+def _head_mask(name, rt, tap):
+    """the head's dropout mask from the tape: exactly the two values {0, 1 / (1 - p)} (fp32), a kept fraction within
+    5 sigma of 1 - p, and the kept features are the pooled bf16 mean times 1 / (1 - p) with ONE rounding to bf16 (at
+    p = 0.1 and 0.2 the fp32 product rounds like the fp64 one: a bf16 value times 10 / 9 or 5 / 4 lies at least 1/18
+    ulp from a rounding midpoint) -> the (0/1 keep mask, p) of oracle.ref_model.resnet_head_vjp"""
+    from convnet.pytorch_b200 import ops
+    p, mask, feat = rt.dropout_p, tap.head['mask'], tap.head['feat']
+    N, C = feat.shape[0], feat.shape[-1]
+    mask, feat = mask.reshape(N, C), feat.reshape(N, C)
+    scale = float(np.float32(1.0 / (1.0 - p)))
+    values = sorted(torch.unique(mask).tolist())
+    assert mask.dtype == torch.float32 and values == [0.0, scale], \
+        '%s head: dropout mask %s with values %s, not {0, %r}' % (name, mask.dtype, values[:4], scale)
+    keep = mask != 0
+    frac, sigma = float(keep.double().mean()), (p * (1.0 - p) / keep.numel()) ** 0.5
+    print('%s head dropout p = %g: kept fraction %.4f (1 - p %.4f, sigma %.1e)' % (name, p, frac, 1.0 - p, sigma))
+    assert abs(frac - (1.0 - p)) < 5 * sigma, '%s head: kept fraction %.4f for p = %g' % (name, frac, p)
+    pooled = ops.avgpool_fwd(tap.head['h']).reshape(N, C)
+    want = (pooled.double() * (1.0 / (1.0 - p))).to(torch.bfloat16)
+    assert torch.equal(feat[keep], want[keep]), '%s head: %d of the kept features are not bf16(mean / (1 - p))' % (
+        name, int((feat[keep] != want[keep]).sum()))
+    assert float(feat[~keep].abs().max()) == 0.0, '%s head: a dropped feature is not zero' % name
+    return keep.double(), p
+
+
 def _unit_names(rt, mine):
-    """id of each _BN / _Conv of the runtime -> (block prefix or 'stem', module name inside it)"""
-    bns, convs = {id(rt.stem_bn): ('stem', 'bn1')}, {}
+    """id of each _BN / _Conv of the runtime -> (block prefix or 'stem', module name inside it), from the module names"""
+    mods = {id(m): n for n, m in mine.named_modules()}
+    bns, convs = {id(rt.stem_bn): ('stem', mods[id(rt.stem_bn.mod)])}, {}
     for (p, _), spec in zip(_prefixes(mine), rt.blocks):
-        for i, (c, b) in enumerate(zip(spec['convs'], spec['bns'])):
-            convs[id(c)], bns[id(b)] = (p, 'conv%d' % (i + 1)), (p, 'bn%d' % (i + 1))
-        if spec['down'] is not None:
-            convs[id(spec['down'][0])], bns[id(spec['down'][1])] = (p, 'downsample.0'), (p, 'downsample.1')
+        if 'units' in spec:
+            pairs = [(c, b) for c, b, _ in spec['units']]
+        else:
+            pairs = list(zip(spec['convs'], spec['bns'])) + ([tuple(spec['down'])] if spec['down'] is not None else [])
+        for c, b in pairs:
+            convs[id(c)] = (p, c.slot.name[len(p) + 1:-len('.weight')])
+            bns[id(b)] = (p, mods[id(b.mod)][len(p) + 1:])
     return bns, convs
 
 
@@ -410,7 +529,7 @@ def _replay_units(name, mine, tap, masks, failures):
     + dropout) on the engine's own z and dy -- dz, g = dy * act', d gamma / d beta -- and the running statistics against
     fp64 statistics of the same z; every convolution backward against fp64 dgrad / wgrad on the engine's own x and dz.
     One rounding separates the two sides, however ill-conditioned the whole block is."""
-    from convnet.pytorch_b200.lib import ACT_NONE
+    from convnet.pytorch_b200.lib import ACT_NONE, ACT_RELU6
     from oracle import ref_model
     rt, sd, l1 = mine._b200, tap.sd, _is_l1(mine)
     bn_names, conv_names = _unit_names(rt, mine)
@@ -423,7 +542,7 @@ def _replay_units(name, mine, tap, masks, failures):
             where, local = conv_names[id(c)]
             w = sd['%s.%s.weight' % (where, local)].double()
             x, dz = _nchw(u.x), _nchw(rec['dz'])
-            kw = dict(stride=c.stride, padding=c.pad, groups=c.groups)
+            kw = dict(stride=c.stride, padding=c.pad, groups=c.C if c.kind == 'dw' else c.groups)
             if rec['dx'] is not None:
                 dx = torch.nn.grad.conv2d_input(x.shape, w, dz, **kw)
                 if rec['res'] is not None:
@@ -447,15 +566,24 @@ def _replay_units(name, mine, tap, masks, failures):
         elif rec['join']:                 # the pre-activation includes the skip: its sign is that of the output
             gout = dy * (_nchw(u.y) > 0)
         else:
-            # the ReLU gate as the kernels decide it, from the forward's fp32 coefficients: where bn(z) sits within
-            # fp32 rounding of zero the fp64 decision differs, and a flipped gate moves d beta by a whole dy element
-            pre = u.z.float() * u.scale + u.shift
-            gate = (pre > 0).permute(0, 3, 1, 2).double()
+            # the ReLU / ReLU6 gate as the kernels decide it, from the forward's fp32 coefficients with ONE rounding,
+            # fmaf(z, scale, shift) (z * scale is exact in fp64): where bn(z) sits within fp32 rounding of 0 or 6 the
+            # fp64 decision differs, and a flipped gate moves d beta by a whole dy element.  Two fp32 roundings are
+            # not enough either: a depthwise convolution repeats one z value over every all-zero window, and a
+            # MobileNet-v2 step has shown 20 copies of a pre-activation of 1.6e-9 whose sign the unfused sum flips
+            pre = (u.z.double() * u.scale.double() + u.shift.double()).float()
+            gate = (pre > 0) & (pre < 6) if rec['act'] == ACT_RELU6 else pre > 0
+            gate = gate.permute(0, 3, 1, 2).double()
             if where != 'stem' and local == 'bn1' and masks is not None and where in masks:
                 keep, rate = masks[where]
                 gate = gate * keep.double() * dropout_oracle.threshold(rate)[1]
             gout = dy * gate
         dz, dg, db = torch.autograd.grad(out, [z, loc[full + '.weight'], loc[full + '.bias']], gout)
+        bias = sd.get(u.conv.slot.name[:-len('weight')] + 'bias') if u.conv is not None else None
+        if bias is not None:
+            # a convolution bias in front of the BN: z holds the convolution without it; the true pre-BN tensor is
+            # z + b, which moves only the running mean
+            bufs[full + '.running_mean'] = bufs[full + '.running_mean'] + 0.1 * bias.double()
         with torch.no_grad():           # the forward's coefficients: y = z * scale + shift
             zd = z.detach()
             mean = zd.mean((0, 2, 3))
@@ -490,7 +618,25 @@ def _run(name, mine, x, y):
     failures = _replay(name, mine, x, y, tap, soft=soft, smooth=c.get('smooth', 0.0), upstream=c.get('upstream', 1.0))
     masks = _dropout_masks(mine, tap.key, x) if tap.key is not None else None
     _replay_units(name, mine, tap, masks, failures)
+    if 'clip' in c:
+        _check_clipping(name, mine, tap, c['clip'])
     return failures
+
+
+def _check_clipping(name, mine, tap, bns):
+    """the raised BatchNorms of the configuration clip: at least 1 % of their pre-activations lie above 6"""
+    bn_names = _unit_names(mine._b200, mine)[0]
+    seen = {}
+    for rec in tap.units:
+        if rec['kind'] == 'bn':
+            where, local = bn_names[id(rec['u'].bn)]
+            full = local if where == 'stem' else where + '.' + local
+            if full in bns:
+                u = rec['u']
+                seen[full] = float(((u.z.float() * u.scale + u.shift) > 6).double().mean())
+    print('%s: fraction of pre-activations above 6: %s' % (name, ', '.join('%s %.3f' % kv for kv in sorted(seen.items()))))
+    assert sorted(seen) == sorted(bns)
+    assert min(seen.values()) >= 0.01, '%s: a raised BatchNorm does not clip: %s' % (name, seen)
 
 
 # ---------------------------------------------------------------------------------------------------- tests
@@ -506,12 +652,14 @@ def test_block_replay(name):
     assert not failures, '%s: %s' % (name, ['%s %s %.3e > %.0e' % f for f in failures])
 
 
-@pytest.mark.parametrize('name', ['resnet20', 'resnext_se50'])
+@pytest.mark.parametrize('name', ['resnet20', 'resnext_se50', 'mobilenet_v2_relu6', 'mobilenet_v1'])
 def test_gradients_accumulate(name):
     """two train_steps on one batch without zero_grad: every arena gradient is twice the one-step gradient (the
     accumulate contract of include/b200conv.h that chunked batches rely on: the stem's space-to-depth gather, the
-    grouped unpack, the SE and fc column sums, BN d gamma / d beta), and the running buffers saw two momentum updates.
-    A path that overwrites instead of accumulating shows an error of 0.5."""
+    grouped unpack, the SE and fc column sums, BN d gamma / d beta, the depthwise weight gradients through their shared
+    workspace on the side stream), and the running buffers saw two momentum updates.  A path that overwrites instead of
+    accumulating shows an error of 0.5.  MobileNet-v1's depthwise biases stay exactly zero.  (The MobileNet-v2
+    configuration has no head dropout: two steps would draw two masks.)"""
     _setup()
     ref, mine, x, y = _build(name)
     rt = mine._b200
@@ -526,6 +674,9 @@ def test_gradients_accumulate(name):
     torch.cuda.synchronize()
     worst = (0.0, '')
     for n, p in mine.named_parameters():
+        if _conv_bias(n, g1):
+            assert float(g1[n].abs().max()) == 0.0 and float(p.grad.abs().max()) == 0.0, n
+            continue
         assert float(g1[n].norm()) > 0, n
         worst = max(worst, (_rel(p.grad, 2 * g1[n]), n))
     bworst = (0.0, '')
@@ -541,10 +692,13 @@ def test_gradients_accumulate(name):
     assert bworst[0] <= 1e-6, bworst
 
 
-@pytest.mark.parametrize('name', ['resnet18', 'resnext20', 'resnet_se50', 'resnet20_l1'])
+@pytest.mark.parametrize('name', ['resnet18', 'resnext20', 'resnet_se50', 'resnet20_l1', 'mobilenet_v2',
+                                  'mobilenet_v1'])
 def test_eval_blocks(name):
     """eval-mode forwards, BatchNorm folded into the convolutions and not folded: every block against the fp64 block in
-    eval mode on the running statistics.  The folded weights carry one more bf16 rounding, of w * gamma / sigma."""
+    eval mode on the running statistics.  The folded weights carry one more bf16 rounding, of w * gamma / sigma.  The
+    MobileNet runtimes never fold (fold_bn_eval = False): both settings must give the same logits bit for bit, and
+    MobileNet-v1's depthwise bias enters the BatchNorm shift."""
     from oracle import ref_model
     from convnet.pytorch_b200 import engine
     _setup()
@@ -553,20 +707,26 @@ def test_eval_blocks(name):
     sd = {k: v.detach().clone() for k, v in mine.state_dict().items()}
     prefixes = _prefixes(mine)
     mine.eval()
-    failures = []
+    failures, logits = [], []
     saved = engine.FOLD_BN_EVAL
     try:
         for fold in (False, True):
             engine.FOLD_BN_EVAL = fold
             with _Tap(rt) as tap, torch.no_grad():
-                mine(x)
+                logits.append(mine(x))
             torch.cuda.synchronize()
+            folded = fold and rt.fold_bn_eval
             for (p, stride), b in zip(prefixes, tap.blocks):
-                r = ref_model.resnet_block_vjp(sd, p, _nchw(b['x']), None, stride, block=_block_fn(mine, p, None),
-                                               training=False)
-                _note('eval y folded' if fold else 'eval y', _rel(_nchw(b['y']), r['y']), name, p, failures)
+                if _is_mobilenet(mine):
+                    r = ref_model.mobilenet_block_vjp(sd, p, _nchw(b['x']), None, training=False)
+                else:
+                    r = ref_model.resnet_block_vjp(sd, p, _nchw(b['x']), None, stride, block=_block_fn(mine, p, None),
+                                                   training=False)
+                _note('eval y folded' if folded else 'eval y', _rel(_nchw(b['y']), r['y']), name, p, failures)
     finally:
         engine.FOLD_BN_EVAL = saved
+    if not rt.fold_bn_eval:
+        assert torch.equal(logits[0], logits[1]), '%s: FOLD_BN_EVAL changed the eval forward of a non-folding runtime' % name
     _report('after eval %s' % name)
     assert not failures, '%s: %s' % (name, ['%s %s %.3e > %.0e' % f for f in failures])
 
@@ -671,6 +831,42 @@ def _mutant_upstream_bias(monkeypatch, rt, mine):
     return 'head', lambda q: q == 'fc.bias'
 
 
+def _mutant_mb_skip(monkeypatch, rt, mine):
+    """MobileNet-v2 identity block bottleneck2: its first unit's dgrad gets no residual (the skip gradient is dropped)"""
+    first = _spec(rt, mine, 'features.bottleneck2.block')['units'][0][0]
+    orig = rt._conv_bwd
+
+    def conv_bwd(u, dz, need_dx=True, residual=None):
+        return orig(u, dz, need_dx, None if u.conv is first else residual)
+    monkeypatch.setattr(rt, '_conv_bwd', conv_bwd, raising=False)
+    return 'features.bottleneck2.block', lambda q: q == 'dx'
+
+
+def _mutant_relu6_as_relu(monkeypatch, rt, mine):
+    """the clipping depthwise BN of bottleneck2 (mobilenet_v2_relu6) runs its backward with ReLU's gate"""
+    from convnet.pytorch_b200.lib import ACT_RELU
+    bn = _spec(rt, mine, 'features.bottleneck2.block')['units'][1][1]
+
+    def fn(orig, u, dy, y_mask, act, want_g):
+        return orig(u, dy, y_mask, ACT_RELU if u.bn is bn else act, want_g)
+    _wrap_bn_bwd(monkeypatch, rt, fn)
+    return 'features.bottleneck2.block', lambda q: q == '4 dz'
+
+
+def _mutant_dw_bias_mean(monkeypatch, rt, mine):
+    """MobileNet-v1 features.5: the depthwise convolution's bias is left out of its BN's running-mean update"""
+    monkeypatch.setattr(_spec(rt, mine, 'features.5.components')['units'][0][0], 'bias32', None)
+    return 'features.5.components', lambda q: q == '1.running_mean'
+
+
+def _mutant_head_mask_bwd(monkeypatch, rt, mine):
+    """MobileNet-v2: the head's backward does not apply the dropout mask to d feat"""
+    orig = rt._head_bwd
+    monkeypatch.setattr(rt, '_head_bwd', lambda tape, dlogits, dl_bf16=None: orig(dict(tape, mask=None), dlogits,
+                                                                                  dl_bf16), raising=False)
+    return 'head', lambda q: q == 'dh'
+
+
 MUTANTS = {
     'skip_dy': ('resnet20', _mutant_skip_dy),
     'down_dy': ('resnet18', _mutant_down_dy),
@@ -680,6 +876,10 @@ MUTANTS = {
     'drop_layer': ('wrn16_4_dropout', _mutant_drop_layer),
     'sign_sum': ('resnet20_l1', _mutant_sign_sum),
     'upstream_bias': ('resnet18_upstream8', _mutant_upstream_bias),
+    'mb_skip': ('mobilenet_v2_112', _mutant_mb_skip),
+    'relu6_as_relu': ('mobilenet_v2_relu6', _mutant_relu6_as_relu),
+    'dw_bias_mean': ('mobilenet_v1', _mutant_dw_bias_mean),
+    'head_mask_bwd': ('mobilenet_v2_112', _mutant_head_mask_bwd),
 }
 
 

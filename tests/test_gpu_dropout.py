@@ -379,6 +379,34 @@ def test_graph_replay_matches_eager():
     assert not diff, 'graph replay differs from eager in %s' % diff[:5]
 
 
+def test_mobilenet_v2_head_dropout_graph_replay_matches_eager():
+    """MobileNet-v2 with its head Dropout(0.2): Trainer.train with captured graphs against graphs disabled under the same
+    torch.manual_seed, parameters, running buffers and losses bit for bit after 6 steps -- the head's keep mask comes
+    from torch's CUDA generator, whose Philox offset a captured graph advances on every replay, so each replayed step
+    draws the mask the eager step draws"""
+    from convnet.pytorch_b200.models import mobilenet_v2
+    from convnet.pytorch_b200.engine import convert_b200
+    _setup()
+    g = torch.Generator().manual_seed(0)
+    batches = [(torch.randn(32, 3, 64, 64, generator=g), torch.randint(0, 1000, (32,), generator=g)) for _ in range(6)]
+    results = []
+    for use_graphs in (False, True):
+        torch.manual_seed(123)
+        model = convert_b200(mobilenet_v2(dataset='imagenet'), 'cuda')
+        assert model._b200.dropout_p == 0.2
+        tr = _trainer(model)
+        tr.use_graphs = use_graphs
+        res = tr.train(batches)
+        assert (tr.graph_replays > 0) == use_graphs
+        if use_graphs:
+            assert tr.graph_replays == len(batches) - 2
+        results.append((res, {k: v.detach().clone() for k, v in model.state_dict().items()}))
+    (r0, s0), (r1, s1) = results
+    assert r0['loss'] == r1['loss'], (r0['loss'], r1['loss'])
+    diff = [k for k in s0 if not torch.equal(s0[k], s1[k])]
+    assert not diff, 'graph replay differs from eager in %s' % diff[:5]
+
+
 @pytest.mark.parametrize('kind', ['mixup', 'device_augment'])
 def test_combines_with_mixup_and_device_augment(kind):
     """a dropout WRN-16-4 trains through Trainer.train with MixUp, or on uint8 batches augmented on the device: finite

@@ -203,9 +203,28 @@ def test_resnet50_imagenet_step_and_eval():
 
 def test_optimizer_step_matches_reference_chain():
     """OptimRegime on the B200 arenas vs torch SGD + WeightDecay hooks on the torch model, same gradients."""
-    from convnet.pytorch_b200.models import resnet
+    _optimizer_chain('resnet20')
+
+
+@pytest.mark.parametrize('name', ['mobilenet_v2', 'mobilenet_v1'])
+def test_mobilenet_optimizer_step_matches_reference_chain(name):
+    """the same for MobileNet: the dense convolution weights and the classifier weight are decayed, the depthwise
+    weights, the depthwise biases, the BatchNorm parameters and the classifier bias are not"""
+    _optimizer_chain(name)
+
+
+def _optimizer_chain(name):
+    """three steps of OptimRegime on the arenas and on the torch model from the same gradients: every parameter agrees.
+    The WeightDecay filter folds into the fused SGD as an arena prefix; that prefix must be the reference's decayed set
+    (oracle.ref_model.is_decayed)."""
+    from convnet.pytorch_b200 import models
     from convnet.pytorch_b200.utils.optim import OptimRegime
-    ref, mine, x, y = _pair(resnet, dict(dataset='cifar10', depth=20), (3, 32, 32), 10, batch=32)
+    from oracle import ref_model
+    factory, cfg, shape, classes = {
+        'resnet20': (models.resnet, dict(dataset='cifar10', depth=20), (3, 32, 32), 10),
+        'mobilenet_v2': (models.mobilenet_v2, dict(dataset='imagenet'), (3, 64, 64), 1000),
+        'mobilenet_v1': (models.mobilenet, dict(dataset='imagenet'), (3, 64, 64), 1000)}[name]
+    ref, mine, x, y = _pair(factory, cfg, shape, classes, batch=32)
     o_ref = OptimRegime(ref, copy.deepcopy(ref.regime))
     o_mine = OptimRegime(mine, copy.deepcopy(mine.regime))
     for step in range(3):
@@ -220,8 +239,15 @@ def test_optimizer_step_matches_reference_chain():
         o_ref.step()
         o_mine.step()
         with torch.no_grad():
+            worst = max((_rel(p, q), n) for (n, p), (_, q) in zip(mine.named_parameters(), ref.named_parameters()))
+            print('optimizer chain %s step %d: worst parameter rel-L2 %.3e (%s)' % ((name, step) + worst))
             for (n, p), (_, q) in zip(mine.named_parameters(), ref.named_parameters()):
                 assert _rel(p, q) < 1e-6, '%s after step %d: %.3e' % (n, step, _rel(p, q))
+    wd, count = o_mine.optimizer.extra_wd
+    sd = {k: v.cpu() for k, v in ref.state_dict().items()}
+    decayed = {s.name for s in mine._b200.arena.slots if s.offset < count}
+    assert wd == 1e-4 and decayed == {k for k in ref_model.param_names(sd) if ref_model.is_decayed(k, sd)}, \
+        'the folded WeightDecay prefix is not the decayed set: %s' % sorted(decayed)[:8]
     sd = o_mine.state_dict()
     assert len(sd['state']) == len(list(mine.parameters()))
     k0 = sorted(sd['state'].keys())[0]
