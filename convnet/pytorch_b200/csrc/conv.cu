@@ -56,6 +56,8 @@ struct IgemmParams {
   int window;            // > 0: block-diagonal convolution -- output channels [window*b, window*b + window) read source
                          // channels [window*b, window*b + window) only; the weight operand is [N_total][taps][window]
   uint32_t epi_bytes;    // one warpgroup's output staging tile
+  int epi_bufs;          // staging tiles per warpgroup (1 or 2), used alternately: with 2, a tile's epilogue does not
+                         // wait for the TMA store of the warpgroup's previous tile to leave shared memory
   double* stats;         // fused BN statistics accumulators [kReplicas][2][N_total] (BN workspace) or nullptr
   void* out;
   const void* res;
@@ -104,6 +106,23 @@ __device__ __forceinline__ void store_pair(const IgemmParams& p, float v0, float
   }
 }
 
+// store_pair for every column pair of one output row of a fragment (accumulators a[j + 2h], a[j + 2h + 1] at column
+// 2j), bf16, no bias or activation, all columns inside N_total and ldo even; off = element offset of the row's first
+// column pair.  The same arithmetic as store_pair, without its run-time branches.
+template <int BN, bool RES>
+__device__ __forceinline__ void store_row_bf16(const IgemmParams& p, const float (&a)[BN / 2], int h, long long off) {
+#pragma unroll
+  for (int j = 0; j < BN / 2; j += 4) {
+    float v0 = a[j + 2 * h], v1 = a[j + 2 * h + 1];
+    if (RES) {
+      const float2 t = unpack_bf16x2(*(reinterpret_cast<const uint32_t*>(reinterpret_cast<const __nv_bfloat16*>(p.res) + off + 2 * j)));
+      v0 += t.x;
+      v1 += t.y;
+    }
+    *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(p.out) + off + 2 * j) = pack_bf16x2(v0, v1);
+  }
+}
+
 // The MMAs of one operand stage for a warpgroup's 128-row tile: per 16-deep k-step, two m64 wgmmas (rows 0-63 and
 // 64-127) that share the B descriptor.  KS is the stage's k-steps (ck / 16); scale0 == 0 starts the accumulators.
 template <int KS, int SZ>
@@ -116,6 +135,40 @@ __device__ __forceinline__ void igemm_stage_mma(float (&acc)[2][SZ], uint64_t da
     wgmma_bf16<0, 0>(acc[1], da + a_half + 2 * k, db + 2 * k, k != 0 ? 1u : scale0);
   }
   wgmma_commit();
+}
+
+// Writes a warpgroup's 128 x BN accumulator tile, + bias, + residual (fetched into the same staging tile beforehand),
+// activation, rounded to bf16, into the 128B-swizzled staging tile epi_w (64-column boxes of [128 rows][128 B]).
+// FIXED = 1: no bias, no activation and the residual given by RES at compile time -- the epilogues of training (the
+// statistics-fusing forward pass, the data gradient with or without residual) -- so that the unrolled loop has no
+// branch.  With a run-time switch per value the scheduler could not overlap one value's residual load, adds, pack and
+// store with the next value's, and staging a 128-column tile took several times as long as its MMAs.  FIXED = 0 reads
+// the bias, residual and activation at run time.
+template <int BN, int FIXED, bool RES>
+__device__ __forceinline__ void stage_tile(uint8_t* epi_w, const float (&acc)[2][BN / 2], const IgemmParams& p,
+                                           int nbase, int r_lo, int c_lo) {
+  const bool res = FIXED ? RES : p.res != nullptr;
+  const int act = FIXED ? B200_ACT_NONE : p.act;
+#pragma unroll
+  for (int j = 0; j < BN / 2; j += 4) {
+    const int c = 2 * j + c_lo;
+    float bias0 = 0.f, bias1 = 0.f;   // added even without a bias: x + 0 turns -0 into +0
+    if (!FIXED && p.bias != nullptr) { bias0 = __ldg(p.bias + nbase + c); bias1 = __ldg(p.bias + nbase + c + 1); }
+#pragma unroll
+    for (int mh = 0; mh < 2; ++mh)
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int row = mh * 64 + r_lo + 8 * h;
+        uint32_t* dst = reinterpret_cast<uint32_t*>(epi_w + staged_offset(row, c, kTileM * 128));
+        float v0 = acc[mh][j + 2 * h] + bias0, v1 = acc[mh][j + 2 * h + 1] + bias1;
+        if (res) {
+          const float2 t = unpack_bf16x2(*dst);
+          v0 += t.x;
+          v1 += t.y;
+        }
+        *dst = pack_bf16x2(apply_act(v0, act), apply_act(v1, act));
+      }
+  }
 }
 
 // BN = block_n, the tile width: it sizes the accumulators exactly and fixes the wgmma shape at compile time.
@@ -226,7 +279,6 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   const int ksteps = p.ck / 16;
   const uint32_t bstat_addr = smem_u32(sBstat);
   constexpr int nbox = BN / 64;
-  uint8_t* epi_w = epi + wg * p.epi_bytes;           // this warpgroup's staging tile: 64-column boxes of [128 rows][128 B]
   // fused-statistics bookkeeping (BN = 64 or 128): this thread owns column st_col, rows [st_row0, st_row0 + st_rows)
   // of each tile
   const int st_col = wt % BN;
@@ -245,10 +297,16 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     const int n_tile = p.own_ntile ? own_n : tile - m_tile * p.n_tiles;
     const int nbase = n_tile * BN;
     const int mine = local >> 1;   // this warpgroup's tile count so far
+    // this tile's staging buffer: 64-column boxes of [128 rows][128 B]
+    uint8_t* epi_w = epi + (wg * p.epi_bufs + (p.epi_bufs == 2 ? (mine & 1) : 0)) * p.epi_bytes;
     if (p.tma_store) {
-      // The staging tile is reused: this warpgroup's store of its previous tile must have read it and its threads must
-      // be done with their statistics reads.  Then the residual tile is fetched into it, landing while the MMAs run.
-      if (leader && mine > 0) bulk_wait_group_read0();
+      // The staging tile is reused: the store of the warpgroup's tile that last used it must have read it (with two
+      // buffers, the store of the tile just before may still be reading the other one) and its threads must be done
+      // with their statistics reads.  Then the residual tile is fetched into it, landing while the MMAs run.
+      if (leader && mine > 0) {
+        if (p.epi_bufs == 2) bulk_wait_group_read1();
+        else bulk_wait_group_read0();
+      }
       named_bar_sync(1 + wg, 128);
       if (leader && p.res != nullptr) {
         fence_proxy_async();
@@ -292,26 +350,9 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         // Dense bf16 output: stage the tile in 128B-swizzled shared memory and write it with TMA (coalesced, clipped at
         // the M tail); the residual was fetched into the same buffer.
         if (p.res != nullptr) mbar_wait(&res_bar[wg], static_cast<uint32_t>(mine & 1));
-#pragma unroll
-        for (int j = 0; j < BN / 2; j += 4) {
-          const int c = 2 * j + c_lo;
-          float bias0 = 0.f, bias1 = 0.f;
-          if (p.bias != nullptr) { bias0 = __ldg(p.bias + nbase + c); bias1 = __ldg(p.bias + nbase + c + 1); }
-#pragma unroll
-          for (int mh = 0; mh < 2; ++mh)
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-              const int row = mh * 64 + r_lo + 8 * h;
-              uint32_t* dst = reinterpret_cast<uint32_t*>(epi_w + staged_offset(row, c, kTileM * 128));
-              float v0 = acc[mh][j + 2 * h] + bias0, v1 = acc[mh][j + 2 * h + 1] + bias1;
-              if (p.res != nullptr) {
-                const float2 t = unpack_bf16x2(*dst);
-                v0 += t.x;
-                v1 += t.y;
-              }
-              *dst = pack_bf16x2(apply_act(v0, p.act), apply_act(v1, p.act));
-            }
-        }
+        if (p.bias != nullptr || p.act != B200_ACT_NONE) stage_tile<BN, 0, false>(epi_w, acc, p, nbase, r_lo, c_lo);
+        else if (p.res != nullptr) stage_tile<BN, 1, true>(epi_w, acc, p, nbase, r_lo, c_lo);
+        else stage_tile<BN, 1, false>(epi_w, acc, p, nbase, r_lo, c_lo);
         fence_proxy_async();                             // generic-proxy smem writes -> visible to TMA
         named_bar_sync(1 + wg, 128);
         if (leader) {
@@ -345,6 +386,9 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       }
       continue;
     }
+    // bf16 output, no bias or activation, no column tail (the strided data gradients): stored without a branch per value
+    const bool plain = !p.out_fp32 && p.bias == nullptr && p.act == B200_ACT_NONE && (p.ldo & 1) == 0 &&
+                       nbase + BN <= p.N_total;
 #pragma unroll
     for (int mh = 0; mh < 2; ++mh)
 #pragma unroll
@@ -357,8 +401,12 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         const int bj = rem - bi * p.J;
         const long long off = ((static_cast<long long>(img) * p.OH + (bi * p.os + p.oh0)) * p.OW + (bj * p.os + p.ow0)) *
                               static_cast<long long>(p.ldo);
+        if (plain && p.res != nullptr) store_row_bf16<BN, true>(p, acc[mh], h, off + nbase + c_lo);
+        else if (plain) store_row_bf16<BN, false>(p, acc[mh], h, off + nbase + c_lo);
+        else {
 #pragma unroll
-        for (int j = 0; j < BN / 2; j += 4) store_pair(p, acc[mh][j + 2 * h], acc[mh][j + 2 * h + 1], off, nbase + 2 * j + c_lo);
+          for (int j = 0; j < BN / 2; j += 4) store_pair(p, acc[mh][j + 2 * h], acc[mh][j + 2 * h + 1], off, nbase + 2 * j + c_lo);
+        }
       }
   }
   if constexpr (BN == 64 || BN == 128)
@@ -729,8 +777,14 @@ static int launch_igemm(const IgemmLaunch& L, cudaStream_t stream) {
   // dense bf16 outputs with 64-channel granularity go out through shared memory + TMA store
   p.tma_store = (L.os == 1 && !L.out_fp32 && (p.block_n % 64) == 0 && (L.Nout % p.block_n) == 0 && L.ldo == L.Nout &&
                  L.OH == L.I && L.OW == L.J && L.oh0 == 0 && L.ow0 == 0) ? 1 : 0;
-  const int epi_bytes = p.tma_store ? kTileM * p.block_n * 2 : 0;   // per consumer warpgroup
-  const int epi_total = 2 * epi_bytes;
+  const int epi_bytes = p.tma_store ? kTileM * p.block_n * 2 : 0;   // per staging tile
+  // A tile that stores at least as many bytes as it loads (the expanding 1x1 layers and their data gradients with
+  // C <= 128) is bound by its output stream.  With one staging tile per warpgroup, each epilogue first waits for the
+  // warpgroup's previous TMA store to drain, so only about one store per warpgroup is in flight; two staging tiles let
+  // the next epilogue start while that store is still leaving.
+  const int k_iters = L.ntaps * p.c_chunks;
+  p.epi_bufs = (p.tma_store && k_iters * (int)p.a_bytes <= epi_bytes) ? 2 : 1;
+  int epi_total = 2 * p.epi_bufs * epi_bytes;
   // small 1x1 layers (all weight slices <= 64 KB): keep the weights resident, stream only the activations
   const int b_all = L.ntaps * p.c_chunks * (int)p.b_bytes;
   int bstat_bytes = 0;
@@ -761,6 +815,11 @@ static int launch_igemm(const IgemmLaunch& L, cudaStream_t stream) {
   }
   p.epi_bytes = (uint32_t)epi_bytes;
   p.num_stages = (kSmemBudgetMax - epi_total - bstat_bytes) / (int)stage;
+  if (p.epi_bufs == 2 && p.num_stages < 2 * k_iters) {   // the ring must still hold two tiles' operands
+    p.epi_bufs = 1;
+    epi_total = 2 * epi_bytes;
+    p.num_stages = (kSmemBudgetMax - epi_total - bstat_bytes) / (int)stage;
+  }
   if (p.num_stages > kMaxStages) p.num_stages = kMaxStages;
   if (p.num_stages < 2) p.num_stages = 2;
   p.OH = L.OH; p.OW = L.OW; p.os = L.os; p.oh0 = L.oh0; p.ow0 = L.ow0; p.ldo = L.ldo;
@@ -813,10 +872,11 @@ static int launch_igemm(const IgemmLaunch& L, cudaStream_t stream) {
                                       : (total_tiles + grid - 1) / grid;
     fprintf(stderr, "[igemm] M=%d C=%d N=%d taps=%d os=%d block_n=%d n_tiles=%d m_tiles=%d ck=%d k_iters=%d stages=%d "
             "tma_store=%d plain_a=%d bstat=%d own=%d out_fp32=%d bias=%d res=%d act=%d stats=%d grid=%d max_tiles=%d "
-            "smem=%d window=%d xs=%d\n",
+            "smem=%d window=%d xs=%d epi_bufs=%d\n",
             p.M_total, L.SC, L.Nout, L.ntaps, L.os, p.block_n, p.n_tiles, p.m_tiles, p.ck, L.ntaps * p.c_chunks,
             p.num_stages, p.tma_store, p.plain_a, p.b_stationary, p.own_ntile, p.out_fp32, L.bias != nullptr,
-            L.res != nullptr, p.act, L.stats != nullptr, grid, max_tiles, smem_bytes, L.window, (int)L.s_pix);
+            L.res != nullptr, p.act, L.stats != nullptr, grid, max_tiles, smem_bytes, L.window, (int)L.s_pix,
+            p.epi_bufs);
   }
   b200::launch(kfn, grid, kThreads, smem_bytes, stream, tmA, tmB, tmC, tmR, p);
   B200_CHECK_LAUNCH("conv_igemm_kernel");
