@@ -16,6 +16,7 @@
 #include "common.cuh"
 #include "host.h"
 #include <stdlib.h>
+#include <type_traits>
 
 namespace b200 {
 
@@ -27,7 +28,9 @@ struct HaloParams {
   int RT, Wp;              // output rows per tile, halo row pitch W+S-1
   int tiles_per_img, m_tiles, n_tiles, block_n, c_chunks;
   int sa, sb;              // ring depths (sb unused when the weights are stationary)
-  uint32_t a_bytes, a_box_bytes, b_bytes;
+  int epi_bufs;            // staging tiles (1 or 2), used alternately: with 2, a tile's epilogue does not wait for the
+                           // TMA store of the tile just before to leave shared memory
+  uint32_t a_bytes, a_box_bytes, b_bytes, epi_bytes;
   int act;
   int has_res;
   double* stats;
@@ -41,6 +44,38 @@ struct HaloParams {
   uint16_t a_off[kHMaxTaps];  // pixel-row offset of each tap's view inside the halo buffer
   uint16_t b_tap[kHMaxTaps];  // weight tap slice used with it
 };
+
+// Writes a warpgroup's 64 x BN accumulator rows (fragment rows h = 0, 1 of this thread go to staged rows srow[h], and
+// only where keep[h]), + bias, + residual (fetched into the staging tile beforehand), activation, rounded to bf16, into
+// the 128B-swizzled staging tile epi_t (64-column boxes box_pitch bytes apart).  FIXED = 1: no bias, no activation and
+// the residual given by RES at compile time -- the epilogues of training (the statistics-fusing forward pass and the
+// data gradient) -- so that the unrolled loop has no branch per value.  FIXED = 0 reads the bias, residual and
+// activation at run time.  The bias is added only when there is one, so a -0 accumulator stays -0.
+template <int BN, int FIXED, bool RES>
+__device__ __forceinline__ void halo_stage_tile(uint8_t* epi_t, const float (&acc)[BN / 2], const HaloParams& p,
+                                                int nbase, const int (&srow)[2], const bool (&keep)[2], int c_lo,
+                                                uint32_t box_pitch) {
+  const bool res = FIXED ? RES : p.has_res != 0;
+  const bool bias = !FIXED && p.bias != nullptr;
+  const int act = FIXED ? B200_ACT_NONE : p.act;
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    if (!keep[h]) continue;
+#pragma unroll
+    for (int j = 0; j < BN / 2; j += 4) {
+      const int c = 2 * j + c_lo;
+      uint32_t* dst = reinterpret_cast<uint32_t*>(epi_t + staged_offset(srow[h], c, box_pitch));
+      float v0 = acc[j + 2 * h], v1 = acc[j + 2 * h + 1];
+      if (bias) { v0 += __ldg(p.bias + nbase + c); v1 += __ldg(p.bias + nbase + c + 1); }
+      if (res) {
+        const float2 t2 = unpack_bf16x2(*dst);
+        v0 += t2.x;
+        v1 += t2.y;
+      }
+      *dst = pack_bf16x2(apply_act(v0, act), apply_act(v1, act));
+    }
+  }
+}
 
 // Descriptors are built once per operand buffer and advanced by adding (byte offset >> 4) to the address field, with
 // the tap / k-step loops fully unrolled.  BN = block_n (64, 128 or 256) sizes the accumulators exactly.
@@ -149,14 +184,22 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant_
     const int img = m_tile / p.tiles_per_img;
     const int h0 = (m_tile - img * p.tiles_per_img) * p.RT;
     const int nbase = n_tile * BN;
-    // the staging tile is reused: the previous TMA store must have read it, every thread must be done with its
-    // statistics reads; then the residual tile is fetched into it while the MMAs run
-    if (leader && local > 0) bulk_wait_group_read0();
-    named_bar_sync(1, 256);
-    if (leader && p.has_res) {
-      fence_proxy_async();
-      mbar_arrive_expect_tx(&res_bar, static_cast<uint32_t>(nbox) * box_bytes);
-      for (int b = 0; b < nbox; ++b) tma_load_4d(&tmR, &res_bar, epi + b * box_pitch, nbase + b * 64, 0, h0, img);
+    uint8_t* epi_t = epi + (p.epi_bufs == 2 ? (local & 1) : 0) * p.epi_bytes;   // this tile's staging tile
+    // The staging tile is reused: the TMA store of the tile that last used it must have read it (with two, the store of
+    // the tile just before may still be reading the other one) and every thread must be done with its statistics reads
+    // of it.  Without a residual nothing touches it before the staging, so the store drains under this tile's MMAs;
+    // with one, the residual tile is fetched into it first, landing while the MMAs run.
+    if (p.has_res) {
+      if (leader && local > 0) {
+        if (p.epi_bufs == 2) bulk_wait_group_read1();
+        else bulk_wait_group_read0();
+      }
+      named_bar_sync(1, 256);
+      if (leader) {
+        fence_proxy_async();
+        mbar_arrive_expect_tx(&res_bar, static_cast<uint32_t>(nbox) * box_bytes);
+        for (int b = 0; b < nbox; ++b) tma_load_4d(&tmR, &res_bar, epi_t + b * box_pitch, nbase + b * 64, 0, h0, img);
+      }
     }
 
     // one commit group per tap (streamed weights: each tap frees a weight slot) or per channel block (resident weights);
@@ -167,30 +210,40 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant_
     for (int cc = 0; cc < p.c_chunks; ++cc) {
       mbar_wait(&a_full[ia], pa);
       const uint64_t da0 = proto + (smem_u32(sA + ia * p.a_bytes) >> 4) + a_wg;
+      // The tap loop is compiled once for each weight residency.  With resident weights no run-time test and no
+      // commit sits between the MMAs of two taps, and one fence per channel block suffices, so the MMAs of all taps
+      // issue as one group.  With the residency tested at run time, ptxas closed the MMAs of every tap as a group of
+      // their own and injected a warpgroup.arrive before the next tap: the MMA phase of a stem tile took 2.5 times as
+      // long, that of a 128-wide layer2 tile 1.3 times.
+      auto taps = [&](auto stationary) {
+        constexpr bool kStat = decltype(stationary)::value;
 #pragma unroll
-      for (int t = 0; t < NTAPS; ++t) {
-        uint64_t db0;
-        if (p.b_stationary) {
-          db0 = proto + (smem_u32(sB + (cc * NTAPS + t) * p.b_bytes) >> 4);
-        } else {
-          mbar_wait(&b_full[ib], pb);
-          db0 = proto + (smem_u32(sB + ib * p.b_bytes) >> 4);
-        }
-        const uint32_t tap_inc = (static_cast<uint32_t>(p.a_off[t]) * p.row_bytes) >> 4;
-        wgmma_fence();
+        for (int t = 0; t < NTAPS; ++t) {
+          uint64_t db0;
+          if (kStat) {
+            db0 = proto + (smem_u32(sB + (cc * NTAPS + t) * p.b_bytes) >> 4);
+          } else {
+            mbar_wait(&b_full[ib], pb);
+            db0 = proto + (smem_u32(sB + ib * p.b_bytes) >> 4);
+          }
+          const uint32_t tap_inc = (static_cast<uint32_t>(p.a_off[t]) * p.row_bytes) >> 4;
+          if (!kStat || t == 0) wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < KSTEPS; ++k)
-          wgmma_bf16<0, 0>(acc, da0 + tap_inc + 2 * k, db0 + 2 * k, (cc | t | k) != 0 ? 1u : 0u);
-        if (!p.b_stationary || t == NTAPS - 1) {
-          wgmma_commit();
-          wgmma_wait<1>();
-          if (rel_b >= 0) release_stage(&b_empty[rel_b], lane);
-          if (rel_a >= 0) release_stage(&a_empty[rel_a], lane);
-          rel_a = (t == NTAPS - 1) ? ia : -1;
-          rel_b = p.b_stationary ? -1 : ib;
+          for (int k = 0; k < KSTEPS; ++k)
+            wgmma_bf16<0, 0>(acc, da0 + tap_inc + 2 * k, db0 + 2 * k, (cc | t | k) != 0 ? 1u : 0u);
+          if (!kStat || t == NTAPS - 1) {
+            wgmma_commit();
+            wgmma_wait<1>();
+            if (rel_b >= 0) release_stage(&b_empty[rel_b], lane);
+            if (rel_a >= 0) release_stage(&a_empty[rel_a], lane);
+            rel_a = (t == NTAPS - 1) ? ia : -1;
+            rel_b = kStat ? -1 : ib;
+          }
+          if (!kStat && ++ib == p.sb) { ib = 0; pb ^= 1u; }
         }
-        if (!p.b_stationary && ++ib == p.sb) { ib = 0; pb ^= 1u; }
-      }
+      };
+      if (p.b_stationary) taps(std::true_type{});
+      else taps(std::false_type{});
       if (++ia == p.sa) { ia = 0; pa ^= 1u; }
     }
     wgmma_wait<0>();
@@ -198,29 +251,28 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant_
     if (rel_b >= 0) release_stage(&b_empty[rel_b], lane);
     if (rel_a >= 0) release_stage(&a_empty[rel_a], lane);
 
-    if (p.has_res) mbar_wait(&res_bar, static_cast<uint32_t>(local & 1));
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      if (!in_tile[h] || h0 + (r_lo + 8 * h) / p.Wp >= p.H) continue;
-      const int row = srow[h];
-#pragma unroll
-      for (int j = 0; j < BN / 2; j += 4) {
-        const int c = 2 * j + c_lo;
-        uint32_t* dst = reinterpret_cast<uint32_t*>(epi + staged_offset(row, c, box_pitch));
-        float v0 = acc[j + 2 * h], v1 = acc[j + 2 * h + 1];
-        if (p.bias != nullptr) { v0 += __ldg(p.bias + nbase + c); v1 += __ldg(p.bias + nbase + c + 1); }
-        if (p.has_res) {
-          const float2 t2 = unpack_bf16x2(*dst);
-          v0 += t2.x;
-          v1 += t2.y;
-        }
-        *dst = pack_bf16x2(apply_act(v0, p.act), apply_act(v1, p.act));
+    if (p.has_res) {
+      mbar_wait(&res_bar, static_cast<uint32_t>(local & 1));
+    } else {
+      if (leader && local > 0) {
+        if (p.epi_bufs == 2) bulk_wait_group_read1();
+        else bulk_wait_group_read0();
       }
+      named_bar_sync(1, 256);
     }
+    bool keep[2];   // fragment rows inside the tile and the image (the last row tile of an image may be ragged)
+#pragma unroll
+    for (int h = 0; h < 2; ++h) keep[h] = in_tile[h] && h0 + (r_lo + 8 * h) / p.Wp < p.H;
+    if (p.bias != nullptr || p.act != B200_ACT_NONE)
+      halo_stage_tile<BN, 0, false>(epi_t, acc, p, nbase, srow, keep, c_lo, box_pitch);
+    else if (p.has_res)
+      halo_stage_tile<BN, 1, true>(epi_t, acc, p, nbase, srow, keep, c_lo, box_pitch);
+    else
+      halo_stage_tile<BN, 1, false>(epi_t, acc, p, nbase, srow, keep, c_lo, box_pitch);
     fence_proxy_async();
     named_bar_sync(1, 256);
     if (leader) {
-      for (int b = 0; b < nbox; ++b) tma_store_4d(&tmC, epi + b * box_pitch, nbase + b * 64, 0, h0, img);
+      for (int b = 0; b < nbox; ++b) tma_store_4d(&tmC, epi_t + b * box_pitch, nbase + b * 64, 0, h0, img);
       bulk_commit_group();
     }
     if (p.stats != nullptr) {
@@ -231,7 +283,8 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant_
       const int vrows = min(p.RT, p.H - h0) * p.W;   // staged rows that belong to the image
       const int r_end = min(st_row0 + st_rows, vrows);
       for (int r = st_row0; r < r_end; ++r) {
-        const float x = __bfloat162float(*reinterpret_cast<const __nv_bfloat16*>(epi + staged_offset(r, st_col, box_pitch)));
+        const float x =
+            __bfloat162float(*reinterpret_cast<const __nv_bfloat16*>(epi_t + staged_offset(r, st_col, box_pitch)));
         st_s1 += x;
         st_s2 = fmaf(x, x, st_s2);
       }
@@ -313,27 +366,32 @@ int launch_halo(const void* src, const void* wmat, void* out, const void* res, c
       p.a_off[t] = (uint16_t)(dir == 0 ? r * p.Wp + s : (R - 1 - r) * p.Wp + (S - 1 - s));
     }
   const uint32_t box_pitch = (((uint32_t)(p.RT * W) * 128u) + 1023u) & ~1023u;
-  const uint32_t epi_bytes = (uint32_t)(p.block_n / 64) * box_pitch;
-  int budget = 212 * 1024 - (int)epi_bytes;
+  p.epi_bytes = (uint32_t)(p.block_n / 64) * box_pitch;
   const int b_all = p.c_chunks * p.ntaps * (int)p.b_bytes;
   p.b_stationary = ((p.n_tiles == 1 || p.diag) && b_all <= 80 * 1024) ? 1 : 0;
   B200_REQUIRE(!p.diag || p.b_stationary, B200_ERR_UNSUPPORTED, "conv halo: window mode expects resident weights");
-  int b_region;
-  if (p.b_stationary) {
-    b_region = b_all;
-    p.sb = 0;
-    p.sa = (budget - b_region) / (int)p.a_bytes;
-    if (p.sa > kHMaxA) p.sa = kHMaxA;
-  } else {
-    p.sa = 2;
-    p.sb = (budget - p.sa * (int)p.a_bytes) / (int)p.b_bytes;
-    if (p.sb > kHMaxB) p.sb = kHMaxB;
-    if (p.sb >= 6 && (int)(3 * p.a_bytes + 4 * p.b_bytes) <= budget) {
-      p.sa = 3;
-      p.sb = (budget - 3 * (int)p.a_bytes) / (int)p.b_bytes;
+  // Two staging tiles where the operand ring still gets two slots (sa >= 2, streamed weights sb >= 2), else one: with
+  // one, each epilogue first waits for the store of the tile before to leave shared memory.
+  int b_region = 0;
+  for (p.epi_bufs = 2; p.epi_bufs >= 1; --p.epi_bufs) {
+    const int budget = 212 * 1024 - p.epi_bufs * (int)p.epi_bytes;
+    if (p.b_stationary) {
+      b_region = b_all;
+      p.sb = 0;
+      p.sa = (budget - b_region) / (int)p.a_bytes;
+      if (p.sa > kHMaxA) p.sa = kHMaxA;
+    } else {
+      p.sa = 2;
+      p.sb = (budget - p.sa * (int)p.a_bytes) / (int)p.b_bytes;
       if (p.sb > kHMaxB) p.sb = kHMaxB;
+      if (p.sb >= 6 && (int)(3 * p.a_bytes + 4 * p.b_bytes) <= budget) {
+        p.sa = 3;
+        p.sb = (budget - 3 * (int)p.a_bytes) / (int)p.b_bytes;
+        if (p.sb > kHMaxB) p.sb = kHMaxB;
+      }
+      b_region = p.sb * (int)p.b_bytes;
     }
-    b_region = p.sb * (int)p.b_bytes;
+    if (p.sa >= 2 && (p.b_stationary || p.sb >= 2)) break;
   }
   B200_REQUIRE(p.sa >= 2 && (p.b_stationary || p.sb >= 2), B200_ERR_UNSUPPORTED,
                "conv halo: shared memory budget exceeded (W=%d, block_n=%d)", W, p.block_n);
@@ -351,7 +409,7 @@ int launch_halo(const void* src, const void* wmat, void* out, const void* res, c
     rc = encode_tiled(&tmR, res, 4, {Nout, W, H, N}, {64, W, p.RT, 1}, "conv halo residual");
     if (rc) return rc;
   }
-  const int smem_bytes = p.sa * (int)p.a_bytes + b_region + (int)epi_bytes + 1024;
+  const int smem_bytes = p.sa * (int)p.a_bytes + b_region + p.epi_bufs * (int)p.epi_bytes + 1024;
   HaloKernelFn kfn = halo_kernel_for(p.ntaps, p.block_n);
   B200_REQUIRE(kfn != nullptr, B200_ERR_UNSUPPORTED, "conv halo: %d taps with block_n %d unsupported", p.ntaps, p.block_n);
   rc = set_smem_attr((const void*)kfn, smem_bytes);
@@ -366,9 +424,9 @@ int launch_halo(const void* src, const void* wmat, void* out, const void* res, c
   }
   if (getenv("B200_HALO_DEBUG"))
     fprintf(stderr, "[halo] dir=%d N=%d H=%d W=%d C=%d K=%d taps=%d block_n=%d n_tiles=%d m_tiles=%d bstat=%d diag=%d "
-            "sa=%d sb=%d bias=%d res=%d act=%d stats=%d grid=%d\n", dir, N, H, W, Cs, Nout, p.ntaps, p.block_n,
-            p.n_tiles, p.m_tiles, p.b_stationary, p.diag, p.sa, p.sb, bias != nullptr, res != nullptr, act,
-            stats != nullptr, grid);
+            "sa=%d sb=%d bias=%d res=%d act=%d stats=%d grid=%d epi_bufs=%d\n", dir, N, H, W, Cs, Nout, p.ntaps,
+            p.block_n, p.n_tiles, p.m_tiles, p.b_stationary, p.diag, p.sa, p.sb, bias != nullptr, res != nullptr, act,
+            stats != nullptr, grid, p.epi_bufs);
   b200::launch(kfn, grid, kThreads, smem_bytes, stream, tmX, tmB, tmC, tmR, p);
   B200_CHECK_LAUNCH("conv_halo_kernel");
   return B200_OK;
