@@ -29,6 +29,13 @@ Resize + CenterCrop on the device (transform key ``device_scale_crop``, ImageNet
 decode and compute each image's resized size, crop offsets and support region; the loader yields
 (utils.augment.ScaleCropBatch of the regions and geometry, target) and the stem relayout kernel resamples the crop
 window of each whole image's resize and normalises it.  Same datasets as ``device_resized_crop``.
+
+JPEG decode on the device (transform key ``device_decode``, together with one of the two device crops): the workers
+read the file bytes and parse the headers (utils/jpeg.py) but do not decode baseline JPEGs; the loader yields
+(utils.augment.JpegBatch, target) and csrc/jpeg.cu decodes each image's region into the region buffer the crop's
+relayout reads, byte for byte what Pillow decodes.  Other files (progressive, CMYK, PNG, ...) are decoded by PIL in the
+worker and ride in the same batch.  Real imagenet reads the files' bytes; synthetic_imagenet encodes its seeded pool
+in memory with PIL (quality 90, 4:2:0).
 """
 import os
 from copy import deepcopy
@@ -38,8 +45,8 @@ import torch
 from torch.utils.data import Dataset, Subset
 from torch.utils.data.distributed import DistributedSampler
 
-from .utils.augment import AugmentCollate, BatchAugment, Cutout, ResizedCrop, ResizedCropCollate, ScaleCrop, \
-    ScaleCropCollate
+from .utils.augment import AugmentCollate, BatchAugment, Cutout, JpegCollate, JpegDecode, ResizedCrop, \
+    ResizedCropCollate, ScaleCrop, ScaleCropCollate
 from .utils.regime import Regime
 
 
@@ -163,7 +170,7 @@ def get_dataset(name, split='train', transform=None, target_transform=None, down
 
 def device_augment_spec(transform_name='cifar10', input_size=None, scale_size=None, normalize=None, augment=True,
                         cutout=None, autoaugment=False, padding=None, duplicates=1, num_crops=1, device_augment=True,
-                        device_resized_crop=False, device_scale_crop=False):
+                        device_resized_crop=False, device_scale_crop=False, device_decode=False):
     """The BatchAugment of a ``device_augment`` transform setting: the CIFAR training transform of
     real_dataset_transform (pad-4 random crop + flip + ToTensor + Normalize [+ Cutout]) with its duplicates.  The
     settings it cannot reproduce raise."""
@@ -215,7 +222,7 @@ def u8_dataset(name, input_size=None, scale_size=None, split='train', download=T
 def resized_crop_spec(transform_name='imagenet', input_size=None, scale_size=None, normalize=None, augment=True,
                       cutout=None, autoaugment=False, padding=None, duplicates=1, num_crops=1, device_augment=False,
                       device_resized_crop=True, interpolation='bilinear', color_jitter=None, lighting=None,
-                      device_scale_crop=False):
+                      device_scale_crop=False, device_decode=False):
     """The ResizedCrop of a ``device_resized_crop`` transform setting: the imagenet training transform of
     real_dataset_transform (RandomResizedCrop(input_size) + flip + ToTensor + Normalize) with its duplicates.  The
     settings it cannot reproduce raise."""
@@ -240,7 +247,7 @@ def resized_crop_spec(transform_name='imagenet', input_size=None, scale_size=Non
 
 def scale_crop_spec(transform_name='imagenet', input_size=None, scale_size=None, normalize=None, augment=False,
                     cutout=None, autoaugment=False, padding=None, duplicates=1, num_crops=1, device_augment=False,
-                    device_resized_crop=False, device_scale_crop=True, interpolation='bilinear'):
+                    device_resized_crop=False, device_scale_crop=True, interpolation='bilinear', device_decode=False):
     """The ScaleCrop of a ``device_scale_crop`` transform setting: the imagenet evaluation transform of
     real_dataset_transform (Resize(scale_size) + CenterCrop(input_size) + ToTensor + Normalize, scale_size =
     int(input_size * 8 / 7) unless set).  The settings it cannot reproduce raise."""
@@ -305,11 +312,46 @@ def decoded_dataset(name, transform, split='train', datasets_path='~/Datasets', 
                               % name)
 
 
+def read_bytes(path):
+    """ImageFolder loader of ``device_decode``: the file's bytes (the workers parse headers, they do not decode)."""
+    with open(path, 'rb') as f:
+        return f.read()
+
+
+def synthetic_imagenet_jpegs(seed=0):
+    """synthetic_imagenet_pool(seed) encoded in memory by PIL (quality 90, 4:2:0): the files of ``device_decode``."""
+    import io
+    out = []
+    for img in synthetic_imagenet_pool(seed=seed):
+        buf = io.BytesIO()
+        img.save(buf, 'JPEG', quality=90, subsampling=2)
+        out.append(buf.getvalue())
+    return out
+
+
+def encoded_dataset(name, transform, split='train', datasets_path='~/Datasets', synthetic_length=None, **_):
+    """File-bytes samples of ``device_decode``: ImageFolder with read_bytes for imagenet, synthetic_imagenet_jpegs for
+    synthetic_imagenet; ``transform`` (a utils.augment.JpegDecode) does the per-image host work."""
+    train = split == 'train'
+    if name == 'synthetic_imagenet':
+        _, classes, n_train, n_val = _SYNTHETIC[name]
+        length = synthetic_length or int(os.environ.get('B200_SYNTHETIC_LENGTH', n_train if train else n_val))
+        g = torch.Generator().manual_seed(2 if train else 3)
+        return DecodedImages(synthetic_imagenet_jpegs(seed=0 if train else 1),
+                             torch.randint(0, classes, (length,), generator=g), transform)
+    if name == 'imagenet':
+        import torchvision.datasets as tvd
+        return tvd.ImageFolder(root=os.path.join(os.path.expanduser(datasets_path), name, 'train' if train else 'val'),
+                               transform=transform, loader=read_bytes)
+    raise NotImplementedError('device_decode supports imagenet and synthetic_imagenet; got %r' % name)
+
+
 _DATA_ARGS = {'name', 'split', 'transform', 'target_transform', 'download', 'datasets_path', 'synthetic_length'}
 _DATALOADER_ARGS = {'batch_size', 'shuffle', 'sampler', 'batch_sampler', 'num_workers', 'collate_fn', 'pin_memory',
                     'drop_last', 'timeout', 'worker_init_fn'}
 _TRANSFORM_ARGS = {'transform_name', 'input_size', 'scale_size', 'normalize', 'augment', 'cutout', 'duplicates',
-                   'num_crops', 'autoaugment', 'device_augment', 'device_resized_crop', 'device_scale_crop'}
+                   'num_crops', 'autoaugment', 'device_augment', 'device_resized_crop', 'device_scale_crop',
+                   'device_decode'}
 _OTHER_ARGS = {'distributed'}
 
 
@@ -340,7 +382,15 @@ class DataRegime(object):
             data_kwargs = dict(setting['data'])
             name = data_kwargs.get('name', '')
             collate = None
-            if setting['transform'].get('device_scale_crop'):
+            tf_set = setting['transform']
+            if tf_set.get('device_decode') and not (tf_set.get('device_scale_crop') or tf_set.get('device_resized_crop')):
+                raise NotImplementedError('device_decode decodes into the region buffer of device_resized_crop or '
+                                          'device_scale_crop; set one of them')
+            if tf_set.get('device_decode'):
+                spec = (scale_crop_spec if tf_set.get('device_scale_crop') else resized_crop_spec)(**tf_set)
+                self._data = encoded_dataset(transform=JpegDecode(spec), **data_kwargs)
+                collate = JpegCollate(spec)
+            elif setting['transform'].get('device_scale_crop'):
                 spec = scale_crop_spec(**setting['transform'])
                 self._data = decoded_dataset(transform=spec, **data_kwargs)
                 collate = ScaleCropCollate(spec)
@@ -360,7 +410,8 @@ class DataRegime(object):
                 # real images: build the transform the regime asks for (reference data.py:101-102) -- never fall back
                 # to a bare ToTensor(), which would train on unnormalised, unaugmented, variable-size images
                 tf = {k: v for k, v in setting['transform'].items()
-                      if v is not None and k not in ('device_augment', 'device_resized_crop', 'device_scale_crop')}
+                      if v is not None and k not in ('device_augment', 'device_resized_crop', 'device_scale_crop',
+                                                     'device_decode')}
                 data_kwargs['transform'] = real_dataset_transform(**tf)
             if collate is None:
                 self._data = get_dataset(**data_kwargs)

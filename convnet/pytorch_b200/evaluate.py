@@ -58,6 +58,9 @@ def build_parser():
     a('--device-scale-crop', action='store_true', default=False,
       help='ImageNet: the loader workers only decode; the input relayout on the GPU resizes (Pillow-exact bilinear), '
            'centre-crops and normalises the images')
+    a('--device-decode', action='store_true', default=False,
+      help='ImageNet, with --device-scale-crop: the loader workers only read the files and parse their headers; '
+           'baseline JPEGs are decoded on the GPU, byte for byte what Pillow decodes')
     a('--calibrate-bn', action='store_true', default=False, help='calibrate bn stats')
     a('--calibrate-steps', default=200, type=int, help='forward passes of --calibrate-bn (reference: 200)')
     a('--avg-out', action='store_true', default=False, help='average outputs over the duplicates')
@@ -110,6 +113,10 @@ def main_worker(args):
     os.makedirs(save_path, exist_ok=True)
     setup_logging(os.path.join(save_path, 'log.txt'))
     cuda = 'cuda' in args.device and torch.cuda.is_available()
+    if args.device_decode and not args.device_scale_crop:
+        raise NotImplementedError('--device-decode decodes into the regions of --device-scale-crop; set it')
+    if args.device_decode and not cuda:
+        raise NotImplementedError('--device-decode decodes on the GPU: it needs a CUDA device')
     if cuda:
         torch.cuda.manual_seed_all(args.seed)
         torch.cuda.set_device(args.device_ids[0])
@@ -150,7 +157,8 @@ def main_worker(args):
     common = {'datasets_path': args.datasets_dir, 'name': args.dataset, 'input_size': args.input_size,
               'batch_size': args.batch_size, 'num_workers': args.workers, 'pin_memory': cuda, 'drop_last': False}
     val_data = DataRegime(None, defaults=dict(common, split='val', augment=args.augment, shuffle=False,
-                                              duplicates=args.duplicates, device_scale_crop=args.device_scale_crop))
+                                              duplicates=args.duplicates, device_scale_crop=args.device_scale_crop,
+                                              device_decode=args.device_decode))
     if args.calibrate_bn:
         train_data = DataRegime(None, defaults=dict(common, split='train', augment=True, shuffle=True))
         trainer.calibrate_bn(train_data.get_loader(), num_steps=args.calibrate_steps)

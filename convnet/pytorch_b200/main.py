@@ -10,7 +10,8 @@ masters in the arena), ``synthetic_*`` datasets, ``--b200 {auto,on,off}`` (auto:
 ``--device-augment`` (batch augmentation of the CIFAR transform done in the input relayout kernel, with the Resize of
 the Mix&Match ``sampled*`` regimes),
 ``--device-resized-crop`` (the ImageNet RandomResizedCrop + flip resampled in the input relayout kernel),
-``--device-scale-crop`` (the ImageNet evaluation Resize + CenterCrop resampled in the input relayout kernel), and
+``--device-scale-crop`` (the ImageNet evaluation Resize + CenterCrop resampled in the input relayout kernel),
+``--device-decode`` (baseline JPEGs decoded on the GPU ahead of either device crop), and
 rank/world are read from the torchrun environment when ``--local_rank`` is not given.
 """
 import argparse
@@ -83,6 +84,10 @@ def build_parser():
     a('--device-scale-crop', action='store_true', default=False,
       help='ImageNet validation: the loader workers only decode; the input relayout on the GPU resizes (Pillow-exact '
            'bilinear), centre-crops and normalises the images')
+    a('--device-decode', action='store_true', default=False,
+      help='ImageNet, with --device-resized-crop (training) and / or --device-scale-crop (validation): the loader '
+           'workers only read the files and parse their headers; baseline JPEGs are decoded on the GPU into the '
+           'regions the crops read, byte for byte what Pillow decodes (other files are decoded by the workers)')
     a('--autoaugment', action='store_true', default=False, help='autoaugment policies (ignored for synthetic data)')
     a('--grad-clip', default=-1, type=float, help='maximum grad norm value, -1 for none')
     a('--loss-scale', default=1, type=float, help='loss scale for mixed precision training')
@@ -164,6 +169,11 @@ def main_worker(args):
         args.device = 'cuda:%d' % args.device_ids[0]
     else:
         args.device_ids = None
+    if args.device_decode and not (args.device_resized_crop or args.device_scale_crop):
+        raise NotImplementedError('--device-decode decodes into the regions of --device-resized-crop or '
+                                  '--device-scale-crop; set one of them')
+    if args.device_decode and not on_cuda:
+        raise NotImplementedError('--device-decode decodes on the GPU: it needs a CUDA device')
     use_b200 = args.b200 == 'on' or (args.b200 == 'auto' and on_cuda)
     if use_b200 and not on_cuda:
         raise RuntimeError('--b200 on requires a CUDA device: the B200 kernel path has no CPU fallback')
@@ -245,7 +255,8 @@ def main_worker(args):
                                     'augment': False, 'input_size': args.input_size,
                                     'batch_size': args.eval_batch_size, 'shuffle': False,
                                     'num_workers': args.workers, 'pin_memory': True, 'drop_last': False,
-                                    'device_scale_crop': args.device_scale_crop})
+                                    'device_scale_crop': args.device_scale_crop,
+                                    'device_decode': args.device_decode and args.device_scale_crop})
     if args.evaluate:
         res = trainer.validate(val_data.get_loader())
         logging.info(res)
@@ -256,7 +267,8 @@ def main_worker(args):
                       'num_workers': args.workers, 'pin_memory': True, 'drop_last': True,
                       'distributed': args.distributed, 'duplicates': args.duplicates,
                       'autoaugment': args.autoaugment, 'cutout': {'holes': 1, 'length': 16} if args.cutout else None,
-                      'device_augment': args.device_augment, 'device_resized_crop': args.device_resized_crop}
+                      'device_augment': args.device_augment, 'device_resized_crop': args.device_resized_crop,
+                      'device_decode': args.device_decode and args.device_resized_crop}
     if hasattr(model, 'sampled_data_regime'):
         probs, configs = zip(*model.sampled_data_regime)
         train_data = SampledDataRegime([DataRegime(None, defaults={**train_defaults, **cfg}) for cfg in configs],

@@ -6,6 +6,7 @@ Every call is asynchronous on the current torch CUDA stream.
 """
 import ctypes
 
+import numpy as np
 import torch
 
 from . import lib as _l
@@ -714,6 +715,92 @@ def _window(out, window):
     if p < 0 or n < 1 or p + n > out.shape[0]:
         raise _l.B200Error('relayout window (%d, %d) outside its %d rows' % (p, n, out.shape[0]))
     return out[p:p + n]
+
+
+JPEG_STATUS = {1: 'bad Huffman code', 2: 'premature end of data', 4: 'wrong restart marker',
+               8: 'coefficient index past 63'}
+
+
+def check_jpeg_layout(layout, payload_bytes, out_bytes):
+    """Host-side validation of a JpegBatch layout (utils/augment.py JpegCollate) before b200_jpeg_decode trusts it:
+    every table, segment and region inside its buffer, the coefficient, plane and pixel prefixes consistent with the
+    images' sizes, every restart interval inside its image's segment.  Raises B200Error."""
+    from .utils import augment as A, jpeg as J
+    d, iv = layout['desc'], layout['intervals']
+    B = d.shape[0]
+    if d.ndim != 2 or d.shape[1] != A.DESC_WORDS or iv.ndim != 2 or iv.shape[1] != 3:
+        raise _l.B200Error('jpeg_decode: descriptor must be [B, %d] and intervals [n, 3]' % A.DESC_WORDS)
+    kind, rh, rw = d[:, A._D_KIND], d[:, A._D_RH], d[:, A._D_RW]
+    dev = kind != A.KIND_HOST
+    pix = rh * rw
+    bad = (kind < 0) | (kind > 2) | (rh < 1) | (rw < 1) | (d[:, A._D_OUT] < 0) | (d[:, A._D_OUT] + 3 * pix > out_bytes)
+    bad |= d[:, A._D_PIX] != np.concatenate([[0], np.cumsum(pix)[:-1]])
+    hmax, vmax = np.maximum(d[:, A._D_HMAX], 1), np.maximum(d[:, A._D_VMAX], 1)
+    H, W = d[:, A._D_H], d[:, A._D_W]
+    gray = kind == A.KIND_GRAY
+    samp_ok = np.where(gray, (hmax == 1) & (vmax == 1), ((hmax == 1) | (hmax == 2)) & ((vmax == 1) | (vmax == hmax)))
+    blocks = np.where(gray, 1, hmax * vmax + 2) * d[:, A._D_MCUX] * d[:, A._D_MCUY]
+    blocks = np.where(dev, blocks, 0)
+    bad |= d[:, A._D_COEF] != np.concatenate([[0], np.cumsum(blocks)[:-1]])
+    bad |= d[:, A._D_PLANE] != 64 * d[:, A._D_COEF]
+    bad |= ~dev & ((d[:, A._D_SRC] < 0) | (d[:, A._D_SRC] + 3 * pix > payload_bytes))
+    hsize = 4 * J.HUFF_WORDS
+    dv = (~samp_ok) | (H < 1) | (W < 1) | (H > 65535) | (W > 65535)
+    dv |= (d[:, A._D_MCUX] != -(-W // (8 * hmax))) | (d[:, A._D_MCUY] != -(-H // (8 * vmax)))
+    dv |= (d[:, A._D_MCUROWS] < 0) | (d[:, A._D_MCUROWS] > d[:, A._D_MCUY]) | (d[:, A._D_RI] < 0)
+    dv |= (d[:, A._D_ECS0] < 0) | (d[:, A._D_ECS0] > d[:, A._D_ECS1]) | (d[:, A._D_ECS1] > payload_bytes)
+    dv |= (d[:, A._D_Y0] < 0) | (d[:, A._D_X0] < 0) | (d[:, A._D_Y0] + rh > H) | (d[:, A._D_X0] + rw > W)
+    for c in range(3):
+        used = ~gray | (c == 0)
+        for w, size in ((A._D_Q + c, 256), (A._D_DC + c, hsize), (A._D_AC + c, hsize)):
+            dv |= used & ((d[:, w] < 0) | (d[:, w] % 16 != 0) | (d[:, w] + size > payload_bytes))
+    bad |= dev & dv
+    if bool(bad.any()) or int(blocks.sum()) != layout['coef_blocks'] or int(pix.sum()) != layout['pixels']:
+        raise _l.B200Error('jpeg_decode: the descriptor of image(s) %s does not describe the payload'
+                           % np.flatnonzero(bad).tolist())
+    if len(iv):
+        b = iv[:, 0]
+        if bool(((b < 0) | (b >= B)).any()):
+            raise _l.B200Error('jpeg_decode: a restart interval names no image')
+        e0, e1 = d[b, A._D_ECS0], d[b, A._D_ECS1]
+        if bool(((iv[:, 1] < 0) | (iv[:, 2] < e0) | (iv[:, 2] > e1) | (d[b, A._D_KIND] == A.KIND_HOST)).any()):
+            raise _l.B200Error('jpeg_decode: a restart interval lies outside its image\'s segment')
+    if layout['intervals_at'] + iv.nbytes > payload_bytes or d.nbytes > payload_bytes:
+        raise _l.B200Error('jpeg_decode: the payload is shorter than its tables')
+
+
+def jpeg_decode(payload, layout, out):
+    """Decode a JpegBatch payload (uint8, on the device) into the flat uint8 region buffer ``out``: each image's region
+    of its RGB decode as Pillow makes it, HWC at its index offset.  -> int32 [B] device status words (see
+    JPEG_STATUS; check_jpeg_status reads them)."""
+    _chk(payload, torch.uint8, "payload"); _chk(out, torch.uint8, "out")
+    check_jpeg_layout(layout, payload.numel(), out.numel())
+    B = layout['desc'].shape[0]
+    dev = payload.device
+    nb = int(layout['coef_blocks'])
+    coef = torch.empty((max(nb, 1), 64), dtype=torch.int16, device=dev)
+    planes = torch.empty(max(nb, 1) * 64, dtype=torch.uint8, device=dev)
+    status = torch.empty(B, dtype=torch.int32, device=dev)
+    base = payload.data_ptr()
+    n_iv = layout['intervals'].shape[0]
+    with _T('jpeg_decode', 0, payload.numel() + 130 * nb + 3 * int(layout['pixels'])):
+        _l.check(_l.load().b200_jpeg_decode(base, payload.numel(), base, B, base + layout['intervals_at'], n_iv,
+                                            coef.data_ptr(), nb, planes.data_ptr(), planes.numel(),
+                                            int(layout['pixels']), out.data_ptr(), out.numel(), status.data_ptr(),
+                                            _stream()),
+                 "b200_jpeg_decode")
+    return status
+
+
+def check_jpeg_status(status):
+    """Raise B200Error naming every image of the batch (by its position) whose decode failed: ``status`` the host
+    copy of jpeg_decode's status words."""
+    st = status.cpu().numpy() if torch.is_tensor(status) else np.asarray(status)
+    failed = np.flatnonzero(st)
+    if failed.size:
+        raise _l.B200Error('jpeg_decode: sample(s) %s of the batch failed to decode (%s)' % (
+            failed.tolist(), '; '.join('%d: %s' % (i, ', '.join(v for k, v in JPEG_STATUS.items() if st[i] & k))
+                                       for i in failed[:8])))
 
 
 class ScaleCropTables(object):

@@ -41,7 +41,7 @@ from torch.nn.utils import clip_grad_norm_
 
 from .lib import B200Error, MIX_CUTMIX, MIX_MIXUP
 from .utils import regularization
-from .utils.augment import DeviceBatch, ResizedCropBatch, ScaleCropBatch
+from .utils.augment import DeviceBatch, JpegBatch, ResizedCropBatch, ScaleCropBatch
 from .utils.meters import AverageMeter, accuracy
 from .utils.mixup import CutMix, MixUp
 
@@ -89,7 +89,12 @@ def _cuda_prefetch(loader, device, dtype):
     step (a fresh 154 MB tensor per batch that is handed across streams made the allocator stall now and then).
     A DeviceBatch's tensors travel together, in the same slot.  The region buffer of a ResizedCropBatch or ScaleCropBatch
     changes size every step: its slots are keyed on a capacity instead, which grows by at least half when a batch does
-    not fit."""
+    not fit.
+    A JpegBatch (data.py ``device_decode``) is decoded right after its copies, on the copy stream, into a region buffer
+    of its slot, so the decode overlaps the previous step; the consumer receives the ResizedCropBatch / ScaleCropBatch
+    of that buffer once the decode's status words say every image decoded (B200Error otherwise: no step trains on a
+    failed decode, where the reference would train on libjpeg's recovered pixels)."""
+    from . import ops
     copy_stream = torch.cuda.Stream(device=device)
     ring = {}          # shapes and dtypes -> [[x_buf, y_buf, consumed_event or None, (other device tensors)], ...]
     turn = {}
@@ -100,7 +105,7 @@ def _cuda_prefetch(loader, device, dtype):
         host = batch.tensors if batch is not None else (inputs,)
         x, rest = host[0], host[1:]
         x_dtype = x.dtype if x.dtype == torch.uint8 else dtype     # uint8 image batches stay uint8
-        ragged = isinstance(batch, (ResizedCropBatch, ScaleCropBatch))
+        ragged = isinstance(batch, (ResizedCropBatch, ScaleCropBatch, JpegBatch))
         key = (type(batch), None if ragged else tuple(x.shape), x_dtype, tuple(target.shape), target.dtype,
                tuple((tuple(t.shape), t.dtype) for t in rest))
         shape = tuple(x.shape)
@@ -130,12 +135,28 @@ def _cuda_prefetch(loader, device, dtype):
             slot[1].copy_(target, non_blocking=True)
             for d, t in zip(slot[3], rest):
                 d.copy_(t, non_blocking=True)
+            decoded = None
+            if isinstance(batch, JpegBatch):
+                if len(slot) < 5 or slot[4].numel() < batch.nbytes:
+                    if len(slot) >= 5 and slot[2] is not None:
+                        slot[2].synchronize()             # the step that read the old region buffer has run
+                    buf = torch.empty(-(-max(batch.nbytes, 1) * 3 // 2 // (1 << 20)) * (1 << 20), device=device,
+                                      dtype=torch.uint8)
+                    slot[4:] = [buf]
+                decoded, status = batch.replace((slot[0],) + slot[3]).decode(slot[4])
+                status_host = torch.empty(status.shape, dtype=status.dtype, pin_memory=True)
+                status_host.copy_(status, non_blocking=True)
+                decoded = (decoded, status_host)
             ready = torch.cuda.Event()
             ready.record(copy_stream)
-        return slot, ready, batch
+        return slot, ready, batch, decoded
 
-    def hand_over(slot, ready, batch):
+    def hand_over(slot, ready, batch, decoded):
         torch.cuda.current_stream(device).wait_event(ready)
+        if decoded is not None:
+            ready.synchronize()                            # the decode and its status copy, not the running step
+            ops.check_jpeg_status(decoded[1])
+            return decoded[0], slot[1]
         return (slot[0] if batch is None else batch.replace((slot[0],) + slot[3])), slot[1]
 
     def release(slot):
@@ -443,6 +464,8 @@ class Trainer(object):
         tensor {loss, top-1 %, top-5 %} of the loss kernel, which Trainer.forward reads back asynchronously
         (the reference synchronises three times per step here: trainer.py:153,226-227)."""
         grad = None
+        if isinstance(inputs_batch, JpegBatch) and self.b200 is not None and 'cuda' in str(self.device):
+            inputs_batch = self._decode(inputs_batch)
         if training:
             self.optimizer.zero_grad()
             self.optimizer.update(self.epoch, self.training_steps)
@@ -664,6 +687,15 @@ class Trainer(object):
         return ops.Mix(dev[:B], dev[B:].view(torch.int32), kind)
 
     # ------------------------------------------------------------------ batch augmentation on the device
+    def _decode(self, batch):
+        """A JpegBatch that did not come through the prefetch ring: copied and decoded on the current stream (the one
+        decode path, JpegBatch.decode), its status checked -> the ResizedCropBatch / ScaleCropBatch it stands for."""
+        from . import ops
+        device = torch.device(self.device)
+        decoded, status = batch.replace(tuple(t.to(device, non_blocking=True) for t in batch.tensors)).decode()
+        ops.check_jpeg_status(status.cpu())
+        return decoded
+
     def _device_aug(self, batch):
         """-> (ops.Aug, ops.Rrc or ops.ScaleCropTables over the batch's tables on the device and a persistent device LUT
         of its normalisation -- one per statistics, channel count and device, so that a captured graph keeps reading a

@@ -258,11 +258,16 @@ class ResizedCrop(object):
             out[d] = torch.tensor([i, j, h, w, int(torch.rand(1) < 0.5)], dtype=torch.int32)
         return out
 
+    @staticmethod
+    def region(draws):
+        """(y0, x0, y1, x1): the bounding box of the crop boxes ``draws``."""
+        return int(draws[:, 0].min()), int(draws[:, 1].min()), int((draws[:, 0] + draws[:, 2]).max()), \
+            int((draws[:, 1] + draws[:, 3]).max())
+
     def __call__(self, img):
         """PIL image -> (uint8 HWC region, int32 [D, 5] draws relative to the region): the loader's per-image work."""
         draws = self.draw(img)
-        y0, x0 = int(draws[:, 0].min()), int(draws[:, 1].min())
-        y1, x1 = int((draws[:, 0] + draws[:, 2]).max()), int((draws[:, 1] + draws[:, 3]).max())
+        y0, x0, y1, x1 = self.region(draws)
         a = np.asarray(img)
         region = torch.from_numpy(np.array(a[y0:y1, x0:x1].reshape(y1 - y0, x1 - x0, -1), copy=True))
         draws[:, 0] -= y0
@@ -495,3 +500,205 @@ class ScaleCropCollate(object):
         target = torch.as_tensor([int(t) for _, t in batch], dtype=torch.long)
         flat = torch.cat([r.reshape(-1) for r in regions])
         return ScaleCropBatch(flat, index, geom, self.spec, regions[0].shape[2]), target
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# JPEG decode on the device (transform key ``device_decode``, with ``device_resized_crop`` or ``device_scale_crop``).
+# The workers read the file bytes and parse the headers (utils/jpeg.py); each image's crop or support region is drawn
+# from the header's size, and csrc/jpeg.cu decodes just the entropy-coded data the region needs into the region buffer
+# the relayouts read.  Files outside the device's baseline subset are decoded by PIL in the worker and ride in the same
+# batch.
+
+_D_KIND, _D_H, _D_W, _D_HMAX, _D_VMAX, _D_MCUX, _D_MCUY, _D_MCUROWS, _D_RI, _D_ECS0, _D_ECS1 = range(11)
+_D_Q, _D_DC, _D_AC = 11, 14, 17
+_D_COEF, _D_PLANE, _D_Y0, _D_X0, _D_RH, _D_RW, _D_OUT, _D_SRC, _D_PIX = range(20, 29)
+DESC_WORDS = 32
+KIND_COLOR, KIND_GRAY, KIND_HOST = 0, 1, 2
+
+
+def _image_size(h, w):
+    """A stand-in with an h x w image's size for the torchvision draws (they read nothing but the size)."""
+    return torch.empty((1, 1, 1), dtype=torch.uint8).expand(3, h, w)
+
+
+class JpegDecode(object):
+    """Worker-side transform of ``device_decode``: file bytes -> (JpegInfo of a device-class file or None, (y0, x0, h, w)
+    region box, draws or geometry relative to the region, the bytes, the uint8 HWC region decoded by PIL for the other
+    files or None).  ``spec`` (a ResizedCrop or a ScaleCrop) draws with the calls and order of its PIL path from the
+    header's size, so the random stream and the draws are unchanged."""
+
+    def __init__(self, spec):
+        self.spec = spec
+
+    def __call__(self, data):
+        import io
+        from . import jpeg
+        data = bytes(data)
+        info = jpeg.parse(data)
+        img = None
+        if info.device:
+            h, w = info.height, info.width
+        else:
+            from PIL import Image
+            img = Image.open(io.BytesIO(data)).convert('RGB')
+            w, h = img.size
+        if isinstance(self.spec, ResizedCrop):
+            table = self.spec.draw(img if img is not None else _image_size(h, w))
+            y0, x0, y1, x1 = self.spec.region(table)
+            table[:, 0] -= y0
+            table[:, 1] -= x0
+            box = (y0, x0, y1 - y0, x1 - x0)
+        else:
+            table, (rh, rw) = self.spec.geometry(h, w)
+            box = (int(table[0]), int(table[1]), rh, rw)
+        region = None
+        if img is not None:
+            y0, x0, rh, rw = box
+            region = np.ascontiguousarray(np.asarray(img)[y0:y0 + rh, x0:x0 + rw])
+        return (info if info.device else None), box, table, data, region
+
+
+def _mcu_rows_needed(info, y1):
+    """MCU rows the decode of image rows [0, y1) needs, the upsampling context row below included."""
+    hmax, vmax = info.sampling
+    mcuy = info.mcus[1]
+    rows = (y1 - 1) // (8 * vmax) + 1
+    if vmax > 1:
+        ch = -(-info.height // vmax)
+        rows = max(rows, min((y1 - 1) // vmax + 1, ch - 1) // 8 + 1)
+    return min(rows, mcuy)
+
+
+class JpegCollate(object):
+    """DataLoader ``collate_fn`` of a ``device_decode`` loader: packs the JpegDecode samples into one JpegBatch.
+    -> (batch, target repeated to the batch's rows)."""
+
+    def __init__(self, spec):
+        self.spec = spec
+
+    def __call__(self, batch):
+        from . import jpeg
+        samples = [s for s, _ in batch]
+        target = torch.as_tensor([int(t) for _, t in batch], dtype=torch.long)
+        B = len(samples)
+        chunks, pos, cache = [], [0], {}
+
+        def put(a, key=None):
+            if key is not None and key in cache:
+                return cache[key]
+            a = np.ascontiguousarray(a).view(np.uint8).reshape(-1)
+            off = pos[0]
+            chunks.append(a)
+            pad = -a.size % 16
+            if pad:
+                chunks.append(np.zeros(pad, np.uint8))
+            pos[0] += a.size + pad
+            if key is not None:
+                cache[key] = off
+            return off
+
+        desc = np.zeros((B, DESC_WORDS), np.int64)
+        put(desc)                                          # the descriptor heads the payload (filled in below)
+        sizes = [3 * s[1][2] * s[1][3] for s in samples]
+        offsets = np.concatenate([[0], np.cumsum(sizes)[:-1]]).astype(np.int64)
+        intervals, coef, pix = [], 0, 0
+        for b, (info, (y0, x0, rh, rw), _, data, region) in enumerate(samples):
+            d = desc[b]
+            d[_D_Y0], d[_D_X0], d[_D_RH], d[_D_RW] = y0, x0, rh, rw
+            d[_D_OUT], d[_D_PIX], d[_D_COEF], d[_D_PLANE] = offsets[b], pix, coef, coef * 64
+            pix += rh * rw
+            if info is None:
+                d[_D_KIND] = KIND_HOST
+                d[_D_SRC] = put(region)
+                continue
+            hmax, vmax = info.sampling
+            mcux, mcuy = info.mcus
+            d[_D_KIND] = KIND_COLOR if info.channels == 3 else KIND_GRAY
+            d[_D_H], d[_D_W], d[_D_HMAX], d[_D_VMAX], d[_D_MCUX], d[_D_MCUY] = \
+                info.height, info.width, hmax, vmax, mcux, mcuy
+            d[_D_MCUROWS] = _mcu_rows_needed(info, y0 + rh)
+            d[_D_RI] = info.restart
+            e0, e1 = info.ecs
+            d[_D_ECS0] = put(np.frombuffer(data, np.uint8, count=e1 - e0, offset=e0))
+            d[_D_ECS1] = d[_D_ECS0] + e1 - e0
+            for c, (ci, td, ta) in enumerate(info.scan):
+                q = info.qt[info.comps[ci][3]]
+                d[_D_Q + c] = put(q, ('q', q.tobytes()))
+                for w, t in ((_D_DC + c, info.dc[td]), (_D_AC + c, info.ac[ta])):
+                    packed = t.pack()
+                    d[w] = put(packed, ('h', packed.tobytes()))
+            coef += mcux * mcuy * (hmax * vmax + 2 if info.channels == 3 else 1)
+            ri = info.restart or mcux * mcuy
+            n = -(-int(d[_D_MCUROWS]) * mcux // ri)
+            starts = np.full(n, d[_D_ECS1], np.int64)
+            starts[0] = d[_D_ECS0]
+            rst = info.rst[:n - 1] - e0 + d[_D_ECS0]
+            starts[1:1 + rst.size] = rst
+            intervals.append(np.stack([np.full(n, b), np.arange(n), starts], 1))
+        intervals = np.concatenate(intervals).astype(np.int64) if intervals else np.zeros((0, 3), np.int64)
+        iv_off = put(intervals) if len(intervals) else pos[0]
+        chunks[0][:] = desc.view(np.uint8).reshape(-1)
+        payload = torch.from_numpy(np.concatenate(chunks))
+        index = torch.tensor([[o, s[1][2], s[1][3]] for o, s in zip(offsets, samples)], dtype=torch.int64)
+        if isinstance(self.spec, ResizedCrop):
+            table, reps = torch.cat([s[2] for s in samples]), self.spec.duplicates
+        else:
+            table, reps = torch.stack([s[2] for s in samples]), 1
+        layout = {'desc': desc, 'intervals': intervals, 'intervals_at': iv_off, 'coef_blocks': coef, 'pixels': pix}
+        return JpegBatch(payload, index, table, self.spec, layout, [s[3] for s in samples]), \
+            target.repeat_interleave(reps)
+
+
+class JpegBatch(DeviceBatch):
+    """B JPEG files packed for the device decode: ``payload`` uint8 (descriptor int64 [B, 32] at byte 0, then the
+    entropy-coded segments, tables, host-decoded regions and the restart-interval table), ``index`` int64 [B, 3]
+    {byte offset, h, w} of each region in the region buffer, ``table`` the draws (ResizedCrop) or geometry (ScaleCrop)
+    as in ResizedCropBatch / ScaleCropBatch, ``layout`` the host copies and sizes of the payload's tables, ``files`` the
+    file bytes (for apply()).  ``decode()`` yields the ResizedCropBatch / ScaleCropBatch the relayout reads."""
+    __slots__ = ('payload', 'index', 'table', 'spec', 'layout', 'files', 'host')
+
+    def __init__(self, payload, index, table, spec, layout, files, host=None):
+        self.payload, self.index, self.table, self.spec = payload, index, table, spec
+        self.layout, self.files = layout, files
+        self.host = host if host is not None else (index, table)
+
+    @property
+    def rows(self):
+        return self.table.shape[0] if isinstance(self.spec, ResizedCrop) else self.index.shape[0]
+
+    @property
+    def nbytes(self):
+        return int(self.layout['pixels']) * 3
+
+    @property
+    def tensors(self):
+        return (self.payload, self.index, self.table)
+
+    def replace(self, tensors):
+        return JpegBatch(tensors[0], tensors[1], tensors[2], self.spec, self.layout, self.files, self.host)
+
+    def decode(self, out=None):
+        """-> (ResizedCropBatch or ScaleCropBatch over ``out`` (a new device buffer when None), int32 [B] device status
+        words, 0 for every image decoded): the decode is enqueued on the current stream of the payload's device."""
+        from .. import ops
+        if out is None:
+            out = torch.empty(max(self.nbytes, 1), dtype=torch.uint8, device=self.payload.device)
+        status = ops.jpeg_decode(self.payload, self.layout, out)
+        cls = ResizedCropBatch if isinstance(self.spec, ResizedCrop) else ScaleCropBatch
+        return cls(out, self.index, self.table, self.spec, 3, self.nbytes, self.host), status
+
+    def regions(self):
+        """uint8 flat region buffer decoded by PIL: each image's np.asarray(Image.open(f).convert('RGB'))[region]."""
+        import io
+        from PIL import Image
+        desc = self.layout['desc']
+        out = []
+        for f, d in zip(self.files, desc):
+            y0, x0, rh, rw = (int(v) for v in d[_D_Y0:_D_RW + 1])
+            a = np.asarray(Image.open(io.BytesIO(f)).convert('RGB'))
+            out.append(np.ascontiguousarray(a[y0:y0 + rh, x0:x0 + rw]).reshape(-1))
+        return torch.from_numpy(np.concatenate(out))
+
+    def apply(self):
+        """-> fp32 NCHW rows on the host: the regions decoded by PIL through the spec's own apply()."""
+        return self.spec.apply(self.regions(), self.host[0], self.host[1], 3)

@@ -5,7 +5,7 @@
  * The reference has no FFI of its own (it is pure Python on top of torch.nn); every entry point
  * below replaces one implicit torch/cuDNN/ATen operator the reference invokes, cited per function
  * as reference file:line (paths under the reference tree).  INTEGRATION.md shows the ctypes stubs.
- * 53 entry points.
+ * 54 entry points.
  *
  * Conventions
  *  - every function returns 0 on success or a negative B200_ERR_* code; b200_last_error() gives text.
@@ -274,6 +274,21 @@ int b200_input_prep_u8_rrc(const uint8_t* regions, long long region_bytes, const
 int b200_input_prep_u8_scale_crop(const uint8_t* regions, long long region_bytes, const long long* index,
                                   const int* geom, int B, int C, int OH, int OW, int Cpad, int mode, const float* lut,
                                   void* out, b200_stream_t stream);
+/* Baseline JPEG decode into the region buffer of b200_input_prep_u8_rrc / b200_input_prep_u8_scale_crop (csrc/jpeg.cu,
+ * tests/jpeg_oracle.py): out receives, for each of the B images, its region (desc words y0, x0, rh, rw) of the RGB
+ * image np.asarray(Image.open(f).convert('RGB')) as Pillow (libjpeg-turbo: ISLOW IDCT, fancy upsampling) decodes it,
+ * uint8 HWC at byte offset desc[b][26].  payload (DEVICE, 16-byte aligned): the entropy-coded segments, packed Huffman
+ * and quantisation tables and the regions the loader decoded on the host, at the offsets of desc (DEVICE int64
+ * [B][32], utils/augment.py JpegCollate); intervals (DEVICE int64 [n_intervals][3]) = {image, interval, first byte}
+ * of each restart interval.  coef (int16 [coef_blocks][64]) and planes (plane_bytes >= 64 * coef_blocks) are
+ * workspaces.  status (DEVICE int32 [B]) is reset, then ORs 1 (bad Huffman code), 2 (premature end of data),
+ * 4 (wrong restart marker) or 8 (coefficient index past 63) per image; such an image's pixels are unspecified.  Reads
+ * of the entropy-coded data stay inside each image's segment; the descriptor's other offsets are trusted (ops.py
+ * jpeg_decode validates them on the host). */
+int b200_jpeg_decode(const uint8_t* payload, long long payload_bytes, const long long* desc, int B,
+                     const long long* intervals, int n_intervals, int16_t* coef, long long coef_blocks, uint8_t* planes,
+                     long long plane_bytes, long long pixels, uint8_t* out, long long out_bytes, int* status,
+                     b200_stream_t stream);
 /* bf16 [K][T][C] -> bf16 [C][T][K] (dgrad weight layout), multi-tensor: n tensors described by
  * device arrays. */
 int b200_weight_transpose(const void* src, void* dst, int K, int T, int C, b200_stream_t stream);

@@ -2,7 +2,9 @@
 Trainer.train with captured graphs, on a temporary ImageFolder of seeded synthetic JPEGs of ImageNet-like sizes
 (about 500x375, varied; written before any timing).
 
-Three data paths, alternated round by round on the same model and Trainer, so drift of the card affects all alike:
+Four data paths, alternated round by round on the same model and Trainer, so drift of the card affects all alike:
+  decode  -- --device-resized-crop --device-decode: the workers read the files, parse headers and draw; the loader
+             yields JpegBatch and csrc/jpeg.cu decodes the crops' regions on the copy stream ahead of the relayout;
   device  -- --device-resized-crop: --workers DataLoader workers decode and draw only; the loader yields
              ResizedCropBatch (the crops' regions + draws) and the relayout kernel resamples, flips and normalises;
   host    -- today's host transform (real_dataset_transform('imagenet'): RandomResizedCrop, flip, ToTensor,
@@ -11,7 +13,9 @@ Three data paths, alternated round by round on the same model and Trainer, so dr
 Each round of a path runs --warmup + --steps steps from one persistent loader iterator; only the last --steps are
 timed (device synchronise to device synchronise).  Round 0 of every path is warm-up.  Also reports the relayout
 kernel's time and bytes/s (CUDA events over --kernel-iters launches on a loader batch), the host-to-device bytes per
-step of each path, and the cost of the region copy from pageable memory against staging it through a pinned buffer.
+step of each path, and the cost of the region copy from pageable memory against staging it through a pinned buffer,
+the decode kernels' times (torch.profiler over a loader batch, a run of its own after the timed rounds) and the host
+CPU time per image of the workers' per-image work and collate, with and without the device decode.
 Prints one JSON line (also written to --out) with the card's name and power limit and the host's CPU count.
 
     python tools/resized_crop_bench.py [--rounds 3] [--steps 20] [--warmup 4] [--workers N] [--out FILE]
@@ -107,6 +111,44 @@ def copy_costs(batch, iters=10):
     return res
 
 
+def decode_kernels(batch, iters=5):
+    """ms per batch of each decode kernel: torch.profiler with CUDA activities over ``iters`` decodes of a JpegBatch."""
+    from torch.profiler import ProfilerActivity, profile
+    dev = batch.replace(tuple(t.cuda() for t in batch.tensors))
+    dev.decode()
+    torch.cuda.synchronize()
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        for _ in range(iters):
+            dev.decode()
+        torch.cuda.synchronize()
+    out = {}
+    for e in prof.key_averages():
+        for k in ('jpeg_huffman_kernel', 'jpeg_idct_kernel', 'jpeg_color_kernel'):
+            if k in e.key:
+                t = getattr(e, 'device_time_total', None) or getattr(e, 'cuda_time_total', 0)
+                out[k] = round(t / 1e3 / iters, 3)
+    out['total'] = round(sum(out.values()), 3)
+    return out
+
+
+def worker_cpu_ms(root, spec, n=128):
+    """Host CPU ms per image of the workers' work (per-image transform, then collate of the batch): the PIL decode
+    path of the device crop against the header-only path of device_decode."""
+    import glob
+    from PIL import Image
+    from convnet.pytorch_b200.utils.augment import JpegCollate, JpegDecode, ResizedCropCollate, ScaleCropCollate
+    files = sorted(glob.glob(os.path.join(root, '**', '*.jpg'), recursive=True))[:n]
+    datas = [open(f, 'rb').read() for f in files]
+    host_collate = ResizedCropCollate(spec) if hasattr(spec, 'draw') else ScaleCropCollate(spec)
+    res = {}
+    for name, fn, collate in (('pil_decode', lambda d: spec(Image.open(__import__('io').BytesIO(d)).convert('RGB')),
+                               host_collate), ('device_decode', JpegDecode(spec), JpegCollate(spec))):
+        t0 = time.process_time()
+        collate([(fn(d), 0) for d in datas])
+        res[name] = round(1e3 * (time.process_time() - t0) / len(datas), 3)
+    return res
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--rounds', type=int, default=3)
@@ -139,10 +181,13 @@ def main():
     device_it = iter(DataRegime(None, defaults=dict(base, device_resized_crop=True, pin_memory=False)).get_loader())
     # the host path does not pin either: a pin-memory thread may not allocate while the Trainer captures a graph
     host_it = iter(DataRegime(None, defaults=dict(base, pin_memory=False)).get_loader())
+    decode_it = iter(DataRegime(None, defaults=dict(base, device_resized_crop=True, device_decode=True,
+                                                    pin_memory=False)).get_loader())
+    jpeg_batch, _ = next(decode_it)
     sample, _ = next(device_it)
     bound = [(sample.apply().cuda(), torch.randint(0, CLASSES, (B,)).cuda()) for _ in range(2)]
     bound_it = itertools.cycle(bound)
-    paths = (('bound', bound_it), ('device', device_it), ('host', host_it))
+    paths = (('bound', bound_it), ('decode', decode_it), ('device', device_it), ('host', host_it))
     times = {k: [] for k, _ in paths}
     data_wait = {k: [] for k, _ in paths}
     for r in range(args.rounds + 1):
@@ -153,6 +198,8 @@ def main():
                 data_wait[name].append(1e3 * data)
     kern = kernel_time(sample, args.kernel_iters)
     copies = copy_costs(sample)
+    dec = decode_kernels(jpeg_batch)
+    cpu = worker_cpu_ms(os.path.join(tmp, 'imagenet'), sample.spec)
     gpu, power = card()
     med = {k: statistics.median(v) for k, v in times.items()}
     res = {'model': 'resnet50', 'batch': B, 'size': SIZE, 'images': IMAGES, 'jpeg_setup_s': round(setup_s, 1),
@@ -162,7 +209,10 @@ def main():
            'img_per_s': {k: round(B / (v / 1e3), 1) for k, v in med.items()},
            'data_wait_ms_mean': {k: round(statistics.mean(v), 3) for k, v in data_wait.items()},
            'h2d_bytes_per_step': {'device': sample.nbytes + 8 * sample.index.numel() + 4 * sample.draws.numel() + 8 * B,
-                                  'host': 4 * B * 3 * SIZE * SIZE + 8 * B, 'bound': 0},
+                                  'host': 4 * B * 3 * SIZE * SIZE + 8 * B, 'bound': 0,
+                                  'decode': jpeg_batch.payload.numel() + 8 * jpeg_batch.index.numel()
+                                  + 4 * jpeg_batch.table.numel() + 8 * B},
+           'decode_kernels_ms': dec, 'worker_cpu_ms_per_image': cpu,
            'relayout_kernel': kern, 'relayout_share_of_device_step': round(kern['ms'] / med['device'], 5),
            'region_copy_host_ms': copies, 'graph_replays': tr.graph_replays, 'gpu': gpu, 'power_limit': power,
            'host_cpus': os.cpu_count()}

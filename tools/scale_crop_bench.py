@@ -2,7 +2,9 @@
 from scale 256, through Trainer.validate, on a temporary ImageFolder of seeded synthetic JPEGs of ImageNet-like sizes
 (about 500x375, varied; written before any timing).
 
-Three data paths, alternated round by round on the same model and Trainer, so drift of the card affects all alike:
+Four data paths, alternated round by round on the same model and Trainer, so drift of the card affects all alike:
+  decode  -- --device-scale-crop --device-decode: the workers read the files and parse headers only; the loader yields
+             JpegBatch and csrc/jpeg.cu decodes the support regions on the copy stream ahead of the relayout;
   device  -- --device-scale-crop: --workers DataLoader workers decode and cut each image's support region only; the
              loader yields ScaleCropBatch and the relayout kernel resizes, centre-crops and normalises;
   host    -- the host transform (real_dataset_transform('imagenet', augment=False): Resize, CenterCrop, ToTensor,
@@ -11,7 +13,8 @@ Three data paths, alternated round by round on the same model and Trainer, so dr
 Each round of a path runs --warmup + --steps steps from one persistent loader iterator; only the last --steps are
 timed (device synchronise to device synchronise).  Round 0 of every path is warm-up.  Also reports the host-to-device
 bytes per batch of each path and the relayout kernel's time from a torch.profiler trace of --kernel-iters launches on a
-loader batch, with the bytes it moves.  Prints one JSON line (also written to --out) with the card's name and power
+loader batch, with the bytes it moves, the decode kernels' times (torch.profiler, a run of its own) and the host CPU
+time per image of the workers' work with and without the device decode.  Prints one JSON line (also written to --out) with the card's name and power
 limit and the host's CPU count.
 
     python tools/scale_crop_bench.py [--rounds 3] [--steps 20] [--warmup 4] [--workers 16] [--out FILE]
@@ -121,10 +124,12 @@ def main():
             'drop_last': True, 'pin_memory': False}
     device_it = iter(DataRegime(None, defaults=dict(base, device_scale_crop=True)).get_loader())
     host_it = iter(DataRegime(None, defaults=base).get_loader())
+    decode_it = iter(DataRegime(None, defaults=dict(base, device_scale_crop=True, device_decode=True)).get_loader())
+    jpeg_batch, _ = next(decode_it)
     sample, _ = next(device_it)
     bound = [(sample.apply().cuda(), torch.randint(0, CLASSES, (B,)).cuda()) for _ in range(2)]
     bound_it = itertools.cycle(bound)
-    paths = (('bound', bound_it), ('device', device_it), ('host', host_it))
+    paths = (('bound', bound_it), ('decode', decode_it), ('device', device_it), ('host', host_it))
     times = {k: [] for k, _ in paths}
     data_wait = {k: [] for k, _ in paths}
     for r in range(args.rounds + 1):
@@ -134,6 +139,9 @@ def main():
                 times[name].append(ms)
                 data_wait[name].append(1e3 * data)
     kern = kernel_time(sample, args.kernel_iters)
+    from resized_crop_bench import decode_kernels, worker_cpu_ms
+    dec = decode_kernels(jpeg_batch)
+    cpu = worker_cpu_ms(os.path.join(tmp, 'imagenet'), sample.spec)
     gpu, power = card()
     med = {k: statistics.median(v) for k, v in times.items()}
     res = {'model': 'resnet50-eval-folded', 'batch': B, 'size': SIZE, 'scale': SCALE, 'images': IMAGES,
@@ -146,7 +154,10 @@ def main():
                                for k, v in times.items()},
            'data_wait_ms_mean': {k: round(statistics.mean(v), 3) for k, v in data_wait.items()},
            'h2d_bytes_per_batch': {'device': sample.nbytes + 8 * sample.index.numel() + 4 * sample.geom.numel() + 8 * B,
-                                   'host': 4 * B * 3 * SIZE * SIZE + 8 * B, 'bound': 0},
+                                   'host': 4 * B * 3 * SIZE * SIZE + 8 * B, 'bound': 0,
+                                   'decode': jpeg_batch.payload.numel() + 8 * jpeg_batch.index.numel()
+                                   + 4 * jpeg_batch.table.numel() + 8 * B},
+           'decode_kernels_ms': dec, 'worker_cpu_ms_per_image': cpu,
            'relayout_kernel': kern, 'relayout_share_of_device_batch': round(kern['ms'] / med['device'], 5),
            'gpu': gpu, 'power_limit': power, 'host_cpus': os.cpu_count()}
     line = json.dumps(res)
