@@ -1,11 +1,12 @@
 // Baseline JPEG decode on the device (b200_jpeg_decode): the loader workers parse headers (utils/jpeg.py) and ship the
 // entropy-coded segments; three kernels turn them into the uint8 HWC regions the resized-crop and scale-crop relayouts
-// read, byte for byte what Pillow (libjpeg-turbo, ISLOW IDCT, fancy upsampling) decodes.  tests/jpeg_oracle.py is the
-// numpy statement of the same arithmetic.
+// read, byte for byte what Pillow (libjpeg-turbo on x86-64, SIMD ISLOW IDCT, fancy upsampling) decodes.
+// tests/jpeg_oracle.py is the numpy statement of the same arithmetic.
 //   1. jpeg_huffman_kernel: one thread per restart interval (the whole image without restart markers) decodes Huffman
 //      codes into int16 coefficient blocks (natural order), up to the last MCU row the region needs;
 //   2. jpeg_idct_kernel: one thread per 8x8 block the region's pixels (and their upsampling context) depend on runs
-//      libjpeg's jpeg_idct_islow with its range-limit table into block-padded uint8 component planes;
+//      the ISLOW IDCT as libjpeg-turbo's x86-64 SIMD code computes it (16-bit dequantisation and sums, saturating
+//      stores; its C jpeg_idct_islow differs on out-of-range blocks) into block-padded uint8 component planes;
 //   3. jpeg_color_kernel: one thread per region pixel upsamples the chroma (h2v1 / h2v2 fancy, box when the chroma is
 //      at most 2 samples wide), converts YCbCr -> RGB in libjpeg's fixed point and writes HWC RGB; grayscale images are
 //      replicated to RGB, and images the workers decoded with PIL are copied from the payload.
@@ -196,37 +197,30 @@ __device__ __forceinline__ void comp_span(long long a, long long n, int f, int f
   }
 }
 
-constexpr long long F0298 = 2446, F0390 = 3196, F0541 = 4433, F0765 = 6270, F0899 = 7373, F1175 = 9633,
-                    F1501 = 12299, F1847 = 15137, F1961 = 16069, F2053 = 16819, F2562 = 20995, F3072 = 25172;
+constexpr int F0298 = 2446, F0390 = 3196, F0541 = 4433, F0765 = 6270, F0899 = 7373, F1175 = 9633, F1501 = 12299,
+              F1847 = 15137, F1961 = 16069, F2053 = 16819, F2562 = 20995, F3072 = 25172;
 
-// one pass of jidctint.c's jpeg_idct_islow over x[0..7] (stride s), DESCALEd by n into o[0..7]
-template <typename In, typename Out>
-__device__ __forceinline__ void idct8(const In* x, int s, Out* o, int os, int n) {
-  const long long x0 = x[0], x1 = x[s], x2 = x[2 * s], x3 = x[3 * s], x4 = x[4 * s], x5 = x[5 * s], x6 = x[6 * s],
-                  x7 = x[7 * s];
-  long long z1 = (x2 + x6) * F0541;
-  const long long tmp2 = z1 + x6 * -F1847, tmp3 = z1 + x2 * F0765;
-  const long long tmp0 = (x0 + x4) * 8192, tmp1 = (x0 - x4) * 8192;
-  const long long tmp10 = tmp0 + tmp3, tmp13 = tmp0 - tmp3, tmp11 = tmp1 + tmp2, tmp12 = tmp1 - tmp2;
-  long long t0 = x7, t1 = x5, t2 = x3, t3 = x1;
-  z1 = t0 + t3;
-  long long z2 = t1 + t2, z3 = t0 + t2, z4 = t1 + t3;
-  const long long z5 = (z3 + z4) * F1175;
-  t0 *= F0298; t1 *= F2053; t2 *= F3072; t3 *= F1501;
-  z1 *= -F0899; z2 *= -F2562;
-  z3 = z3 * -F1961 + z5; z4 = z4 * -F0390 + z5;
-  t0 += z1 + z3; t1 += z2 + z4; t2 += z2 + z3; t3 += z1 + z4;
-  const long long r = 1LL << (n - 1);
-  o[0] = (Out)((tmp10 + t3 + r) >> n); o[7 * os] = (Out)((tmp10 - t3 + r) >> n);
-  o[os] = (Out)((tmp11 + t2 + r) >> n); o[6 * os] = (Out)((tmp11 - t2 + r) >> n);
-  o[2 * os] = (Out)((tmp12 + t1 + r) >> n); o[5 * os] = (Out)((tmp12 - t1 + r) >> n);
-  o[3 * os] = (Out)((tmp13 + t0 + r) >> n); o[4 * os] = (Out)((tmp13 - t0 + r) >> n);
-}
+__device__ __forceinline__ int s16(int x) { return (short)x; }        // paddw / pmullw: keep the low 16 bits
+__device__ __forceinline__ short sat16(int x) { return (short)(x < -32768 ? -32768 : (x > 32767 ? 32767 : x)); }
 
-// libjpeg's IDCT range-limit table at (x & 1023)
-__device__ __forceinline__ uint8_t range_limit(long long x) {
-  const int k = (int)(x & 1023);
-  return (uint8_t)(k < 128 ? k + 128 : (k < 512 ? 255 : (k < 896 ? 0 : k - 896)));
+// one pass of libjpeg-turbo's SIMD ISLOW IDCT (jidctint-sse2 / -avx2) over x[0..7] (stride s), DESCALEd by n and
+// saturated to int16 (packssdw) into o[0..7]: jidctint.c's algorithm with its products paired as pmaddwd forms them,
+// and x0 +- x4 and the odd part's z3 = x7 + x3, z4 = x5 + x1 summed in 16 bits.  No 32-bit sum can overflow.
+__device__ __forceinline__ void idct8(const short* x, int s, short* o, int os, int n) {
+  const int x0 = x[0], x1 = x[s], x2 = x[2 * s], x3 = x[3 * s], x4 = x[4 * s], x5 = x[5 * s], x6 = x[6 * s],
+            x7 = x[7 * s];
+  const int tmp3 = x2 * (F0541 + F0765) + x6 * F0541, tmp2 = x2 * F0541 + x6 * (F0541 - F1847);
+  const int tmp0 = s16(x0 + x4) * 8192, tmp1 = s16(x0 - x4) * 8192;
+  const int tmp10 = tmp0 + tmp3, tmp13 = tmp0 - tmp3, tmp11 = tmp1 + tmp2, tmp12 = tmp1 - tmp2;
+  const int z3 = s16(x7 + x3), z4 = s16(x5 + x1);
+  const int z3f = z3 * (F1175 - F1961) + z4 * F1175, z4f = z3 * F1175 + z4 * (F1175 - F0390);
+  const int t0 = x7 * (F0298 - F0899) + x1 * -F0899 + z3f, t3 = x7 * -F0899 + x1 * (F1501 - F0899) + z4f;
+  const int t1 = x5 * (F2053 - F2562) + x3 * -F2562 + z4f, t2 = x5 * -F2562 + x3 * (F3072 - F2562) + z3f;
+  const int r = 1 << (n - 1);
+  o[0] = sat16((tmp10 + t3 + r) >> n); o[7 * os] = sat16((tmp10 - t3 + r) >> n);
+  o[os] = sat16((tmp11 + t2 + r) >> n); o[6 * os] = sat16((tmp11 - t2 + r) >> n);
+  o[2 * os] = sat16((tmp12 + t1 + r) >> n); o[5 * os] = sat16((tmp12 - t1 + r) >> n);
+  o[3 * os] = sat16((tmp13 + t0 + r) >> n); o[4 * os] = sat16((tmp13 - t0 + r) >> n);
 }
 
 __global__ void jpeg_idct_kernel(const uint8_t* __restrict__ payload, const long long* __restrict__ desc, int B,
@@ -255,19 +249,30 @@ __global__ void jpeg_idct_kernel(const uint8_t* __restrict__ payload, const long
     const int* q = reinterpret_cast<const int*>(payload + d[D_Q0 + c]);
     alignas(16) short in[64];
     const int4* src = reinterpret_cast<const int4*>(coef + t * 64);
+    int ac = 0;                                               // OR of coefficient rows 1..7 (one int4 per row)
 #pragma unroll
-    for (int i = 0; i < 8; ++i) reinterpret_cast<int4*>(in)[i] = src[i];
-    int dq[64], ws[64];
+    for (int i = 0; i < 8; ++i) {
+      const int4 w = src[i];
+      reinterpret_cast<int4*>(in)[i] = w;
+      if (i > 0) ac |= w.x | w.y | w.z | w.w;
+    }
+    short dq[64], ws[64];
 #pragma unroll
-    for (int i = 0; i < 64; ++i) dq[i] = (int)in[i] * __ldg(q + i);
+    for (int i = 0; i < 64; ++i) dq[i] = (short)((int)in[i] * __ldg(q + i));   // pmullw: the low 16 bits
+    if (ac == 0) {
+      // pass 1's shortcut when every AC row is zero: each column is dq0 << 2, wrapped to 16 bits (psllw)
 #pragma unroll
-    for (int col = 0; col < 8; ++col) idct8(dq + col, 8, ws + col, 8, 11);     // pass 1: columns
+      for (int i = 0; i < 64; ++i) ws[i] = (short)(dq[i & 7] * 4);
+    } else {
+#pragma unroll
+      for (int col = 0; col < 8; ++col) idct8(dq + col, 8, ws + col, 8, 11);     // pass 1: columns
+    }
     alignas(8) uint8_t row[8];
-    long long o[8];
+    short o[8];
     for (int y = 0; y < 8; ++y) {
       idct8(ws + 8 * y, 1, o, 1, 18);                                         // pass 2: rows
 #pragma unroll
-      for (int i = 0; i < 8; ++i) row[i] = range_limit(o[i]);
+      for (int i = 0; i < 8; ++i) row[i] = (uint8_t)(o[i] < -128 ? 0 : (o[i] > 127 ? 255 : o[i] + 128));
       *reinterpret_cast<uint2*>(planes + plane + (by * 8 + y) * (bw * 8) + bx * 8) =
           *reinterpret_cast<const uint2*>(row);
     }

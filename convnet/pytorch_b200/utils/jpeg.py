@@ -3,7 +3,7 @@
 
 ``parse(data)`` walks SOI, APPn, DQT, DHT, SOF, DRI and SOS, locates the entropy-coded segment (ECS) and its restart
 markers, and returns a ``JpegInfo``.  ``info.device`` says whether csrc/jpeg.cu decodes the file to the bytes Pillow
-(libjpeg-turbo, ISLOW IDCT, fancy upsampling) gives for ``Image.open(f).convert('RGB')``:
+(libjpeg-turbo on x86-64: its SIMD ISLOW IDCT, fancy upsampling) gives for ``Image.open(f).convert('RGB')``:
   - SOF0 / SOF1, 8-bit samples, Huffman coding, one scan holding every component in frame order;
   - 1 component, or 3 with luma sampling 1x1, 2x1 or 2x2 and chroma 1x1;
   - a YCbCr colour space as libjpeg infers it (JFIF APP0, Adobe APP14 transform 1, or no Adobe marker and component
@@ -204,12 +204,14 @@ def _parse(d, info):
 
 def _locate_ecs(d, start, info):
     """The ECS runs from ``start`` to the first marker that is neither a stuffed 0xFF00 nor RSTn (the end of the data
-    when there is none: a truncated file keeps its bytes, and the decoder reports the premature end)."""
+    when there is none: a truncated file keeps its bytes, and the decoder reports the premature end).  0xFF fill bytes
+    before a marker (T.81 B.1.1.2) stay inside it: the decoders stop reading an interval at its first 0xFF that is not
+    stuffing."""
     a = np.frombuffer(d, np.uint8)
     ff = np.flatnonzero(a[start:-1] == 0xFF) + start
     nxt = a[ff + 1]
     is_rst = (nxt >= 0xD0) & (nxt <= 0xD7)
-    ends = ff[(nxt != 0) & ~is_rst]
+    ends = ff[(nxt != 0) & (nxt != 0xFF) & ~is_rst]
     end = int(ends[0]) if ends.size else len(a)
     info.ecs = (start, end)
     rst = ff[is_rst]

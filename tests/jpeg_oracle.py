@@ -1,5 +1,6 @@
-"""numpy restatement of the device JPEG decode (csrc/jpeg.cu): baseline Huffman decode, libjpeg's integer ISLOW IDCT
-with its range-limit table, fancy upsampling (h2v1, h2v2) and libjpeg's fixed-point YCbCr -> RGB.  It is the spec the
+"""numpy restatement of the device JPEG decode (csrc/jpeg.cu): baseline Huffman decode, the integer ISLOW IDCT as
+libjpeg-turbo's x86-64 SIMD code computes it (16-bit dequantisation and sums, saturating stores), fancy upsampling
+(h2v1, h2v2) and libjpeg's fixed-point YCbCr -> RGB.  It is the spec the
 kernels are written against; the CPU tests pin it to Pillow's decode and the GPU tests pin the kernels to Pillow.
 
 decode(data) -> uint8 [H, W, 3], the bytes of np.asarray(Image.open(f).convert('RGB')), for a file whose
@@ -86,41 +87,46 @@ _F = dict(f0298=2446, f0390=3196, f0541=4433, f0765=6270, f0899=7373, f1175=9633
           f1961=16069, f2053=16819, f2562=20995, f3072=25172)
 
 
-def _idct_1d(x0, x1, x2, x3, x4, x5, x6, x7, shift_in, descale):
-    """One pass of jidctint.c's jpeg_idct_islow over int64 arrays -> the 8 outputs, DESCALEd by ``descale``."""
+def s16(x):
+    """The low 16 bits of int64 values, as a signed int16 (two's-complement wrap)."""
+    return ((x + 32768) & 0xFFFF) - 32768
+
+
+def _idct_1d(x0, x1, x2, x3, x4, x5, x6, x7, descale):
+    """One pass of libjpeg-turbo's SIMD ISLOW IDCT (jidctint-sse2 / -avx2) over int64 arrays of int16 values -> the 8
+    outputs, DESCALEd by ``descale`` and saturated to int16.  It is jidctint.c's algorithm with the products paired
+    as its comments rewrite them (pmaddwd), and with x0 +- x4 and the odd part's z3 = x7 + x3, z4 = x5 + x1 added in
+    16 bits (paddw, wrapping)."""
     f = _F
-    z1 = (x2 + x6) * f['f0541']
-    tmp2 = z1 + x6 * -f['f1847']
-    tmp3 = z1 + x2 * f['f0765']
-    tmp0 = (x0 + x4) << 13
-    tmp1 = (x0 - x4) << 13
+    tmp3 = x2 * (f['f0541'] + f['f0765']) + x6 * f['f0541']
+    tmp2 = x2 * f['f0541'] + x6 * (f['f0541'] - f['f1847'])
+    tmp0 = s16(x0 + x4) << 13
+    tmp1 = s16(x0 - x4) << 13
     tmp10, tmp13, tmp11, tmp12 = tmp0 + tmp3, tmp0 - tmp3, tmp1 + tmp2, tmp1 - tmp2
-    t0, t1, t2, t3 = x7, x5, x3, x1
-    z1, z2, z3, z4 = t0 + t3, t1 + t2, t0 + t2, t1 + t3
-    z5 = (z3 + z4) * f['f1175']
-    t0, t1, t2, t3 = t0 * f['f0298'], t1 * f['f2053'], t2 * f['f3072'], t3 * f['f1501']
-    z1, z2 = z1 * -f['f0899'], z2 * -f['f2562']
-    z3, z4 = z3 * -f['f1961'] + z5, z4 * -f['f0390'] + z5
-    t0, t1, t2, t3 = t0 + z1 + z3, t1 + z2 + z4, t2 + z2 + z3, t3 + z1 + z4
+    z3, z4 = s16(x7 + x3), s16(x5 + x1)
+    z3, z4 = z3 * (f['f1175'] - f['f1961']) + z4 * f['f1175'], z3 * f['f1175'] + z4 * (f['f1175'] - f['f0390'])
+    t0 = x7 * (f['f0298'] - f['f0899']) + x1 * -f['f0899'] + z3
+    t3 = x7 * -f['f0899'] + x1 * (f['f1501'] - f['f0899']) + z4
+    t1 = x5 * (f['f2053'] - f['f2562']) + x3 * -f['f2562'] + z4
+    t2 = x5 * -f['f2562'] + x3 * (f['f3072'] - f['f2562']) + z3
     r = 1 << (descale - 1)
-    return [(v + r) >> descale for v in (tmp10 + t3, tmp11 + t2, tmp12 + t1, tmp13 + t0,
-                                          tmp13 - t0, tmp12 - t1, tmp11 - t2, tmp10 - t3)]
-
-
-def range_limit(x):
-    """libjpeg's IDCT range-limit table at (x & 1023): x + 128 clamped to [0, 255] for |x| < 384, wrapping beyond."""
-    k = x & 1023
-    return np.where(k < 128, k + 128, np.where(k < 512, 255, np.where(k < 896, 0, k - 896))).astype(np.uint8)
+    return [np.clip((v + r) >> descale, -32768, 32767) for v in (tmp10 + t3, tmp11 + t2, tmp12 + t1, tmp13 + t0,
+                                                                tmp13 - t0, tmp12 - t1, tmp11 - t2, tmp10 - t3)]
 
 
 def idct(blocks, q):
-    """int16 [..., 64] coefficient blocks, int [64] quantisation (natural order) -> uint8 [..., 8, 8] samples."""
-    c = blocks.astype(np.int64).reshape(-1, 8, 8) * np.asarray(q, np.int64).reshape(8, 8)
-    cols = _idct_1d(*[c[:, k, :] for k in range(8)], 0, 13 - 2)          # pass 1: columns, [N, 8 cols] per row
-    ws = np.stack(cols, axis=1)                                          # [N, row, col]
-    rows = _idct_1d(*[ws[:, :, k] for k in range(8)], 0, 13 + 2 + 3)      # pass 2: rows
+    """int16 [..., 64] coefficient blocks, int [64] quantisation (natural order) -> uint8 [..., 8, 8] samples, as
+    libjpeg-turbo's x86-64 SIMD ISLOW makes them: dequantisation keeps the low 16 bits of coef * q; a block whose
+    coefficient rows 1..7 are all zero takes the shortcut of pass 1, every column s16(dq0 << 2); the final store
+    saturates to [-128, 127] and adds 128."""
+    raw = blocks.astype(np.int64).reshape(-1, 8, 8)
+    c = s16(raw * np.asarray(q, np.int64).reshape(8, 8))
+    ws = np.stack(_idct_1d(*[c[:, k, :] for k in range(8)], 13 - 2), axis=1)    # pass 1: columns -> [N, row, col]
+    flat = ~raw[:, 1:, :].any(axis=(1, 2))
+    ws[flat] = s16(c[flat, 0:1, :] << 2)
+    rows = _idct_1d(*[ws[:, :, k] for k in range(8)], 13 + 2 + 3)              # pass 2: rows
     out = np.stack(rows, axis=2)
-    return range_limit(out).reshape(blocks.shape[:-1] + (8, 8))
+    return (np.clip(out, -128, 127) + 128).astype(np.uint8).reshape(blocks.shape[:-1] + (8, 8))
 
 
 def planes(data, info):
